@@ -2,12 +2,14 @@
 //
 // Same math as conv_gemm_tc.cu; differs in how the A operand reaches shared memory: instead of the LDGSTS
 // gather of that kernel, every [128 positions x 32 channels] atom is ONE cp.async.bulk.tensor (TMA) box of a
-// 3-D tensor map (channel, position, frustum) with hardware 128-byte swizzle.  M tiles are aligned to
-// frustums (tile = 128 consecutive positions of one frustum), so
-//   * kernel taps are a coordinate offset (t*stride + tap, may be -1): out-of-range rows are zero-filled by
-//     the TMA unit — that IS the conv zero padding (nn.Conv1d(..., padding=1));
+// 3-D tensor map (channel, position, frustum) with hardware 128-byte swizzle.  An M tile is 128
+// consecutive rows of the flattened (frustum, padded position) sequence (the maps are encoded with B = 1,
+// T = frustums x pitch), so
+//   * kernel taps are a coordinate offset (t*stride + tap, may be -1): the zero pad row(s) that follow every
+//     frustum, and the TMA unit's zero fill before the first and after the last row, ARE the conv zero padding
+//     (nn.Conv1d(..., padding=1)); a tap never reaches the neighbouring frustum's rows;
 //   * stride-2 convs use the map's elementStrides (box 256 -> 128 loaded rows);
-//   * rows past T never bleed into the next frustum (separate tensor dimension).
+//   * channels past ld and the K padding blocks are zero-filled by the TMA unit.
 // One elected thread issues A boxes + the weight bulk copy of a 64-wide K stage onto ONE mbarrier; two
 // consumer warpgroups (64 rows each) issue 8 wgmma per stage and store their accumulators.  No proxy fence,
 // no producer warps.

@@ -1,5 +1,7 @@
 // Self-test of the wgmma building blocks in isolation (descriptor encodings, swizzled operand
-// layouts, accumulator fragment layout): D[128 x N] = A[128 x K] * W[N x K]^T with one warpgroup.
+// layouts, accumulator fragment layout): D[128 x N] = A[128 x K] * W[N x K]^T with one warpgroup,
+// N in {64, 128, 256} (m64nNk8).  The two 64-row halves run one after the other, so at most 128
+// accumulators per thread are live (the N = 256 tile of the persistent FCN kernel).
 // A is written to shared memory by threads (as the PointNet epilogues do), W arrives as the
 // pre-swizzled stage image produced by the host packer through a bulk copy.
 #include "common.cuh"
@@ -36,30 +38,33 @@ wgmma_selftest_kernel(int K, const float *__restrict__ A, const uint8_t *__restr
     }
     __syncthreads();
     mbar_wait(bar, 0);
-    float acc[2][N / 2];
+    for (int h = 0; h < 2; ++h) {
+        float acc[N / 2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+        wgmma_fence();
+        fence_acc(acc);
+        for (int kb = 0; kb < KB; ++kb)
 #pragma unroll
-        for (int i = 0; i < N / 2; ++i) acc[h][i] = 0.f;
-    wgmma_fence();
-    fence_acc(acc[0]);
-    fence_acc(acc[1]);
-    for (int kb = 0; kb < KB; ++kb)
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-                wgmma_tf32<N>(acc[h], make_desc_sw128(smem_u32(sA) + kb * 16384 + h * 8192 + k * 32),
+            for (int k = 0; k < 4; ++k)
+                wgmma_tf32<N>(acc, make_desc_sw128(smem_u32(sA) + kb * 16384 + h * 8192 + k * 32),
                               make_desc_sw128(smem_u32(sW) + kb * N * 128 + k * 32), (kb | k) != 0);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_acc(acc[0]);
-    fence_acc(acc[1]);
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_acc(acc);
 #pragma unroll
         for (int i = 0; i < N / 2; ++i)
-            D[(size_t)(64 * h + frag_row(i, warp, lane)) * N + frag_col(i, lane)] = acc[h][i];
+            D[(size_t)(64 * h + frag_row(i, warp, lane)) * N + frag_col(i, lane)] = acc[i];
+    }
+}
+
+template <int N>
+static int launch_selftest(int K, const float *A, const void *w_img, float *D, cudaStream_t stream) {
+    const int smem = (K / 32) * (16384 + N * 128) + 8 + 1024;
+    FCN_CUDA(cudaFuncSetAttribute(wgmma_selftest_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    wgmma_selftest_kernel<N><<<1, 128, smem, stream>>>(K, A, (const uint8_t *)w_img, D);
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
 }
 
 }  // namespace fcn
@@ -68,17 +73,12 @@ using namespace fcn;
 
 extern "C" int fcn_selftest_umma(int N, int K, const float *A, const void *w_img, float *D,
                                  fcn_stream_t stream) {
-    FCN_REQUIRE(N == 64 || N == 128, "N must be 64 or 128");
-    FCN_REQUIRE(K >= 32 && K % 32 == 0 && K <= 256, "K must be a multiple of 32 in [32,256]");
+    FCN_REQUIRE(N == 64 || N == 128 || N == 256, "N must be 64, 128 or 256");
+    FCN_REQUIRE(K >= 32 && K % 32 == 0, "K must be a positive multiple of 32");
+    FCN_REQUIRE((K / 32) * (16384 + N * 128) + 8 + 1024 <= 232448,
+                "K too large for shared memory: K <= 256 (N = 64), 224 (N = 128), 128 (N = 256)");
     FCN_REQUIRE(A && w_img && D, "NULL pointer");
-    const int smem = (K / 32) * (16384 + N * 128) + 8 + 1024;
-    if (N == 64) {
-        FCN_CUDA(cudaFuncSetAttribute(wgmma_selftest_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        wgmma_selftest_kernel<64><<<1, 128, smem, (cudaStream_t)stream>>>(K, A, (const uint8_t *)w_img, D);
-    } else {
-        FCN_CUDA(cudaFuncSetAttribute(wgmma_selftest_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        wgmma_selftest_kernel<128><<<1, 128, smem, (cudaStream_t)stream>>>(K, A, (const uint8_t *)w_img, D);
-    }
-    FCN_LAUNCH_CHECK();
-    return FCN_OK;
+    if (N == 64) return launch_selftest<64>(K, A, w_img, D, (cudaStream_t)stream);
+    if (N == 128) return launch_selftest<128>(K, A, w_img, D, (cudaStream_t)stream);
+    return launch_selftest<256>(K, A, w_img, D, (cudaStream_t)stream);
 }

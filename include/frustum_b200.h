@@ -107,6 +107,8 @@ FCN_API int fcn_group_rows(const fcn_group_args *args, fcn_stream_t stream);
  *                PointNetModule.forward (det_base.py:103); rows must come from unique_rows=0.
  *     precision: 0 = fp32 SIMT, 1 = TF32 tensor cores (wgmma) for the C1->C2->C3 layers,
  *                2 = same on 2-CTA clusters, weight stages multicast to both CTAs (C1 >= 128).
+ *     Tiles: the rows of one section are contiguous within a tile (a section may continue in another tile);
+ *     record slots past a tile's nrows are never read.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
     int C1, C2, C3, T, K, ld_feat, row_cap, tile_rows, unpooled, precision, B;
@@ -132,6 +134,7 @@ FCN_API int fcn_pointnet_tiles(const fcn_pointnet_args *args, fcn_stream_t strea
  *       out[b, t*up + j, c_off + co] = act( sum_seg sum_c src[b, t*stride + tap, c] * W + bias )
  *     K is the concatenation of the segments, each padded to a multiple of 32 (zero weights); K_pad
  *     is that sum, optionally rounded up to a multiple of 64 (required by the tensor-core variants).
+ *     The channel pad [C, ld) of a source is read (against those zero weights) and must hold finite values.
  *     wt: [K_pad][n_cols] fp32 (n_cols = up*Cout rounded up to 64), bias: [n_cols].
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
@@ -397,8 +400,9 @@ FCN_API int fcn_btc_to_bct(int B, int C, int T, int pitch, int ld, const float *
                            fcn_stream_t stream);
 
 /* Self-test of the wgmma/bulk-copy building blocks: D (128,N) = A (128,K) * W^T with W given
- * as the pre-swizzled stage image of the host packer (engine.pack_sw128).  N in {64,128},
- * K multiple of 32 (<= 256).  Used by tests/ to pin the descriptor encodings on real hardware. */
+ * as the pre-swizzled stage image of the host packer (engine.pack_sw128).  N in {64,128,256},
+ * K multiple of 32 that fits shared memory: K <= 256 (N = 64), 224 (N = 128), 128 (N = 256).
+ * Used by tests/ to pin the descriptor encodings on real hardware. */
 FCN_API int fcn_selftest_umma(int N, int K, const float *A, const void *w_img, float *D,
                               fcn_stream_t stream);
 

@@ -19,7 +19,7 @@ pytestmark = pytest.mark.gpu
 TF32_TOL = 2.5e-3
 
 
-@pytest.mark.parametrize("N,K", [(128, 32), (128, 64), (64, 64), (128, 192), (64, 128), (64, 256)])
+@pytest.mark.parametrize("N,K", [(128, 32), (128, 64), (64, 64), (128, 192), (64, 128), (64, 256), (256, 128)])
 def test_umma_selftest_matches_fp64_matmul(N, K):
     from frustum_convnet_b200 import _lib
     from frustum_convnet_b200.engine import pack_sw128, tf32_rna
@@ -36,6 +36,36 @@ def test_umma_selftest_matches_fp64_matmul(N, K):
     err = float((D.cpu().double() - ref).abs().max())
     print("umma selftest N=%d K=%d max err %.3e" % (N, K, err))
     assert err < 1e-3 * max(1.0, float(ref.abs().max())), err
+
+
+@pytest.mark.parametrize("N,K", [(64, 256), (128, 224), (256, 128), (256, 32)])
+def test_umma_selftest_exact_integer_operands(N, K):
+    """m64nNk8 for N = 64, 128, 256 with integer operands (every partial sum an integer < 2^22, so the fp32
+    accumulation is exact in any order): the product must be bit-identical to the int64 matmul."""
+    from frustum_convnet_b200 import _lib
+    from frustum_convnet_b200.engine import pack_sw128
+    g = torch.Generator().manual_seed(N + K)
+    A = torch.randint(-1000, 1001, (128, K), generator=g)       # < 2^11: TF32 values
+    W = torch.randint(-15, 16, (N, K), generator=g)
+    assert int((A.abs() @ W.abs().t()).max()) < (1 << 22)
+    img = pack_sw128(W.float().to(dev()), N)
+    D = torch.full((128, N), float("nan"), device=dev())
+    Ad = A.float().to(dev()).contiguous()
+    _lib.call("fcn_selftest_umma", N, K, Ad.data_ptr(), img.data_ptr(), D.data_ptr(),
+              torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    ref = (A @ W.t()).float()
+    bad = int((D.cpu() != ref).sum())
+    assert bad == 0, "%d of %d elements differ from the exact product" % (bad, ref.numel())
+
+
+def test_umma_selftest_rejects_k_beyond_shared_memory():
+    from frustum_convnet_b200 import _lib
+    x = torch.zeros(128 * 256, device=dev())
+    for N, K in ((128, 256), (256, 160)):
+        with pytest.raises(RuntimeError, match="shared memory"):
+            _lib.call("fcn_selftest_umma", N, K, x.data_ptr(), x.data_ptr(), x.data_ptr(),
+                      torch.cuda.current_stream().cuda_stream)
 
 
 @pytest.mark.parametrize("cluster", ["1", "0"])
