@@ -164,6 +164,27 @@ class InputArgs(C.Structure):
                 ("rot_angle", C.c_void_p)]
 
 
+class DetRecord(C.Structure):
+    _fields_ = [("seg", C.c_int32), ("frustum", C.c_int32), ("t", C.c_int32), ("reserved", C.c_int32),
+                ("box", C.c_float * 8)]
+
+
+class DetCandidateArgs(C.Structure):
+    _fields_ = [("B", C.c_int), ("T2", C.c_int), ("NS", C.c_int), ("dataset", C.c_int), ("method", C.c_int),
+                ("first", C.c_int), ("num_frustums", C.c_int), ("capacity", C.c_int)] + \
+               [(n, C.c_void_p) for n in ("cls_probs", "center", "heading", "size", "size_probs", "rot_angle",
+                                          "rgb_prob", "ref_center", "seg_of_frustum", "counter", "records")]
+
+
+class DetFinalizeArgs(C.Structure):
+    _fields_ = [("num_segments", C.c_int), ("num_frustums", C.c_int), ("capacity", C.c_int), ("method", C.c_int),
+                ("dataset", C.c_int), ("top_k", C.c_int), ("thresh", C.c_float), ("n_counted", C.c_int),
+                ("counter", C.c_void_p), ("records", C.c_void_p), ("box2d", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_longlong), ("info", C.c_void_p),
+                ("seg_offsets", C.c_void_p), ("keep_count", C.c_void_p), ("rows", C.c_void_p),
+                ("mask", C.c_void_p), ("mask_words", C.c_longlong)]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -195,6 +216,10 @@ SIGNATURES = {
     "fcn_ipc_open": (_I, [_P, C.POINTER(C.c_void_p)]),
     "fcn_ipc_close": (_I, [_P]),
     "fcn_rbbox_iou_3d_pair": (_I, [_I, _P, _P, _P, _F, _P, _P]),
+    "fcn_det_candidates": (_I, [C.POINTER(DetCandidateArgs), _P]),
+    "fcn_det_workspace_bytes": (C.c_longlong, [_I, _I]),
+    "fcn_det_prepare": (_I, [C.POINTER(DetFinalizeArgs), _P]),
+    "fcn_det_select": (_I, [C.POINTER(DetFinalizeArgs), _P]),
 }
 
 _lib = None

@@ -12,6 +12,7 @@
 //      metric, incl. its degenerate-ring rule) is >= thresh (nms_cpu.h:226-227);
 //   4. greedy scan in rank order by one warp (keep i unless suppressed, then OR row i into the suppressed set);
 //   5. the first top_k kept indices (rbbox_iou.py:311 `keep[:top_k]`) in rank order, count per segment.
+#include "box_corners.cuh"
 #include "box_iou.cuh"
 #include "common.cuh"
 
@@ -20,21 +21,6 @@ namespace fcn {
 constexpr int NMS_MAX_DETS = 512;
 constexpr int NMS_WORDS = NMS_MAX_DETS / 32;
 constexpr int NMS_THREADS = 256;
-
-// corners in the reference order (rbbox_iou.py:131-147 == models/model_util.py:48-72)
-__device__ __forceinline__ void box_to_corners(const float *d, float *c) {
-    const float cx = d[0], cy = d[1], cz = d[2], l = d[3], w = d[4], h = d[5], r = d[6];
-    const float cs = cosf(r), sn = sinf(r);
-    const float xs[8] = {l / 2, l / 2, -l / 2, -l / 2, l / 2, l / 2, -l / 2, -l / 2};
-    const float ys[8] = {h / 2, h / 2, h / 2, h / 2, -h / 2, -h / 2, -h / 2, -h / 2};
-    const float zs[8] = {w / 2, -w / 2, -w / 2, w / 2, w / 2, -w / 2, -w / 2, w / 2};
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        c[3 * i + 0] = cs * xs[i] + sn * zs[i] + cx;
-        c[3 * i + 1] = ys[i] + cy;
-        c[3 * i + 2] = -sn * xs[i] + cs * zs[i] + cz;
-    }
-}
 
 __global__ void __launch_bounds__(NMS_THREADS)
 nms3d_kernel(const float *__restrict__ dets, const int *__restrict__ seg_offsets, float thresh, int top_k,
@@ -85,10 +71,7 @@ nms3d_kernel(const float *__restrict__ dets, const int *__restrict__ seg_offsets
         while (rem >= n - 1 - i) { rem -= n - 1 - i; ++i; }
         const int j = i + 1 + rem;
         const float *a = cube + i * 6, *b = cube + j * 6;
-        // standup IoU > 0 <=> the bounding cubes overlap with positive volume (rbbox_iou.py:62-96)
-        const bool cubes = fminf(a[3], b[3]) - fmaxf(a[0], b[0]) > 0.f && fminf(a[4], b[4]) - fmaxf(a[1], b[1]) > 0.f &&
-                           fminf(a[5], b[5]) - fmaxf(a[2], b[2]) > 0.f;
-        if (!cubes) continue;
+        if (!cubes_overlap(a, b)) continue;      // standup IoU > 0 (rbbox_iou.py:62-96)
         float iou[2];
         rbbox_iou_pair(corners + i * 24, corners + j * 24, iou);
         if (iou[1] >= thresh) atomicOr(&mask[i * NMS_WORDS + (j >> 5)], 1u << (j & 31));

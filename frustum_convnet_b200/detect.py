@@ -1,0 +1,156 @@
+"""Per-image 3-D detections on the device: the step between the forward and the result files of
+train/test_net_det.py:243-305 (test_net_det_sunrgbd.py:197-266), with no per-batch host copy.
+
+    col = DetectionCollector(test_dataset.id_list, test_dataset.type_list, test_dataset.box2d_list,
+                             dataset=cfg.DATA.DATASET_NAME, method=cfg.TEST.METHOD, thresh=cfg.TEST.THRESH)
+    for i, data_dicts in enumerate(test_loader):
+        outputs = model(data_dicts_var)
+        col.add(outputs, data_dicts_var, first=load_batch_size * i)   # one launch, no host sync, capturable
+    nms_results = col.finalize()      # == the dict test() hands to write_detection_results
+
+`add` appends the foreground rows of a batch to device records (csrc/detect.cu, ``fcn_det_candidates``);
+`finalize` orders them as the reference's lists, runs rotated 3-D NMS on every image x class list of any length and
+returns {data_idx: {class_type: float32 (n, 12)}} in the reference's dict order, zero-row lists included (as
+(0, 12) arrays).  The collector belongs to one process and one device.  No CPU fallback: CPU tensors raise."""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+
+from . import _lib
+
+_DATASETS = {"KITTI": 0, "SUNRGBD": 1}
+_METHODS = {"nms": 0}          # every other cfg.TEST.METHOD behaves as 'top' (test_net_det.py:256-263)
+
+
+class DetectionCollector:
+    def __init__(self, id_list, type_list, box2d_list, dataset="KITTI", method="nms", thresh=0.1, top_k=300,
+                 capacity=None, device=None):
+        if dataset not in _DATASETS:
+            raise ValueError("dataset must be one of %s" % sorted(_DATASETS))
+        n = len(id_list)
+        if len(type_list) != n or len(box2d_list) != n:
+            raise ValueError("id_list, type_list and box2d_list must have the same length")
+        self.dataset, self.method = dataset, ("nms" if method == "nms" else "top")
+        self.thresh, self.top_k = float(thresh), int(top_k)
+        self.num_frustums = n
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        if self.device.type != "cuda":
+            raise RuntimeError("DetectionCollector: a CUDA device is required (there is no CPU fallback)")
+        # segment table in the reference's dict order: images by first appearance, classes by first appearance
+        # within the image (test_net_det.py:278-282)
+        seg_of, self.segments = {}, []
+        table = np.empty(n, dtype=np.int32)
+        for f in range(n):
+            key = (id_list[f], type_list[f])
+            s = seg_of.get(key)
+            if s is None:
+                s = seg_of[key] = len(self.segments)
+                self.segments.append(key)
+            table[f] = s
+        self._seg_host = table
+        self.capacity = int(capacity) if capacity is not None else max(65536, 16 * n)
+        dev = self.device
+        self.seg_of_frustum = torch.from_numpy(table).to(dev)
+        self.box2d = torch.from_numpy(np.asarray(box2d_list, dtype=np.float32).reshape(n, 4)).to(dev)
+        self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.records = torch.empty((max(self.capacity, 1), 12), dtype=torch.int32, device=dev)   # fcn_det_record
+        self.added = np.zeros(n, dtype=bool)
+        self._streams = {}
+
+    def reset(self):
+        """Start a new pass (stream-ordered on the current stream)."""
+        self.counter.zero_()
+        self.added[:] = False
+        self._streams = {}
+
+    def add(self, outputs, data_dicts, first):
+        """Append the rows of one batch: `outputs` = the model's six-tuple, `data_dicts` supplies rot_angle and the
+        optional rgb_prob / ref_center, frustum b of the batch is dataset entry first + b.  One launch on the
+        current stream; no host sync, so it may be captured in a CUDA graph (a captured add marks its frustums when
+        it is captured, and every replay appends its rows again)."""
+        cls_probs, center, heading, size, _, size_probs = outputs
+        for t in (cls_probs, center, heading, size, size_probs):
+            if not t.is_cuda:
+                raise RuntimeError("DetectionCollector.add: CUDA tensors required (there is no CPU fallback)")
+        B, T2 = int(cls_probs.shape[0]), int(cls_probs.shape[1])
+        first = int(first)
+        if first < 0 or first + B > self.num_frustums:
+            raise ValueError("frustums [%d, %d) are outside the dataset of %d" % (first, first + B, self.num_frustums))
+        f32 = lambda t: t.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        keep_alive = [f32(cls_probs), f32(center), f32(heading).reshape(B, T2), f32(size), f32(size_probs)]
+        rot = data_dicts["rot_angle"]
+        if not rot.is_cuda:
+            raise RuntimeError("DetectionCollector.add: rot_angle must be a CUDA tensor")
+        keep_alive.append(f32(rot).reshape(B))
+        opt = []
+        for k, shape in (("rgb_prob", (B,)), ("ref_center", (B, 3))):
+            v = data_dicts.get(k)
+            if v is not None:
+                if not v.is_cuda:
+                    raise RuntimeError("DetectionCollector.add: %s must be a CUDA tensor" % k)
+                v = f32(v).reshape(shape)
+                keep_alive.append(v)
+            opt.append(v)
+        cp, ce, he, sz, sp, ra = keep_alive[:6]
+        a = _lib.DetCandidateArgs()
+        a.B, a.T2, a.NS = B, T2, int(sp.shape[-1])
+        a.dataset, a.method = _DATASETS[self.dataset], _METHODS.get(self.method, 1)
+        a.first, a.num_frustums, a.capacity = first, self.num_frustums, self.capacity
+        a.cls_probs, a.center, a.heading, a.size, a.size_probs = (t.data_ptr() for t in (cp, ce, he, sz, sp))
+        a.rot_angle = ra.data_ptr()
+        a.rgb_prob = opt[0].data_ptr() if opt[0] is not None else None
+        a.ref_center = opt[1].data_ptr() if opt[1] is not None else None
+        a.seg_of_frustum, a.counter, a.records = (self.seg_of_frustum.data_ptr(), self.counter.data_ptr(),
+                                                  self.records.data_ptr())
+        stream = torch.cuda.current_stream(self.device)
+        with torch.cuda.device(self.device):
+            _lib.call("fcn_det_candidates", C.byref(a), stream.cuda_stream)
+        self._streams[stream.cuda_stream] = stream
+        self.added[first:first + B] = True
+
+    def finalize(self):
+        """-> {data_idx: {class_type: float32 (n, 12)}}; one host sync to size the NMS bit matrix, one copy back."""
+        dev = self.device
+        cur = torch.cuda.current_stream(dev)
+        for st in self._streams.values():
+            if st.cuda_stream != cur.cuda_stream:
+                cur.wait_stream(st)
+        S = len(self.segments)
+        with torch.cuda.device(dev):
+            nbytes = _lib.load().fcn_det_workspace_bytes(self.capacity, S)
+            if nbytes < 0:
+                _lib.check(-1, "fcn_det_workspace_bytes")
+            ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+            info = torch.zeros(4, dtype=torch.int64, device=dev)
+            off = torch.zeros(S + 1, dtype=torch.int32, device=dev)
+            kc = torch.zeros(max(S, 1), dtype=torch.int32, device=dev)
+            rows = torch.empty((max(self.capacity, 1), 12), dtype=torch.float32, device=dev)
+            a = _lib.DetFinalizeArgs()
+            a.num_segments, a.num_frustums, a.capacity = S, self.num_frustums, self.capacity
+            a.method, a.dataset = _METHODS.get(self.method, 1), _DATASETS[self.dataset]
+            a.top_k, a.thresh = self.top_k, self.thresh
+            a.counter, a.records, a.box2d = self.counter.data_ptr(), self.records.data_ptr(), self.box2d.data_ptr()
+            a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), int(nbytes), info.data_ptr()
+            a.seg_offsets, a.keep_count, a.rows = off.data_ptr(), kc.data_ptr(), rows.data_ptr()
+            _lib.call("fcn_det_prepare", C.byref(a), cur.cuda_stream)
+            n_counted, mask_words = (int(v) for v in info[:2].tolist())          # the one host sync
+            a.n_counted = n_counted
+            mask = torch.empty(max(mask_words, 1), dtype=torch.int32, device=dev)
+            a.mask, a.mask_words = mask.data_ptr(), mask_words
+            _lib.call("fcn_det_select", C.byref(a), cur.cuda_stream)
+            n = n_counted
+            rows_h = rows[:n].cpu().numpy()
+            off_h, kc_h = off.cpu().numpy(), kc[:S].cpu().numpy()
+        self.last_counts = {"rows": n, "kept": int(kc_h.sum()) if S else 0}
+        # dict order of the frustums that were added, in dataset order
+        segs = self._seg_host[self.added]
+        _, first_pos = np.unique(segs, return_index=True)
+        order = segs[np.sort(first_pos)]
+        res = {}
+        for s in order:
+            idx, ct = self.segments[s]
+            res.setdefault(idx, {})[ct] = rows_h[off_h[s]: off_h[s] + kc_h[s]].copy()
+        return res

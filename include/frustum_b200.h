@@ -419,6 +419,73 @@ FCN_API int fcn_selftest_umma(int N, int K, const float *A, const void *w_img, f
 FCN_API int fcn_rbbox_iou_3d_pair(int M, const float *corners, const float *qcorners, float *iou,
                                   float iou_thresh, float *stats, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (10) Per-image 3-D detections on the device.  Replaces the host loop of train/test_net_det.py:243-293
+ *      (test_net_det_sunrgbd.py:197-252) and write_detection_results_nms (:126-152 / :120-145): foreground
+ *      selection, from_prediction_to_label_format, the image x class grouping and rotated 3-D NMS of lists of
+ *      any length.
+ *
+ *      fcn_det_candidates (once per batch, no host sync, capturable): one CTA per frustum b selects its
+ *      foreground positions t (method 0 'nms': KITTI p0 < p1, SUN-RGBD p1 > 0.5, else the first argmax of p1;
+ *      method 1 'top': the first argmax), scores them (KITTI p1 + rgb_prob, SUN-RGBD rgb_prob + max size_prob),
+ *      decodes them in fp32 (ry = heading + rot_angle; centre rotated by -rot_angle about y, + ref_center,
+ *      KITTI: ty += h/2), drops boxes with h, w or l < 0.01 and appends one record per row.  Rows are reserved
+ *      with one atomicAdd on *counter per frustum; rows at or past `capacity` are counted but not written.
+ *      seg_of_frustum[first + b] is the dense image x class id of frustum b.  rgb_prob (B) and ref_center
+ *      (B,3) may be NULL (1 and 0).  Outputs are contiguous: cls_probs (B,T2,2), center (B,T2,3),
+ *      heading (B,T2), size (B,T2,3) = (l, w, h), size_probs (B,T2,NS).
+ *
+ *      Finalize (once per pass, two calls around one host read of `info`):
+ *        fcn_det_prepare : orders the records by (segment, frustum, t) - the reference's list order whichever
+ *                          call or stream appended them - and, for 'nms', ranks every segment by descending
+ *                          score (ties: larger list index first); writes seg_offsets (S+1) and
+ *                          info = {rows counted, mask words needed, pair tiles, 0} (int64).
+ *        fcn_det_select  : needs n_counted = info[0] <= capacity (else an error naming the capacity needed) and
+ *                          a `mask` of >= info[1] words (no initialisation needed).  'nms': suppression bits of all
+ *                          pairs of every segment (bounding cubes overlap, then rotated 3-D IoU >= thresh), tiled
+ *                          32 x 32 over the whole grid; greedy scan per segment; keep[:top_k].  'top': every row.
+ *                          rows (capacity, 12): kept row k of segment s at seg_offsets[s] + k, k < keep_count[s],
+ *                          KITTI [x1,y1,x2,y2, tx,ty,tz, h,w,l, ry, score], SUN-RGBD [.., tx,ty,tz, l,w,h, ry, score],
+ *                          box2d (num_frustums, 4) gives the first four columns.
+ *      fcn_det_workspace_bytes = the workspace both finalize calls share (needs the device; -1 on error).
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_DET_KITTI 0
+#define FCN_DET_SUNRGBD 1
+#define FCN_DET_NMS 0
+#define FCN_DET_TOP 1
+typedef struct {
+    int32_t seg, frustum, t, reserved;
+    float box[8];                  /* tx, ty, tz, l, w, h, ry, score: the NMS box and the label-format values */
+} fcn_det_record;
+typedef struct {
+    int B, T2, NS, dataset, method, first, num_frustums, capacity;
+    const float *cls_probs, *center, *heading, *size, *size_probs;
+    const float *rot_angle, *rgb_prob, *ref_center;
+    const int32_t *seg_of_frustum; /* (num_frustums) */
+    int32_t *counter;              /* device scalar, zeroed by the caller before the pass */
+    fcn_det_record *records;       /* (capacity) */
+} fcn_det_candidate_args;
+FCN_API int fcn_det_candidates(const fcn_det_candidate_args *args, fcn_stream_t stream);
+typedef struct {
+    int num_segments, num_frustums, capacity, method, dataset, top_k;
+    float thresh;
+    int n_counted;                 /* fcn_det_select: info[0] as read by the host */
+    const int32_t *counter;
+    const fcn_det_record *records;
+    const float *box2d;            /* (num_frustums, 4) */
+    void *workspace;
+    long long workspace_bytes;
+    long long *info;               /* device int64[4] */
+    int32_t *seg_offsets;          /* (num_segments + 1) */
+    int32_t *keep_count;           /* (num_segments) */
+    float *rows;                   /* (capacity, 12) */
+    uint32_t *mask;                /* fcn_det_select, method 'nms': >= info[1] words (may be NULL when info[1] == 0) */
+    long long mask_words;
+} fcn_det_finalize_args;
+FCN_API long long fcn_det_workspace_bytes(int capacity, int num_segments);
+FCN_API int fcn_det_prepare(const fcn_det_finalize_args *args, fcn_stream_t stream);
+FCN_API int fcn_det_select(const fcn_det_finalize_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
