@@ -185,6 +185,29 @@ class DetFinalizeArgs(C.Structure):
                 ("mask", C.c_void_p), ("mask_words", C.c_longlong)]
 
 
+TRAIN_DET, TRAIN_REFINE = 0, 1
+
+
+class TrainFrustum(C.Structure):
+    _fields_ = [("rot", C.c_double), ("cs", C.c_double), ("sn", C.c_double),
+                ("box2d", C.c_double * 4), ("P", C.c_double * 12), ("ref_center", C.c_double * 3),
+                ("line0", C.c_double * 3), ("line_delta", C.c_double * 3), ("z_start", C.c_double),
+                ("z_step", C.c_double * MAX_SCALES), ("center", C.c_double * 3), ("heading", C.c_double),
+                ("size", C.c_double * 3), ("dist", C.c_double), ("rgb_prob", C.c_double),
+                ("T", C.c_int32 * MAX_SCALES), ("cls_index", C.c_int32), ("reserved", C.c_int32)]
+
+
+class TrainInputArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("kind", "labels", "rtc", "extra_feat", "random_flip", "random_shift", "B", "N",
+                                        "num_scales", "num_classes", "num_frustums", "points_f64")] + \
+               [("stride", C.c_double * MAX_SCALES), ("max_depth", C.c_double)] + \
+               [(n, C.c_void_p) for n in ("points", "point_offsets", "seg", "frustums", "index", "choice", "flip_u",
+                                          "shift_n", "point_cloud")] + \
+               [("centers", C.c_void_p * MAX_SCALES)] + \
+               [(n, C.c_void_p) for n in ("cls_label", "seg_label", "box3d_center", "box3d_heading", "box3d_size",
+                                          "size_class", "rot_angle", "one_hot", "ref_center", "rgb_prob")]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -220,6 +243,7 @@ SIGNATURES = {
     "fcn_det_workspace_bytes": (C.c_longlong, [_I, _I]),
     "fcn_det_prepare": (_I, [C.POINTER(DetFinalizeArgs), _P]),
     "fcn_det_select": (_I, [C.POINTER(DetFinalizeArgs), _P]),
+    "fcn_build_train_inputs": (_I, [C.POINTER(TrainInputArgs), _P]),
 }
 
 _lib = None

@@ -10,15 +10,15 @@
 // Arithmetic is float64 with the float32 casts exactly where numpy makes them, so results are bit-identical to
 // the reference up to the last-ulp difference between CUDA's and glibc's double sin/cos.
 #include "common.cuh"
+#include "input_builder.cuh"
 
 namespace fcn {
 
 __global__ void __launch_bounds__(256)
 build_inputs_kernel(const __grid_constant__ fcn_input_args a) {
     const int b = blockIdx.x, tid = threadIdx.x;
-    const double rot = 1.5707963267948966 + a.frustum_angle[b];      // np.pi / 2.0 + frustum_angle
     double sn, cs;
-    sincos(rot, &sn, &cs);
+    const double rot = centre_view_angle(a.frustum_angle[b], &sn, &cs);
     if (tid == 0 && a.rot_angle != nullptr) a.rot_angle[b] = (float)rot;
     // ---- resampled, centre-view rotated point cloud (B,3,N)
     const float *pts = a.points + 3 * (size_t)a.point_offsets[b];
@@ -27,28 +27,26 @@ build_inputs_kernel(const __grid_constant__ fcn_input_args a) {
     for (int j = tid; j < a.N; j += blockDim.x) {
         int i = a.choice[(size_t)b * a.N + j];
         i = i < 0 ? 0 : (i >= n_raw ? n_raw - 1 : i);               // defensive clamp (valid inputs are in range)
-        const double x = (double)pts[3 * i], z = (double)pts[3 * i + 2];
-        // pc[:, [0, 2]] = dot(pc[:, [0, 2]], rotmat.T), rotmat = [[c, -s], [s, c]]  ->  x' = x c - z s, z' = x s + z c
-        pc[j] = (float)(x * cs - z * sn);
+        double x, z;
+        rotate_y<false>((double)pts[3 * i], (double)pts[3 * i + 2], cs, sn, &x, &z);
+        pc[j] = (float)x;
         pc[a.N + j] = pts[3 * i + 1];
-        pc[2 * a.N + j] = (float)(x * sn + z * cs);
+        pc[2 * a.N + j] = (float)z;
     }
     // ---- section centres of every scale
-    const double *bx = a.box2d + 4 * (size_t)b, *P = a.P + 12 * (size_t)b;
-    const double cx = (bx[0] + bx[2]) / 2.0, cy = (bx[1] + bx[3]) / 2.0;
-    const double c_u = P[2], c_v = P[6], f_u = P[0], f_v = P[5];
-    const double b_x = P[3] / (-f_u), b_y = P[7] / (-f_v);
+    const RectProjection proj(a.box2d + 4 * (size_t)b, a.P + 12 * (size_t)b);
     for (int s = 0; s < a.num_scales; ++s) {
         const int T = a.T[s];
         const double st = a.stride[s];
         float *c = a.centers[s] + (size_t)b * 3 * T;
         for (int t = tid; t < T; t += blockDim.x) {
-            const double z = (double)t * st + st / 2.0;              // np.arange(0, max_depth, s) + s / 2.
-            const double x = ((cx - c_u) * z) / f_u + b_x;
-            const double y = ((cy - c_v) * z) / f_v + b_y;
-            c[t] = (float)(x * cs - z * sn);
+            const double z = section_depth<false>(t, st);
+            double x, y, xr, zr;
+            proj.at(z, &x, &y);
+            rotate_y<false>(x, z, cs, sn, &xr, &zr);
+            c[t] = (float)xr;
             c[T + t] = (float)y;
-            c[2 * T + t] = (float)(x * sn + z * cs);
+            c[2 * T + t] = (float)zr;
         }
     }
     if (a.one_hot != nullptr)

@@ -486,6 +486,77 @@ FCN_API long long fcn_det_workspace_bytes(int capacity, int num_segments);
 FCN_API int fcn_det_prepare(const fcn_det_finalize_args *args, fcn_stream_t stream);
 FCN_API int fcn_det_select(const fcn_det_finalize_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (11) Labelled training batches on the device: ProviderDataset.__getitem__ + collate for a whole batch in one
+ *      launch (one CTA per item, no host sync, no allocation, capturable), from a dataset resident in HBM.
+ *      cfg.DATA.RTC = True and WITH_EXTRA_FEAT = False only (every reference cfg); anything else is rejected.
+ *        FCN_TRAIN_DET, labels = 1     datasets/provider_sample.py:133-270 (train branch), generate_labels :272-289,
+ *                                      generate_ref :291-327, default_collate
+ *        FCN_TRAIN_REFINE, labels = 1  datasets/provider_sample_refine.py:174-316 (train branch), generate_labels
+ *                                      :318-334, generate_ref :336-385, collate_fn :388-419
+ *        FCN_TRAIN_REFINE, labels = 0  the same file's from_rgb_detection branch :228-248 (no labels, no augmentation)
+ *      Per frustum the host stores one fcn_train_frustum of float64 values computed ONCE with the reference's own
+ *      numpy expressions (exact by construction); per step only index (B), choice (B,N), flip_u (B), shift_n (B)
+ *      cross PCIe (the caller's np.random draws, :164-166,227,241 / :207,270,284).  The kernel does the rest in
+ *      float64 with every product and sum rounded separately, casting where numpy casts:
+ *        point_cloud (B,3,N)   points[choice] rotated to the centre view (det: rot = pi/2 + frustum_angle, :157,354-362;
+ *                              refine: minus the predicted centre, rotated by the predicted angle, :149-154,199), cast
+ *                              to the dataset's dtype (points_f64 = 0: float32), x negated when flip_u > 0.5
+ *                              (:227-235 / :270-278), z += shift (:237-244 / :280-286), then float32;
+ *        centers[s] (B,3,P_s)  det: project_image_to_rect of the 2-D box centre at arange(0, max_depth, s) + s/2,
+ *                              rotated; refine: the predicted box's line from its front to its back face mean at
+ *                              arange(z_start, ., s) + s/2 (arange element i = z_start + i * z_step[s]); x negated by
+ *                              the flip.  P_s = max over the batch of T[s] of the items (collate_fn :388-419 pads
+ *                              with mode='edge': columns >= T[s] of an item repeat its last column);
+ *        cls_label (B,P_2)     int64 on the float64 ref2: -1 inside the full box (det 1.0x, refine 0.6x the GT size),
+ *                              1 inside the half box (det 0.5x, refine 0.3x), 1 at the first argmin of the distance
+ *                              to the GT centre when no ref is inside the half box; edge padded like the refs.  The
+ *                              inside test is the half-space test in the box frame (the reference uses a Delaunay
+ *                              triangulation of the 8 corners, data_utils.py:24-34: they differ within ~1e-15 m of a face);
+ *        box3d_center (B,3), box3d_heading (B,1), box3d_size (B,3) float32, size_class (B,1) int64: the GT box in the
+ *                              frame of the inputs, flipped (heading = pi - heading) and shifted like the points;
+ *        seg_label (B,N)       int64 (det only), rot_angle (B,1), one_hot (B,num_classes) (NULL: none), ref_center
+ *                              (B,3) (refine), rgb_prob (B,1) (refine, labels = 0).
+ *      Shift: det clip(n * dist * 0.2, +-0.5 dist), then clip(shift + c_z, 0, max_depth) - c_z; refine
+ *      clip(n * dist * 0.1, +-2 stride[0]); dist = sqrt(l^2 + w^2) of the GT size.
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_TRAIN_DET 0
+#define FCN_TRAIN_REFINE 1
+typedef struct {
+    double rot, cs, sn;            /* rot_angle output and np.cos / np.sin of the centre-view rotation angle */
+    double box2d[4], P[12];        /* det: 2-D box x1, y1, x2, y2 and calib P2 (row-major 3x4) */
+    double ref_center[3];          /* refine: predicted box centre (pred_box3d[0] + pred_box3d[6]) / 2 */
+    double line0[3], line_delta[3];/* refine: front face mean of the centre-view predicted box, back mean - front mean */
+    double z_start;                /* refine: min z of the centre-view predicted box (the arange start) */
+    double z_step[FCN_MAX_SCALES]; /* refine: (z_start + s) - z_start, numpy's arange increment */
+    double center[3], heading;     /* GT centre and heading in the frame of the inputs (before flip / shift) */
+    double size[3], dist;          /* GT size (l, w, h) and sqrt(l^2 + w^2) */
+    double rgb_prob;               /* refine, labels = 0 */
+    int32_t T[FCN_MAX_SCALES];     /* sections per scale (refine: len(np.arange(z_start, z_end, s))) */
+    int32_t cls_index, reserved;   /* size class = one-hot index */
+} fcn_train_frustum;
+typedef struct {
+    int kind, labels, rtc, extra_feat, random_flip, random_shift;
+    int B, N, num_scales, num_classes, num_frustums, points_f64;
+    double stride[FCN_MAX_SCALES];
+    double max_depth;
+    const void *points;                  /* (sum n, 3) float32, or float64 when points_f64 */
+    const long long *point_offsets;      /* (num_frustums + 1) */
+    const int32_t *seg;                  /* (sum n) det seg labels (label_list[i].astype(int64)), else NULL */
+    const fcn_train_frustum *frustums;   /* (num_frustums) */
+    const int32_t *index;                /* (B) dataset indices, repeats allowed */
+    const int32_t *choice;               /* (B, N) indices into each item's own points */
+    const double *flip_u, *shift_n;      /* (B) np.random.random() / np.random.randn() (read when enabled) */
+    float *point_cloud;
+    float *centers[FCN_MAX_SCALES];      /* (B, 3, P_s) contiguous, capacity B * 3 * max T[s] */
+    long long *cls_label;                /* (B, P_2) */
+    long long *seg_label;                /* (B, N) det */
+    float *box3d_center, *box3d_heading, *box3d_size;
+    long long *size_class;
+    float *rot_angle, *one_hot, *ref_center, *rgb_prob;
+} fcn_train_input_args;
+FCN_API int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
