@@ -40,6 +40,7 @@ constexpr int MG_THREADS = (MG_MMA_WARPS + 1) * 32;
 constexpr int MG_NSTAGE = 3;         // stage slot: 2 x 16 KB of A + 32 KB of W (NT <= 128: 64-wide K; NT = 256: 32-wide)
 constexpr int MG_A_ATOM = MG_ROWS * 128, MG_A_STAGE = 2 * MG_A_ATOM;
 constexpr int MG_W_STAGE = 2 * 128 * 128;                     // two [128 x 32] atoms or one [256 x 32] atom
+__host__ __device__ constexpr int mg_k_atoms(int NT) { return NT == 256 ? 1 : 2; }   // 32-wide K atoms per stage
 constexpr int MG_OFF_W = MG_NSTAGE * MG_A_STAGE;
 constexpr int MG_OFF_BAR = MG_OFF_W + MG_NSTAGE * MG_W_STAGE;
 constexpr int MG_JOBQ = 4;                                    // job descriptors in flight inside a CTA
@@ -86,22 +87,26 @@ __device__ __forceinline__ void mg_job(const MegaParams &P, const fcn_mega_layer
                                        int *flags) {
     const fcn_mega_args &p = P.a;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3, t = tid & 127;
-    const int NS = L.n_stage, ka = L.k_atoms == 1 ? 1 : 2;
+    // 32-wide K atoms per stage (the layer table's k_atoms, checked on the host): a compile-time count keeps every
+    // wgmma of a stage in straight-line code
+    constexpr int KA = mg_k_atoms(NT);
+    const int NS = L.n_stage;
     const uint32_t w_atom16 = (uint32_t)(NT * 128) >> 4;              // second 32-wide K atom of a W stage
     const uint64_t adesc0 = make_desc_sw128(smem_u32(sA) + wg * (64 * 128));
     const uint64_t bdesc0 = make_desc_sw128(smem_u32(sW));
     float acc[NT / 2];
 #pragma unroll
     for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
-    wgmma_fence();
     int prev = -1;
     for (int s = 0; s < NS; ++s, ++stage) {
         const uint32_t st = stage % MG_NSTAGE, ph = (stage / MG_NSTAGE) & 1;
         mbar_wait(&full[st], ph);
         const uint64_t ad = adesc0 + (uint64_t)(st * (MG_A_STAGE >> 4));
         const uint64_t bd = bdesc0 + (uint64_t)(st * (MG_W_STAGE >> 4));
+        wgmma_fence();
         fence_acc(acc);
-        for (int a = 0; a < ka; ++a)
+#pragma unroll
+        for (int a = 0; a < KA; ++a)
 #pragma unroll
             for (int k = 0; k < 4; ++k)
                 wgmma_tf32<NT>(acc, ad + (uint64_t)(a * (MG_A_ATOM >> 4) + 2 * k), bd + (uint64_t)(a * w_atom16 + 2 * k),
@@ -275,7 +280,7 @@ fcn_mega_kernel(const __grid_constant__ MegaParams P) {
                 if (dbg) { dbg[0] = clock64(); dbg[1] = jcur; }
                 const int r0 = job.m_tile * MG_ROWS;
                 const int NS = L.n_stage;
-                const int ka = L.k_atoms == 1 ? 1 : 2;                   // 32-wide K atoms per stage
+                const int ka = mg_k_atoms(L.NT);
                 const uint32_t w_bytes = (uint32_t)(L.NT * 128 * ka);    // [NT rows x 32 tf32] per atom
                 const uint32_t a_bytes = (uint32_t)(ka * MG_A_ATOM);
                 const uint8_t *wsrc = (const uint8_t *)L.w_tc + (size_t)job.n_tile * NS * w_bytes;
@@ -387,6 +392,11 @@ extern "C" int fcn_mega_forward(const fcn_mega_args *args, fcn_stream_t stream) 
     FCN_REQUIRE(a.n_out >= 0 && a.n_out <= FCN_MAX_PEERS && a.n_flag_out >= 0 && a.n_flag_out <= FCN_MAX_PEERS,
                 "too many output sets");
     FCN_REQUIRE(a.NH >= 1 && a.NH <= DEC_MAX_BINS && a.NS >= 1 && a.NS <= DEC_MAX_BINS, "bad decode sizes");
+    for (int i = 0; i < a.n_layers; ++i) {
+        const fcn_mega_layer &L = a.layers[i];
+        FCN_REQUIRE((L.NT == 64 || L.NT == 128 || L.NT == 256) && L.k_atoms == mg_k_atoms(L.NT),
+                    "layer tile width must be 64, 128 or 256, with k_atoms = 1 for 256 and 2 otherwise");
+    }
     if (a.n_jobs == 0) return FCN_OK;
     static_assert(sizeof(DecodeOut) == sizeof(fcn_decode_out), "decode output block layout");
     int grid = a.grid > 0 ? a.grid : sm_count();

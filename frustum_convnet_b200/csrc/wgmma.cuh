@@ -120,6 +120,15 @@ __device__ __forceinline__ void bulk_g2s_multicast(void *smem_dst, const void *g
 }
 
 // ------------------------------------------------------------------ wgmma
+// Fence protocol.  wgmma.fence must separate any other access to an accumulator register from the next
+// wgmma.mma_async that uses it (PTX ISA, "wgmma.fence").  Zero-initialisation, epilogue reads and fence_acc() below
+// all count as such accesses (fence_acc's "+f" operands tell the compiler the registers may have changed), so a
+// K loop issues wgmma_fence() at the top of EVERY stage - after the stage's mbarrier wait, before fence_acc() and
+// the stage's wgmmas - not once before the loop.  Keep the wgmmas of a stage in straight-line code as well
+// (compile-time trip counts, unrolled).  Otherwise ptxas inserts its own warpgroup.arrive (advisory C7519) and,
+// where that lands on a divergent path (next to a lane-0 mbarrier arrive), serializes every wgmma of the kernel
+// (C7520): results stay the same, but no two MMAs are ever in flight.  tests/test_wgmma_sass_cpu.py checks this.
+//
 // K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA descriptor bit layout):
 //  [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major) | [32,46) SBO>>4 = 1024>>4 |
 //  [49,52) base offset = 0 (tiles are 1024-byte aligned) | [62,64) layout = 1 (SWIZZLE_128B)

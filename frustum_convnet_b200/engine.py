@@ -103,8 +103,9 @@ class FrustumEngine:
         self.use_tma = os.environ.get("FCN_CONV_TMA", "1") != "0"   # conv A operand via TMA tensor maps
         # FCN_PN_CLUSTER=1: PointNet on 2-CTA clusters (precision 2: every weight stage is read from L2 once per
         # cluster and multicast to both CTAs) for the scales whose layer-1 width is >= FCN_PN_CLUSTER_MIN.  Off by
-        # default: on an H100 (400 W limit, B=32, 200-step regions) it measured 2-3 % below the 1-CTA kernel
-        # (car 98.2 k vs 100.4 k frustums/s, SUN-RGBD 63.4 k vs 65.6 k).
+        # default: with overlapped wgmmas, on an H100 SXM (700 W limit, B=32, 200-step regions, two runs each) it
+        # measured 2-3 % below the 1-CTA kernel on every workload (resident frustums/s: car 109.8-111.6 k vs
+        # 113.5-114.7 k, people 66.9-67.7 k vs 69.1-69.3 k, SUN-RGBD 72.3-72.6 k vs 74.7-75.1 k).
         self.pn_cluster = os.environ.get("FCN_PN_CLUSTER", "0") == "1"
         self.pn_cluster_min = int(os.environ.get("FCN_PN_CLUSTER_MIN", "128"))
         self.group_scan = os.environ.get("FCN_GROUP_SCAN") is not None   # A/B: section-scan grouping kernels
