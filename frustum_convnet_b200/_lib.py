@@ -208,6 +208,23 @@ class TrainInputArgs(C.Structure):
                                           "size_class", "rot_angle", "one_hot", "ref_center", "rgb_prob")]
 
 
+VAL_VALUES, VAL_ROW = 14, 18
+VAL_NO_FG, VAL_OVERFLOW = 1, 2
+
+
+class ValBatchArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("B", "T2", "NH", "NS", "with_iou", "capacity", "logit_pitch", "ld_logit")] + \
+               [(n, C.c_void_p) for n in ("logits", "center_ref2", "cls_label", "size_class", "box3d_center",
+                                          "box3d_heading", "box3d_size", "mean_size")] + \
+               [(n, C.c_float) for n in ("w_box", "w_head_reg", "w_size_reg", "w_corner", "iou_thresh", "reserved")] + \
+               [(n, C.c_void_p) for n in ("partials", "state", "table")]
+
+
+class ValResult(C.Structure):
+    _fields_ = [("avg", C.c_double * VAL_VALUES), ("sum", C.c_double * VAL_VALUES), ("count", C.c_double),
+                ("rows", C.c_int32), ("added", C.c_int32), ("status", C.c_int32), ("first_no_fg", C.c_int32)]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -244,6 +261,9 @@ SIGNATURES = {
     "fcn_det_prepare": (_I, [C.POINTER(DetFinalizeArgs), _P]),
     "fcn_det_select": (_I, [C.POINTER(DetFinalizeArgs), _P]),
     "fcn_build_train_inputs": (_I, [C.POINTER(TrainInputArgs), _P]),
+    "fcn_val_partials_floats": (C.c_longlong, [_I, _I]),
+    "fcn_val_batch": (_I, [C.POINTER(ValBatchArgs), _P]),
+    "fcn_val_finalize": (_I, [_P, _I, _P, _P, _P]),
 }
 
 _lib = None

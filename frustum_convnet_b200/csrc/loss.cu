@@ -13,15 +13,9 @@
 //   det_loss_final_kernel : the eight losses (det_base.py:505-514) and six metrics (:516-523)
 // Means over the foreground rows are sum(w * term) / nfg, exactly the reference's `nonzero()` row selection
 // (tests/test_train_host_cpu.py proves the weighted form equal to the selected form incl. gradients).
-#include "box_iou.cuh"
-#include "common.cuh"
+#include "loss_terms.cuh"
 
 namespace fcn {
-
-constexpr int LOSS_MAX_BINS = 32;
-constexpr float LOSS_PI = 3.14159265358979323846f;
-
-enum { A_CLS = 0, A_CENTER, A_HCLS, A_HRES, A_SCLS, A_SRES, A_CORNER, A_CLSACC, A_HACC, A_SACC, A_IOU2, A_IOU3, A_IOUGT, A_N };
 
 __global__ void det_loss_count_kernel(int N, const long long *__restrict__ lab, float *__restrict__ counts) {
     __shared__ int s[2];
@@ -37,25 +31,6 @@ __global__ void det_loss_count_kernel(int N, const long long *__restrict__ lab, 
     atomicAdd(&s[1], keep);
     __syncthreads();
     if (threadIdx.x == 0) { atomicAdd(&counts[0], (float)s[0]); atomicAdd(&counts[1], (float)s[1]); }
-}
-
-__device__ __forceinline__ float huber(float a_abs, float delta) {
-    const float q = fminf(a_abs, delta);
-    return 0.5f * q * q + delta * (a_abs - q);
-}
-
-// corners of models/model_util.py:48-72 (x: +-l/2, y: +-h/2, z: +-w/2; rotation about y)
-__device__ __forceinline__ void corners_of(const float *ctr, float heading, const float *size, float *c) {
-    const float l = size[0], w = size[1], h = size[2];
-    const float cs = cosf(heading), sn = sinf(heading);
-    const float sx[8] = {1, 1, -1, -1, 1, 1, -1, -1}, sy[8] = {1, 1, 1, 1, -1, -1, -1, -1}, sz[8] = {1, -1, -1, 1, 1, -1, -1, 1};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const float x = sx[j] * l * 0.5f, y = sy[j] * h * 0.5f, z = sz[j] * w * 0.5f;
-        c[3 * j + 0] = cs * x + sn * z + ctr[0];
-        c[3 * j + 1] = y + ctr[1];
-        c[3 * j + 2] = -sn * x + cs * z + ctr[2];
-    }
 }
 
 __global__ void __launch_bounds__(128)
@@ -76,16 +51,15 @@ det_loss_rows_kernel(const __grid_constant__ fcn_loss_args a, const float *__res
         float *dc = a.dcls + (size_t)r * 2, *dr = a.dreg + (size_t)r * W;
         for (int i = 0; i < W; ++i) dr[i] = 0.f;
         // ---------------- focal classification loss (all rows with label != -1), common.py:217-232
-        const float m = fmaxf(cl[0], cl[1]);
-        const float e0 = expf(cl[0] - m), e1 = expf(cl[1] - m);
-        const float p0 = e0 / (e0 + e1), p1 = e1 / (e0 + e1);
+        float p0, p1;
+        softmax2(cl, p0, p1);
         float d0 = 0.f, d1 = 0.f;
         if (lab != -1) {
             const int tl = lab >= 1 ? 1 : 0;
             const float alpha = tl == 0 ? 0.75f : 0.25f;
             const float pt = tl == 0 ? p0 : p1;
-            const float lg = logf(pt + 1e-14f);
-            v[A_CLS] = -alpha * (1.f - pt) * (1.f - pt) * lg;
+            float lg;
+            v[A_CLS] = focal_term(pt, alpha, lg);
             // d/dpt [ -alpha (1-pt)^2 log(pt+eps) ]
             const float dpt = -alpha * (-2.f * (1.f - pt) * lg + (1.f - pt) * (1.f - pt) / (pt + 1e-14f));
             const float scale = dpt / (counts[0] + 1e-14f);           // loss.sum() / (num_fg + 1e-14)
@@ -103,13 +77,9 @@ det_loss_rows_kernel(const __grid_constant__ fcn_loss_args a, const float *__res
             const float hgt = a.box3d_heading[b];
             const float sgt[3] = {a.box3d_size[b * 3], a.box3d_size[b * 3 + 1], a.box3d_size[b * 3 + 2]};
             const int sc = (int)a.size_class[b];
-            const float two_pi = 2.f * LOSS_PI, apc = two_pi / (float)NH;
-            float g = fmodf(hgt, two_pi);
-            if (g < 0.f) g += two_pi;                                  // python-style modulo
-            float shifted = fmodf(g + apc * 0.5f, two_pi);
-            if (shifted < 0.f) shifted += two_pi;
-            const int hc = min(max((int)floorf(shifted / apc), 0), NH - 1);
-            const float hres_lab = (shifted - ((float)hc * apc + apc * 0.5f)) / (apc * 0.5f);
+            const float apc = 2.f * LOSS_PI / (float)NH;
+            float hres_lab;
+            const int hc = angle_encode(hgt, NH, hres_lab);
             const float *ctr = o, *hs = o + 3, *hr = hs + NH, *ss = hr + NH, *sr = ss + NS;
             float ex[3];
 #pragma unroll
@@ -129,10 +99,8 @@ det_loss_rows_kernel(const __grid_constant__ fcn_loss_args a, const float *__res
             // ---------------- heading class CE + residual Huber (delta 1)
             int h_arg = 0;
             {
-                float mx = hs[0];
-                for (int i = 1; i < NH; ++i) mx = fmaxf(mx, hs[i]);
-                float sum = 0.f;
-                for (int i = 0; i < NH; ++i) sum += expf(hs[i] - mx);
+                float mx;
+                const float sum = softmax_denom(hs, NH, mx);
                 v[A_HCLS] = -(hs[hc] - mx - logf(sum));
                 float best = -1.f;
                 for (int i = 0; i < NH; ++i) {
@@ -148,10 +116,8 @@ det_loss_rows_kernel(const __grid_constant__ fcn_loss_args a, const float *__res
             // ---------------- size class CE + residual Huber (delta 1) on the norm
             int s_arg = 0;
             {
-                float mx = ss[0];
-                for (int i = 1; i < NS; ++i) mx = fmaxf(mx, ss[i]);
-                float sum = 0.f;
-                for (int i = 0; i < NS; ++i) sum += expf(ss[i] - mx);
+                float mx;
+                const float sum = softmax_denom(ss, NS, mx);
                 v[A_SCLS] = -(ss[sc] - mx - logf(sum));
                 float best = -1.f;
                 for (int i = 0; i < NS; ++i) {
@@ -172,8 +138,7 @@ det_loss_rows_kernel(const __grid_constant__ fcn_loss_args a, const float *__res
             // ---------------- corner loss (det_base.py:449-461): predicted box with the GT class labels
             {
                 const float cp[3] = {ref[0] + ctr[0], ref[1] + ctr[1], ref[2] + ctr[2]};
-                float ang = (float)hc * apc + hr[hc] * (apc * 0.5f);
-                if (ang > LOSS_PI) ang -= two_pi;
+                const float ang = angle_decode(hc, hr[hc], apc);
                 float sz[3];
 #pragma unroll
                 for (int i = 0; i < 3; ++i) sz[i] = sr[sc * 3 + i] * ex[i] + ex[i];
@@ -224,8 +189,7 @@ det_loss_rows_kernel(const __grid_constant__ fcn_loss_args a, const float *__res
                 dr[3 + 2 * NH + NS + sc * 3 + 2] += gh * ex[2];
                 // ---------------- IoU metrics: predicted box with the PREDICTED class labels (det_base.py:488-500)
                 if (a.with_iou) {
-                    float angp = (float)h_arg * apc + hr[h_arg] * (apc * 0.5f);
-                    if (angp > LOSS_PI) angp -= two_pi;
+                    const float angp = angle_decode(h_arg, hr[h_arg], apc);
                     float szp[3];
 #pragma unroll
                     for (int i = 0; i < 3; ++i) szp[i] = sr[s_arg * 3 + i] * a.mean_size[s_arg * 3 + i] + a.mean_size[s_arg * 3 + i];

@@ -724,6 +724,27 @@ class _Plan:
             seq()
         self.graph = g
 
+    def forward_staged(self, pc, centers, one_hot):
+        """Eval forward for a consumer of the head logits (``head_logits``): the inputs are copied into the plan's own
+        block and the forward graph is replayed (captured on the first call, which synchronizes once).  While the
+        current stream is being captured, the launch sequence itself is recorded into the caller's graph instead.
+        No host sync otherwise; the decoded outputs are written as by ``run``."""
+        self._check_inputs(pc, centers, one_hot)
+        with torch.cuda.device(self.eng.device):
+            self._stage(pc, centers, one_hot)
+            if torch.cuda.is_current_stream_capturing():
+                self._launch_feat(self.in_pc, self.in_centers, self.in_onehot)
+                self._launch_tail(self.in_centers[1])
+                return
+            if self.graph is None:
+                self._capture()
+            self.graph.replay()
+
+    def head_logits(self):
+        """(logits, pitch, ld_logit, center_ref2) of the last ``forward_staged``: the pitched head-logit buffer
+        (B, pitch, ld_logit) whose row (b, t < T2) is [cls0, cls1, regression...], and the staged (B, 3, T2) refs."""
+        return self.buf["logits"], self.P[1], self.eng.ld_logit, self.in_centers[1]
+
     def run_feat(self, pc, centers, one_hot):
         self._check_inputs(pc, centers, one_hot)
         eng = self.eng

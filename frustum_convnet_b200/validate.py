@@ -1,0 +1,192 @@
+"""The validation pass of train/train_net_det.py ``validate()`` (:162-203) on the device: eval-mode losses and metrics
+of every batch from the fused forward's head logits, averaged over the epoch without a host sync per batch.
+
+    val = Validator(model)                       # model.eval(); reuse the object across epochs
+    for data_dicts in val_loader:
+        val.add({k: v.cuda() for k, v in data_dicts.items()})   # forward graph + two launches, no host sync
+    states = val.finalize()                      # == TrainingStates.get_states(avg=True) of the reference loop
+    val.reset()
+
+`add` stages the batch into the forward plan of its (B, N, T) shape, replays the plan's forward graph and runs
+``fcn_val_batch`` (csrc/validate.cu) on the plan's pitched head logits; the batch's 14 values are appended to a
+device table.  `finalize` replays the reference's float64 AverageMeter over that table (``fcn_val_finalize``) and
+reads the result once.  Weights are taken from ``model.engine()`` on every `add`, so optimizer steps between epochs
+are picked up.  ``PointNetDet.forward`` itself is unchanged.  No CPU fallback: CPU tensors raise."""
+from __future__ import annotations
+
+import ctypes as C
+from collections import OrderedDict
+
+import numpy as np
+import torch
+
+from . import _lib
+from .config import get_cfg
+
+LOSS_KEYS = ("total_loss", "cls_loss", "center_loss", "head_cls_loss", "head_res_loss", "size_cls_loss",
+             "size_res_loss", "corners_loss")
+
+
+class _PlanLabels:
+    """Label buffers and the fcn_val_batch arguments of one forward plan (kept on the plan, so they live and die
+    with its workspace)."""
+
+    def __init__(self, plan):
+        eng, B, T2 = plan.eng, plan.B, plan.T[1]
+        dev, f32, i64 = eng.device, torch.float32, torch.int64
+        self.cls_label = torch.zeros((B, T2), dtype=i64, device=dev)
+        self.size_class = torch.zeros(B, dtype=i64, device=dev)
+        self.center = torch.zeros((B, 3), dtype=f32, device=dev)
+        self.heading = torch.zeros(B, dtype=f32, device=dev)
+        self.size = torch.zeros((B, 3), dtype=f32, device=dev)
+        n = int(_lib.load().fcn_val_partials_floats(B, T2))
+        self.partials = torch.zeros(max(n, 1), dtype=f32, device=dev)
+        logits, pitch, ld, ref2 = plan.head_logits()
+        a = _lib.ValBatchArgs()
+        a.B, a.T2, a.NH, a.NS = B, T2, eng.num_bins, eng.num_size
+        a.logit_pitch, a.ld_logit = pitch, ld
+        a.logits, a.center_ref2, a.mean_size = logits.data_ptr(), ref2.data_ptr(), eng.mean_size.data_ptr()
+        a.cls_label, a.size_class = self.cls_label.data_ptr(), self.size_class.data_ptr()
+        a.box3d_center, a.box3d_heading, a.box3d_size = (self.center.data_ptr(), self.heading.data_ptr(),
+                                                          self.size.data_ptr())
+        a.partials = self.partials.data_ptr()
+        self.args = a
+
+    def stage(self, data, B, T2):
+        self.cls_label.copy_(data["cls_label"].reshape(B, T2), non_blocking=True)
+        self.size_class.copy_(data["size_class"].reshape(B), non_blocking=True)
+        self.center.copy_(data["box3d_center"].reshape(B, 3), non_blocking=True)
+        self.heading.copy_(data["box3d_heading"].reshape(B), non_blocking=True)
+        self.size.copy_(data["box3d_size"].reshape(B, 3), non_blocking=True)
+
+
+class Validator:
+    """Eval-mode losses and metrics of one epoch on the device (see the module docstring).  One process, one
+    device; `capacity` = batches one epoch may add (default 4096)."""
+
+    LABEL_KEYS = ("cls_label", "size_class", "box3d_center", "box3d_heading", "box3d_size")
+
+    def __init__(self, model, capacity=None):
+        self.model = model
+        p = next(model.parameters(), None)
+        if p is None or p.device.type != "cuda":
+            raise RuntimeError("Validator: the model must live on a CUDA device (there is no CPU fallback)")
+        self.device = p.device
+        self.capacity = int(capacity) if capacity is not None else 4096
+        if self.capacity < 1:
+            raise ValueError("capacity must be >= 1")
+        cfg = get_cfg()
+        self.iou_key = "IoU_" + str(cfg.IOU_THRESH)
+        self.keys = LOSS_KEYS + ("cls_acc", "head_acc", "size_acc", "IoU_2D", "IoU_3D", self.iou_key)
+        L = cfg.LOSS
+        self._weights = (float(L.BOX_LOSS_WEIGHT), float(L.HEAD_REG_WEIGHT), float(L.SIZE_REG_WEIGHT),
+                         float(L.CORNER_LOSS_WEIGHT), float(cfg.IOU_THRESH))
+        dev = self.device
+        self.table = torch.zeros((self.capacity, _lib.VAL_ROW), dtype=torch.float32, device=dev)
+        self.state = torch.zeros(4, dtype=torch.int32, device=dev)
+        self._result = torch.zeros(C.sizeof(_lib.ValResult), dtype=torch.uint8, device=dev)
+        self._streams = {}
+        self.last_result = None
+        self._reset_event, self._reset_waited = None, set()
+        self._engine, self._pinned = None, {}
+
+    def reset(self):
+        """Start a new epoch.  The counter is zeroed on the current stream; the next `add` on any other stream waits
+        for it."""
+        with torch.cuda.device(self.device):
+            self.state.zero_()
+            self._reset_event = torch.cuda.Event()
+            self._reset_event.record()
+        self._reset_waited = {torch.cuda.current_stream(self.device).cuda_stream}
+        self._streams = {}
+
+    def add(self, data):
+        """One reference-style batch with labels (CUDA tensors): stage it into the forward plan of its shape, replay
+        the plan's forward graph, then compute and append the batch's losses and metrics.  No host sync (except the
+        first time a shape is seen on a stream, when its forward plan and graph are built), so the caller may capture
+        `add` itself after one un-captured `add` per shape on the capture stream.  Such a graph stays valid while the
+        model's weight pack does: the Validator keeps every plan it used alive (also past the engine's plan limit)
+        until a weight change rebuilds the engine, whose old workspaces are then released."""
+        m = self.model
+        if m.training:
+            raise RuntimeError("Validator.add: call model.eval() first (the reference validate() runs in eval mode)")
+        pc = data["point_cloud"]
+        if pc.dim() != 3 or pc.shape[1] != 3:
+            raise ValueError("Validator.add: point_cloud must be (B, 3, N); inputs with extra channels are not supported")
+        missing = [k for k in self.LABEL_KEYS if data.get(k) is None]
+        if missing:
+            raise ValueError("Validator.add: labels missing: %s" % ", ".join(missing))
+        for k in ("point_cloud",) + self.LABEL_KEYS:
+            if not data[k].is_cuda:
+                raise RuntimeError("Validator.add: %s must be a CUDA tensor (there is no CPU fallback)" % k)
+        eng = m.engine()
+        S = eng.arch.num_scales
+        centers = [data["center_ref%d" % (i + 1)].contiguous() for i in range(S)]
+        one_hot = data.get("one_hot") if eng.num_vec > 0 else None
+        if one_hot is not None:
+            one_hot = one_hot.contiguous()
+        pc = pc.contiguous()
+        B, N = int(pc.shape[0]), int(pc.shape[2])
+        plan = eng.plan(B, N, [int(c.shape[2]) for c in centers])
+        if eng is not self._engine:                  # a rebuilt engine: its plans replace the old ones
+            self._engine, self._pinned = eng, {}
+        self._pinned[id(plan)] = plan
+        lab = plan.__dict__.get("_val_labels")
+        if lab is None:
+            lab = plan._val_labels = _PlanLabels(plan)
+        stream = torch.cuda.current_stream(self.device)
+        with torch.cuda.device(self.device):
+            if stream.cuda_stream not in self._reset_waited and not torch.cuda.is_current_stream_capturing():
+                if self._reset_event is not None:
+                    stream.wait_event(self._reset_event)
+                self._reset_waited.add(stream.cuda_stream)
+            lab.stage(data, B, plan.T[1])
+            plan.forward_staged(pc, centers, one_hot)
+            a = lab.args
+            a.with_iou = 1 if getattr(m, "gpu_iou_metrics", True) else 0
+            a.w_box, a.w_head_reg, a.w_size_reg, a.w_corner, a.iou_thresh = self._weights
+            a.capacity, a.state, a.table = self.capacity, self.state.data_ptr(), self.table.data_ptr()
+            _lib.call("fcn_val_batch", C.byref(a), stream.cuda_stream)
+        self._streams[stream.cuda_stream] = stream
+
+    def _join(self):
+        cur = torch.cuda.current_stream(self.device)
+        for st in self._streams.values():
+            if st.cuda_stream != cur.cuda_stream:
+                cur.wait_stream(st)
+        return cur
+
+    def finalize(self):
+        """-> OrderedDict of the 14 epoch averages in the order of the reference's
+        ``TrainingStates.get_states(avg=True)``; one host read.  Raises if a batch had no foreground row or the
+        table overflowed."""
+        with torch.cuda.device(self.device):
+            cur = self._join()
+            _lib.call("fcn_val_finalize", self.table.data_ptr(), self.capacity, self.state.data_ptr(),
+                      self._result.data_ptr(), cur.cuda_stream)
+            raw = self._result.cpu().numpy().tobytes()
+        r = _lib.ValResult.from_buffer_copy(raw)
+        self.last_result = r
+        if r.status & _lib.VAL_NO_FG:
+            raise RuntimeError("Validator: batch %d of the epoch has no foreground row (cls_label == 1); the reference "
+                               "validate() rejects it (assert fg_idx.numel() != 0)" % r.first_no_fg)
+        if r.status & _lib.VAL_OVERFLOW:
+            raise RuntimeError("Validator: %d batches were added but the capacity is %d; construct "
+                               "Validator(model, capacity=%d) or more" % (r.added, self.capacity, r.added))
+        return OrderedDict((k, float(r.avg[i])) for i, k in enumerate(self.keys))
+
+    def meters(self):
+        """(sum, count) of each AverageMeter after the last `finalize`, keyed like its result."""
+        r = self.last_result
+        if r is None:
+            raise RuntimeError("Validator.meters: call finalize() first")
+        return OrderedDict((k, (float(r.sum[i]), float(r.count))) for i, k in enumerate(self.keys))
+
+    def per_batch(self, full=False):
+        """(n, 14) float32 values of the batches added so far (the `val` of each meter, for logging); full=True
+        returns the whole rows (n, 18) with B, nfg and nkeep in columns 14-16."""
+        with torch.cuda.device(self.device):
+            self._join()
+            n = min(int(self.state[0].item()), self.capacity)
+            t = self.table[:n].cpu().numpy()
+        return np.ascontiguousarray(t if full else t[:, :_lib.VAL_VALUES])

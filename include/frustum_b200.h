@@ -557,6 +557,55 @@ typedef struct {
 } fcn_train_input_args;
 FCN_API int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (12) Validation pass on the device: the eval-mode losses and metrics of models/det_base.py:414-525 for every
+ *      batch of an epoch, and their AverageMeter averages (utils/utils.py:51-67, utils/training_states.py).
+ *
+ *      fcn_val_batch (once per batch, after the eval forward; no host sync, no allocation, capturable): two
+ *      launches.  Reads the head logits where the forward left them: logits (B, logit_pitch, ld_logit), row
+ *      [cls0, cls1, centre 3, heading scores NH, heading residuals NH, size scores NS, size residuals 3*NS, ...];
+ *      center_ref2 (B,3,T2); cls_label (B,T2) int64; size_class (B) int64; box3d_center (B,3), box3d_heading (B),
+ *      box3d_size (B,3) fp32; mean_size (NS,3).  Computes the 8 losses and 6 metrics with the reference's
+ *      denominators (focal loss / (nfg + 1e-14), cls_acc over label != -1, the rest over label == 1; IoU from the
+ *      predicted classes; with_iou = 0 gives NaN IoU values).  Each CTA of the first launch writes its sums to
+ *      its own slot of `partials` (fcn_val_partials_floats(B, T2) floats); the second sums the slots in CTA
+ *      order, so results are bit-identical across runs, streams and graph replays (no float atomics).  It then
+ *      appends one row to `table` (capacity, FCN_VAL_ROW) at row index state[0]++:
+ *        [0..7]  total, cls, center, head_cls, head_res, size_cls, size_res, corners  (det_base.py:505-514)
+ *        [8..13] cls_acc, head_acc, size_acc, IoU_2D, IoU_3D, IoU_>=thresh          (:516-523)
+ *        [14] B, [15] nfg, [16] nkeep, [17] 0.
+ *      state (device int32[4], zeroed by the caller at the start of an epoch): rows appended, status bits,
+ *      index of the first batch without a foreground row (the reference's `assert fg_idx.numel() != 0`), 0.
+ *      Rows at or past `capacity` are counted but not written (FCN_VAL_OVERFLOW).
+ *
+ *      fcn_val_finalize (once per epoch): one thread per value replays sum += (double)val * B, count += B with
+ *      count starting at 1e-14, in row order, and writes avg = sum / count with the row count and status.
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_VAL_VALUES 14
+#define FCN_VAL_ROW 18
+#define FCN_VAL_NO_FG 1
+#define FCN_VAL_OVERFLOW 2
+typedef struct {
+    int B, T2, NH, NS, with_iou, capacity;
+    int logit_pitch, ld_logit;
+    const float *logits;
+    const float *center_ref2;
+    const long long *cls_label, *size_class;
+    const float *box3d_center, *box3d_heading, *box3d_size, *mean_size;
+    float w_box, w_head_reg, w_size_reg, w_corner, iou_thresh, reserved;
+    float *partials;
+    int32_t *state;
+    float *table;
+} fcn_val_batch_args;
+typedef struct {
+    double avg[FCN_VAL_VALUES], sum[FCN_VAL_VALUES], count;
+    int32_t rows, added, status, first_no_fg;   /* rows in the table, rows appended (the capacity needed) */
+} fcn_val_result;
+FCN_API long long fcn_val_partials_floats(int B, int T2);
+FCN_API int fcn_val_batch(const fcn_val_batch_args *args, fcn_stream_t stream);
+FCN_API int fcn_val_finalize(const float *table, int capacity, const int32_t *state, fcn_val_result *result,
+                             fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
