@@ -574,7 +574,8 @@ __device__ __forceinline__ float dy_apply(const DyCoef &c, float da, float y, bo
     return c.scale * (dz - c.m1 - (y - c.mean) * c.invstd * c.m2);
 }
 
-// dX[M,K] = dY[M,N] * W   (W (N,K): contiguous along K);  plain store (single consumer)
+// dX[M,K] += dY[M,N] * W   (W (N,K): contiguous along K).  One CTA owns each element and there is no N split, so
+// the accumulation into the source gradient (shared with its other consumers) is a plain read-add-store.
 __global__ void __launch_bounds__(FP_THREADS)
 train_dx_plain_kernel(const __grid_constant__ fcn_train_layer L) {
     __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
@@ -629,8 +630,11 @@ train_dx_plain_kernel(const __grid_constant__ fcn_train_layer L) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int r = r0 + ty * 8 + i;
-        if (r < M)
-            *(float4 *)(s.grad + (size_t)r * s.ld + c0 + tx * 4) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+        if (r < M) {
+            float4 *dst = (float4 *)(s.grad + (size_t)r * s.ld + c0 + tx * 4);
+            const float4 o = *dst;
+            *dst = make_float4(o.x + acc[i][0], o.y + acc[i][1], o.z + acc[i][2], o.w + acc[i][3]);
+        }
     }
 }
 

@@ -306,7 +306,10 @@ typedef struct {
 FCN_API long long fcn_train_workspace_floats(const fcn_train_layer *layer);
 FCN_API int fcn_train_forward(const fcn_train_layer *layer, float *workspace, long long workspace_floats,
                               fcn_stream_t stream);
-/* backward of one layer: column reduction, dW (all segments), dX for the segments in need_dx_mask */
+/* backward of one layer: column reduction, dW (all segments), dX for the segments in need_dx_mask.
+ * Every output of the training kernels except Y ACCUMULATES into what its buffer holds: dX (into src.grad, so a
+ * source read by several segments or layers receives the sum of their gradients), dW, dbias, dgamma / dbeta,
+ * `sums` and `dsums`.  The forward OVERWRITES Y. */
 FCN_API int fcn_train_backward(const fcn_train_layer *layer, int need_dx_mask, fcn_stream_t stream);
 /* PointNet pooling: feat[(b,t), c] = (cnt > 0) * max_k relu(bn(Y[(b,t,k), c])), one-hot columns appended
  * (det_base.py:100-101,134-157); backward scatters dfeat to the arg-max rows of a zero-filled dA. */
