@@ -185,7 +185,7 @@ class DetFinalizeArgs(C.Structure):
                 ("mask", C.c_void_p), ("mask_words", C.c_longlong)]
 
 
-TRAIN_DET, TRAIN_REFINE = 0, 1
+TRAIN_DET, TRAIN_REFINE, TRAIN_SUNRGBD = 0, 1, 2
 
 
 class TrainFrustum(C.Structure):
@@ -194,7 +194,8 @@ class TrainFrustum(C.Structure):
                 ("line0", C.c_double * 3), ("line_delta", C.c_double * 3), ("z_start", C.c_double),
                 ("z_step", C.c_double * MAX_SCALES), ("center", C.c_double * 3), ("heading", C.c_double),
                 ("size", C.c_double * 3), ("dist", C.c_double), ("rgb_prob", C.c_double),
-                ("T", C.c_int32 * MAX_SCALES), ("cls_index", C.c_int32), ("reserved", C.c_int32)]
+                ("T", C.c_int32 * MAX_SCALES), ("cls_index", C.c_int32), ("reserved", C.c_int32),
+                ("cx", C.c_double), ("cy", C.c_double), ("K", C.c_double * 9), ("Rtilt", C.c_double * 9)]
 
 
 class TrainInputArgs(C.Structure):
@@ -205,7 +206,8 @@ class TrainInputArgs(C.Structure):
                                           "shift_n", "point_cloud")] + \
                [("centers", C.c_void_p * MAX_SCALES)] + \
                [(n, C.c_void_p) for n in ("cls_label", "seg_label", "box3d_center", "box3d_heading", "box3d_size",
-                                          "size_class", "rot_angle", "one_hot", "ref_center", "rgb_prob")]
+                                          "size_class", "rot_angle", "one_hot", "ref_center", "rgb_prob",
+                                          "height_u")]
 
 
 VAL_VALUES, VAL_ROW = 14, 18

@@ -1,13 +1,16 @@
 // Device-side training-batch builder (C ABI section 11): what ProviderDataset.__getitem__ of
-// datasets/provider_sample.py (train branch) and datasets/provider_sample_refine.py (train and from_rgb_detection
-// branches) compute per item on DataLoader workers, plus the collate (default_collate / refine collate_fn with edge
-// padding), for a whole batch in one launch.  One CTA per batch item.
+// datasets/provider_sample.py (train branch), datasets/provider_sample_refine.py and
+// datasets/provider_sample_sunrgbd.py (train and from_rgb_detection branches) compute per item on DataLoader workers,
+// plus the collate (default_collate / refine collate_fn with edge padding), for a whole batch in one launch.  One CTA
+// per batch item.
 //
 // Per-frustum values that never change (rotation cos/sin, GT box in the frame of the inputs, the refine predicted
 // box's face means and arange start/step) come from the host, computed once with numpy's own expressions.  Everything
 // that depends on the step's draws is done here in float64 with each product and sum rounded separately
 // (__dmul_rn / __dadd_rn), as numpy rounds its elementwise expressions.  The rotations of rotate_pc_along_y go
 // through BLAS in the reference (np.dot), which may fuse them; results then differ by at most one float32 ulp.
+// The SUN-RGBD kind follows BLAS's order instead (see dot_fma): its frustum angle is the angle of the box-2D centre's
+// own ray, so the refs' centre-view x is a cancellation down to ~1e-17 m, whose rounding noise a float32 ulp bar sees.
 #include "common.cuh"
 #include "input_builder.cuh"
 
@@ -20,10 +23,23 @@ constexpr double kPi = 3.141592653589793;
 __device__ __forceinline__ double dsub(double a, double b) { return __dadd_rn(a, -b); }
 __device__ __forceinline__ double clip(double v, double lo, double hi) { return fmin(fmax(v, lo), hi); }
 
+// x . y over k = 0, 1, 2 as OpenBLAS's dgemm accumulates it: a0 b0 rounded, then one FMA per further term
+__device__ __forceinline__ double dot_fma(double a0, double b0, double a1, double b1) {
+    return __fma_rn(a1, b1, __dmul_rn(a0, b0));
+}
+__device__ __forceinline__ double dot_fma(double a0, double b0, double a1, double b1, double a2, double b2) {
+    return __fma_rn(a2, b2, dot_fma(a0, b0, a1, b1));
+}
+// rotate_pc_along_y's np.dot(pc[:, [0, 2]], rotmat.T) in that order: x' = x c + z (-s), z' = x s + z c
+__device__ __forceinline__ void rotate_y_fma(double x, double z, double cs, double sn, double *xo, double *zo) {
+    *xo = dot_fma(x, cs, z, -sn);
+    *zo = dot_fma(x, sn, z, cs);
+}
+
 struct Item {
     const fcn_train_frustum *fr;
     bool flip;
-    double shift, c[3], heading;   // GT centre / heading after flip and shift
+    double shift, height, c[3], heading;   // GT centre / heading after flip and shifts
 };
 
 // ref centre t (< T[s]) of scale s, flipped like the reference's ref1..ref4 (float64)
@@ -37,6 +53,15 @@ __device__ __forceinline__ void ref_point(const fcn_train_input_args &a, const I
         double xx;
         proj.at(zz, &xx, y);                                                  // project_image_to_rect
         rotate_y<true>(xx, zz, f.cs, f.sn, x, z);                             // get_center_view
+    } else if (a.kind == FCN_TRAIN_SUNRGBD) {
+        // project_image_to_upright_camera: camera (x, y, z) -> depth (x, z, -y) -> Rtilt @ . -> (X, -Z, Y)
+        const double *K = f.K, *R = f.Rtilt;
+        const double zz = section_depth<true>(t, st);
+        const double xc = __dmul_rn(dsub(f.cx, K[2]), zz) / K[0];
+        const double yc = -(__dmul_rn(dsub(f.cy, K[5]), zz) / K[4]);
+        auto row = [&](int i) { return dot_fma(R[3 * i], xc, R[3 * i + 1], zz, R[3 * i + 2], yc); };
+        *y = -row(2);
+        rotate_y_fma(row(0), row(1), f.cs, f.sn, x, z);                       // get_center_view
     } else {
         // cz = np.arange(z1, z2, s) + s / 2.;  c{x,y} = (cz - c1[2]) / delta[2] * delta[{0,1}] + c1[{0,1}]
         *z = __dadd_rn(__dadd_rn(f.z_start, __dmul_rn((double)t, f.z_step[s])), st / 2.);
@@ -58,7 +83,7 @@ __device__ __forceinline__ int ref_label(const fcn_train_input_args &a, const It
     const double lx = __dadd_rn(__dmul_rn(hc, dx), -__dmul_rn(hs, dz));
     const double lz = __dadd_rn(__dmul_rn(hs, dx), __dmul_rn(hc, dz));
     const double *sz = it.fr->size;
-    const bool det = a.kind == FCN_TRAIN_DET;
+    const bool det = a.kind != FCN_TRAIN_REFINE;
     const double f1 = det ? 0.5 : 0.3, f2 = det ? 1.0 : 0.6;                  // dimension * 0.5 | 1  /  * 0.3 | 0.6
     auto inside = [&](double fac) {
         const double l = __dmul_rn(sz[0], fac) / 2., w = __dmul_rn(sz[1], fac) / 2., h = __dmul_rn(sz[2], fac) / 2.;
@@ -69,7 +94,10 @@ __device__ __forceinline__ int ref_label(const fcn_train_input_args &a, const It
 
 }  // namespace
 
-__global__ void __launch_bounds__(kThreads) build_train_inputs_kernel(const __grid_constant__ fcn_train_input_args a) {
+// B CTAs per launch (B = 32 in the reference cfgs) never fill the GPU, so occupancy is worth nothing here.  With
+// minBlocks = 1 ptxas keeps the whole kernel in registers (74, no spills on sm_90a); without it, it picked 64
+// registers and spilled once the SUN-RGBD projection was inlined.
+__global__ void __launch_bounds__(kThreads, 1) build_train_inputs_kernel(const __grid_constant__ fcn_train_input_args a) {
     const int b = blockIdx.x, tid = threadIdx.x;
     __shared__ int s_pad[FCN_MAX_SCALES];
     __shared__ double s_wd[kThreads / 32];
@@ -84,11 +112,12 @@ __global__ void __launch_bounds__(kThreads) build_train_inputs_kernel(const __gr
     it.flip = a.labels && a.random_flip && a.flip_u[b] > 0.5;
     it.c[0] = f.center[0], it.c[1] = f.center[1], it.c[2] = f.center[2], it.heading = f.heading;
     if (it.flip) it.c[0] = -it.c[0], it.heading = dsub(kPi, it.heading);
-    it.shift = 0.0;
+    it.shift = it.height = 0.0;
     const bool shifting = a.labels && a.random_shift;
+    const bool sun = a.kind == FCN_TRAIN_SUNRGBD;
     if (shifting) {
         const double n = a.shift_n[b], dist = f.dist;
-        if (a.kind == FCN_TRAIN_DET) {
+        if (a.kind != FCN_TRAIN_REFINE) {
             const double sh = clip(__dmul_rn(__dmul_rn(n, dist), 0.2), -0.5 * dist, 0.5 * dist);
             it.shift = dsub(clip(__dadd_rn(sh, it.c[2]), 0.0, a.max_depth), it.c[2]);
         } else {
@@ -96,6 +125,10 @@ __global__ void __launch_bounds__(kThreads) build_train_inputs_kernel(const __gr
             it.shift = clip(__dmul_rn(__dmul_rn(n, dist), 0.1), -s1 * 2, 2 * s1);
         }
         it.c[2] = __dadd_rn(it.c[2], it.shift);
+        if (sun) {                                                            // np.random.random() * 0.4 - 0.2
+            it.height = dsub(__dmul_rn(a.height_u[b], 0.4), 0.2);
+            it.c[1] = __dadd_rn(it.c[1], it.height);
+        }
     }
     // ---- collate width of every scale: the batch's largest T (edge padding beyond an item's own T)
     if (tid < a.num_scales) {
@@ -128,10 +161,13 @@ __global__ void __launch_bounds__(kThreads) build_train_inputs_kernel(const __gr
             }
         }
         if (refine) x = dsub(x, f.ref_center[0]), y = dsub(y, f.ref_center[1]), z = dsub(z, f.ref_center[2]);
-        rotate_y<true>(x, z, f.cs, f.sn, &x, &z);
+        if (sun) rotate_y_fma(x, z, f.cs, f.sn, &x, &z);
+        else rotate_y<true>(x, z, f.cs, f.sn, &x, &z);
         if (!a.points_f64) x = (float)x, y = (float)y, z = (float)z;       // written back into the dataset's dtype
         if (it.flip) x = -x;
         if (shifting) z = __dadd_rn(z, it.shift);
+        // a Python float added to a float32 array is added in float32
+        if (shifting && sun) y = a.points_f64 ? __dadd_rn(y, it.height) : (double)__fadd_rn((float)y, (float)it.height);
         pc[j] = (float)x;
         pc[a.N + j] = (float)y;
         pc[2 * a.N + j] = (float)z;
@@ -214,9 +250,10 @@ using namespace fcn;
 extern "C" int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stream_t stream) {
     FCN_REQUIRE(args != nullptr, "args is NULL");
     const fcn_train_input_args &a = *args;
-    FCN_REQUIRE(a.kind == FCN_TRAIN_DET || a.kind == FCN_TRAIN_REFINE, "kind must be FCN_TRAIN_DET or FCN_TRAIN_REFINE");
+    FCN_REQUIRE(a.kind == FCN_TRAIN_DET || a.kind == FCN_TRAIN_REFINE || a.kind == FCN_TRAIN_SUNRGBD,
+                "kind must be FCN_TRAIN_DET, FCN_TRAIN_REFINE or FCN_TRAIN_SUNRGBD");
     FCN_REQUIRE(a.labels == 0 || a.labels == 1, "labels must be 0 or 1");
-    FCN_REQUIRE(a.kind == FCN_TRAIN_REFINE || a.labels == 1,
+    FCN_REQUIRE(a.kind != FCN_TRAIN_DET || a.labels == 1,
                 "the detection provider's from_rgb_detection branch is fcn_build_inputs");
     FCN_REQUIRE(a.rtc == 1, "only cfg.DATA.RTC = True is supported");
     FCN_REQUIRE(a.extra_feat == 0, "only cfg.DATA.WITH_EXTRA_FEAT = False is supported");
@@ -224,6 +261,7 @@ extern "C" int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stre
     FCN_REQUIRE(a.num_scales >= 2 && a.num_scales <= FCN_MAX_SCALES, "num_scales must be in [2, FCN_MAX_SCALES]");
     FCN_REQUIRE(a.num_classes >= 0 && a.num_classes <= 1024, "bad num_classes");
     for (int s = 0; s < a.num_scales; ++s) FCN_REQUIRE(a.stride[s] > 0 && a.centers[s] != nullptr, "bad scale");
+    FCN_REQUIRE(a.kind != FCN_TRAIN_SUNRGBD || a.num_scales == 5, "the SUN-RGBD provider takes exactly 5 scales");
     FCN_REQUIRE(a.kind == FCN_TRAIN_REFINE || a.max_depth > 0, "max_depth must be > 0");
     if (a.B == 0) return FCN_OK;
     FCN_REQUIRE(a.points && a.point_offsets && a.frustums && a.index && a.choice && a.point_cloud && a.rot_angle,
@@ -233,9 +271,11 @@ extern "C" int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stre
                     "NULL label pointer");
         FCN_REQUIRE((!a.random_flip || a.flip_u) && (!a.random_shift || a.shift_n), "NULL draw pointer");
     }
-    FCN_REQUIRE(a.kind == FCN_TRAIN_REFINE || (a.seg && a.seg_label), "detection needs seg and seg_label");
-    FCN_REQUIRE(a.kind == FCN_TRAIN_DET || a.ref_center, "refinement needs ref_center");
+    FCN_REQUIRE(a.kind == FCN_TRAIN_REFINE || !a.labels || (a.seg && a.seg_label), "detection needs seg and seg_label");
+    FCN_REQUIRE(a.kind != FCN_TRAIN_REFINE || a.ref_center, "refinement needs ref_center");
     FCN_REQUIRE(a.kind == FCN_TRAIN_DET || a.labels || a.rgb_prob, "from_rgb_detection needs rgb_prob");
+    FCN_REQUIRE(a.kind != FCN_TRAIN_SUNRGBD || !a.labels || !a.random_shift || a.height_u,
+                "the SUN-RGBD shift needs height_u");
     build_train_inputs_kernel<<<a.B, kThreads, 0, (cudaStream_t)stream>>>(a);
     FCN_LAUNCH_CHECK();
     return FCN_OK;

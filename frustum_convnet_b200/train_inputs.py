@@ -10,10 +10,13 @@ kind="det"     datasets/provider_sample.py, train branch (:133-270), default_col
 kind="refine"  datasets/provider_sample_refine.py, train branch (:174-316) or, with labels=False, the
                from_rgb_detection branch (:228-248); collate_fn (:388-419) edge-pads center_ref* / cls_label to the
                batch's largest T per scale.
+kind="sunrgbd" datasets/provider_sample_sunrgbd.py, train branch (:116-263; random_flip = random_shift = False is the
+               val split) or, with labels=False, the from_rgb_detection branch (:165-186); default_collate.  Exactly
+               5 strides (the reference unpacks s1..s5), 10 classes, max depth 8 (cfgs/det_sample_sunrgbd.yaml).
 
 ``draw(index)`` replays the np.random calls the reference's ``__getitem__`` makes, item after item (choice, then
-random() when flipping, then randn() when shifting), so a seeded run draws what a ``num_workers=0`` loader over the same
-indices would.  Nothing random runs on the device.  Only cfg.DATA.RTC = True, WITH_EXTRA_FEAT = False (every reference
+random() when flipping, then randn() when shifting, then for SUN-RGBD the height shift's random()), so a seeded run
+draws what a ``num_workers=0`` loader over the same indices would.  Nothing random runs on the device.  Only cfg.DATA.RTC = True, WITH_EXTRA_FEAT = False (every reference
 cfg) is supported.
 
 To capture the kernel in a CUDA graph, capture ``launch()``; before each replay ``upload(index, draws)`` the next batch
@@ -28,6 +31,9 @@ import torch
 from . import _lib
 
 KITTI_CLASSES = ("Car", "Pedestrian", "Cyclist")
+SUNRGBD_CLASSES = ("bathtub", "bed", "bookshelf", "chair", "desk", "dresser", "night_stand", "sofa", "table", "toilet")
+_KINDS = {"det": _lib.TRAIN_DET, "refine": _lib.TRAIN_REFINE, "sunrgbd": _lib.TRAIN_SUNRGBD}
+_MAX_DEPTH = {"det": 70.0, "refine": 70.0, "sunrgbd": 8.0}      # cfg.DATA.MAX_DEPTH of the reference cfgs
 _F32, _I64 = torch.float32, torch.int64
 
 
@@ -70,12 +76,13 @@ def refine_ref_line(pred_box3d, pred_box3d_size, pred_box3d_angle, strides):
     return c1, c2 - c1, z1, steps, Ts
 
 
-def draw_items(counts, index, npoints, random_flip, random_shift, rng=np.random):
+def draw_items(counts, index, npoints, random_flip, random_shift, rng=np.random, height=False):
     """The np.random calls of ProviderDataset.__getitem__ for the items `index` (frustum point counts `counts`), in the
-    reference's order -> dict(choice (B, npoints), flip_u (B), shift_n (B)); disabled draws read 0."""
+    reference's order -> dict(choice (B, npoints), flip_u (B), shift_n (B)); disabled draws read 0.  height=True (the
+    SUN-RGBD provider) adds height_u (B): the random() it draws after randn() when shifting (:231)."""
     B = len(index)
     choice = np.empty((B, npoints), dtype=np.int64)
-    flip_u, shift_n = np.zeros(B), np.zeros(B)
+    flip_u, shift_n, height_u = np.zeros(B), np.zeros(B), np.zeros(B)
     for b, i in enumerate(index):
         n = int(counts[i])
         choice[b] = rng.choice(n, npoints, n < npoints)                              # :166 / :207
@@ -83,12 +90,18 @@ def draw_items(counts, index, npoints, random_flip, random_shift, rng=np.random)
             flip_u[b] = rng.random()                                                 # :227 / :270
         if random_shift:
             shift_n[b] = rng.randn()                                                 # :241 / :284
-    return {"choice": choice, "flip_u": flip_u, "shift_n": shift_n}
+            if height:
+                height_u[b] = rng.random()
+    out = {"choice": choice, "flip_u": flip_u, "shift_n": shift_n}
+    if height:
+        out["height_u"] = height_u
+    return out
 
 
 def frustum_table(kind, strides, max_depth, labels, classes, type_list, label_list=None, box3d_list=None,
                   heading_list=None, size_list=None, frustum_angle_list=None, box2d_list=None, calib_list=None,
-                  prob_list=None, pred_box3d_list=None, pred_box3d_size_list=None, pred_box3d_angle_list=None):
+                  prob_list=None, pred_box3d_list=None, pred_box3d_size_list=None, pred_box3d_angle_list=None,
+                  calib_K_list=None, calib_R_list=None):
     """The per-frustum constants (fcn_train_frustum records) of the provider's lists, computed once in float64 with
     the reference's own numpy expressions."""
     classes = list(classes)
@@ -106,6 +119,20 @@ def frustum_table(kind, strides, max_depth, labels, classes, type_list, label_li
             b3 = box3d_list[i]
             r["center"] = rotate_pc_along_y(np.expand_dims((b3[0, :] + b3[6, :]) / 2.0, 0), rot).squeeze()
             r["heading"] = heading_list[i] - rot
+            r["T"][:S] = det_T
+        elif kind == "sunrgbd":
+            rot = np.pi / 2.0 + frustum_angle_list[i]                           # provider_sample_sunrgbd.py:328-331
+            r["rot"], r["cs"], r["sn"] = rot, np.cos(rot), np.sin(rot)
+            box = box2d_list[i]
+            r["cx"], r["cy"] = (box[0] + box[2]) / 2., (box[1] + box[3]) / 2.  # :294, in box2d's dtype (float32)
+            r["K"] = np.asarray(calib_K_list[i], dtype=np.float64).reshape(9)
+            r["Rtilt"] = np.asarray(calib_R_list[i], dtype=np.float64).reshape(9)
+            if labels:
+                b3 = box3d_list[i]
+                r["center"] = rotate_pc_along_y(np.expand_dims((b3[0, :] + b3[6, :]) / 2.0, 0), rot).squeeze()
+                r["heading"] = heading_list[i] - rot
+            else:
+                r["rgb_prob"] = prob_list[i]
             r["T"][:S] = det_T
         else:
             pb = pred_box3d_list[i]
@@ -131,10 +158,14 @@ def frustum_table(kind, strides, max_depth, labels, classes, type_list, label_li
 
 
 class TrainBatchBuilder:
-    def __init__(self, kind, strides, npoints, max_depth=70.0, num_classes=3, random_flip=True, random_shift=True,
+    def __init__(self, kind, strides, npoints, max_depth=None, num_classes=None, random_flip=True, random_shift=True,
                  labels=True, one_hot=True, rtc=True, with_extra_feat=False, device="cuda"):
-        if kind not in ("det", "refine"):
-            raise ValueError("kind must be 'det' or 'refine', got %r" % (kind,))
+        """max_depth / num_classes default to the kind's reference cfg (70 / 3 for KITTI, 8 / 10 for SUN-RGBD)."""
+        if kind not in _KINDS:
+            raise ValueError("kind must be 'det', 'refine' or 'sunrgbd', got %r" % (kind,))
+        if kind == "sunrgbd" and len(strides) != 5:
+            raise ValueError("the SUN-RGBD provider takes exactly 5 strides (s1, ..., s5 = cfg.DATA.STRIDE), got %d"
+                             % len(strides))
         if not rtc or with_extra_feat:
             raise ValueError("only cfg.DATA.RTC = True and WITH_EXTRA_FEAT = False are supported (every reference cfg)")
         if kind == "det" and not labels:
@@ -146,36 +177,48 @@ class TrainBatchBuilder:
         self.strides = [float(s) for s in strides]
         if not 2 <= len(self.strides) <= _lib.MAX_SCALES:
             raise ValueError("need 2..%d strides" % _lib.MAX_SCALES)
-        self.N, self.V, self.max_depth = int(npoints), int(num_classes), float(max_depth)
+        if num_classes is None:
+            num_classes = len(SUNRGBD_CLASSES if kind == "sunrgbd" else KITTI_CLASSES)
+        self.N, self.V = int(npoints), int(num_classes)
+        self.max_depth = float(_MAX_DEPTH[kind] if max_depth is None else max_depth)
         self.random_flip = bool(random_flip) and self.labels
         self.random_shift = bool(random_shift) and self.labels
         self.one_hot = bool(one_hot)
+        self._has_seg = kind == "det" or (kind == "sunrgbd" and self.labels)
         self.num_frustums = 0
         self.B_cap = 0
         self._B = 0
 
     # ------------------------------------------------------------------ dataset (once)
     @classmethod
-    def from_dataset(cls, ds, kind, strides, npoints=None, max_depth=70.0, **kw):
+    def from_dataset(cls, ds, kind, strides, npoints=None, max_depth=None, classes=None, **kw):
         """Reads the lists off a reference ``ProviderDataset`` instance by attribute name (the reference itself need
-        not be importable).  npoints / random_flip / random_shift / one_hot / labels default to the instance's."""
+        not be importable).  npoints / random_flip / random_shift / one_hot / labels default to the instance's;
+        classes to its category_info, else the dataset's class list (the SUN-RGBD provider has no category_info)."""
         kw.setdefault("random_flip", getattr(ds, "random_flip", False))
         kw.setdefault("random_shift", getattr(ds, "random_shift", False))
         kw.setdefault("one_hot", getattr(ds, "one_hot", True))
         kw.setdefault("labels", not getattr(ds, "from_rgb_detection", False))
-        classes = list(ds.category_info.CLASSES) if hasattr(ds, "category_info") else list(KITTI_CLASSES)
+        if classes is None:
+            classes = ds.category_info.CLASSES if hasattr(ds, "category_info") else \
+                (SUNRGBD_CLASSES if kind == "sunrgbd" else KITTI_CLASSES)
+        classes = list(classes)
         kw.setdefault("num_classes", len(classes))
         tb = cls(kind, strides, ds.npoints if npoints is None else npoints, max_depth=max_depth, **kw)
         names = ("label_list", "box3d_list", "heading_list", "size_list", "frustum_angle_list", "box2d_list",
-                 "calib_list", "prob_list", "pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list")
+                 "calib_list", "prob_list", "pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list",
+                 "calib_K_list", "calib_R_list")
         tb.set_dataset(ds.input_list, ds.type_list, classes, **{n: getattr(ds, n, None) for n in names})
         return tb
 
-    def set_dataset(self, input_list, type_list, classes=KITTI_CLASSES, label_list=None, box3d_list=None,
+    def set_dataset(self, input_list, type_list, classes=None, label_list=None, box3d_list=None,
                     heading_list=None, size_list=None, frustum_angle_list=None, box2d_list=None, calib_list=None,
-                    prob_list=None, pred_box3d_list=None, pred_box3d_size_list=None, pred_box3d_angle_list=None):
+                    prob_list=None, pred_box3d_list=None, pred_box3d_size_list=None, pred_box3d_angle_list=None,
+                    calib_K_list=None, calib_R_list=None):
         """Copies the provider's lists to the device once; per-frustum constants are computed here in float64 with the
-        reference's own numpy expressions."""
+        reference's own numpy expressions.  classes defaults to the kind's dataset (KITTI, or SUN-RGBD's 10)."""
+        if classes is None:
+            classes = SUNRGBD_CLASSES if self.kind == "sunrgbd" else KITTI_CLASSES
         F = len(input_list)
         if F == 0:
             raise ValueError("empty dataset")
@@ -189,11 +232,15 @@ class TrainBatchBuilder:
         need = {"det": ["label_list", "box3d_list", "heading_list", "size_list", "frustum_angle_list", "box2d_list",
                         "calib_list"],
                 "refine": ["pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list"] +
-                          (["box3d_list", "heading_list", "size_list"] if self.labels else ["prob_list"])}[self.kind]
+                          (["box3d_list", "heading_list", "size_list"] if self.labels else ["prob_list"]),
+                "sunrgbd": ["frustum_angle_list", "box2d_list", "calib_K_list", "calib_R_list"] +
+                           (["label_list", "box3d_list", "heading_list", "size_list"] if self.labels else
+                            ["prob_list"])}[self.kind]
         lists = dict(label_list=label_list, box3d_list=box3d_list, heading_list=heading_list, size_list=size_list,
                      frustum_angle_list=frustum_angle_list, box2d_list=box2d_list, calib_list=calib_list,
                      prob_list=prob_list, pred_box3d_list=pred_box3d_list, pred_box3d_size_list=pred_box3d_size_list,
-                     pred_box3d_angle_list=pred_box3d_angle_list)
+                     pred_box3d_angle_list=pred_box3d_angle_list, calib_K_list=calib_K_list,
+                     calib_R_list=calib_R_list)
         for n in need:
             if lists[n] is None or len(lists[n]) != F:
                 raise ValueError("kind=%r needs %s with one entry per frustum" % (self.kind, n))
@@ -208,7 +255,7 @@ class TrainBatchBuilder:
         self.d_offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)).to(dev)
         self.d_frustums = torch.from_numpy(fr.view(np.uint8)).to(dev)
         self.d_seg = None
-        if self.kind == "det":
+        if self._has_seg:
             seg = np.concatenate([np.asarray(s).astype(np.int64) for s in label_list])  # provider_sample.py:206
             if len(seg) != len(pts) or (np.abs(seg) >= 2 ** 31).any():
                 raise ValueError("label_list must hold one int32-range label per point")
@@ -220,7 +267,8 @@ class TrainBatchBuilder:
     def draw(self, index, rng=np.random):
         """The reference's np.random calls for these items, in its order -> dict(choice, flip_u, shift_n).
         ``rng``: the np.random module (the reference's global stream) or a np.random.RandomState."""
-        return draw_items(self.counts, self._index(index), self.N, self.random_flip, self.random_shift, rng)
+        return draw_items(self.counts, self._index(index), self.N, self.random_flip, self.random_shift, rng,
+                          height=self.kind == "sunrgbd")
 
     def _index(self, index):
         if isinstance(index, torch.Tensor):
@@ -252,19 +300,20 @@ class TrainBatchBuilder:
                 self._flat[k] = torch.empty(B * 3, dtype=_F32, device=dev)
             self._flat["box3d_heading"] = torch.empty(B, dtype=_F32, device=dev)
             self._flat["size_class"] = torch.empty(B, dtype=_I64, device=dev)
-        if self.kind == "det":
+        if self._has_seg:
             self._flat["seg_label"] = torch.empty(B * self.N, dtype=_I64, device=dev)
-        else:
+        if self.kind == "refine":
             self._flat["ref_center"] = torch.empty(B * 3, dtype=_F32, device=dev)
-            if not self.labels:
-                self._flat["rgb_prob"] = torch.empty(B, dtype=_F32, device=dev)
+        if not self.labels:
+            self._flat["rgb_prob"] = torch.empty(B, dtype=_F32, device=dev)
         # draws: one packed host staging buffer -> one H2D copy per step into fixed device buffers
-        self._nbytes = 16 * B + 4 * B + 4 * B * self.N
+        # [flip_u f64 | shift_n f64 | height_u f64 | index i32 | choice i32]
+        self._nbytes = 24 * B + 4 * B + 4 * B * self.N
         self._host = np.zeros(self._nbytes, dtype=np.uint8)
         self._dev = torch.empty(self._nbytes, dtype=torch.uint8, device=dev)
         base = self._dev.data_ptr()
         a = _lib.TrainInputArgs()
-        a.kind = _lib.TRAIN_DET if self.kind == "det" else _lib.TRAIN_REFINE
+        a.kind = _KINDS[self.kind]
         a.labels, a.rtc, a.extra_feat = int(self.labels), 1, 0
         a.random_flip, a.random_shift = int(self.random_flip), int(self.random_shift)
         a.B, a.N, a.num_scales, a.num_classes, a.num_frustums = B, self.N, S, self.V, self.num_frustums
@@ -276,7 +325,8 @@ class TrainBatchBuilder:
         a.points, a.point_offsets, a.frustums = self.d_points.data_ptr(), self.d_offsets.data_ptr(), \
             self.d_frustums.data_ptr()
         a.seg = None if self.d_seg is None else self.d_seg.data_ptr()
-        a.flip_u, a.shift_n, a.index, a.choice = base, base + 8 * B, base + 16 * B, base + 20 * B
+        a.flip_u, a.shift_n, a.height_u = base, base + 8 * B, base + 16 * B
+        a.index, a.choice = base + 24 * B, base + 28 * B
         for k in ("point_cloud", "cls_label", "seg_label", "box3d_center", "box3d_heading", "box3d_size", "size_class",
                   "rot_angle", "one_hot", "ref_center", "rgb_prob"):
             setattr(a, k, self._flat[k].data_ptr() if k in self._flat else None)
@@ -299,8 +349,10 @@ class TrainBatchBuilder:
         h[:8 * B].view(np.float64)[:] = np.asarray(draws.get("flip_u", np.zeros(B)), dtype=np.float64).reshape(B)
         h[8 * B: 16 * B].view(np.float64)[:] = np.asarray(draws.get("shift_n", np.zeros(B)),
                                                           dtype=np.float64).reshape(B)
-        h[16 * B: 20 * B].view(np.int32)[:] = index
-        h[20 * B:].view(np.int32)[:] = choice.reshape(-1)
+        h[16 * B: 24 * B].view(np.float64)[:] = np.asarray(draws.get("height_u", np.zeros(B)),
+                                                           dtype=np.float64).reshape(B)
+        h[24 * B: 28 * B].view(np.int32)[:] = index
+        h[28 * B:].view(np.int32)[:] = choice.reshape(-1)
         self._dev.copy_(torch.from_numpy(h), non_blocking=True)
         self._B, self._pad = B, self.T_of[index].max(0)
         return B

@@ -498,6 +498,10 @@ FCN_API int fcn_det_select(const fcn_det_finalize_args *args, fcn_stream_t strea
  *        FCN_TRAIN_REFINE, labels = 1  datasets/provider_sample_refine.py:174-316 (train branch), generate_labels
  *                                      :318-334, generate_ref :336-385, collate_fn :388-419
  *        FCN_TRAIN_REFINE, labels = 0  the same file's from_rgb_detection branch :228-248 (no labels, no augmentation)
+ *        FCN_TRAIN_SUNRGBD, labels = 1 datasets/provider_sample_sunrgbd.py:116-263 (train branch; with random_flip =
+ *                                      random_shift = 0 the val split), generate_labels :265-280, generate_ref :283-326,
+ *                                      default_collate; exactly 5 scales (the reference unpacks s1..s5)
+ *        FCN_TRAIN_SUNRGBD, labels = 0 the same file's from_rgb_detection branch :165-186 (no labels, no augmentation)
  *      Per frustum the host stores one fcn_train_frustum of float64 values computed ONCE with the reference's own
  *      numpy expressions (exact by construction); per step only index (B), choice (B,N), flip_u (B), shift_n (B)
  *      cross PCIe (the caller's np.random draws, :164-166,227,241 / :207,270,284).  The kernel does the rest in
@@ -507,24 +511,32 @@ FCN_API int fcn_det_select(const fcn_det_finalize_args *args, fcn_stream_t strea
  *                              to the dataset's dtype (points_f64 = 0: float32), x negated when flip_u > 0.5
  *                              (:227-235 / :270-278), z += shift (:237-244 / :280-286), then float32;
  *        centers[s] (B,3,P_s)  det: project_image_to_rect of the 2-D box centre at arange(0, max_depth, s) + s/2,
- *                              rotated; refine: the predicted box's line from its front to its back face mean at
+ *                              rotated; sunrgbd: project_image_to_upright_camera (:28-57) of the host's box-2D
+ *                              centre (cx, cy) at the same depths - x = ((cx - K[0,2]) z) / K[0,0], y likewise with
+ *                              K[1,2], K[1,1]; (x, z, -y); Rtilt @ that; (X, -Z, Y) - then rotated; refine: the
+ *                              predicted box's line from its front to its back face mean at
  *                              arange(z_start, ., s) + s/2 (arange element i = z_start + i * z_step[s]); x negated by
  *                              the flip.  P_s = max over the batch of T[s] of the items (collate_fn :388-419 pads
  *                              with mode='edge': columns >= T[s] of an item repeat its last column);
  *        cls_label (B,P_2)     int64 on the float64 ref2: -1 inside the full box (det 1.0x, refine 0.6x the GT size),
- *                              1 inside the half box (det 0.5x, refine 0.3x), 1 at the first argmin of the distance
- *                              to the GT centre when no ref is inside the half box; edge padded like the refs.  The
- *                              inside test is the half-space test in the box frame (the reference uses a Delaunay
+ *                              1 inside the half box (det and sunrgbd 0.5x, refine 0.3x), 1 at the first argmin of
+ *                              the distance to the GT centre when no ref is inside the half box; edge padded like the
+ *                              refs.  The inside test is the half-space test in the box frame (the reference uses a Delaunay
  *                              triangulation of the 8 corners, data_utils.py:24-34: they differ within ~1e-15 m of a face);
  *        box3d_center (B,3), box3d_heading (B,1), box3d_size (B,3) float32, size_class (B,1) int64: the GT box in the
  *                              frame of the inputs, flipped (heading = pi - heading) and shifted like the points;
  *        seg_label (B,N)       int64 (det only), rot_angle (B,1), one_hot (B,num_classes) (NULL: none), ref_center
- *                              (B,3) (refine), rgb_prob (B,1) (refine, labels = 0).
- *      Shift: det clip(n * dist * 0.2, +-0.5 dist), then clip(shift + c_z, 0, max_depth) - c_z; refine
- *      clip(n * dist * 0.1, +-2 stride[0]); dist = sqrt(l^2 + w^2) of the GT size.
+ *                              (B,3) (refine), rgb_prob (B,1) (labels = 0).  seg_label: det, and sunrgbd with labels.
+ *      Shift: det and sunrgbd clip(n * dist * 0.2, +-0.5 dist), then clip(shift + c_z, 0, max_depth) - c_z; refine
+ *      clip(n * dist * 0.1, +-2 stride[0]); dist = sqrt(l^2 + w^2) of the GT size.  sunrgbd then adds the height shift
+ *      h = height_u * 0.4 - 0.2 (np.random.random(), :231-233, drawn after randn()) to the GT centre's y in float64 and
+ *      to the points' y in float32 (numpy adds a Python float to a float32 array in float32).  sunrgbd's np.dot
+ *      products (Rtilt @ and the centre-view rotation) follow OpenBLAS's dgemm order: the first product rounded, then
+ *      one FMA per further term (its refs' centre-view x cancels to ~0, where the order shows).
  * ------------------------------------------------------------------------------------------ */
 #define FCN_TRAIN_DET 0
 #define FCN_TRAIN_REFINE 1
+#define FCN_TRAIN_SUNRGBD 2
 typedef struct {
     double rot, cs, sn;            /* rot_angle output and np.cos / np.sin of the centre-view rotation angle */
     double box2d[4], P[12];        /* det: 2-D box x1, y1, x2, y2 and calib P2 (row-major 3x4) */
@@ -537,6 +549,8 @@ typedef struct {
     double rgb_prob;               /* refine, labels = 0 */
     int32_t T[FCN_MAX_SCALES];     /* sections per scale (refine: len(np.arange(z_start, z_end, s))) */
     int32_t cls_index, reserved;   /* size class = one-hot index */
+    double cx, cy;                 /* sunrgbd: (box[0] + box[2]) / 2., (box[1] + box[3]) / 2. in box2d's own dtype */
+    double K[9], Rtilt[9];         /* sunrgbd: calib K and Rtilt (row-major 3x3) */
 } fcn_train_frustum;
 typedef struct {
     int kind, labels, rtc, extra_feat, random_flip, random_shift;
@@ -557,6 +571,7 @@ typedef struct {
     float *box3d_center, *box3d_heading, *box3d_size;
     long long *size_class;
     float *rot_angle, *one_hot, *ref_center, *rgb_prob;
+    const double *height_u;              /* (B) sunrgbd: np.random.random() after randn() (read when shifting) */
 } fcn_train_input_args;
 FCN_API int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stream_t stream);
 

@@ -4,9 +4,10 @@ csrc/train_inputs.cu) next to the reference-equivalent host path.
 
     python scripts/bench_train_inputs.py [--frustums 8192] [--steps 200] [--regions 5] [--ref-batches 10]
 
-Workloads: car detection (B=32, N=1024, strides 0.25..2, max depth 70) and refinement (B=32, N=512, strides 0.1..0.8)
-over a resident synthetic dataset of `--frustums` frustums (refine predicted-box widths in [1.91, 1.95] m, so every
-batch has T = (20, 10, 5, 3) and one training-step shape).  Per workload:
+Workloads: car detection (B=32, N=1024, strides 0.25..2, max depth 70), refinement (B=32, N=512, strides 0.1..0.8)
+and SUN-RGBD (B=32, N=2048, strides 0.1..1.6, max depth 8, synthetic tilted K / Rtilt, float32 box2d, 6-column
+points) over a resident synthetic dataset of `--frustums` frustums (refine predicted-box widths in [1.91, 1.95] m, so
+every batch has T = (20, 10, 5, 3) and one training-step shape).  Per workload:
   build_ms_per_batch     device time of `--steps` build() calls (one H2D copy of the draws + one launch), CUDA events,
                          draws prepared in advance;
   launch_ms_per_batch    the same for the kernel alone (launch());
@@ -14,8 +15,8 @@ batch has T = (20, 10, 5, 3) and one training-step shape).  Per workload:
   reference_ms_per_batch host time of the reference-equivalent numpy path, single process: the providers' per-item
                          numpy code (oracle/train_inputs.py) with scipy Delaunay inside-box tests as the reference's
                          in_hull does, the collate and torch.from_numpy, no H2D copy;
-and for refinement, train_extra_ms_per_step: regions of `--steps` TrainStep.step calls on one prebuilt batch alternate
-with regions where build() precedes each step (same stream), median(with) - median(without).
+and for refinement and SUN-RGBD, train_extra_ms_per_step: regions of `--steps` TrainStep.step calls on one prebuilt
+batch alternate with regions where build() precedes each step (same stream), median(with) - median(without).
 Prints one JSON line with the card name and its power limit.  Writes nothing to the tree."""
 from __future__ import annotations
 
@@ -33,7 +34,37 @@ if ROOT not in sys.path:
 
 from bench_detect import gpu_identity  # noqa: E402
 
-CAR, REFINE = (0.25, 0.5, 1.0, 2.0), (0.1, 0.2, 0.4, 0.8)
+CAR, REFINE, SUN = (0.25, 0.5, 1.0, 2.0), (0.1, 0.2, 0.4, 0.8), (0.1, 0.2, 0.4, 0.8, 1.6)
+MAX_DEPTH = {"det": 70.0, "refine": 70.0, "sunrgbd": 8.0}
+
+
+def synthetic_sun_lists(F, seed):
+    """F SUN-RGBD frustums in the prepared pickles' dtypes (float32 points with 6 columns, float32 box2d, bool seg)."""
+    from frustum_convnet_b200.train_inputs import SUNRGBD_CLASSES, compute_box_3d
+    rng = np.random.default_rng(seed)
+    n = rng.integers(200, 2500, F)
+    L = {k: [] for k in ("input_list", "type_list", "box2d_list", "frustum_angle_list", "calib_K_list",
+                         "calib_R_list", "label_list", "box3d_list", "heading_list", "size_list")}
+    for i in range(F):
+        K = np.array([[529.5, 0, 365.0], [0, 531.0, 262.0], [0, 0, 1]])
+        ax = rng.uniform(-0.15, 0.15)
+        R = np.array([[1, 0, 0], [0, np.cos(ax), -np.sin(ax)], [0, np.sin(ax), np.cos(ax)]])
+        C = np.array([rng.uniform(-2, 2), rng.uniform(-0.5, 1.0), rng.uniform(1, 7.5)])
+        size, heading = rng.uniform(0.4, 2.2, 3), rng.uniform(-np.pi, np.pi)
+        up = R.T @ np.array([C[0], C[2], -C[1]])                     # upright camera -> depth -> pixel
+        u, v = K[0, 0] * up[0] / up[1] + K[0, 2], K[1, 1] * -up[2] / up[1] + K[1, 2]
+        L["input_list"].append(np.concatenate([C + rng.normal(0, 0.5, (n[i], 3)), rng.uniform(0, 1, (n[i], 3))],
+                                              1).astype(np.float32))
+        L["type_list"].append(SUNRGBD_CLASSES[rng.integers(0, 10)])
+        L["box2d_list"].append(np.array([u - 40, v - 30, u + 40, v + 30], dtype=np.float32))
+        L["frustum_angle_list"].append(float(-np.arctan2(C[2], C[0])))
+        L["calib_K_list"].append(K)
+        L["calib_R_list"].append(R)
+        L["label_list"].append(rng.uniform(0, 1, n[i]) < 0.3)
+        L["box3d_list"].append(compute_box_3d(C, size, heading))
+        L["heading_list"].append(float(heading))
+        L["size_list"].append(size)
+    return L
 
 
 def synthetic_lists(kind, F, seed):
@@ -66,11 +97,12 @@ def synthetic_lists(kind, F, seed):
     return L
 
 
-def reference_path_ms(kind, L, batches, strides):
+def reference_path_ms(kind, L, batches, strides, max_depth):
     """Host time per batch of the reference-equivalent path (numpy items, Delaunay labels, collate)."""
     import torch
     from scipy.spatial import Delaunay
     from oracle import train_inputs as oti
+    from oracle import train_inputs_sunrgbd as ots
     from frustum_convnet_b200.train_inputs import compute_box_3d
 
     def in_hull(pc, center, dimension, angle):                      # datasets/data_utils.py:24-34
@@ -81,7 +113,7 @@ def reference_path_ms(kind, L, batches, strides):
     try:
         t0 = time.perf_counter()
         for index, draws in batches:
-            out = oti.build(kind, L, index, draws, strides, 70.0)
+            out = ots.build(kind, L, index, draws, strides, max_depth)
             out.pop("_margins", None)
             {k: torch.from_numpy(v) for k, v in out.items()}
         return (time.perf_counter() - t0) * 1e3 / len(batches)
@@ -100,7 +132,6 @@ def main():
 
     import torch
     from frustum_convnet_b200 import config, synth
-    from frustum_convnet_b200.det_base import PointNetDet
     from frustum_convnet_b200.train_engine import TrainStep
     from frustum_convnet_b200.train_inputs import TrainBatchBuilder
     assert torch.cuda.is_available(), "bench_train_inputs.py needs a CUDA device; there is no CPU fallback"
@@ -108,9 +139,10 @@ def main():
     torch.cuda.set_device(dev)
     B = args.batch
     line = {"frustums": args.frustums, "batch": B, "steps": args.steps}
-    for kind, strides, N in (("det", CAR, 1024), ("refine", REFINE, 512)):
-        L = synthetic_lists(kind, args.frustums, seed=3)
-        tb = TrainBatchBuilder(kind, strides, N, max_depth=70.0)
+    for kind, strides, N in (("det", CAR, 1024), ("refine", REFINE, 512), ("sunrgbd", SUN, 2048)):
+        L = synthetic_sun_lists(args.frustums, seed=3) if kind == "sunrgbd" else synthetic_lists(kind, args.frustums,
+                                                                                                 seed=3)
+        tb = TrainBatchBuilder(kind, strides, N, max_depth=MAX_DEPTH[kind])
         tb.set_dataset(L["input_list"], L["type_list"], **{k: v for k, v in L.items()
                                                            if k not in ("input_list", "type_list")})
         rng = np.random.RandomState(0)
@@ -134,14 +166,18 @@ def main():
         build_ms = [timed(lambda i: tb.build(idx[i], draws[i])) for _ in range(args.regions)]
         tb.upload(idx[0], draws[0])
         launch_ms = [timed(lambda i: tb.launch()) for _ in range(args.regions)]
-        ref_ms = reference_path_ms(kind, L, list(zip(idx, draws))[: args.ref_batches], strides)
+        ref_ms = reference_path_ms(kind, L, list(zip(idx, draws))[: args.ref_batches], strides, MAX_DEPTH[kind])
         res = {"build_ms_per_batch": float(np.median(build_ms)), "build_ms_min_max": [min(build_ms), max(build_ms)],
                "launch_ms_per_batch": float(np.median(launch_ms)), "draw_ms_per_batch": draw_ms,
                "reference_ms_per_batch": ref_ms, "reference_batches": args.ref_batches, "npoints": N}
-        if kind == "refine":
-            cfg, w = config.load_workload("refine_car")
-            sd = synth.make_state_dict(w["arch"], 3, "KITTI", seed=7)
-            m = PointNetDet(3, num_vec=3)
+        if kind in ("refine", "sunrgbd"):
+            cfg, w = config.load_workload("refine_car" if kind == "refine" else "sunrgbd")
+            if kind == "sunrgbd":
+                from frustum_convnet_b200.det_base_sunrgbd import PointNetDet
+            else:
+                from frustum_convnet_b200.det_base import PointNetDet
+            sd = synth.make_state_dict(w["arch"], w["num_vec"], cfg.DATA.DATASET_NAME, seed=7)
+            m = PointNetDet(3, num_vec=w["num_vec"])
             m.load_state_dict({k: torch.from_numpy(np.asarray(v)) for k, v in sd.items()})
             ts = TrainStep(m.to(dev).train(), lr=1e-3, weight_decay=1e-4)
             fixed = {k: v.clone() for k, v in tb.build(idx[0], draws[0]).items()}
