@@ -77,7 +77,7 @@ det_loss_rows_kernel(const __grid_constant__ fcn_loss_args a, const float *__res
             const float hgt = a.box3d_heading[b];
             const float sgt[3] = {a.box3d_size[b * 3], a.box3d_size[b * 3 + 1], a.box3d_size[b * 3 + 2]};
             const int sc = (int)a.size_class[b];
-            const float apc = 2.f * LOSS_PI / (float)NH;
+            const float apc = heading_bin_width(NH);
             float hres_lab;
             const int hc = angle_encode(hgt, NH, hres_lab);
             const float *ctr = o, *hs = o + 3, *hr = hs + NH, *ss = hr + NH, *sr = ss + NS;

@@ -47,9 +47,15 @@ __device__ __forceinline__ float focal_term(float pt, float alpha, float &lg) {
     return -alpha * (1.f - pt) * (1.f - pt) * lg;
 }
 
+// width of one heading bin: 2 pi / NH rounded once from double, as the model's python constant enters its float32
+// tensor arithmetic (and as decode.cuh computes it).  float32(2 pi) / NH differs by 1 ulp for NH = 9, 11, 13, ...
+__device__ __forceinline__ float heading_bin_width(int NH) {
+    return (float)(2.0 * 3.14159265358979323846 / (double)NH);
+}
+
 // angle_encode (box_transform.py:34-47): heading class and normalised residual of a GT heading
 __device__ __forceinline__ int angle_encode(float hgt, int NH, float &hres_lab) {
-    const float two_pi = 2.f * LOSS_PI, apc = two_pi / (float)NH;
+    const float two_pi = 2.f * LOSS_PI, apc = heading_bin_width(NH);
     float g = fmodf(hgt, two_pi);
     if (g < 0.f) g += two_pi;                                  // python-style modulo
     float shifted = fmodf(g + apc * 0.5f, two_pi);
