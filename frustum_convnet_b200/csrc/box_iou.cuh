@@ -2,9 +2,12 @@
 // call `rbbox_iou_3d_pair` (ops/pybind11/box_ops.h:173-260, called at models/det_base.py:495) that forces a
 // device->host copy of every predicted box per training step.
 //
-// The arithmetic lives in this header as plain C++ so that tests/test_box_iou_cpu.py can compile the SAME
-// functions for the host (g++) and check them against oracle/box_iou.py without a GPU; the kernels in
-// box_iou.cu only add the thread mapping.  No part of the product calls the host build.
+// The arithmetic lives in this header as plain C++ so that the CPU tests can compile the same source for the host
+// (g++) and check it without a GPU: tests/test_box_iou_cpu.py against oracle/box_iou.py, and
+// tests/test_box_iou_exact_cpu.py against exact rational arithmetic with and without multiply-add contraction
+// (nvcc contracts; the five kernels that inline rbbox_iou_pair are pinned on the device by
+// tests/test_gpu_box_iou_exact.py).  The kernels in box_iou.cu only add the thread mapping.  No part of the
+// product calls the host build.
 #pragma once
 
 #ifdef __CUDACC__
@@ -29,43 +32,76 @@ FCN_HD float shoelace_ccw(const Pt2 *p, int n) {
     return 0.5f * a;
 }
 
-// Sutherland-Hodgman: clip the convex quadrilateral `subj` against the convex quadrilateral `clip`
-// (either orientation).  Returns the vertex count (<= 8) of the intersection written to `out`.
-FCN_HD int clip_quads(const Pt2 *subj, const Pt2 *clip, Pt2 *out) {
-    Pt2 buf[2][8];
-    int n = 4, cur = 0;
-    for (int i = 0; i < 4; ++i) buf[0][i] = subj[i];
+// Sutherland-Hodgman: clip the convex quadrilateral `subj` against the convex quadrilateral `clip` (either
+// orientation) and return the signed area (counter-clockwise positive) of the intersection; `*count` receives its
+// vertex count.  The last clip edge feeds its vertices straight into the shoelace sum (same terms, same order as
+// shoelace_ccw on the stored polygon), so that polygon is never stored.
+//
+// Each vertex is classified ONCE per clip edge: its side value is computed when it first appears as the next
+// vertex `q`, carried into the following iteration as `sp`, and the first vertex's value is kept for the wrap-around.
+// Computing it twice (as `sq` of edge j and as `sp` of edge j+1) lets a compiler that contracts multiply-adds
+// round the two expressions differently; for a vertex within rounding of the clip line (shared or collinear
+// edges: boxes slid along their heading, nested boxes) the two signs then disagree, the clip emits a crossing on
+// one edge and drops the vertex on the next, and a triangle of the intersection is lost (IoU errors up to ~0.5).
+//
+// Vertex counts.  In exact arithmetic a convex polygon gains at most one vertex per clip edge (4 -> 5 -> 6 -> 7 ->
+// 8).  Rounding can classify vertices within rounding of the line inconsistently with convexity, and then only the
+// counting bound holds: with p vertices kept and n - p dropped the output has p + (sign changes) <= p + 2 min(p, n-p)
+// <= floor(3n/2) vertices, i.e. at most 6, 9 and 13 after the first three clip edges (and 19 after the last, which
+// is not stored).  The two ping-pong buffers are sized for that (9 + 13 entries), so no vertex is ever dropped.
+FCN_HD float clip_quads_area(const Pt2 *subj, const Pt2 *clip, int *count) {
+    Pt2 buf[9 + 13];                      // edges 0, 2 write buf + 9 (<= 6, <= 13); edge 1 writes buf (<= 9)
+    int n = 4;
+    for (int i = 0; i < 4; ++i) buf[i] = subj[i];
     const float sgn = shoelace_ccw(clip, 4) >= 0.f ? 1.f : -1.f;
+    float a2 = 0.f;                       // twice the signed area, accumulated by the last clip edge
     for (int e = 0; e < 4 && n > 0; ++e) {
         const Pt2 a = clip[e], b = clip[(e + 1) & 3];
         const float ex = b.x - a.x, ey = b.y - a.y;
-        const Pt2 *in = buf[cur];
-        Pt2 *o = buf[cur ^ 1];
+        const Pt2 *in = (e & 1) ? buf + 9 : buf;
+        Pt2 *o = (e & 1) ? buf : buf + 9;
+        const bool last = e == 3;
         int m = 0;
-        for (int j = 0; j < n; ++j) {
-            const Pt2 p = in[j], q = in[j + 1 == n ? 0 : j + 1];
-            const float sp = sgn * (ex * (p.y - a.y) - ey * (p.x - a.x));
-            const float sq = sgn * (ex * (q.y - a.y) - ey * (q.x - a.x));
-            if (sp >= 0.f && m < 8) o[m++] = p;
-            if ((sp >= 0.f) != (sq >= 0.f) && m < 8) {
-                const float t = sp / (sp - sq);
-                o[m].x = p.x + t * (q.x - p.x);
-                o[m].y = p.y + t * (q.y - p.y);
-                ++m;
+        Pt2 first = {0.f, 0.f}, prev = {0.f, 0.f};
+        auto emit = [&](const Pt2 r) {
+            if (!last) {
+                o[m] = r;
+            } else if (m == 0) {
+                first = r;
+            } else {
+                a2 += prev.x * r.y - r.x * prev.y;
             }
+            prev = r;
+            ++m;
+        };
+        const Pt2 p0 = in[0];
+        const float s0 = sgn * (ex * (p0.y - a.y) - ey * (p0.x - a.x));
+        Pt2 p = p0;
+        float sp = s0;
+        for (int j = 0; j < n; ++j) {
+            const bool wrap = j + 1 == n;
+            const Pt2 q = wrap ? p0 : in[j + 1];
+            const float sq = wrap ? s0 : sgn * (ex * (q.y - a.y) - ey * (q.x - a.x));
+            if (sp >= 0.f) emit(p);
+            if ((sp >= 0.f) != (sq >= 0.f)) {
+                const float t = sp / (sp - sq);
+                emit(Pt2{p.x + t * (q.x - p.x), p.y + t * (q.y - p.y)});
+            }
+            p = q;
+            sp = sq;
         }
+        if (last && m > 0) a2 += prev.x * first.y - first.x * prev.y;
         n = m;
-        cur ^= 1;
     }
-    for (int i = 0; i < n; ++i) out[i] = buf[cur][i];
-    return n;
+    *count = n;
+    return 0.5f * a2;
 }
 
 // c, q: the 8 corners (x, y, z) of one box pair in the reference's corner order (model_util.py:48-72).
 // iou[0] = bird's-eye-view IoU, iou[1] = 3-D IoU; (0, 0) when the BEV polygons do not overlap.
 FCN_HD void rbbox_iou_pair(const float *c, const float *q, float *iou) {
     const int order[4] = {6, 7, 4, 5};                       // box_ops.h:206-224
-    Pt2 P[4], Q[4], I[8];
+    Pt2 P[4], Q[4];
     // coordinates relative to the first polygon vertex: areas are translation invariant and the fp32 cross
     // products then work on box-sized (metres) instead of scene-sized (tens of metres) magnitudes
     const float ox = c[order[0] * 3 + 0], oz = c[order[0] * 3 + 2];
@@ -86,9 +122,9 @@ FCN_HD void rbbox_iou_pair(const float *c, const float *q, float *iou) {
     // yield a zero 3-D IoU, exactly as the reference arithmetic does.
     const float area = -shoelace_ccw(P, 4), qarea = -shoelace_ccw(Q, 4);   // clockwise positive (Boost default)
     if (!(area > 0.f) || !(qarea > 0.f)) return;
-    const int n = clip_quads(P, Q, I);
+    int n;
+    float inter = clip_quads_area(P, Q, &n);
     if (n < 3) return;
-    float inter = shoelace_ccw(I, n);
     inter = inter < 0.f ? -inter : inter;
     if (!(inter > 0.f)) return;
     const float uni = area + qarea - inter;

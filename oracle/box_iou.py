@@ -15,7 +15,10 @@ PARITY UNPINNED for the polygon clipping itself: the reference delegates it to B
 system dependency, absent from /root/reference and from this image).  This file restates the published
 algorithm for two CONVEX polygons (Sutherland-Hodgman clipping + shoelace area; the union of two overlapping
 convex polygons is one polygon of area a + b - inter) in float64 and is cross-checked in
-tests/test_box_iou_cpu.py against closed-form cases and an independent point-sampling estimate.
+tests/test_box_iou_cpu.py against closed-form cases and an independent point-sampling estimate.  Against EXACT
+arithmetic the clip is pinned: tests/test_box_iou_exact_cpu.py holds this file (and the pair IoU oracle/nms.py takes
+from it) within 1e-9 of a rational-arithmetic IoU (tests/iou_exact_ref.py) on the reference-generated fixture and on
+pair families with shared, collinear and touching edges.  Boost parity stays unpinned.
 
 DEGENERATE RINGS (decision of round 2, pinned by tests/test_box_iou_cpu.py::test_degenerate_boxes): the reference
 appends the four BEV corners without `bg::correct` (box_ops.h:206-224).  A decoded box with exactly ONE negative

@@ -1,6 +1,8 @@
 """Rotated-box IoU row (SURVEY.md 8(f)-1) on the CPU: the oracle against closed forms, an independent sampling
-estimate and the reference-generated corner fixture; and the DEVICE arithmetic (csrc/box_iou.cuh, the very
-functions the CUDA kernel calls) compiled for the host with g++ against the oracle."""
+estimate and the reference-generated corner fixture; and the device source (csrc/box_iou.cuh) compiled for the host
+with g++ against the oracle.  The host build here uses one contraction mode (-ffp-contract=off); nvcc contracts
+multiply-adds, so this is the same source, not the same arithmetic.  tests/test_box_iou_exact_cpu.py builds the
+header with and without contraction and checks both against exact arithmetic."""
 import ctypes
 import os
 import subprocess
