@@ -227,6 +227,23 @@ class ValResult(C.Structure):
                 ("rows", C.c_int32), ("added", C.c_int32), ("status", C.c_int32), ("first_no_fg", C.c_int32)]
 
 
+KITTI_GT_COLS, KITTI_DET_COLS, KITTI_PTS = 15, 14, 41
+
+
+class KittiEvalArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("num_images", "num_gt", "num_det", "reserved0")] + \
+               [(n, C.c_void_p) for n in ("gt", "det", "gt_offsets", "det_offsets", "host_gt_offsets",
+                                          "host_det_offsets", "workspace")] + \
+               [("workspace_bytes", C.c_longlong), ("result", C.c_void_p)]
+
+
+class KittiEvalResult(C.Structure):
+    _fields_ = [("precision", C.c_double * KITTI_PTS * 3 * 3 * 3), ("aos", C.c_double * KITTI_PTS * 3 * 3),
+                ("ap", C.c_float * 3 * 3 * 3), ("ap_aos", C.c_float * 3 * 3),
+                ("n_thresholds", C.c_int32 * 3 * 3 * 3), ("n_gt", C.c_int32 * 3 * 3 * 3),
+                ("evaluated", C.c_int32 * 3 * 3), ("compute_aos", C.c_int32), ("reserved", C.c_int32)]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -266,6 +283,10 @@ SIGNATURES = {
     "fcn_val_partials_floats": (C.c_longlong, [_I, _I]),
     "fcn_val_batch": (_I, [C.POINTER(ValBatchArgs), _P]),
     "fcn_val_finalize": (_I, [_P, _I, _P, _P, _P]),
+    "fcn_kitti_eval_workspace_bytes": (C.c_longlong, [C.POINTER(KittiEvalArgs)]),
+    "fcn_kitti_eval_overlaps": (_I, [C.POINTER(KittiEvalArgs), _P]),
+    "fcn_kitti_eval_thresholds": (_I, [C.POINTER(KittiEvalArgs), _P]),
+    "fcn_kitti_eval_statistics": (_I, [C.POINTER(KittiEvalArgs), _P]),
 }
 
 _lib = None

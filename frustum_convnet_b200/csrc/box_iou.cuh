@@ -18,18 +18,24 @@
 
 namespace fcn {
 
-struct Pt2 {
-    float x, y;
+// The polygon clip is written once for the scalar type: float for the train metric and NMS (below), double for
+// the KITTI evaluator's bird's-eye-view and 3-D overlaps (kitti_eval.cu), which works in float64 like the reference.
+template <typename T>
+struct Vec2 {
+    T x, y;
 };
+using Pt2 = Vec2<float>;
+using Pt2d = Vec2<double>;
 
 // signed area, counter-clockwise positive
-FCN_HD float shoelace_ccw(const Pt2 *p, int n) {
-    float a = 0.f;
+template <typename T>
+FCN_HD T shoelace_ccw(const Vec2<T> *p, int n) {
+    T a = T(0);
     for (int i = 0; i < n; ++i) {
-        const Pt2 u = p[i], v = p[i + 1 == n ? 0 : i + 1];
+        const Vec2<T> u = p[i], v = p[i + 1 == n ? 0 : i + 1];
         a += u.x * v.y - v.x * u.y;
     }
-    return 0.5f * a;
+    return T(0.5) * a;
 }
 
 // Sutherland-Hodgman: clip the convex quadrilateral `subj` against the convex quadrilateral `clip` (either
@@ -49,21 +55,22 @@ FCN_HD float shoelace_ccw(const Pt2 *p, int n) {
 // counting bound holds: with p vertices kept and n - p dropped the output has p + (sign changes) <= p + 2 min(p, n-p)
 // <= floor(3n/2) vertices, i.e. at most 6, 9 and 13 after the first three clip edges (and 19 after the last, which
 // is not stored).  The two ping-pong buffers are sized for that (9 + 13 entries), so no vertex is ever dropped.
-FCN_HD float clip_quads_area(const Pt2 *subj, const Pt2 *clip, int *count) {
-    Pt2 buf[9 + 13];                      // edges 0, 2 write buf + 9 (<= 6, <= 13); edge 1 writes buf (<= 9)
+template <typename T>
+FCN_HD T clip_quads_area(const Vec2<T> *subj, const Vec2<T> *clip, int *count) {
+    Vec2<T> buf[9 + 13];                  // edges 0, 2 write buf + 9 (<= 6, <= 13); edge 1 writes buf (<= 9)
     int n = 4;
     for (int i = 0; i < 4; ++i) buf[i] = subj[i];
-    const float sgn = shoelace_ccw(clip, 4) >= 0.f ? 1.f : -1.f;
-    float a2 = 0.f;                       // twice the signed area, accumulated by the last clip edge
+    const T sgn = shoelace_ccw(clip, 4) >= T(0) ? T(1) : T(-1);
+    T a2 = T(0);                          // twice the signed area, accumulated by the last clip edge
     for (int e = 0; e < 4 && n > 0; ++e) {
-        const Pt2 a = clip[e], b = clip[(e + 1) & 3];
-        const float ex = b.x - a.x, ey = b.y - a.y;
-        const Pt2 *in = (e & 1) ? buf + 9 : buf;
-        Pt2 *o = (e & 1) ? buf : buf + 9;
+        const Vec2<T> a = clip[e], b = clip[(e + 1) & 3];
+        const T ex = b.x - a.x, ey = b.y - a.y;
+        const Vec2<T> *in = (e & 1) ? buf + 9 : buf;
+        Vec2<T> *o = (e & 1) ? buf : buf + 9;
         const bool last = e == 3;
         int m = 0;
-        Pt2 first = {0.f, 0.f}, prev = {0.f, 0.f};
-        auto emit = [&](const Pt2 r) {
+        Vec2<T> first = {T(0), T(0)}, prev = {T(0), T(0)};
+        auto emit = [&](const Vec2<T> r) {
             if (!last) {
                 o[m] = r;
             } else if (m == 0) {
@@ -74,18 +81,18 @@ FCN_HD float clip_quads_area(const Pt2 *subj, const Pt2 *clip, int *count) {
             prev = r;
             ++m;
         };
-        const Pt2 p0 = in[0];
-        const float s0 = sgn * (ex * (p0.y - a.y) - ey * (p0.x - a.x));
-        Pt2 p = p0;
-        float sp = s0;
+        const Vec2<T> p0 = in[0];
+        const T s0 = sgn * (ex * (p0.y - a.y) - ey * (p0.x - a.x));
+        Vec2<T> p = p0;
+        T sp = s0;
         for (int j = 0; j < n; ++j) {
             const bool wrap = j + 1 == n;
-            const Pt2 q = wrap ? p0 : in[j + 1];
-            const float sq = wrap ? s0 : sgn * (ex * (q.y - a.y) - ey * (q.x - a.x));
-            if (sp >= 0.f) emit(p);
-            if ((sp >= 0.f) != (sq >= 0.f)) {
-                const float t = sp / (sp - sq);
-                emit(Pt2{p.x + t * (q.x - p.x), p.y + t * (q.y - p.y)});
+            const Vec2<T> q = wrap ? p0 : in[j + 1];
+            const T sq = wrap ? s0 : sgn * (ex * (q.y - a.y) - ey * (q.x - a.x));
+            if (sp >= T(0)) emit(p);
+            if ((sp >= T(0)) != (sq >= T(0))) {
+                const T t = sp / (sp - sq);
+                emit(Vec2<T>{p.x + t * (q.x - p.x), p.y + t * (q.y - p.y)});
             }
             p = q;
             sp = sq;
@@ -94,7 +101,7 @@ FCN_HD float clip_quads_area(const Pt2 *subj, const Pt2 *clip, int *count) {
         n = m;
     }
     *count = n;
-    return 0.5f * a2;
+    return T(0.5) * a2;
 }
 
 // c, q: the 8 corners (x, y, z) of one box pair in the reference's corner order (model_util.py:48-72).

@@ -624,6 +624,65 @@ FCN_API int fcn_val_batch(const fcn_val_batch_args *args, fcn_stream_t stream);
 FCN_API int fcn_val_finalize(const float *table, int capacity, const int32_t *state, fcn_val_result *result,
                              fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (13) KITTI object evaluation on the device: the offline evaluator train/kitti_eval/evaluate_object_3d_offline.cpp
+ *      (:56-916) with its semantics unchanged - image 2-D AP with AOS, ground-plane (bird's-eye-view) AP and 3-D AP
+ *      for car, pedestrian and cyclist at the easy, moderate and hard levels, in float64 like the reference.
+ *
+ *      Records are float64 rows, one image after the other; image i owns rows [offsets[i], offsets[i+1]):
+ *        gt  (num_gt, FCN_KITTI_GT_COLS)   [code, truncation, occlusion, alpha, x1, y1, x2, y2, h, w, l, t1, t2, t3, ry]
+ *                                          (a label_2 line, loadGroundtruth :180-204, with the type as its code)
+ *        det (num_det, FCN_KITTI_DET_COLS) [code, alpha, x1, y1, x2, y2, h, w, l, t1, t2, t3, ry, score]
+ *                                          (a result line, loadDetections :133-178, without the two unused fields)
+ *      Type codes FCN_KITTI_*: type names match case-insensitively; every other type is FCN_KITTI_OTHER.
+ *      gt_offsets / det_offsets are DEVICE int32 arrays of num_images + 1 entries; host_gt_offsets /
+ *      host_det_offsets are HOST copies of the same values (validated on the host and used for the buffer sizes:
+ *      they must start at 0, never decrease and end at num_gt / num_det).
+ *
+ *      Three calls in order on one stream, sharing the caller's workspace (fcn_kitti_eval_workspace_bytes: reads
+ *      neither workspace nor result, needs the device, -1 on invalid arguments), no host sync, no allocation:
+ *        fcn_kitti_eval_overlaps   : run-level flags, and every (detection, ground truth) pair's overlap once per
+ *                                    metric (criterion 0 against DontCare);
+ *        fcn_kitti_eval_thresholds : per evaluation the TP scores, sorted, and the recall-step thresholds;
+ *        fcn_kitti_eval_statistics : TP / FP / FN and AOS per threshold, then `result` (DEVICE).
+ *      Results are bit-identical from run to run.  A class without a detection that enables a metric has
+ *      evaluated[metric][class] = 0 and is not part of the output (its vectors are meaningless).
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_KITTI_GT_COLS 15
+#define FCN_KITTI_DET_COLS 14
+#define FCN_KITTI_PTS 41
+#define FCN_KITTI_CAR 0
+#define FCN_KITTI_PEDESTRIAN 1
+#define FCN_KITTI_CYCLIST 2
+#define FCN_KITTI_VAN 3
+#define FCN_KITTI_PERSON_SITTING 4
+#define FCN_KITTI_DONTCARE 5
+#define FCN_KITTI_OTHER 6
+typedef struct {
+    int num_images, num_gt, num_det, reserved0;
+    const double *gt, *det;
+    const int32_t *gt_offsets, *det_offsets;           /* DEVICE (num_images + 1) */
+    const int32_t *host_gt_offsets, *host_det_offsets; /* HOST copies */
+    void *workspace;
+    long long workspace_bytes;
+    struct fcn_kitti_eval_result_ *result;             /* DEVICE */
+} fcn_kitti_eval_args;
+typedef struct fcn_kitti_eval_result_ {
+    double precision[3][3][3][FCN_KITTI_PTS];  /* [metric image|ground|3d][class][difficulty][recall step] */
+    double aos[3][3][FCN_KITTI_PTS];           /* [class][difficulty][step]: image metric, when compute_aos */
+    float ap[3][3][3];                         /* the printed AP: sum of steps 0, 4, ..., 40 in float32, / 11 * 100 */
+    float ap_aos[3][3];
+    int32_t n_thresholds[3][3][3];
+    int32_t n_gt[3][3][3];                     /* recall denominators */
+    int32_t evaluated[3][3];                   /* [metric][class] */
+    int32_t compute_aos;                       /* no detection has alpha == -10 */
+    int32_t reserved;
+} fcn_kitti_eval_result;
+FCN_API long long fcn_kitti_eval_workspace_bytes(const fcn_kitti_eval_args *args);
+FCN_API int fcn_kitti_eval_overlaps(const fcn_kitti_eval_args *args, fcn_stream_t stream);
+FCN_API int fcn_kitti_eval_thresholds(const fcn_kitti_eval_args *args, fcn_stream_t stream);
+FCN_API int fcn_kitti_eval_statistics(const fcn_kitti_eval_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
