@@ -244,6 +244,24 @@ class KittiEvalResult(C.Structure):
                 ("evaluated", C.c_int32 * 3 * 3), ("compute_aos", C.c_int32), ("reserved", C.c_int32)]
 
 
+SUNRGBD_MAX_CLASSES, SUNRGBD_BAD_SEGMENT = 1024, 1
+
+
+class SunrgbdEvalArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("num_classes", "num_gt", "num_gt_segments", "num_det")] + \
+               [("ovthresh", C.c_double)] + \
+               [(n, C.c_void_p) for n in ("gt_corners", "det_corners", "det_scores", "det_segments",
+                                          "gt_segment_offsets", "gt_class_offsets", "det_class_offsets",
+                                          "host_gt_segment_offsets", "host_gt_class_offsets",
+                                          "host_det_class_offsets", "workspace")] + \
+               [("workspace_bytes", C.c_longlong), ("rec", C.c_void_p), ("prec", C.c_void_p), ("result", C.c_void_p)]
+
+
+class SunrgbdEvalResult(C.Structure):
+    _fields_ = [("ap", C.c_double), ("npos", C.c_int32), ("nd", C.c_int32), ("status", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -287,6 +305,9 @@ SIGNATURES = {
     "fcn_kitti_eval_overlaps": (_I, [C.POINTER(KittiEvalArgs), _P]),
     "fcn_kitti_eval_thresholds": (_I, [C.POINTER(KittiEvalArgs), _P]),
     "fcn_kitti_eval_statistics": (_I, [C.POINTER(KittiEvalArgs), _P]),
+    "fcn_sunrgbd_eval_workspace_bytes": (C.c_longlong, [C.POINTER(SunrgbdEvalArgs)]),
+    "fcn_sunrgbd_eval_match": (_I, [C.POINTER(SunrgbdEvalArgs), _P]),
+    "fcn_sunrgbd_eval_curves": (_I, [C.POINTER(SunrgbdEvalArgs), _P]),
 }
 
 _lib = None

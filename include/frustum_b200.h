@@ -683,6 +683,66 @@ FCN_API int fcn_kitti_eval_overlaps(const fcn_kitti_eval_args *args, fcn_stream_
 FCN_API int fcn_kitti_eval_thresholds(const fcn_kitti_eval_args *args, fcn_stream_t stream);
 FCN_API int fcn_kitti_eval_statistics(const fcn_kitti_eval_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (14) SUN-RGBD 3-D detection evaluation on the device: eval_det / eval_det_cls of the reference
+ *      (train/sunrgbd_eval/eval_det.py:41-231, use_07_metric = False) - per class the precision / recall curve and
+ *      the VOC average precision, with the 3-D IoU of rbbox_iou_3d_pair<double> in float64.
+ *
+ *      Boxes are float64 corner sets (8, 3) in the reference's corner order; the bird's-eye-view ring is the (x, z) of
+ *      corners 6, 7, 4, 5, the heights are the y of corners 0 and 4 (ops/pybind11/box_ops.h:173-260).  A ring that is
+ *      not clockwise-positive scores 0 (as in csrc/box_iou.cuh).
+ *        ground truth: class c owns rows [gt_class_offsets[c], gt_class_offsets[c+1]); within a class the rows are
+ *                      grouped into segments, one per image: segment s owns rows [gt_segment_offsets[s], [s+1]), in
+ *                      the reference's per-image order (the first maximum wins), and never crosses a class boundary.
+ *        detections:   class c owns rows [det_class_offsets[c], [c+1]) in gather order; det_segments[d] is the
+ *                      ground-truth segment of the detection's (class, image), or -1 when that image has no ground
+ *                      truth of the class (the detection is a false positive).
+ *      Per class: detections sorted by score, descending, STABLE (the earlier row wins a tie; -0.0 equals 0.0); the
+ *      overlap maximum over the segment's rows in order with strict '>' (a NaN never wins); a hit needs ovmax >
+ *      ovthresh strictly and is a TP when no higher-ranked detection claimed the same ground truth, otherwise an FP
+ *      (no fall-back to another ground truth).  rec = tp / npos and prec = tp / max(tp + fp, DBL_EPSILON) are
+ *      bit-identical to numpy's.  ap sums (delta recall) * (precision envelope) where the recall changes, in a fixed
+ *      order (each of 512 threads sums its positions, one per 512-position chunk from the last chunk back, then
+ *      cub::BlockReduce's fixed tree): within a few ulps of numpy's pairwise sum.  A class without a detection has
+ *      nd = 0 and ap = 0.
+ *
+ *      gt_*_offsets / det_class_offsets are DEVICE int32 arrays; host_* are HOST copies of the same values (validated
+ *      on the host: start at 0, never decrease, end at num_gt / num_det, class boundaries are segment boundaries).
+ *      Two calls in order on one stream, sharing the caller's workspace (fcn_sunrgbd_eval_workspace_bytes: reads
+ *      neither workspace nor outputs, needs the device, -1 on invalid arguments), no host sync, no allocation:
+ *        fcn_sunrgbd_eval_match  : overlap maximum per detection, the per-class stable sort, the first claim of
+ *                                  every ground truth;
+ *        fcn_sunrgbd_eval_curves : rec / prec (DEVICE, num_det each, class c at [det_class_offsets[c], ...), in
+ *                                  score order) and result[c] (DEVICE, num_classes entries).
+ *      A det_segments entry outside [-1, num_gt_segments) or whose segment is not of the detection's class sets
+ *      result[c].status to FCN_SUNRGBD_BAD_SEGMENT (the detection counts as an FP).  Results are bit-identical from run
+ *      to run.
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_SUNRGBD_MAX_CLASSES 1024
+#define FCN_SUNRGBD_BAD_SEGMENT 1
+typedef struct {
+    int num_classes, num_gt, num_gt_segments, num_det;
+    double ovthresh;
+    const double *gt_corners, *det_corners;         /* DEVICE (num_gt, 8, 3), (num_det, 8, 3) */
+    const double *det_scores;                       /* DEVICE (num_det) */
+    const int32_t *det_segments;                    /* DEVICE (num_det) */
+    const int32_t *gt_segment_offsets;              /* DEVICE (num_gt_segments + 1) */
+    const int32_t *gt_class_offsets, *det_class_offsets;   /* DEVICE (num_classes + 1) */
+    const int32_t *host_gt_segment_offsets, *host_gt_class_offsets, *host_det_class_offsets;   /* HOST copies */
+    void *workspace;
+    long long workspace_bytes;
+    double *rec, *prec;                             /* DEVICE (num_det) */
+    struct fcn_sunrgbd_eval_result_ *result;        /* DEVICE (num_classes) */
+} fcn_sunrgbd_eval_args;
+typedef struct fcn_sunrgbd_eval_result_ {
+    double ap;
+    int32_t npos, nd;                               /* ground-truth rows, detections of the class */
+    int32_t status, reserved;
+} fcn_sunrgbd_eval_result;
+FCN_API long long fcn_sunrgbd_eval_workspace_bytes(const fcn_sunrgbd_eval_args *args);
+FCN_API int fcn_sunrgbd_eval_match(const fcn_sunrgbd_eval_args *args, fcn_stream_t stream);
+FCN_API int fcn_sunrgbd_eval_curves(const fcn_sunrgbd_eval_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
