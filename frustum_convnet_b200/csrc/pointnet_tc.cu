@@ -2,14 +2,18 @@
 // registers), weight tiles staged by the TMA engine (1-D bulk copies of pre-swizzled images, mbarrier ring).
 //
 // Per 128-row tile (rows = unique grouped points {dx,dy,dz,section} from group_rows_kernel), two compute
-// warpgroups each own 64 rows and run the whole chain on them without waiting for each other:
-//   layer 1 (3->C1, fp32 FMA, folded BN, ReLU) -> A operand in shared memory (K-major, 128B swizzle, TF32)
-//   layer 2 D2[64 x C2] = A1 * W2^T (wgmma) -> +bias, ReLU, TF32 -> A2 (same rows of the same buffer)
-//   layer 3 D3[64 x 128-channel chunk] = A2 * W3^T -> +bias, ReLU, max over the rows of each section:
-//           a segmented suffix max over the 16 rows of a warp (shuffles), then one integer atomicMax per
+// warpgroups each own 64 rows and run the whole chain on them in registers, without waiting for each other:
+//   layer 1 (3->C1, fp32 FMA, folded BN, ReLU, TF32) -> straight into the A fragments of layer 2 (8 columns per
+//           k-step, double-buffered by K block so that it runs under the previous block's MMAs)
+//   layer 2 D2[64 x C2] = A1 * W2^T (wgmma, A from registers) -> +bias, ReLU, TF32 in place, then an intra-quad
+//           permutation turns the accumulator fragments into the A fragments of layer 3 (resident for the tile)
+//   layer 3 D3[64 x N3-channel chunk] = A2 * W3^T (A from registers) -> +bias, ReLU, max over the rows of each
+//           section: a segmented suffix max over the 16 rows of a warp (shuffles), then one integer atomicMax per
 //           (section part, channel) into the position-major feature map
-// A loader warp streams (or keeps resident) the pre-swizzled W2/W3 stage images; both warpgroups read
-// every stage, and a stage is released when both have retired the wgmma group that read it.
+// Only the weights go through shared memory.  A loader warp streams (or keeps resident) the pre-swizzled W2/W3
+// stage images; both warpgroups read every stage, and a stage is released when both have retired the wgmma group
+// that read it.  The loader is a whole warpgroup that gives its registers to the two consumer warpgroups
+// (setmaxnreg): at C2 = 256 the layer-3 A fragments alone take 128 registers per thread.
 //
 // "precision = 2" runs the same kernel on clusters of two CTAs (CL = 2, streamed-weight scales only): the two
 // CTAs take the two tiles of a tile pair in lock step, and every weight stage is fetched from L2 ONCE per
@@ -18,36 +22,53 @@
 #include "common.cuh"
 #include "wgmma.cuh"
 
+// Streamed weight ring at C1 = 256, in 16 KB stages (A-B builds: -DFCN_PN_RING_C256=N).
+#ifndef FCN_PN_RING_C256
+#define FCN_PN_RING_C256 4
+#endif
+
 namespace fcn {
 using namespace gmma;
 
 constexpr int TC_ROWS = 128;
 constexpr int TC_COMPUTE_WARPS = 8;                         // two warpgroups of 64 tile rows each
-constexpr int TC_THREADS = (TC_COMPUTE_WARPS + 1) * 32;     // + the weight loader warp
 constexpr int TC_STAGE_BYTES = 16384;
+constexpr int TC_SMEM_MAX = 232448;                         // 227 KB of dynamic shared memory per CTA
 
-template <int C1, int C2, int C3>
+template <int C1, int C2, int C3, int CL>
 struct TcCfg {
     static constexpr int KB1 = C1 / 32, KB2 = C2 / 32;
     static constexpr int N2 = C2 < 128 ? C2 : 128;
     static constexpr int NCH2 = C2 / N2;
-    static constexpr int N3 = 128;
-    static constexpr int NCH3 = C3 / N3;
-    static constexpr int A_BYTES = TC_ROWS * (C1 > C2 ? C1 : C2) * 4;
-    static constexpr int JOBS2 = NCH2 * KB1, JOBS3 = NCH3 * KB2, JOBS = JOBS2 + JOBS3;
-    // streamed rings: at C1 = 256, 4 stages measured faster on an H100 than 3 or 5 (5 is the most that fits)
-    static constexpr int NSTAGE = (C1 >= 256) ? 4 : (C1 >= 128 ? 6 : JOBS);
-    static constexpr bool RESIDENT = JOBS <= NSTAGE;
+    // W2 stage images in load order: K block major, its NCH2 column chunks side by side (job kb * NCH2 + nc)
+    static constexpr int JOBS2 = NCH2 * KB1, JOBS3 = (C3 / 128) * KB2, JOBS = JOBS2 + JOBS3;
     // Small-channel scales are latency-bound per tile (tiny MMAs, long SIMT phases): run TWO CTAs per SM
     // so that one CTA's epilogue overlaps the other's loads/MMAs.
     static constexpr int CTAS_PER_SM = (C1 <= 64) ? 2 : 1;
-    static constexpr int OFF_W = A_BYTES;
-    // resident weights are packed tightly (layer-2 stages are only N2 x 128 B), streamed stages use 16 KB slots
-    static constexpr int W_BYTES = RESIDENT ? (JOBS2 * N2 * 128 + JOBS3 * TC_STAGE_BYTES) : NSTAGE * TC_STAGE_BYTES;
+    // + the loader warpgroup (one lane loads), which gives its registers to the consumers: the layer-3 A fragments
+    // alone take C2 / 2 registers per thread.  One CTA per SM: 168 at launch -> 232 / 40 (2 x 232 + 40 per lane of
+    // an SM sub-partition); two CTAs per SM: 80 at launch -> 104 / 24 (8 x 104 + 4 x 24 = 12 x 80 per CTA).
+    static constexpr int THREADS = (TC_COMPUTE_WARPS + 4) * 32;
+    static constexpr int REGS_CONSUMER = CTAS_PER_SM == 1 ? 232 : 104, REGS_PRODUCER = CTAS_PER_SM == 1 ? 40 : 24;
+    static constexpr int OTHER_BYTES = 2 * TC_ROWS * 16 + C1 * 16 + C2 * 4 + C3 * 4 + 2 * TC_ROWS * 4;
+    // weight-resident when every stage fits (packed tightly: layer-2 stages are only N2 x 128 B); 2-CTA clusters
+    // exist to share streamed stages
+    static constexpr int W_RES_BYTES = JOBS2 * N2 * 128 + JOBS3 * TC_STAGE_BYTES;
+    static constexpr bool RESIDENT =
+        CL == 1 && W_RES_BYTES + OTHER_BYTES + 2 * JOBS * 8 + 1024 <= TC_SMEM_MAX / CTAS_PER_SM - (CTAS_PER_SM - 1) * 1024;
+    // streamed rings: 6 stages at C1 = 128 (2-CTA clusters only), 4 at C1 = 256 (with the activations in registers,
+    // car pointnet_s4 measured 0.101-0.103 ms per launch with 4, 8 and 12 stages alike on an H100 SXM at 400 W)
+    static constexpr int NSTAGE = RESIDENT ? JOBS : (C1 >= 256 ? FCN_PN_RING_C256 : 6);
+    // layer-3 chunk: 64 channels at two CTAs per SM (the register budget is 96 per thread there), else 128; a
+    // 64-channel chunk reads one half of a 128-row W3 stage image (resident weights only)
+    static constexpr int N3 = CTAS_PER_SM == 2 ? 64 : 128;
+    static constexpr int SUB3 = 128 / N3, NCH3 = C3 / N3;
+    static constexpr int W_BYTES = RESIDENT ? W_RES_BYTES : NSTAGE * TC_STAGE_BYTES;
     __host__ __device__ static constexpr int stage_off(int st) {
         return !RESIDENT ? st * TC_STAGE_BYTES
                          : (st < JOBS2 ? st * N2 * 128 : JOBS2 * N2 * 128 + (st - JOBS2) * TC_STAGE_BYTES);
     }
+    static constexpr int OFF_W = 0;
     static constexpr int OFF_RECS = OFF_W + W_BYTES;
     static constexpr int OFF_W1 = OFF_RECS + 2 * TC_ROWS * 16;       // recs are double-buffered by tile parity
     static constexpr int OFF_B2 = OFF_W1 + C1 * 16;
@@ -58,18 +79,23 @@ struct TcCfg {
     static constexpr int BYTES = OFF_BAR + NBAR * 8 + 1024;          // + alignment slack
     static_assert(C1 % 32 == 0 && C2 % 32 == 0 && C3 % 128 == 0, "channel counts");
     static_assert(C2 <= 256, "layer-2 accumulators: at most two 128-column chunks");
-    static_assert(BYTES <= 232448, "exceeds the 227 KB shared-memory limit per CTA");
+    static_assert(N3 == 128 || RESIDENT, "64-channel layer-3 chunks read resident W3 stages");
+    static_assert(BYTES <= TC_SMEM_MAX, "exceeds the 227 KB shared-memory limit per CTA");
     static_assert(CTAS_PER_SM == 1 || 2 * (BYTES + 1024) <= 233472, "two CTAs must fit in 228 KB per SM");
 };
 
+// One layer-1 output (fp32 FMA chain, folded BN, ReLU) as a TF32 operand.
+__device__ __forceinline__ uint32_t layer1_tf32(const float4 &r, const float4 &w) {
+    return __float_as_uint(to_tf32(fmaxf(fmaf(r.z, w.z, fmaf(r.y, w.y, fmaf(r.x, w.x, w.w))), 0.f)));
+}
+
 template <int C1, int C2, int C3, int CL>
-__global__ void __launch_bounds__(TC_THREADS, (TcCfg<C1, C2, C3>::CTAS_PER_SM))
+__global__ void __launch_bounds__((TcCfg<C1, C2, C3, CL>::THREADS), (TcCfg<C1, C2, C3, CL>::CTAS_PER_SM))
 pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
-    using Cfg = TcCfg<C1, C2, C3>;
+    using Cfg = TcCfg<C1, C2, C3, CL>;
     static_assert(CL == 1 || (CL == 2 && !Cfg::RESIDENT), "2-CTA clusters share streamed weight stages");
     extern __shared__ uint8_t smem_dyn[];
     uint8_t *smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-    uint8_t *sA = smem;
     uint8_t *sW = smem + Cfg::OFF_W;
     float4 *recs_all = (float4 *)(smem + Cfg::OFF_RECS);
     float4 *w1s = (float4 *)(smem + Cfg::OFF_W1);
@@ -99,10 +125,10 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
     };
 
     // ---- one-time setup
-    for (int i = tid; i < C1; i += TC_THREADS)
+    for (int i = tid; i < C1; i += Cfg::THREADS)
         w1s[i] = make_float4(__ldg(p.w1t + i), __ldg(p.w1t + C1 + i), __ldg(p.w1t + 2 * C1 + i), __ldg(p.b1 + i));
-    for (int i = tid; i < C2; i += TC_THREADS) b2s[i] = __ldg(p.b2 + i);
-    for (int i = tid; i < C3; i += TC_THREADS) b3s[i] = __ldg(p.b3 + i);
+    for (int i = tid; i < C2; i += Cfg::THREADS) b2s[i] = __ldg(p.b2 + i);
+    for (int i = tid; i < C3; i += Cfg::THREADS) b3s[i] = __ldg(p.b3 + i);
     if (tid == 0) {
         for (int i = 0; i < Cfg::NSTAGE; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], TC_COMPUTE_WARPS * CL); }
         fence_barrier_init();
@@ -110,9 +136,10 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
     __syncthreads();
     if (CL == 2) cluster_sync();                 // the peer's barriers are initialised before anyone signals them
 
-    if (warp == TC_COMPUTE_WARPS) {
-        // ================= weight loader (one lane) =================
-        if (lane == 0) {
+    if (warp >= TC_COMPUTE_WARPS) {
+        // ================= weight loader (one lane of the loader warpgroup) =================
+        setmaxnreg_dec<Cfg::REGS_PRODUCER>();
+        if (warp == TC_COMPUTE_WARPS && lane == 0) {
             const int ntile_loads = Cfg::RESIDENT ? 1 : my_tiles;
             uint32_t job = 0;
             for (int it = 0; it < ntile_loads; ++it) {
@@ -121,7 +148,9 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
                     mbar_wait(&w_empty[st], ph ^ 1);   // CL = 2: released by the consumers of both CTAs
                     const bool l2 = j < Cfg::JOBS2;
                     const uint32_t bytes = l2 ? Cfg::N2 * 128 : TC_STAGE_BYTES;
-                    const uint8_t *src = l2 ? (const uint8_t *)p.w2_tc + (size_t)j * (Cfg::N2 * 128)
+                    // the W2 image is chunk major (chunk nc, K block kb at nc * KB1 + kb)
+                    const int j2 = (j % Cfg::NCH2) * Cfg::KB1 + j / Cfg::NCH2;
+                    const uint8_t *src = l2 ? (const uint8_t *)p.w2_tc + (size_t)j2 * (Cfg::N2 * 128)
                                             : (const uint8_t *)p.w3_tc + (size_t)(j - Cfg::JOBS2) * TC_STAGE_BYTES;
                     mbar_arrive_expect_tx(&w_full[st], bytes);   // both halves land on this CTA's barrier
                     if (CL == 2) {
@@ -136,13 +165,17 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
     } else {
 
         // ================= compute warpgroups =================
-        const int wg = warp >> 2, wq = warp & 3, t = tid & 127;
-        const int l1_row = 64 * wg + (t & 63);                 // layer-1 role: row, K blocks kb = t/64, t/64 + 2, ...
-        const uint32_t l1_off = (uint32_t)((l1_row >> 3) * 1024 + (l1_row & 7) * 128);
-        const int rx = l1_row & 7;
-        const uint64_t adesc0 = make_desc_sw128(smem_u32(sA) + wg * (64 * 128));
+        setmaxnreg_inc<Cfg::REGS_CONSUMER>();
+        const int wg = warp >> 2, wq = warp & 3;
+        const int g = lane >> 2, q = lane & 3;
+        const int ra = 64 * wg + 16 * wq + g;                  // fragment rows of this thread: ra and ra + 8
         const uint64_t bdesc0 = make_desc_sw128(smem_u32(sW));
-        const int ra = 64 * wg + 16 * wq + (lane >> 2);        // fragment rows of this thread: ra and ra + 8
+        // Layer-2 accumulators -> layer-3 A fragments.  In each 8-column block, lane q of a quad holds columns
+        // (2q, 2q + 1) and needs (q, q + 4).  Two shuffles move the quad's 8 values: in the first, lane q sends
+        // its column 2q + psel and receives from lane src1; in the second it sends the other one and receives from
+        // src1 ^ 2.  Lanes with psel = 0 receive column q first, lanes with psel = 1 column q + 4.
+        const int psel = (q ^ (q >> 1)) & 1;
+        const int src1 = (lane & ~3) | (q >> 1) | (psel << 1), src2 = src1 ^ 2;
         uint32_t job = 0;
         int4 td_next = tile_of(0);
         float4 rec_next = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -182,72 +215,78 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
                     rec_next = ((const float4 *)p.rows + (size_t)td_next.x * p.row_cap + td_next.y)[tid];
             }
             asm volatile("bar.sync 1, %0;\n" ::"n"(TC_COMPUTE_WARPS * 32));
-            const float4 rec = recs[l1_row];
-            // ---- layer 1 (fp32 FMA) -> A1
-            for (int kb = t >> 6; kb < Cfg::KB1; kb += 2) {
-                uint8_t *dst = sA + kb * (TC_ROWS * 128) + l1_off;
-    #pragma unroll
-                for (int c4 = 0; c4 < 8; ++c4) {
-                    float o[4];
-    #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float4 w = w1s[kb * 32 + c4 * 4 + j];
-                        o[j] = to_tf32(fmaxf(fmaf(rec.z, w.z, fmaf(rec.y, w.y, fmaf(rec.x, w.x, w.w))), 0.f));
-                    }
-                    *(float4 *)(dst + ((c4 ^ rx) << 4)) = make_float4(o[0], o[1], o[2], o[3]);
-                }
-            }
-            fence_proxy_async();
-            asm volatile("bar.sync %0, 128;\n" ::"r"(2 + wg));
+            const float4 reca = recs[ra], recb = recs[ra + 8];
             if (Cfg::RESIDENT) job = 0;
 
-            // ---- layer 2: D2 = A1 * W2^T, all NCH2 chunks in registers (A2 overwrites A1)
+            // ---- layers 1 + 2: per K block, layer 1 computes the A fragments of its 4 k-steps (columns
+            //      32 kb + 8 k + q and + 4 of rows ra, ra + 8) while the previous block's MMAs run; D2 = A1 * W2^T
+            //      for all NCH2 chunks in registers.  The fragments alternate between two buffers: a buffer is
+            //      rewritten two K blocks later, after wait_group 1 has retired every group that read it.
             float acc2[Cfg::NCH2][Cfg::N2 / 2];
     #pragma unroll
-            for (int nc = 0; nc < Cfg::NCH2; ++nc) {
+            for (int nc = 0; nc < Cfg::NCH2; ++nc)
     #pragma unroll
                 for (int i = 0; i < Cfg::N2 / 2; ++i) acc2[nc][i] = 0.f;
-                for (int kb = 0; kb < Cfg::KB1; ++kb, ++job) {
+            uint32_t a1[2][4][4];
+    #pragma unroll
+            for (int kb = 0; kb < Cfg::KB1; ++kb) {
+                uint32_t (&a)[4][4] = a1[kb & 1];
+    #pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const float4 w0 = w1s[kb * 32 + 8 * k + q], w4 = w1s[kb * 32 + 8 * k + q + 4];
+                    a[k][0] = layer1_tf32(reca, w0);
+                    a[k][1] = layer1_tf32(recb, w0);
+                    a[k][2] = layer1_tf32(reca, w4);
+                    a[k][3] = layer1_tf32(recb, w4);
+                    fence_frag(a[k]);
+                }
+    #pragma unroll
+                for (int nc = 0; nc < Cfg::NCH2; ++nc, ++job) {
                     const uint32_t st = job % Cfg::NSTAGE, ph = Cfg::RESIDENT ? 0 : (job / Cfg::NSTAGE) & 1;
                     mbar_wait(&w_full[st], ph);
                     wgmma_fence();
                     fence_acc(acc2[nc]);
     #pragma unroll
                     for (int k = 0; k < 4; ++k)
-                        wgmma_tf32<Cfg::N2>(acc2[nc], adesc0 + (uint64_t)(kb * ((TC_ROWS * 128) >> 4) + 2 * k),
-                                            bdesc0 + (uint64_t)((Cfg::stage_off(st) >> 4) + 2 * k), (kb | k) != 0);
+                        wgmma_tf32_rs<Cfg::N2>(acc2[nc], a[k], bdesc0 + (uint64_t)((Cfg::stage_off(st) >> 4) + 2 * k),
+                                               (kb | k) != 0);
                     wgmma_commit();
                     fence_acc(acc2[nc]);
-                    if (!Cfg::RESIDENT) {
-                        wgmma_wait<1>();
-                        release_prev();
-                        prev = (int)st;
-                    }
+                    wgmma_wait<1>();
+                    release_prev();
+                    prev = (int)st;
                 }
             }
             wgmma_wait<0>();
     #pragma unroll
             for (int nc = 0; nc < Cfg::NCH2; ++nc) fence_acc(acc2[nc]);
             release_prev();
-            // ---- epilogue 2: +bias, ReLU, TF32 -> A2 (this warpgroup's rows; all its layer-2 MMAs are done)
+            // ---- epilogue 2: +bias, ReLU, TF32 in place, then the quad permutation into the A fragments of the
+            //      KB2 * 4 k-steps of layer 3 (k-step s = columns 8 s .. 8 s + 7)
+            uint32_t a2[Cfg::KB2 * 4][4];
     #pragma unroll
             for (int nc = 0; nc < Cfg::NCH2; ++nc)
     #pragma unroll
-                for (int i = 0; i < Cfg::N2 / 2; i += 2) {
-                    const int r = 64 * wg + frag_row(i, wq, lane), c = nc * Cfg::N2 + frag_col(i, lane);
-                    const float2 bb = *(const float2 *)(b2s + c);
-                    const float2 o = make_float2(to_tf32(fmaxf(acc2[nc][i] + bb.x, 0.f)),
-                                                 to_tf32(fmaxf(acc2[nc][i + 1] + bb.y, 0.f)));
-                    *(float2 *)(sA + (c >> 5) * (TC_ROWS * 128) + sw128_offset(r, c & 31)) = o;
+                for (int j = 0; j < Cfg::N2 / 8; ++j) {
+                    const float2 bb = *(const float2 *)(b2s + nc * Cfg::N2 + 8 * j + 2 * q);
+    #pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const float v0 = to_tf32(fmaxf(acc2[nc][4 * j + 2 * h] + bb.x, 0.f));
+                        const float v1 = to_tf32(fmaxf(acc2[nc][4 * j + 2 * h + 1] + bb.y, 0.f));
+                        const float x1 = __shfl_sync(0xffffffffu, psel ? v1 : v0, src1);
+                        const float x2 = __shfl_sync(0xffffffffu, psel ? v0 : v1, src2);
+                        uint32_t (&a)[4] = a2[nc * (Cfg::N2 / 8) + j];
+                        a[h] = __float_as_uint(psel ? x2 : x1);
+                        a[2 + h] = __float_as_uint(psel ? x1 : x2);
+                    }
                 }
-            fence_proxy_async();
-            asm volatile("bar.sync %0, 128;\n" ::"r"(2 + wg));
+    #pragma unroll
+            for (int s = 0; s < Cfg::KB2 * 4; ++s) fence_frag(a2[s]);
 
             // ---- layer 3 + section max.  Rows ra (fragment half 0) and ra + 8 (half 1) of this thread; the suffix
             //      max over the rows of a section runs over the 8 lanes l/4 = 0..7 of each half, then half 0 takes in
             //      half 1's head when the section crosses row 8 of the warp.  +bias, ReLU, TF32 rounding commute with
             //      the max (monotone), values >= 0 so the integer atomicMax on the float bits is exact.
-            const int g = lane >> 2;
             const int sa = sect_s[ra], sb = sect_s[ra + 8], s8 = sect_s[ra - g + 8];
             unsigned oka = 0, okb = 0;                 // bit d: row + (1 << d) is in the same section and 8-row half
     #pragma unroll
@@ -264,15 +303,19 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
                 float acc3[Cfg::N3 / 2];
     #pragma unroll
                 for (int i = 0; i < Cfg::N3 / 2; ++i) acc3[i] = 0.f;
+    #pragma unroll
                 for (int kb = 0; kb < Cfg::KB2; ++kb, ++job) {
-                    const uint32_t st = job % Cfg::NSTAGE, ph = Cfg::RESIDENT ? 0 : (job / Cfg::NSTAGE) & 1;
+                    // resident: W3 stage (128-channel chunk nc / SUB3, K block kb), column half nc % SUB3
+                    const uint32_t st = Cfg::RESIDENT ? Cfg::JOBS2 + (nc / Cfg::SUB3) * Cfg::KB2 + kb : job % Cfg::NSTAGE;
+                    const uint32_t ph = Cfg::RESIDENT ? 0 : (job / Cfg::NSTAGE) & 1;
+                    const uint32_t boff = Cfg::stage_off(st) + (nc % Cfg::SUB3) * (Cfg::N3 * 128);
                     mbar_wait(&w_full[st], ph);
                     wgmma_fence();
                     fence_acc(acc3);
     #pragma unroll
                     for (int k = 0; k < 4; ++k)
-                        wgmma_tf32<Cfg::N3>(acc3, adesc0 + (uint64_t)(kb * ((TC_ROWS * 128) >> 4) + 2 * k),
-                                            bdesc0 + (uint64_t)((Cfg::stage_off(st) >> 4) + 2 * k), (kb | k) != 0);
+                        wgmma_tf32_rs<Cfg::N3>(acc3, a2[4 * kb + k], bdesc0 + (uint64_t)((boff >> 4) + 2 * k),
+                                               (kb | k) != 0);
                     wgmma_commit();
                     fence_acc(acc3);
                     if (!Cfg::RESIDENT) {
@@ -300,7 +343,7 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
                         const float x = __shfl_sync(0xffffffffu, v[2 + e], lane & 3);   // row 8 of this warp
                         if (merge_a) v[e] = fmaxf(v[e], x);
                     }
-                    const int c = nc * Cfg::N3 + 8 * j + 2 * (lane & 3);
+                    const int c = nc * Cfg::N3 + 8 * j + 2 * q;
                     const float2 bb = *(const float2 *)(b3s + c);
     #pragma unroll
                     for (int e = 0; e < 4; ++e) {
@@ -321,14 +364,14 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
 
 template <int C1, int C2, int C3, int CL>
 static int launch_tc(const fcn_pointnet_args &a, cudaStream_t stream) {
-    using Cfg = TcCfg<C1, C2, C3>;
+    using Cfg = TcCfg<C1, C2, C3, CL>;
     auto kern = pointnet_tc_kernel<C1, C2, C3, CL>;
     FCN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::BYTES));
     int clusters = sm_count() * Cfg::CTAS_PER_SM / CL;
     if (clusters > (a.max_tiles + CL - 1) / CL) clusters = (a.max_tiles + CL - 1) / CL;
     if (clusters < 1) return FCN_OK;
     static const int prio = env_priority("FCN_PRIO_PN");
-    FCN_CUDA(launch_pdl_cluster(prio, CL, kern, dim3(clusters * CL), dim3(TC_THREADS), (size_t)Cfg::BYTES, stream, a));
+    FCN_CUDA(launch_pdl_cluster(prio, CL, kern, dim3(clusters * CL), dim3(Cfg::THREADS), (size_t)Cfg::BYTES, stream, a));
     return FCN_OK;
 }
 
