@@ -262,6 +262,21 @@ class SunrgbdEvalResult(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class FrustumFrame(C.Structure):
+    _fields_ = [("P", C.c_double * 12), ("V2C", C.c_double * 12), ("R0", C.c_double * 9),
+                ("height", C.c_int32), ("width", C.c_int32)]
+
+
+class FrustumExtractArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("num_frames", "num_points", "num_dets", "num_kept")] + \
+               [("num_out_points", C.c_longlong)] + \
+               [(n, C.c_void_p) for n in ("scans", "scan_offsets", "host_scan_offsets", "frames", "boxes",
+                                          "det_frame", "workspace")] + \
+               [("workspace_bytes", C.c_longlong)] + \
+               [(n, C.c_void_p) for n in ("info", "det_points", "points", "offsets", "frustum_angle", "box2d", "P",
+                                          "det_index")]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -308,6 +323,9 @@ SIGNATURES = {
     "fcn_sunrgbd_eval_workspace_bytes": (C.c_longlong, [C.POINTER(SunrgbdEvalArgs)]),
     "fcn_sunrgbd_eval_match": (_I, [C.POINTER(SunrgbdEvalArgs), _P]),
     "fcn_sunrgbd_eval_curves": (_I, [C.POINTER(SunrgbdEvalArgs), _P]),
+    "fcn_frustum_extract_workspace_bytes": (C.c_longlong, [C.POINTER(FrustumExtractArgs)]),
+    "fcn_frustum_extract_count": (_I, [C.POINTER(FrustumExtractArgs), _P]),
+    "fcn_frustum_extract_write": (_I, [C.POINTER(FrustumExtractArgs), _P]),
 }
 
 _lib = None

@@ -1,0 +1,344 @@
+// KITTI frustum extraction on the device (C ABI section (15)): extract_frustum_data_rgb_detection of
+// kitti/prepare_data.py:462-568 for several frames and all their 2-D detections in one pair of calls.
+//
+// The reference re-masks the whole scan for every detection and projects every scan twice.  Here:
+//   fcn_frustum_extract_count  flags    one thread per scan point: velo -> rect -> image in float64 (every product and
+//                                       sum rounded separately, kitti_util.py:172-210) and the image test of
+//                                       get_lidar_in_image_fov (draw_util.py:15-18);
+//                              scan     exclusive sum of the flags over all frames (frames stay contiguous, scan order
+//                                       is kept): the position of every in-image point;
+//                              compact  the in-image points, recomputed, stored at those positions: float32 rect and
+//                                       intensity (prepare_data.py:506-508) plus float64 u, v;
+//                              count    one CTA per detection over its frame's in-image points only: the clipped box
+//                                       (:522-524), the box test (:527-532), the frustum angle (:537-543) and the
+//                                       drop rules (:546-548);
+//                              scans    exclusive sums over the kept detections and their point counts, then info;
+//   fcn_frustum_extract_write  write    one CTA per kept detection: the box test again, a block scan for stable
+//                                       positions, the points scattered in scan order, and the per-detection values.
+#include <cub/cub.cuh>
+
+#include <cmath>
+
+#include "common.cuh"
+#include "input_builder.cuh"
+
+namespace fcn {
+
+constexpr int FX_THREADS = 256;
+constexpr int FX_FRAME_DOUBLES = 33;     // P (12), V2C (12), R0 (9) of fcn_frustum_frame
+
+// velo (x, y, z) -> float32 rect and float64 image coordinates; true when the point is in the image.  The order of the
+// operations is restated by oracle/frustum_extract.py.
+__device__ __forceinline__ bool fx_project(const double *__restrict__ m, int height, int width, float4 s, float4 *rect,
+                                           double *u, double *v) {
+    const double *P = m, *V = m + 12, *R = m + 24;
+    const double x = s.x, y = s.y, z = s.z;
+    double ref[3], r[3], img[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+        ref[i] = dadd<true>(dadd<true>(dadd<true>(dmul<true>(V[4 * i], x), dmul<true>(V[4 * i + 1], y)),
+                                       dmul<true>(V[4 * i + 2], z)), V[4 * i + 3]);
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+        r[i] = dadd<true>(dadd<true>(dmul<true>(R[3 * i], ref[0]), dmul<true>(R[3 * i + 1], ref[1])),
+                          dmul<true>(R[3 * i + 2], ref[2]));
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+        img[i] = dadd<true>(dadd<true>(dadd<true>(dmul<true>(P[4 * i], r[0]), dmul<true>(P[4 * i + 1], r[1])),
+                                       dmul<true>(P[4 * i + 2], r[2])), P[4 * i + 3]);
+    *u = __ddiv_rn(img[0], img[2]);
+    *v = __ddiv_rn(img[1], img[2]);
+    *rect = make_float4((float)r[0], (float)r[1], (float)r[2], s.w);
+    return *u >= 0.0 && *u < (double)width && *v >= 0.0 && *v < (double)height && s.x > 2.0f;
+}
+
+// one frame per blockIdx.y; the frame's matrices in shared memory
+__device__ __forceinline__ void fx_load_frame(const fcn_frustum_frame *__restrict__ frames, int f, double *m) {
+    if (threadIdx.x < FX_FRAME_DOUBLES) m[threadIdx.x] = frames[f].P[threadIdx.x];   // P, V2C, R0 are contiguous
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(FX_THREADS)
+fx_flag_kernel(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
+               const fcn_frustum_frame *__restrict__ frames, int32_t *__restrict__ flags) {
+    __shared__ double m[FX_FRAME_DOUBLES];
+    const int f = blockIdx.y;
+    fx_load_frame(frames, f, m);
+    const int i = so[f] + blockIdx.x * FX_THREADS + threadIdx.x;
+    if (i >= so[f + 1]) return;
+    float4 rect;
+    double u, v;
+    flags[i] = fx_project(m, frames[f].height, frames[f].width, scans[i], &rect, &u, &v) ? 1 : 0;
+}
+
+__global__ void __launch_bounds__(FX_THREADS)
+fx_compact_kernel(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
+                  const fcn_frustum_frame *__restrict__ frames, const int32_t *__restrict__ pos,
+                  float4 *__restrict__ fov_pts, double *__restrict__ fov_u, double *__restrict__ fov_v) {
+    __shared__ double m[FX_FRAME_DOUBLES];
+    const int f = blockIdx.y;
+    fx_load_frame(frames, f, m);
+    const int i = so[f] + blockIdx.x * FX_THREADS + threadIdx.x;
+    if (i >= so[f + 1]) return;
+    float4 rect;
+    double u, v;
+    if (fx_project(m, frames[f].height, frames[f].width, scans[i], &rect, &u, &v)) {
+        const int k = pos[i];
+        fov_pts[k] = rect;
+        fov_u[k] = u;
+        fov_v[k] = v;
+    }
+}
+
+// np.clip(a, 0, hi): NaN stays NaN
+__device__ __forceinline__ double fx_clip(double a, double hi) {
+    const double c = a < 0.0 ? 0.0 : a;
+    return c > hi ? hi : c;
+}
+
+__device__ __forceinline__ bool fx_in_box(double u, double v, const double *b) {
+    return u < b[2] && u >= b[0] && v < b[3] && v >= b[1];
+}
+
+__global__ void __launch_bounds__(FX_THREADS)
+fx_count_kernel(int num_frames, const int32_t *__restrict__ so, const fcn_frustum_frame *__restrict__ frames,
+                const double *__restrict__ boxes, const int32_t *__restrict__ det_frame,
+                const int32_t *__restrict__ pos, const double *__restrict__ fov_u, const double *__restrict__ fov_v,
+                int32_t *__restrict__ det_points, int32_t *__restrict__ keep, long long *__restrict__ cnt,
+                double *__restrict__ box_ws, double *__restrict__ angle_ws, int32_t *__restrict__ bad) {
+    using Reduce = cub::BlockReduce<int, FX_THREADS>;
+    __shared__ typename Reduce::TempStorage tmp;
+    const int d = blockIdx.x, f = det_frame[d];
+    if (f < 0 || f >= num_frames) {
+        if (threadIdx.x == 0) {
+            det_points[d] = -1;
+            keep[d] = 0;
+            cnt[d] = 0;
+            atomicAdd(bad, 1);
+        }
+        return;
+    }
+    const fcn_frustum_frame *fr = frames + f;
+    double b[4];
+    b[0] = fx_clip(boxes[4 * d + 0], (double)(fr->width - 1));
+    b[1] = fx_clip(boxes[4 * d + 1], (double)(fr->height - 1));
+    b[2] = fx_clip(boxes[4 * d + 2], (double)(fr->width - 1));
+    b[3] = fx_clip(boxes[4 * d + 3], (double)(fr->height - 1));
+    const int p0 = pos[so[f]], p1 = pos[so[f + 1]];
+    int c = 0;
+    for (int i = p0 + threadIdx.x; i < p1; i += FX_THREADS) c += fx_in_box(fov_u[i], fov_v[i], b);
+    c = Reduce(tmp).Sum(c);
+    if (threadIdx.x == 0) {
+        const bool drop = b[3] - b[1] < 5.0 || b[2] - b[0] < 1.0 || c < 1;
+        det_points[d] = drop ? -1 : c;
+        keep[d] = drop ? 0 : 1;
+        cnt[d] = drop ? 0 : c;
+        const RectProjection rp(b, fr->P);
+        double x, y;
+        rp.at(20.0, &x, &y);
+        angle_ws[d] = -atan2(20.0, x);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) box_ws[4 * d + j] = b[j];
+    }
+}
+
+__global__ void fx_info_kernel(int num_dets, const int32_t *__restrict__ keep_pos,
+                               const long long *__restrict__ cnt_pos, const int32_t *__restrict__ bad,
+                               long long *__restrict__ info) {
+    info[0] = keep_pos[num_dets];
+    info[1] = cnt_pos[num_dets];
+    info[2] = *bad;
+    info[3] = 0;
+}
+
+__global__ void __launch_bounds__(FX_THREADS)
+fx_write_kernel(int num_kept, long long num_out, const int32_t *__restrict__ so,
+                const fcn_frustum_frame *__restrict__ frames, const int32_t *__restrict__ det_frame,
+                const int32_t *__restrict__ det_points, const int32_t *__restrict__ keep_pos,
+                const long long *__restrict__ cnt_pos, const double *__restrict__ box_ws,
+                const double *__restrict__ angle_ws, const int32_t *__restrict__ pos,
+                const float4 *__restrict__ fov_pts, const double *__restrict__ fov_u,
+                const double *__restrict__ fov_v, float4 *__restrict__ points, int32_t *__restrict__ offsets,
+                double *__restrict__ angle, double *__restrict__ box2d, double *__restrict__ P,
+                int32_t *__restrict__ det_index) {
+    using Scan = cub::BlockScan<int, FX_THREADS>;
+    __shared__ typename Scan::TempStorage tmp;
+    const int d = blockIdx.x, c = det_points[d];
+    if (c < 0) return;
+    const int k = keep_pos[d];
+    const long long base = cnt_pos[d];
+    if (k >= num_kept || base + c > num_out) return;     // sizes read by the host disagree with the count pass
+    const int f = det_frame[d];
+    const double *b = box_ws + 4 * d;
+    if (threadIdx.x < 12) P[12 * k + threadIdx.x] = frames[f].P[threadIdx.x];
+    if (threadIdx.x < 4) box2d[4 * k + threadIdx.x] = b[threadIdx.x];
+    if (threadIdx.x == 0) {
+        offsets[k + 1] = (int32_t)(base + c);
+        angle[k] = angle_ws[d];
+        det_index[k] = d;
+    }
+    const double bb[4] = {b[0], b[1], b[2], b[3]};
+    const int p0 = pos[so[f]], p1 = pos[so[f + 1]];
+    int run = 0;
+    for (int i0 = p0; i0 < p1 && run < c; i0 += FX_THREADS) {
+        const int i = i0 + threadIdx.x;
+        const int flag = i < p1 && fx_in_box(fov_u[i], fov_v[i], bb);
+        int off, total;
+        Scan(tmp).ExclusiveSum(flag, off, total);
+        if (flag) points[base + run + off] = fov_pts[i];
+        run += total;
+        __syncthreads();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ host side
+struct FxWs {
+    int32_t *flags, *pos, *keep, *keep_pos, *bad;
+    long long *cnt, *cnt_pos;
+    float4 *fov_pts;
+    double *fov_u, *fov_v, *box, *angle;
+    void *temp;
+    size_t temp_bytes, total;
+};
+
+static size_t fx_align(size_t x) { return (x + 255) & ~(size_t)255; }
+
+static cudaError_t fx_layout(const fcn_frustum_extract_args *a, char *base, FxWs &w) {
+    const size_t N = (size_t)a->num_points, D = (size_t)a->num_dets;
+    size_t t0 = 0, t1 = 0, t2 = 0;
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, t0, (const int32_t *)nullptr, (int32_t *)nullptr,
+                                                  a->num_points + 1);
+    if (e != cudaSuccess) return e;
+    e = cub::DeviceScan::ExclusiveSum(nullptr, t1, (const int32_t *)nullptr, (int32_t *)nullptr, a->num_dets + 1);
+    if (e != cudaSuccess) return e;
+    e = cub::DeviceScan::ExclusiveSum(nullptr, t2, (const long long *)nullptr, (long long *)nullptr,
+                                      a->num_dets + 1);
+    if (e != cudaSuccess) return e;
+    w.temp_bytes = t0 > t1 ? t0 : t1;
+    w.temp_bytes = w.temp_bytes > t2 ? w.temp_bytes : t2;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += fx_align(bytes); return p; };
+    w.flags = (int32_t *)take((N + 1) * 4);
+    w.pos = (int32_t *)take((N + 1) * 4);
+    w.fov_pts = (float4 *)take(N * 16);
+    w.fov_u = (double *)take(N * 8);
+    w.fov_v = (double *)take(N * 8);
+    w.keep = (int32_t *)take((D + 1) * 4);
+    w.keep_pos = (int32_t *)take((D + 1) * 4);
+    w.cnt = (long long *)take((D + 1) * 8);
+    w.cnt_pos = (long long *)take((D + 1) * 8);
+    w.box = (double *)take(D * 32);
+    w.angle = (double *)take(D * 8);
+    w.bad = (int32_t *)take(4);
+    w.temp = take(w.temp_bytes);
+    w.total = off;
+    return cudaSuccess;
+}
+
+// Host-side checks shared by every entry: counts, pointers, the host copy of the scan offsets.  Sets *max_n to the
+// largest scan.
+static int fx_check(const fcn_frustum_extract_args *a, const char *fn, int *max_n) {
+    if (a == nullptr) return invalid(fn, "NULL args");
+    if (a->num_frames < 0 || a->num_points < 0 || a->num_dets < 0)
+        return invalid(fn, "negative count (num_frames, num_points, num_dets must be >= 0)");
+    if (a->num_frames > 65535 || a->num_points > (1 << 30) || a->num_dets > (1 << 28))
+        return invalid(fn, "too large (num_frames <= 65535, num_points <= 2^30, num_dets <= 2^28)");
+    *max_n = 0;
+    if (a->num_frames == 0 || a->num_dets == 0) return FCN_OK;
+    if (!a->host_scan_offsets) return invalid(fn, "NULL host_scan_offsets");
+    if (!a->scan_offsets || !a->frames || !a->boxes || !a->det_frame || (a->num_points > 0 && !a->scans))
+        return invalid(fn, "NULL pointer");
+    if (((uintptr_t)a->scans & 15) != 0) return invalid(fn, "scans must be 16-byte aligned");
+    const int32_t *so = a->host_scan_offsets;
+    if (so[0] != 0 || so[a->num_frames] != a->num_points)
+        return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
+    for (int f = 0; f < a->num_frames; ++f) {
+        if (so[f + 1] < so[f]) return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
+        if (so[f + 1] - so[f] > *max_n) *max_n = so[f + 1] - so[f];
+    }
+    return FCN_OK;
+}
+
+static int fx_prepare(const fcn_frustum_extract_args *a, const char *fn, FxWs &w, int *max_n) {
+    const int st = fx_check(a, fn, max_n);
+    if (st != FCN_OK || a->num_frames == 0 || a->num_dets == 0) return st;
+    if (!a->workspace || !a->info || !a->det_points) return invalid(fn, "NULL workspace, info or det_points");
+    cudaError_t e = fx_layout(a, nullptr, w);
+    if (e != cudaSuccess) return cuda_fail(fn, e);
+    if (a->workspace_bytes < (long long)w.total)
+        return invalid(fn, "workspace smaller than fcn_frustum_extract_workspace_bytes()");
+    e = fx_layout(a, (char *)a->workspace, w);
+    if (e != cudaSuccess) return cuda_fail(fn, e);
+    return FCN_OK;
+}
+
+}  // namespace fcn
+
+using namespace fcn;
+
+extern "C" long long fcn_frustum_extract_workspace_bytes(const fcn_frustum_extract_args *a) {
+    int max_n;
+    if (fx_check(a, __func__, &max_n) != FCN_OK) return -1;
+    if (a->num_frames == 0 || a->num_dets == 0) return 0;
+    FxWs w;
+    const cudaError_t e = fx_layout(a, nullptr, w);
+    if (e != cudaSuccess) {
+        cuda_fail(__func__, e);
+        return -1;
+    }
+    return (long long)w.total;
+}
+
+extern "C" int fcn_frustum_extract_count(const fcn_frustum_extract_args *a, fcn_stream_t stream) {
+    FxWs w;
+    int max_n;
+    const int st = fx_prepare(a, __func__, w, &max_n);
+    if (st != FCN_OK || a->num_frames == 0 || a->num_dets == 0) return st;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int N = a->num_points, D = a->num_dets, F = a->num_frames;
+    const float4 *scans = (const float4 *)a->scans;
+    FCN_CUDA(cudaMemsetAsync(w.flags + N, 0, 4, s));
+    FCN_CUDA(cudaMemsetAsync(w.keep + D, 0, 4, s));
+    FCN_CUDA(cudaMemsetAsync(w.cnt + D, 0, 8, s));
+    FCN_CUDA(cudaMemsetAsync(w.bad, 0, 4, s));
+    const dim3 grid(ceil_div(max_n, FX_THREADS), F);
+    if (max_n > 0) {
+        fx_flag_kernel<<<grid, FX_THREADS, 0, s>>>(scans, a->scan_offsets, a->frames, w.flags);
+        FCN_LAUNCH_CHECK();
+    }
+    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.flags, w.pos, N + 1, s));
+    if (max_n > 0) {
+        fx_compact_kernel<<<grid, FX_THREADS, 0, s>>>(scans, a->scan_offsets, a->frames, w.pos, w.fov_pts, w.fov_u,
+                                                      w.fov_v);
+        FCN_LAUNCH_CHECK();
+    }
+    fx_count_kernel<<<D, FX_THREADS, 0, s>>>(F, a->scan_offsets, a->frames, a->boxes, a->det_frame, w.pos, w.fov_u,
+                                             w.fov_v, a->det_points, w.keep, w.cnt, w.box, w.angle, w.bad);
+    FCN_LAUNCH_CHECK();
+    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.keep, w.keep_pos, D + 1, s));
+    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.cnt, w.cnt_pos, D + 1, s));
+    fx_info_kernel<<<1, 1, 0, s>>>(D, w.keep_pos, w.cnt_pos, w.bad, a->info);
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
+}
+
+extern "C" int fcn_frustum_extract_write(const fcn_frustum_extract_args *a, fcn_stream_t stream) {
+    FxWs w;
+    int max_n;
+    const int st = fx_prepare(a, __func__, w, &max_n);
+    if (st != FCN_OK || a->num_frames == 0 || a->num_dets == 0) return st;
+    if (a->num_kept < 0 || a->num_kept > a->num_dets || a->num_out_points < 0 || a->num_out_points > INT32_MAX)
+        return invalid(__func__, "num_kept must be in [0, num_dets] and num_out_points in [0, 2^31)");
+    if (!a->offsets || (a->num_kept > 0 && (!a->frustum_angle || !a->box2d || !a->P || !a->det_index)) ||
+        (a->num_out_points > 0 && !a->points))
+        return invalid(__func__, "NULL output");
+    cudaStream_t s = (cudaStream_t)stream;
+    FCN_CUDA(cudaMemsetAsync(a->offsets, 0, 4, s));
+    if (a->num_kept == 0) return FCN_OK;
+    fx_write_kernel<<<a->num_dets, FX_THREADS, 0, s>>>(
+        a->num_kept, a->num_out_points, a->scan_offsets, a->frames, a->det_frame, a->det_points, w.keep_pos,
+        w.cnt_pos, w.box, w.angle, w.pos, w.fov_pts, w.fov_u, w.fov_v, (float4 *)a->points, a->offsets,
+        a->frustum_angle, a->box2d, a->P, a->det_index);
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
+}

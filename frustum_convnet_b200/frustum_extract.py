@@ -1,0 +1,211 @@
+"""KITTI frustums from raw LiDAR scans and 2-D detections on the device: extract_frustum_data_rgb_detection of the
+reference (kitti/prepare_data.py:462-568) without its pickle, for a whole set of frames in one call.
+
+    ids, types, probs, boxes = read_rgb_detections(open("rgb_detection_val.txt"))
+    fr = FrustumExtractor(type_whitelist=("Car",)).extract(scans, calibs, image_hw, ids, types, probs, boxes)
+    fb.set_frustums_device(fr.points, fr.offsets, fr.frustum_angle, fr.box2d, fr.P)   # FrustumBatchBuilder
+    col = DetectionCollector(fr.id_list, fr.type_list, fr.box2d_list)
+
+``scans[data_idx]`` is an (n, 4) float32 scan (x, y, z, intensity in Velodyne coordinates; numpy or a CUDA tensor),
+``calibs[data_idx]`` a dict with 'P2', 'Tr_velo_to_cam' and 'R0_rect' (the calib file's float64 values) and
+``image_hw[data_idx]`` the image's (height, width).  The result holds what the reference pickles: device tensors
+``points`` (M, 4) float32, ``offsets`` (K + 1) int32, ``frustum_angle`` (K) float64, ``box2d`` (K, 4) float64 and
+``P`` (K, 12) float64; host ``counts`` and the lists ``id_list``, ``type_list``, ``box2d_list``, ``prob_list``,
+``calib_list`` in the pickle's order.  Points, counts, boxes and order are bit-identical to the reference's wherever
+its matmul rounding and the kernel's fixed elementwise order (csrc/frustum_extract.cu) agree on a point's side of an
+edge; the angle comes from CUDA's atan2 (within 2 ulp of glibc's).  The thresholds (5 px, 1 point) and the 2 m
+distance are the reference's.  One host sync per call, to learn K and M.  No CPU fallback: CPU tensors raise."""
+from __future__ import annotations
+
+import ctypes as C
+import os
+
+import numpy as np
+import torch
+
+from . import _lib
+
+DET_ID2STR = {1: "Pedestrian", 2: "Car", 3: "Cyclist"}
+
+
+def read_rgb_detections(lines):
+    """Lines 'path type prob xmin ymin xmax ymax' (read_det_file, prepare_data.py:428-446) ->
+    (id_list, type_list, prob_list, box2d_list); the type is a detector id of DET_ID2STR or a type name."""
+    id_list, type_list, prob_list, box2d_list = [], [], [], []
+    for line in lines:
+        t = line.rstrip().split(" ")
+        id_list.append(int(os.path.basename(t[0]).rstrip(".png")))
+        try:
+            cls_type = DET_ID2STR[int(t[1])]
+        except ValueError:
+            if t[1] not in DET_ID2STR.values():
+                raise ValueError("unknown detection type %r" % t[1])
+            cls_type = t[1]
+        type_list.append(cls_type)
+        prob_list.append(float(t[2]))
+        box2d_list.append(np.array([float(t[i]) for i in range(3, 7)]))
+    return id_list, type_list, prob_list, box2d_list
+
+
+class Frustums:
+    """One extraction: K kept detections and their M points (see the module docstring)."""
+
+    def __init__(self, points, offsets, frustum_angle, box2d, P, counts, id_list, type_list, box2d_list, prob_list,
+                 calib_list, det_index):
+        self.points, self.offsets, self.frustum_angle, self.box2d, self.P = points, offsets, frustum_angle, box2d, P
+        self.counts = counts
+        self.id_list, self.type_list, self.box2d_list = id_list, type_list, box2d_list
+        self.prob_list, self.calib_list = prob_list, calib_list
+        self.det_index = det_index          # (K,) host int64: the detection line of each kept frustum
+
+    def __len__(self):
+        return len(self.id_list)
+
+
+def on_device(t, dev):
+    """t is a CUDA tensor on dev ('cuda' without an index: the current device)."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        return False
+    return t.device.index == (dev.index if dev.index is not None else torch.cuda.current_device())
+
+
+def _frame_record(calib, hw):
+    f = _lib.FrustumFrame()
+    for name, key, n in (("P", "P2", 12), ("V2C", "Tr_velo_to_cam", 12), ("R0", "R0_rect", 9)):
+        v = np.asarray(calib[key], dtype=np.float64).reshape(-1)
+        if v.size != n:
+            raise ValueError("calib %s must hold %d values, got %d" % (key, n, v.size))
+        getattr(f, name)[:] = v.tolist()
+    h, w = (int(x) for x in hw)
+    if h <= 0 or w <= 0:
+        raise ValueError("image size must be positive, got %r" % (hw,))
+    f.height, f.width = h, w
+    return f
+
+
+class FrustumExtractor:
+    def __init__(self, type_whitelist=("Car",), device=None):
+        self.type_whitelist = tuple(type_whitelist)
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        if self.device.type != "cuda":
+            raise RuntimeError("FrustumExtractor: a CUDA device is required (there is no CPU fallback)")
+
+    def _scan(self, scan):
+        if isinstance(scan, torch.Tensor):
+            if not on_device(scan, self.device):
+                raise RuntimeError("FrustumExtractor: scans must be numpy arrays or CUDA tensors on %s" % self.device)
+            if scan.dtype != torch.float32 or scan.dim() != 2 or scan.shape[1] != 4:
+                raise ValueError("a scan must be an (n, 4) float32 array")
+            return scan
+        a = np.asarray(scan)
+        if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
+            raise ValueError("a scan must be an (n, 4) float32 array")
+        return a
+
+    def extract(self, scans, calibs, image_hw, id_list, type_list, prob_list, box2d_list, stream=None, timer=None):
+        """-> Frustums.  Runs on `stream` (default: the current stream of the extractor's device).  `timer(name)`
+        (optional, benchmarks) is called around the two device calls: "start", "count", "write_start", "write"."""
+        n = len(id_list)
+        if len(type_list) != n or len(prob_list) != n or len(box2d_list) != n:
+            raise ValueError("id_list, type_list, prob_list and box2d_list must have the same length")
+        lines = [i for i in range(n) if type_list[i] in self.type_whitelist]
+        frame_of, frame_ids = {}, []
+        for i in lines:
+            if id_list[i] not in frame_of:
+                frame_of[id_list[i]] = len(frame_ids)
+                frame_ids.append(id_list[i])
+        boxes = np.array([np.asarray(box2d_list[i], dtype=np.float64).reshape(4) for i in lines],
+                         dtype=np.float64).reshape(-1, 4)
+        if not np.isfinite(boxes).all():
+            raise ValueError("2-D boxes must be finite")
+        det_frame = np.array([frame_of[id_list[i]] for i in lines], dtype=np.int32)
+        sc = [self._scan(scans[k]) for k in frame_ids]
+        frames = (_lib.FrustumFrame * len(frame_ids))(*[_frame_record(calibs[k], image_hw[k]) for k in frame_ids])
+        so = np.zeros(len(frame_ids) + 1, dtype=np.int32)
+        np.cumsum([s.shape[0] for s in sc], out=so[1:])
+        dev = self.device
+        F, D, N = len(frame_ids), len(lines), int(so[-1])
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.device(dev), torch.cuda.stream(stream):
+            if F == 0 or D == 0:
+                return self._result(torch.zeros((0, 4), dtype=torch.float32, device=dev),
+                                    torch.zeros(1, dtype=torch.int32, device=dev), *self._empty(dev),
+                                    np.zeros(0, np.int64), [], id_list, type_list, prob_list, box2d_list, calibs,
+                                    image_hw)
+            if all(isinstance(s, np.ndarray) for s in sc):
+                scan_dev = torch.from_numpy(np.concatenate(sc)).to(dev)
+            else:
+                scan_dev = torch.cat([s if isinstance(s, torch.Tensor) else torch.from_numpy(s).to(dev)
+                                      for s in sc]).contiguous()
+            # one host buffer: frames | boxes (D*4 f64) | scan offsets (F+1 i32) | det frames (D i32)
+            nb = [C.sizeof(frames), D * 32, (F + 1) * 4, D * 4]
+            o = np.cumsum([0] + nb)
+            hbuf = np.empty(int(o[-1]), dtype=np.uint8)
+            hbuf[o[0]:o[1]] = np.frombuffer(bytes(frames), dtype=np.uint8)
+            hbuf[o[1]:o[2]] = boxes.view(np.uint8).reshape(-1)
+            hbuf[o[2]:o[3]] = so.view(np.uint8)
+            hbuf[o[3]:o[4]] = det_frame.view(np.uint8)
+            inp = torch.from_numpy(hbuf).to(dev)
+            a = _lib.FrustumExtractArgs()
+            a.num_frames, a.num_points, a.num_dets = F, N, D
+            a.scans = scan_dev.data_ptr() if N > 0 else None
+            ib = inp.data_ptr()
+            a.frames, a.boxes, a.scan_offsets, a.det_frame = (ib + int(v) for v in o[:4])
+            a.host_scan_offsets = so.ctypes.data
+            nbytes = _lib.load().fcn_frustum_extract_workspace_bytes(C.byref(a))
+            if nbytes < 0:
+                _lib.check(-1, "fcn_frustum_extract_workspace_bytes")
+            ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
+            summary = torch.empty(4 + (D + 1) // 2, dtype=torch.int64, device=dev)    # info | det_points
+            a.workspace, a.workspace_bytes = ws.data_ptr(), int(nbytes)
+            a.info, a.det_points = summary.data_ptr(), summary.data_ptr() + 32
+            if timer is not None:
+                timer("start")
+            _lib.call("fcn_frustum_extract_count", C.byref(a), stream.cuda_stream)
+            if timer is not None:
+                timer("count")
+            back = summary.cpu().numpy()                                     # the one host sync
+            K, M, bad = int(back[0]), int(back[1]), int(back[2])
+            if bad:
+                raise RuntimeError("fcn_frustum_extract: %d detections reference no frame" % bad)
+            if M >= 2 ** 31:
+                raise RuntimeError("fcn_frustum_extract: %d frustum points do not fit int32 offsets" % M)
+            det_points = back[4:].view(np.int32)[:D]
+            kept = np.flatnonzero(det_points >= 0)
+            assert len(kept) == K and int(det_points[kept].sum()) == M
+            points = torch.empty((M, 4), dtype=torch.float32, device=dev)
+            offsets = torch.empty(K + 1, dtype=torch.int32, device=dev)
+            angle = torch.empty(K, dtype=torch.float64, device=dev)
+            box2d = torch.empty((K, 4), dtype=torch.float64, device=dev)
+            P = torch.empty((K, 12), dtype=torch.float64, device=dev)
+            det_index = torch.empty(K, dtype=torch.int32, device=dev)
+            a.num_kept, a.num_out_points = K, M
+            a.points, a.offsets, a.frustum_angle = points.data_ptr(), offsets.data_ptr(), angle.data_ptr()
+            a.box2d, a.P, a.det_index = box2d.data_ptr(), P.data_ptr(), det_index.data_ptr()
+            if timer is not None:
+                timer("write_start")
+            _lib.call("fcn_frustum_extract_write", C.byref(a), stream.cuda_stream)
+            if timer is not None:
+                timer("write")
+        line_idx = np.asarray(lines, dtype=np.int64)[kept]
+        return self._result(points, offsets, angle, box2d, P, det_points[kept].astype(np.int64), line_idx, id_list,
+                            type_list, prob_list, box2d_list, calibs, image_hw)
+
+    @staticmethod
+    def _empty(dev):
+        return (torch.zeros(0, dtype=torch.float64, device=dev), torch.zeros((0, 4), dtype=torch.float64, device=dev),
+                torch.zeros((0, 12), dtype=torch.float64, device=dev))
+
+    @staticmethod
+    def _result(points, offsets, angle, box2d, P, counts, line_idx, id_list, type_list, prob_list, box2d_list, calibs,
+                image_hw):
+        ids = [id_list[i] for i in line_idx]
+        boxes = []
+        for i, k in zip(line_idx, ids):              # the reference's own clip (prepare_data.py:522-524), on the host
+            h, w = image_hw[k]
+            b = np.asarray(box2d_list[i], dtype=np.float64).reshape(4).copy()
+            b[[0, 2]] = np.clip(b[[0, 2]], 0, w - 1)
+            b[[1, 3]] = np.clip(b[[1, 3]], 0, h - 1)
+            boxes.append(b)
+        return Frustums(points, offsets, angle, box2d, P, counts, ids, [type_list[i] for i in line_idx], boxes,
+                        [prob_list[i] for i in line_idx], [calibs[k] for k in ids], np.asarray(line_idx, np.int64))

@@ -37,6 +37,40 @@ class FrustumBatchBuilder:
         self.box2d = torch.from_numpy(np.asarray(box2d, dtype=np.float64).reshape(self.B, 4)).to(dev)
         self.P = torch.from_numpy(np.asarray(P2, dtype=np.float64).reshape(self.B, 12)).to(dev)
         self.cls = None if cls_index is None else torch.from_numpy(np.asarray(cls_index, dtype=np.int32)).to(dev)
+        self._bind()
+
+    def set_frustums_device(self, points, offsets, frustum_angle, box2d, P, cls_index=None):
+        """set_frustums from CUDA tensors already on this builder's device (FrustumExtractor's output), with no host
+        round trip: points (M, 4 or 3) float32, offsets (B + 1) int32, frustum_angle (B) float64, box2d (B, 4) and
+        P (B, 12) float64; cls_index (B) int32 (CUDA tensor or host values) or None.  Every frustum must hold at least
+        one point (the extractor drops empty ones; this is not checked here, as that would need the host)."""
+        from .frustum_extract import on_device
+        dev = self.device
+        for name, t, dt, cols in (("points", points, torch.float32, (3, 4)), ("offsets", offsets, torch.int32, None),
+                                  ("frustum_angle", frustum_angle, torch.float64, None),
+                                  ("box2d", box2d, torch.float64, (4,)), ("P", P, torch.float64, (12,))):
+            if not on_device(t, dev):
+                raise RuntimeError("set_frustums_device: %s must be a CUDA tensor on %s" % (name, dev))
+            if t.dtype != dt or t.dim() != (1 if cols is None else 2) or (cols is not None and t.shape[1] not in cols):
+                raise ValueError("set_frustums_device: %s has dtype %s and shape %s" % (name, t.dtype, tuple(t.shape)))
+        self.B = int(offsets.shape[0]) - 1
+        if self.B < 1 or frustum_angle.shape[0] != self.B or box2d.shape[0] != self.B or P.shape[0] != self.B:
+            raise ValueError("set_frustums_device: offsets, frustum_angle, box2d and P disagree on the frustum count")
+        self.points = points[:, :3].contiguous()
+        self.offsets, self.angle = offsets.contiguous(), frustum_angle.contiguous()
+        self.box2d, self.P = box2d.contiguous(), P.contiguous()
+        if isinstance(cls_index, torch.Tensor):
+            if not on_device(cls_index, dev):
+                raise RuntimeError("set_frustums_device: cls_index must be a CUDA tensor on %s or host values" % dev)
+            self.cls = cls_index.to(torch.int32).contiguous()
+        else:
+            self.cls = None if cls_index is None else torch.from_numpy(np.asarray(cls_index, dtype=np.int32)).to(dev)
+        if self.cls is not None and self.cls.numel() != self.B:
+            raise ValueError("set_frustums_device: cls_index must have one entry per frustum")
+        self._bind()
+
+    def _bind(self):
+        dev = self.device
         f32 = torch.float32
         self.out = {"point_cloud": torch.empty((self.B, 3, self.N), dtype=f32, device=dev),
                     "rot_angle": torch.empty((self.B, 1), dtype=f32, device=dev)}

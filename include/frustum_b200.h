@@ -743,6 +743,60 @@ FCN_API long long fcn_sunrgbd_eval_workspace_bytes(const fcn_sunrgbd_eval_args *
 FCN_API int fcn_sunrgbd_eval_match(const fcn_sunrgbd_eval_args *args, fcn_stream_t stream);
 FCN_API int fcn_sunrgbd_eval_curves(const fcn_sunrgbd_eval_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (15) KITTI frustum extraction on the device: extract_frustum_data_rgb_detection of kitti/prepare_data.py:462-568
+ *      (with kitti_util.py:172-210 and draw_util.py:12-23) for several frames and all their 2-D detections at once.
+ *
+ *      Per frame f (scan rows [scan_offsets[f], scan_offsets[f+1]) of `scans`, float32 x, y, z, intensity):
+ *        ref  = V2C . [x, y, z, 1]   rect = R0 . ref   [u', v', w] = P . [rect, 1]   u = u' / w, v = v' / w
+ *      in float64, every product and sum rounded separately, each row summed left to right (column 0 first).
+ *      A point is in the image when 0 <= u < width, 0 <= v < height and x > 2 (NaN fails); those points are
+ *      compacted per frame in scan order.
+ *      Per detection d (frame det_frame[d], box xmin, ymin, xmax, ymax as read): the box clipped to [0, width-1] x
+ *      [0, height-1]; its points are the frame's in-image points with xmin <= u < xmax and ymin <= v < ymax, in scan
+ *      order; it is dropped when ymax - ymin < 5, xmax - xmin < 1 or it has no point.  The type whitelist is the
+ *      caller's: pass only the detections of wanted types.  frustum_angle = -atan2(20, x) of project_image_to_rect
+ *      of the clipped box centre at depth 20.
+ *
+ *      Two calls in order on one stream, sharing the caller's workspace (fcn_frustum_extract_workspace_bytes: needs the
+ *      device, -1 on invalid arguments), no host sync, no allocation:
+ *        fcn_frustum_extract_count : the in-image points, every detection's points, the drop rules and the prefix sums
+ *                                    over the kept detections; writes det_points (DEVICE, num_dets: the detection's
+ *                                    point count when kept, -1 when dropped or when det_frame is out of range) and
+ *                                    info (DEVICE int64[4]: kept detections K, their points M, detections with an
+ *                                    out-of-range frame, 0);
+ *        fcn_frustum_extract_write : needs num_kept = K and num_out_points = M as read by the host; writes the kept
+ *                                    detections in detection order: points (M, 4) float32 rect x, y, z and intensity,
+ *                                    offsets (K + 1) int32, frustum_angle (K), box2d (K, 4) clipped, P (K, 12) the
+ *                                    frame's P2, det_index (K) int32 index d.
+ *      With num_frames == 0 or num_dets == 0 both calls return 0 and do nothing (K = M = 0; info is not written).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+    double P[12], V2C[12], R0[9];   /* P2 (3x4), Tr_velo_to_cam (3x4), R0_rect (3x3), row-major */
+    int32_t height, width;          /* image size */
+} fcn_frustum_frame;
+typedef struct {
+    int num_frames, num_points, num_dets, num_kept;
+    long long num_out_points;
+    const float *scans;                 /* DEVICE (num_points, 4), 16-byte aligned */
+    const int32_t *scan_offsets;        /* DEVICE (num_frames + 1) */
+    const int32_t *host_scan_offsets;   /* HOST copy: starts at 0, never decreases, ends at num_points */
+    const fcn_frustum_frame *frames;    /* DEVICE (num_frames) */
+    const double *boxes;                /* DEVICE (num_dets, 4) */
+    const int32_t *det_frame;           /* DEVICE (num_dets) */
+    void *workspace;
+    long long workspace_bytes;
+    long long *info;                    /* DEVICE int64[4] */
+    int32_t *det_points;                /* DEVICE (num_dets) */
+    float *points;                      /* fcn_frustum_extract_write outputs (DEVICE) */
+    int32_t *offsets;
+    double *frustum_angle, *box2d, *P;
+    int32_t *det_index;
+} fcn_frustum_extract_args;
+FCN_API long long fcn_frustum_extract_workspace_bytes(const fcn_frustum_extract_args *args);
+FCN_API int fcn_frustum_extract_count(const fcn_frustum_extract_args *args, fcn_stream_t stream);
+FCN_API int fcn_frustum_extract_write(const fcn_frustum_extract_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
