@@ -8,8 +8,9 @@
 //   layer 2 D2[64 x C2] = A1 * W2^T (wgmma, A from registers) -> +bias, ReLU, TF32 in place, then an intra-quad
 //           permutation turns the accumulator fragments into the A fragments of layer 3 (resident for the tile)
 //   layer 3 D3[64 x N3-channel chunk] = A2 * W3^T (A from registers) -> +bias, ReLU, max over the rows of each
-//           section: a segmented suffix max over the 16 rows of a warp (shuffles), then one integer atomicMax per
-//           (section part, channel) into the position-major feature map
+//           section part in a warp's 16 rows, then one integer atomicMax per (section part, channel) into the
+//           position-major feature map.  A warp with one or two sections reduce-scatters each section's max over
+//           its lanes (14 shuffles per 64 channels); three or more take a segmented suffix max (112).
 // Only the weights go through shared memory.  A loader warp streams (or keeps resident) the pre-swizzled W2/W3
 // stage images; both warpgroups read every stage, and a stage is released when both have retired the wgmma group
 // that read it.  The loader is a whole warpgroup that gives its registers to the two consumer warpgroups
@@ -87,6 +88,44 @@ struct TcCfg {
 // One layer-1 output (fp32 FMA chain, folded BN, ReLU) as a TF32 operand.
 __device__ __forceinline__ uint32_t layer1_tf32(const float4 &r, const float4 &w) {
     return __float_as_uint(to_tf32(fmaxf(fmaf(r.z, w.z, fmaf(r.y, w.y, fmaf(r.x, w.x, w.w))), 0.f)));
+}
+
+// Max over the 16 rows of a warp that belong to ONE section, for the 32 columns of accumulator blocks
+// j0 .. j0 + 3 (acc[4j + e]: rows ra (e < 2) and ra + 8 (e >= 2), columns 8j + 2q + (e & 1)).  in_a / in_b: row ra /
+// ra + 8 is in the section; any other row (another section, or past nrows, whose staged record is zero-filled)
+// becomes -inf by a select before any fmaxf.  The 8 values of a thread are reduce-scattered over the 8 lanes g = 0..7 that share
+// q (butterfly over lane bits 16, 8, 4: each level keeps one half and receives the partner's max of the other half,
+// 4 + 2 + 1 shuffles), so lane g ends up with the section max of value g, i.e. column 8 (j0 + g / 2) + 2q + g % 2;
+// then +bias, TF32 and one integer atomicMax if positive, as on the general path.  dst / bias point at column 0 of
+// the chunk.  32 columns at a time keep the temporaries at 8 registers next to the A fragments and accumulators.
+template <int H>            // one butterfly level over lane bit 4H: 2H values in, H out
+__device__ __forceinline__ void max_scatter_level(float (&v)[8], int lane) {
+    const bool hi = (lane & (4 * H)) != 0;
+#pragma unroll
+    for (int i = 0; i < H; ++i) {
+        const float send = hi ? v[i] : v[i + H], keep = hi ? v[i + H] : v[i];
+        v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 4 * H));
+    }
+}
+
+template <int R>
+__device__ __forceinline__ void section_max_32(const float (&acc)[R], int j0, bool in_a, bool in_b, int *dst,
+                                               const float *bias, int lane) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+            const float x = in_a ? acc[4 * (j0 + j) + c] : -INFINITY;
+            const float y = in_b ? acc[4 * (j0 + j) + 2 + c] : -INFINITY;
+            v[2 * j + c] = fmaxf(x, y);
+        }
+    max_scatter_level<4>(v, lane);
+    max_scatter_level<2>(v, lane);
+    max_scatter_level<1>(v, lane);
+    const int g = lane >> 2, c = 8 * (j0 + (g >> 1)) + 2 * (lane & 3) + (g & 1);
+    const float o = to_tf32(v[0] + bias[c]);
+    if (o > 0.f) atomicMax(dst + c, __float_as_int(o));
 }
 
 template <int C1, int C2, int C3, int CL>
@@ -176,11 +215,26 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
         // src1 ^ 2.  Lanes with psel = 0 receive column q first, lanes with psel = 1 column q + 4.
         const int psel = (q ^ (q >> 1)) & 1;
         const int src1 = (lane & ~3) | (q >> 1) | (psel << 1), src2 = src1 ^ 2;
+        // Each warpgroup stages its own 64 rows (threads 0..63 of the warpgroup, row srow) into the record / section
+        // buffers of the tile parity.  Tile it + 1's record is loaded before tile it's barrier and stored at the end of
+        // tile it, so that the two dependent global loads have the whole tile to land; at C2 = 256 the layer-3 A
+        // fragments leave no registers to hold it through layer 3, so it is stored once layer 2 has run.
+        constexpr bool STAGE_AFTER_L2 = C2 > 128;
+        const bool stager = (tid & 64) == 0;
+        const int srow = 64 * wg + (tid & 63);
+        auto load_rec = [&](const int4 &t) {
+            return stager && srow < t.z ? ((const float4 *)p.rows + (size_t)t.x * p.row_cap + t.y)[srow]
+                                        : make_float4(0.f, 0.f, 0.f, 0.f);
+        };
+        auto stage_rec = [&](int parity, const float4 &r, int nrows) {
+            if (stager) {
+                recs_all[parity * TC_ROWS + srow] = r;
+                sect_all[parity * TC_ROWS + srow] = srow < nrows ? (__float_as_int(r.w) & 0x7fffffff) : -1;
+            }
+        };
         uint32_t job = 0;
         int4 td_next = tile_of(0);
-        float4 rec_next = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (tid < TC_ROWS && tid < td_next.z)
-            rec_next = ((const float4 *)p.rows + (size_t)td_next.x * p.row_cap + td_next.y)[tid];
+        stage_rec(0, load_rec(td_next), td_next.z);
 
         // one weight stage per call: wait, 4 wgmma (k = 8 each), commit; the stage of the previous call is released
         // once its group has retired (streamed weights only)
@@ -198,23 +252,20 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
         };
 
         for (int it = 0; it < my_tiles; ++it) {
-            const int4 td = td_next;           // tile descriptor + the staged record were prefetched
-            const int b = td.x, nrows = td.z;  // during the previous tile (two dependent global loads)
-            // staging buffers alternate with the tile parity: a warp that runs ahead into tile it+1
-            // must not overwrite what slower warps still read for tile it (they meet at this barrier)
-            float4 *recs = recs_all + (it & 1) * TC_ROWS;
-            int *sect_s = sect_all + (it & 1) * TC_ROWS;
-            if (tid < TC_ROWS) {
-                recs[tid] = rec_next;
-                sect_s[tid] = tid < nrows ? (__float_as_int(rec_next.w) & 0x7fffffff) : -1;
-            }
+            const int b = td_next.x;           // tile descriptor + the staged record were prefetched
+                                               // during the previous tile (two dependent global loads)
+            // The staging buffers alternate with the tile parity.  Tile it + 1's buffer is written after this
+            // barrier, which every warp of the warpgroup reaches only once it has read tile it - 1's; a warpgroup
+            // reads only its own rows, so the two warpgroups never wait for each other here and may drift apart by
+            // up to the weight ring's depth.
+            const float4 *recs = recs_all + (it & 1) * TC_ROWS;
+            const int *sect_s = sect_all + (it & 1) * TC_ROWS;
+            float4 rec_next;
             if (it + 1 < my_tiles) {
                 td_next = tile_of(it + 1);
-                rec_next = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (tid < TC_ROWS && tid < td_next.z)
-                    rec_next = ((const float4 *)p.rows + (size_t)td_next.x * p.row_cap + td_next.y)[tid];
+                rec_next = load_rec(td_next);
             }
-            asm volatile("bar.sync 1, %0;\n" ::"n"(TC_COMPUTE_WARPS * 32));
+            asm volatile("bar.sync %0, 128;\n" ::"r"(2 + wg));
             const float4 reca = recs[ra], recb = recs[ra + 8];
             if (Cfg::RESIDENT) job = 0;
 
@@ -261,6 +312,7 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
     #pragma unroll
             for (int nc = 0; nc < Cfg::NCH2; ++nc) fence_acc(acc2[nc]);
             release_prev();
+            if (STAGE_AFTER_L2 && it + 1 < my_tiles) stage_rec((it + 1) & 1, rec_next, td_next.z);
             // ---- epilogue 2: +bias, ReLU, TF32 in place, then the quad permutation into the A fragments of the
             //      KB2 * 4 k-steps of layer 3 (k-step s = columns 8 s .. 8 s + 7)
             uint32_t a2[Cfg::KB2 * 4][4];
@@ -283,21 +335,11 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
     #pragma unroll
             for (int s = 0; s < Cfg::KB2 * 4; ++s) fence_frag(a2[s]);
 
-            // ---- layer 3 + section max.  Rows ra (fragment half 0) and ra + 8 (half 1) of this thread; the suffix
-            //      max over the rows of a section runs over the 8 lanes l/4 = 0..7 of each half, then half 0 takes in
-            //      half 1's head when the section crosses row 8 of the warp.  +bias, ReLU, TF32 rounding commute with
-            //      the max (monotone), values >= 0 so the integer atomicMax on the float bits is exact.
-            const int sa = sect_s[ra], sb = sect_s[ra + 8], s8 = sect_s[ra - g + 8];
-            unsigned oka = 0, okb = 0;                 // bit d: row + (1 << d) is in the same section and 8-row half
-    #pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                const int o = 1 << d;
-                if (g + o < 8 && sa >= 0 && sect_s[ra + o] == sa) oka |= 1u << d;
-                if (g + o < 8 && sb >= 0 && sect_s[ra + 8 + o] == sb) okb |= 1u << d;
-            }
-            const bool merge_a = sa >= 0 && sa == s8;
-            const bool head_a = sa >= 0 && (g == 0 || sect_s[ra - 1] != sa);
-            const bool head_b = sb >= 0 && sect_s[ra + 7] != sb;
+            // ---- layer 3 + section max.  Warp-uniform shape of the warp's 16 rows: sections are contiguous runs and
+            //      the rows past nrows (sect -1) a suffix, so the rows 1..15 that start a new section give the number
+            //      of sections.  One or two sections (almost every warp at C1 >= 128) take section_max_32 per section;
+            //      three or more the segmented suffix max below.  +bias, ReLU, TF32 rounding commute with the max
+            //      (monotone), values >= 0 so the integer atomicMax on the float bits is exact.
             int *feat = (int *)(p.out + (size_t)b * p.feat_pitch * p.ld_feat);
             for (int nc = 0; nc < Cfg::NCH3; ++nc) {
                 float acc3[Cfg::N3 / 2];
@@ -327,6 +369,42 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
                 wgmma_wait<0>();
                 fence_acc(acc3);
                 release_prev();
+                // the warp's section shape (re-read per chunk from shared memory rather than held in registers
+                // through the MMAs)
+                const int sa = sect_s[ra], sb = sect_s[ra + 8];
+                const int r0 = ra - g, rl = r0 + (lane & 15);
+                const int s0 = sect_s[r0], sl = sect_s[rl];
+                const unsigned starts =
+                    __ballot_sync(0xffffffffu, lane >= 1 && lane < 16 && sl >= 0 && sl != sect_s[rl - 1]);
+                const int nsec = s0 < 0 ? 0 : 1 + __popc(starts);
+                const int s1 = nsec == 2 ? sect_s[r0 + __ffs(starts) - 1] : -1;
+                if (nsec == 0) continue;
+                if (nsec <= 2) {
+                    const int c0 = nc * Cfg::N3;
+    #pragma unroll
+                    for (int h = 0; h < Cfg::N3 / 32; ++h) {
+                        section_max_32(acc3, 4 * h, sa == s0, sb == s0, feat + (size_t)s0 * p.ld_feat + c0, b3s + c0,
+                                       lane);
+                        if (nsec == 2)
+                            section_max_32(acc3, 4 * h, sa == s1, sb == s1, feat + (size_t)s1 * p.ld_feat + c0,
+                                           b3s + c0, lane);
+                    }
+                    continue;
+                }
+                // segmented suffix max: rows ra (fragment half 0) and ra + 8 (half 1) of this thread; the suffix max
+                // over the rows of a section runs over the 8 lanes l/4 = 0..7 of each half, then half 0 takes in
+                // half 1's head when the section crosses row 8 of the warp
+                const int s8 = sect_s[r0 + 8];
+                unsigned oka = 0, okb = 0;             // bit d: row + (1 << d) is in the same section and 8-row half
+    #pragma unroll
+                for (int d = 0; d < 3; ++d) {
+                    const int o = 1 << d;
+                    if (g + o < 8 && sa >= 0 && sect_s[ra + o] == sa) oka |= 1u << d;
+                    if (g + o < 8 && sb >= 0 && sect_s[ra + 8 + o] == sb) okb |= 1u << d;
+                }
+                const bool merge_a = sa >= 0 && sa == s8;
+                const bool head_a = sa >= 0 && (g == 0 || sect_s[ra - 1] != sa);
+                const bool head_b = sb >= 0 && sect_s[ra + 7] != sb;
     #pragma unroll
                 for (int j = 0; j < Cfg::N3 / 8; ++j) {
                     float v[4] = {acc3[4 * j], acc3[4 * j + 1], acc3[4 * j + 2], acc3[4 * j + 3]};
@@ -354,6 +432,7 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
                     }
                 }
             }
+            if (!STAGE_AFTER_L2 && it + 1 < my_tiles) stage_rec((it + 1) & 1, rec_next, td_next.z);
         }
     }
     if (CL == 2) {                               // the peer may still signal this CTA's barriers
