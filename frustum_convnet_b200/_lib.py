@@ -277,6 +277,24 @@ class FrustumExtractArgs(C.Structure):
                                           "det_index")]
 
 
+REFINE_GT, REFINE_MATCHED, REFINE_DET = 0, 1, 2
+
+
+class RefineBox(C.Structure):
+    _fields_ = [("center", C.c_double * 3), ("half", C.c_double * 3), ("cs", C.c_double), ("sn", C.c_double)]
+
+
+class RefineExtractArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("mode", "num_frames", "num_points", "num_jobs", "num_gt", "num_dets",
+                                       "num_pairs", "num_kept")] + \
+               [("num_out_points", C.c_longlong), ("iou_thresh", C.c_double)] + \
+               [(n, C.c_void_p) for n in ("scans", "scan_offsets", "host_scan_offsets", "frames", "jobs", "job_frame",
+                                          "job_ref", "gt_boxes", "gt_corners", "det_corners", "det_frame",
+                                          "gt_offsets", "pair_offsets", "workspace")] + \
+               [("workspace_bytes", C.c_longlong)] + \
+               [(n, C.c_void_p) for n in ("info", "job_points", "job_gt", "points", "labels", "offsets")]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -326,6 +344,9 @@ SIGNATURES = {
     "fcn_frustum_extract_workspace_bytes": (C.c_longlong, [C.POINTER(FrustumExtractArgs)]),
     "fcn_frustum_extract_count": (_I, [C.POINTER(FrustumExtractArgs), _P]),
     "fcn_frustum_extract_write": (_I, [C.POINTER(FrustumExtractArgs), _P]),
+    "fcn_refine_extract_workspace_bytes": (C.c_longlong, [C.POINTER(RefineExtractArgs)]),
+    "fcn_refine_extract_count": (_I, [C.POINTER(RefineExtractArgs), _P]),
+    "fcn_refine_extract_write": (_I, [C.POINTER(RefineExtractArgs), _P]),
 }
 
 _lib = None

@@ -145,4 +145,37 @@ FCN_HD void rbbox_iou_pair(const float *c, const float *q, float *iou) {
     iou[1] = inter_vol / (vol + qvol - inter_vol);
 }
 
+#ifdef __CUDACC__
+// The 3-D IoU of the reference's Boost kernels in float64 (rbbox_iou_3d_pair<double>, box_ops.h:206-249, element [1];
+// the same arithmetic as rbbox_iou_3d, :85-170): the SUN-RGBD evaluator's overlaps (sunrgbd_eval.cu) and the KITTI
+// refinement extractor's detection / ground-truth matching (refine_extract.cu).  Rings are the (x, z) of corners 6, 7,
+// 4, 5; a ring that is not clockwise-positive scores 0 (the rule of rbbox_iou_pair above and oracle/box_iou.py).
+// std::min / std::max semantics are kept (ternaries), as are the reference's separate products.
+__device__ inline double rbbox_iou3d_d(const double *__restrict__ c, const double *__restrict__ q) {
+    const int order[4] = {6, 7, 4, 5};
+    Pt2d P[4], Q[4];
+    for (int i = 0; i < 4; ++i) {
+        P[i].x = c[order[i] * 3 + 0];
+        P[i].y = c[order[i] * 3 + 2];
+        Q[i].x = q[order[i] * 3 + 0];
+        Q[i].y = q[order[i] * 3 + 2];
+    }
+    const double area = -shoelace_ccw(P, 4), qarea = -shoelace_ccw(Q, 4);
+    if (!(area > 0.0) || !(qarea > 0.0)) return 0.0;
+    int n;
+    double inter = clip_quads_area(P, Q, &n);
+    if (n < 3) return 0.0;
+    inter = fabs(inter);
+    if (!(inter > 0.0)) return 0.0;
+    const double ymax = q[1] < c[1] ? q[1] : c[1];
+    const double ymin = c[13] < q[13] ? q[13] : c[13];
+    const double h = c[1] - c[13], qh = q[1] - q[13];
+    const double dy = ymax - ymin;
+    const double inter_vol = __dmul_rn(inter, 0.0 < dy ? dy : 0.0);
+    const double av = __dmul_rn(area, h), qv = __dmul_rn(qarea, qh);
+    const double vol = 0.0 < av ? av : 0.0, qvol = 0.0 < qv ? qv : 0.0;
+    return inter_vol / __dadd_rn(__dadd_rn(vol, qvol), -inter_vol);
+}
+#endif
+
 }  // namespace fcn

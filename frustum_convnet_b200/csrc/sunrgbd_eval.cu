@@ -29,35 +29,6 @@ namespace fcn {
 constexpr int SE_THREADS = 256;
 constexpr int SE_CURVE_THREADS = 512;
 
-// rbbox_iou_3d_pair<double> (box_ops.h:206-249) of one pair, element [1]: the 3-D IoU.  Rings are the (x, z) of
-// corners 6, 7, 4, 5; a ring that is not clockwise-positive scores 0 (the rule of box_iou.cuh and oracle/box_iou.py).
-// std::min / std::max semantics are kept (ternaries), as are the reference's separate products.
-__device__ double se_iou3d(const double *__restrict__ c, const double *__restrict__ q) {
-    const int order[4] = {6, 7, 4, 5};
-    Pt2d P[4], Q[4];
-    for (int i = 0; i < 4; ++i) {
-        P[i].x = c[order[i] * 3 + 0];
-        P[i].y = c[order[i] * 3 + 2];
-        Q[i].x = q[order[i] * 3 + 0];
-        Q[i].y = q[order[i] * 3 + 2];
-    }
-    const double area = -shoelace_ccw(P, 4), qarea = -shoelace_ccw(Q, 4);
-    if (!(area > 0.0) || !(qarea > 0.0)) return 0.0;
-    int n;
-    double inter = clip_quads_area(P, Q, &n);
-    if (n < 3) return 0.0;
-    inter = fabs(inter);
-    if (!(inter > 0.0)) return 0.0;
-    const double ymax = q[1] < c[1] ? q[1] : c[1];
-    const double ymin = c[13] < q[13] ? q[13] : c[13];
-    const double h = c[1] - c[13], qh = q[1] - q[13];
-    const double dy = ymax - ymin;
-    const double inter_vol = __dmul_rn(inter, 0.0 < dy ? dy : 0.0);
-    const double av = __dmul_rn(area, h), qv = __dmul_rn(qarea, qh);
-    const double vol = 0.0 < av ? av : 0.0, qvol = 0.0 < qv ? qv : 0.0;
-    return inter_vol / __dadd_rn(__dadd_rn(vol, qvol), -inter_vol);
-}
-
 // the class of detection d: the last c with det_class_offsets[c] <= d (empty classes skipped)
 __device__ __forceinline__ int se_class_of(const int32_t *__restrict__ off, int num_classes, int d) {
     int lo = 0, hi = num_classes - 1;
@@ -91,7 +62,7 @@ se_overlap_kernel(int num_det, int num_classes, int num_segments, double ovthres
             double ovmax = -INFINITY;
             int jmax = -1;
             for (int j = g0; j < g1; ++j) {
-                const double iou = se_iou3d(bb, gt + (size_t)j * 24);
+                const double iou = rbbox_iou3d_d(bb, gt + (size_t)j * 24);
                 if (iou > ovmax) {
                     ovmax = iou;
                     jmax = j;

@@ -1,0 +1,502 @@
+"""KITTI refinement frustums on the device: the three extraction functions of the reference's
+kitti/prepare_data_refine.py without their pickles, for a whole set of frames in one call.
+
+    rx = RefineFrustumExtractor(type_whitelist=("Car",))
+    train = rx.from_ground_truth(scans, calibs, image_hw, train_ids, gt_dir, perturb=True, augment=5, rng=np.random)
+    val   = rx.from_ground_truth(scans, calibs, image_hw, val_ids, gt_dir, remove_diff=True)
+    vdet  = rx.from_matched_detections(scans, calibs, image_hw, val_ids, col.finalize(), gt_dir, remove_diff=True)
+    test  = rx.from_detections(scans, calibs, image_hw, val_ids, col.finalize())    # or read_result_dir(...)
+    tb = TrainBatchBuilder.from_frustums(test, "refine", strides=cfg.DATA.STRIDE, npoints=cfg.DATA.NUM_SAMPLES,
+                                         labels=False)
+
+  from_ground_truth        extract_frustum_data (:239-403): every ground-truth box of a whitelisted type (after the
+                           remove_diff rule: occlusion > 2, truncation > 0.5 or a 2-D height < 25 drop it), enlarged
+                           x1.2 and, with perturb, perturbed `augment` times in a chain (random_shift_rotate_box3d(.,
+                           0.05), seven rng.random() draws an attempt); labels: the points in the ground-truth box.
+  from_matched_detections  extract_frustum_det_data (:406-592): every whitelisted detection of a frame with ground
+                           truth, enlarged x1.2; its ground truth is the first maximum of the 3-D IoU (rbbox_iou_3d,
+                           float64, on the device) if that maximum is >= 0.5 (Car in the whitelist) or 0.25.
+  from_detections          extract_frustum_data_rgb_detection (:649-773): every whitelisted detection, enlarged x1.2,
+                           dropped when ymax - ymin < 5, xmax - xmin < 1 (the 2-D box as read, not clipped) or it
+                           has no point; no labels, prob_list holds the scores.
+A ground-truth or matched frustum without a labelled point is dropped.  Types match exactly (Object3d.type in
+type_whitelist).  Every per-box constant (the box array, enlargement, perturbation, corners, sizes, angles,
+frustum_angle) is computed here on the host with the reference's own numpy expressions; nothing random runs on the
+device.  The points are the in-image points of section (15) (FrustumExtractor's projection), float32 rect x, y, z
+and intensity in scan order; "in a box" is a float64 half-space test in the box's frame (csrc/refine_extract.cu)
+where the reference triangulates the 8 corners with scipy's Delaunay: the two agree except for points within
+rounding (~1e-9 m) of a face.  A box with a non-positive extent raises ValueError naming its line where the
+reference's Qhull would raise (in matched mode: a matched detection and its ground truth only).  The matching IoU
+substitutes the reference's Boost polygon clip with box_iou.cuh's clip_quads_area<double>; agreement with Boost is
+not pinned.
+
+Detections are the collector's {idx: {class: (n, 12)}} taken as the values the reference reads back from the text
+write_detection_results writes (kitti_eval.detection_records), lines in class then row order; or the result files
+themselves (read_result_dir).  Ground truth is a label_2 directory (or a {idx: [KittiObject]} dict).  One host sync
+per call, to learn the kept frustums and their points.  No CPU fallback: CPU tensors and devices raise."""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import pickle
+
+import numpy as np
+import torch
+
+from . import _lib
+from .frustum_extract import _frame_record, on_device
+from .kitti_eval import detection_records
+
+RATIO = 1.2                # the enlargement of every box that cuts points (prepare_data_refine.py:319, :489, :724)
+PERTURB_RATIO = 0.05       # random_shift_rotate_box3d(., 0.05) of the training set (:328-329)
+
+
+class KittiObject:
+    """One label or result line, parsed as kitti_util.Object3d parses it."""
+
+    def __init__(self, type, truncation, occlusion, alpha, box2d, h, w, l, t, ry, score=1, line=""):
+        self.type, self.truncation, self.occlusion, self.alpha = type, truncation, occlusion, alpha
+        self.box2d = np.array([box2d[0], box2d[1], box2d[2], box2d[3]])
+        self.xmin, self.ymin, self.xmax, self.ymax = (float(v) for v in box2d)
+        self.h, self.w, self.l, self.t, self.ry, self.score = h, w, l, tuple(t), ry, score
+        self.line = line                 # "<file>:<line number>" for error messages
+
+    @classmethod
+    def parse(cls, text, where=""):
+        data = text.split(" ")
+        data[1:] = [float(x) for x in data[1:]]
+        return cls(data[0], data[1], int(data[2]), data[3], data[4:8], data[8], data[9], data[10],
+                   (data[11], data[12], data[13]), data[14], data[15] if len(data) > 15 else 1, where)
+
+
+def read_objects(path):
+    """A label or result file -> [KittiObject] (utils.read_label); a missing file raises, an empty one is empty."""
+    with open(path) as f:
+        return [KittiObject.parse(line.rstrip(), "%s:%d" % (path, n + 1)) for n, line in enumerate(f)]
+
+
+def read_label_dir(label_dir, image_ids):
+    return {int(i): read_objects(os.path.join(label_dir, "%06d.txt" % int(i))) for i in image_ids}
+
+
+def read_result_dir(result_dir, image_ids):
+    """Result files '%06d.txt' of every image of image_ids -> {idx: [KittiObject]}."""
+    return read_label_dir(result_dir, image_ids)
+
+
+def objects_from_detections(dets):
+    """The collector's {idx: {class: float32 (n, 12)}} -> {idx: [KittiObject]}: the values utils.read_label reads
+    back from the lines write_detection_results writes, in its line order (classes in dict order, then rows)."""
+    out = {}
+    for idx, per_class in dets.items():
+        objs = []
+        for cls_type, rows in per_class.items():
+            for n, r in enumerate(detection_records(rows, cls_type)):
+                objs.append(KittiObject(cls_type, -1.0, -1, float(r[1]), [float(v) for v in r[2:6]], float(r[6]),
+                                        float(r[7]), float(r[8]), [float(v) for v in r[9:12]], float(r[12]),
+                                        float(r[13]), "detections[%d][%r] row %d" % (idx, cls_type, n)))
+        out[int(idx)] = objs
+    return out
+
+
+# ------------------------------------------------------------------------------ per-box constants (host, float64)
+def obj_array(obj):
+    """[cx, cy - h / 2, cz, l, w, h, ry] (prepare_data_refine.py:310-315)."""
+    cx, cy, cz = obj.t
+    return np.array([cx, cy - obj.h / 2, cz, obj.l, obj.w, obj.h, obj.ry])
+
+
+def compute_box_3d_obj_array(a):
+    """prepare_data_refine.py:56-79: the 8 corners (8, 3) of [cx, cy, cz, l, w, h, ry]."""
+    cx, cy, cz, l, w, h, angle = a
+    c, s = np.cos(angle), np.sin(angle)
+    R = np.array([[c, 0, s], [0, 1, 0], [-s, 0, c]])
+    x_corners = [l / 2, l / 2, -l / 2, -l / 2, l / 2, l / 2, -l / 2, -l / 2]
+    y_corners = [h / 2, h / 2, h / 2, h / 2, -h / 2, -h / 2, -h / 2, -h / 2]
+    z_corners = [w / 2, -w / 2, -w / 2, w / 2, w / 2, -w / 2, -w / 2, w / 2]
+    corners_3d = np.dot(R, np.vstack([x_corners, y_corners, z_corners]))
+    corners_3d[0, :] = corners_3d[0, :] + cx
+    corners_3d[1, :] = corners_3d[1, :] + cy
+    corners_3d[2, :] = corners_3d[2, :] + cz
+    return np.transpose(corners_3d, (1, 0))
+
+
+def random_shift_rotate_box3d(a, r=PERTURB_RATIO, rng=np.random):
+    """prepare_data_refine.py:203-236 with the generator as an argument: seven rng.random() draws an attempt (l, h, w,
+    cx, cy, cz, angle), again while an extent is <= 0, the angle wrapped to [-pi, pi)."""
+    cx, cy, cz, l, w, h, angle = a
+    angle = angle + np.pi
+    if not (l > 0 and w > 0 and h > 0):
+        raise ValueError("a perturbed box needs positive extents, got l, w, h = %r, %r, %r" % (l, w, h))
+    while True:
+        l1 = l + l * r * (rng.random() * 2 - 1)
+        h1 = h + h * r * (rng.random() * 2 - 1)
+        w1 = w + w * r * (rng.random() * 2 - 1)
+        cx1 = cx + l * r * (rng.random() * 2 - 1)
+        cy1 = cy + h * r * (rng.random() * 2 - 1)
+        cz1 = cz + w * r * (rng.random() * 2 - 1)
+        angle1 = angle + r * (rng.random() * 2 - 1) * np.pi
+        angle1 = angle1 % (2 * np.pi)
+        if l1 > 0 and h1 > 0 and w1 > 0:
+            return np.array([cx1, cy1, cz1, l1, w1, h1, angle1 - np.pi])
+
+
+def iou_corners(boxes):
+    """ops/pybind11/rbbox_iou.py:121-148 (boxes3d2corners): (n, 7) -> (n, 8, 3), as rbbox_iou_3d computes them."""
+    boxes = np.asarray(boxes, dtype=np.float64).reshape(-1, 7)
+    N = boxes.shape[0]
+    l, w, h, hd = boxes[:, 3], boxes[:, 4], boxes[:, 5], boxes[:, 6]
+    x = np.stack([l / 2, l / 2, -l / 2, -l / 2, l / 2, l / 2, -l / 2, -l / 2], 1)
+    y = np.stack([h / 2, h / 2, h / 2, h / 2, -h / 2, -h / 2, -h / 2, -h / 2], 1)
+    z = np.stack([w / 2, -w / 2, -w / 2, w / 2, w / 2, -w / 2, -w / 2, w / 2], 1)
+    corners = np.stack([x, y, z], 1)
+    c, s = np.cos(hd), np.sin(hd)
+    one, zero = np.ones(N), np.zeros(N)
+    R = np.stack([np.stack([c, zero, s], 1), np.stack([zero, one, zero], 1), np.stack([-s, zero, c], 1)], 1)
+    out = np.einsum("bij,bjk->bik", R, corners) + np.expand_dims(boxes[:, :3], 2)
+    return np.transpose(out, (0, 2, 1))
+
+
+def box_record(a):
+    """The half-space test's constants of box array a: centre, half extents (l, h, w) / 2, cos and sin of ry."""
+    r = np.zeros(1, dtype=np.dtype(_lib.RefineBox))[0]
+    r["center"] = a[:3]
+    r["half"] = [a[3] / 2, a[5] / 2, a[4] / 2]
+    r["cs"], r["sn"] = np.cos(a[6]), np.sin(a[6])
+    return r
+
+
+def _check_box(a, obj, extents=True):
+    if not np.isfinite(a).all():
+        raise ValueError("%s: the 3-D box must be finite, got %s" % (obj.line, a.tolist()))
+    if extents and not (a[3] > 0 and a[4] > 0 and a[5] > 0):
+        raise ValueError("%s: the 3-D box needs positive l, w, h, got %r, %r, %r" % (obj.line, a[3], a[4], a[5]))
+
+
+def is_diff(obj):
+    return obj.occlusion > 2 or obj.truncation > 0.5 or obj.ymax - obj.ymin < 25
+
+
+def ground_truth_boxes(objects, type_whitelist, remove_diff):
+    """extract_boxes (:25-53): the whitelisted (exact type) ground truth that remove_diff keeps, in line order."""
+    return [o for o in objects if o.type in type_whitelist and not (remove_diff and is_diff(o))]
+
+
+def job_table(mode, image_ids, objects, gt_objects, type_whitelist, remove_diff=False, perturb=False, augment=1,
+              rng=np.random):
+    """The jobs of one extraction in the reference's order, with every per-box constant.  -> (jobs, gts): jobs a list
+    of dicts (frame id, the cutting box array `cut`, its object, `gt` the label ground truth's position in gts (GT
+    mode), `det` the detection's position in the matched table); gts {frame id: [ground truth KittiObject]}."""
+    jobs, gts = [], {}
+    for idx in image_ids:
+        idx = int(idx)
+        if mode == _lib.REFINE_DET:
+            for obj in objects[idx]:
+                if obj.type not in type_whitelist:
+                    continue
+                a = obj_array(obj)
+                _check_box(a, obj)
+                if obj.ymax - obj.ymin < 5 or obj.xmax - obj.xmin < 1:     # :739-741, decided on the host
+                    continue
+                enl = a.copy()
+                enl[3:6] = enl[3:6] * RATIO
+                jobs.append(dict(frame=idx, obj=obj, cut=enl))
+            continue
+        g = ground_truth_boxes(gt_objects[idx], type_whitelist, remove_diff)
+        if mode == _lib.REFINE_MATCHED:
+            if not g:
+                continue                                                     # :458-459
+            gts[idx] = g
+            for obj in objects[idx]:
+                if obj.type not in type_whitelist:
+                    continue
+                a = obj_array(obj)
+                _check_box(a, obj, extents=False)       # extents: once matched (check_matched_extents)
+                enl = a.copy()
+                enl[3:6] = enl[3:6] * RATIO
+                jobs.append(dict(frame=idx, obj=obj, cut=enl, box=a))
+            continue
+        gts[idx] = g
+        for k, obj in enumerate(g):
+            a = obj_array(obj)
+            _check_box(a, obj)
+            enl = a.copy()
+            enl[3:6] = enl[3:6] * RATIO
+            for _ in range(augment):
+                if perturb:
+                    enl = random_shift_rotate_box3d(enl, PERTURB_RATIO, rng)
+                jobs.append(dict(frame=idx, obj=obj, cut=enl, gt=k))
+    return jobs, gts
+
+
+def check_matched_extents(jobs, gt_flat, job_gt):
+    """Matched mode: extract_frustum_det_data triangulates a detection's box and its ground truth's only once the
+    detection is matched (:493-532), so only matched pairs need positive extents.  job_gt[j] >= 0: job j matched
+    gt_flat[job_gt[j]]."""
+    for j, g in enumerate(job_gt):
+        if g >= 0:
+            _check_box(jobs[j]["box"], jobs[j]["obj"])
+            _check_box(obj_array(gt_flat[g]), gt_flat[g])
+
+
+def frustum_angle(cut):
+    return -1 * np.arctan2(cut[2], cut[0])
+
+
+# ------------------------------------------------------------------------------ result
+_GT_NAMES = ("id_list", "box3d_list", "input_list", "label_list", "type_list", "heading_list", "size_list",
+             "frustum_angle_list", "box2d_list", "calib_list", "pred_box3d_list", "pred_box3d_size_list",
+             "pred_box3d_angle_list")
+_DET_NAMES = ("id_list", "box2d_list", "input_list", "type_list", "frustum_angle_list", "prob_list", "calib_list",
+              "pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list")
+
+
+class RefineFrustums:
+    """One extraction: K kept frustums and their M points.  Device: points (M, 4) float32, offsets (K + 1) int32,
+    label (M) uint8 (None for detections), written on the extraction's stream.  Host: the provider's lists
+    (datasets/provider_sample_refine.py:85-117).  input_list(), label_list() and TrainBatchBuilder.from_frustums make
+    the current stream wait for that stream first (wait()); other readers of the tensors on another stream call
+    wait() themselves."""
+
+    def __init__(self, mode, points, offsets, label, counts, job_index, lists, stream=None):
+        self.mode, self.points, self.offsets, self.label = mode, points, offsets, label
+        self.stream = stream
+        self.counts = counts                  # (K,) host int64
+        self.job_index = job_index            # (K,) host int64: the job (box, augmentation) of each frustum
+        self.has_labels = mode != _lib.REFINE_DET
+        for n in ("id_list", "box2d_list", "type_list", "frustum_angle_list", "prob_list", "calib_list",
+                  "box3d_list", "heading_list", "size_list", "pred_box3d_list", "pred_box3d_size_list",
+                  "pred_box3d_angle_list"):
+            setattr(self, n, lists.get(n))
+
+    def __len__(self):
+        return len(self.id_list)
+
+    def _split(self, t):
+        off = np.concatenate([[0], np.cumsum(self.counts)])
+        return [t[off[k]:off[k + 1]] for k in range(len(self))]
+
+    def wait(self):
+        """Make the current stream of the tensors' device wait for the extraction's stream."""
+        if self.stream is not None:
+            torch.cuda.current_stream(self.points.device).wait_stream(self.stream)
+
+    def input_list(self):
+        """The per-frustum (n, 4) float32 point arrays, copied to the host."""
+        self.wait()
+        return self._split(self.points.cpu().numpy())
+
+    def label_list(self):
+        """The per-frustum (n,) float64 labels (1 inside the ground-truth box), copied to the host."""
+        if not self.has_labels:
+            raise ValueError("frustums from detections have no labels")
+        self.wait()
+        return self._split(self.label.cpu().numpy().astype(np.float64))
+
+    def to_pickle(self, path):
+        """The lists in the order the reference's function pickles them (readable by the reference's provider)."""
+        names = _GT_NAMES if self.has_labels else _DET_NAMES
+        values = {"input_list": self.input_list()}
+        if self.has_labels:
+            values["label_list"] = self.label_list()
+        with open(path, "wb") as fp:
+            for n in names:
+                pickle.dump(values[n] if n in values else getattr(self, n), fp, -1)
+
+
+class RefineFrustumExtractor:
+    def __init__(self, type_whitelist=("Car",), device=None):
+        self.type_whitelist = tuple(type_whitelist)
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        if self.device.type != "cuda":
+            raise RuntimeError("RefineFrustumExtractor: a CUDA device is required (there is no CPU fallback)")
+
+    # ------------------------------------------------------------------ public modes
+    def from_ground_truth(self, scans, calibs, image_hw, image_ids, gt, perturb=False, augment=1, rng=np.random,
+                          remove_diff=False, stream=None, timer=None):
+        """gt: a label_2 directory or {idx: [KittiObject]}.  rng: the np.random module or a RandomState."""
+        gt = self._objects(gt, image_ids)
+        jobs, gts = job_table(_lib.REFINE_GT, image_ids, None, gt, self.type_whitelist, remove_diff, perturb,
+                              int(augment), rng)
+        return self._run(_lib.REFINE_GT, scans, calibs, image_hw, jobs, gts, stream, timer)
+
+    def from_matched_detections(self, scans, calibs, image_hw, image_ids, dets, gt, remove_diff=False, stream=None,
+                                timer=None):
+        """dets: the collector's dict or {idx: [KittiObject]} (read_result_dir); gt as for from_ground_truth."""
+        dets, gt = self._dets(dets, image_ids), self._objects(gt, image_ids)
+        jobs, gts = job_table(_lib.REFINE_MATCHED, image_ids, dets, gt, self.type_whitelist, remove_diff)
+        return self._run(_lib.REFINE_MATCHED, scans, calibs, image_hw, jobs, gts, stream, timer)
+
+    def from_detections(self, scans, calibs, image_hw, image_ids, dets, stream=None, timer=None):
+        dets = self._dets(dets, image_ids)
+        jobs, _ = job_table(_lib.REFINE_DET, image_ids, dets, None, self.type_whitelist)
+        return self._run(_lib.REFINE_DET, scans, calibs, image_hw, jobs, {}, stream, timer)
+
+    @property
+    def iou_thresh(self):
+        return 0.5 if "Car" in self.type_whitelist else 0.25          # prepare_data_refine.py:447
+
+    @staticmethod
+    def _objects(gt, image_ids):
+        if isinstance(gt, (str, os.PathLike)):
+            return read_label_dir(gt, image_ids)
+        return {int(k): v for k, v in gt.items()}
+
+    @staticmethod
+    def _dets(dets, image_ids):
+        """Images without an entry have no detections (the collector's dict omits them)."""
+        if any(len(v) and not isinstance(v, list) for v in dets.values()):
+            dets = objects_from_detections(dets)
+        return {int(i): list(dets.get(int(i), [])) for i in image_ids}
+
+    def _scan(self, scan):
+        if isinstance(scan, torch.Tensor):
+            if not on_device(scan, self.device):
+                raise RuntimeError("RefineFrustumExtractor: scans must be numpy arrays or CUDA tensors on %s"
+                                   % self.device)
+            if scan.dtype != torch.float32 or scan.dim() != 2 or scan.shape[1] != 4:
+                raise ValueError("a scan must be an (n, 4) float32 array")
+            return scan
+        a = np.asarray(scan)
+        if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
+            raise ValueError("a scan must be an (n, 4) float32 array")
+        return a
+
+    # ------------------------------------------------------------------ device call
+    def _run(self, mode, scans, calibs, image_hw, jobs, gts, stream, timer):
+        dev = self.device
+        frame_ids = []
+        for jb in jobs:
+            if not frame_ids or frame_ids[-1] != jb["frame"]:
+                frame_ids.append(jb["frame"])
+        fpos = {k: f for f, k in enumerate(frame_ids)}
+        gt_flat, gt_off = [], [0]
+        for k in frame_ids:
+            gt_flat += gts.get(k, [])
+            gt_off.append(len(gt_flat))
+        gt_base = {k: gt_off[fpos[k]] for k in frame_ids}
+        J, F, G = len(jobs), len(frame_ids), len(gt_flat)
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.device(dev), torch.cuda.stream(stream):
+            if F == 0 or J == 0:
+                return self._result(mode, torch.zeros((0, 4), dtype=torch.float32, device=dev),
+                                    torch.zeros(1, dtype=torch.int32, device=dev),
+                                    None if mode == _lib.REFINE_DET else torch.zeros(0, dtype=torch.uint8, device=dev),
+                                    np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, np.int64), jobs,
+                                    gt_flat, calibs, stream)
+            sc = [self._scan(scans[k]) for k in frame_ids]
+            if all(isinstance(s, np.ndarray) for s in sc):
+                scan_dev = torch.from_numpy(np.concatenate(sc)).to(dev)
+            else:
+                scan_dev = torch.cat([s if isinstance(s, torch.Tensor) else torch.from_numpy(s).to(dev)
+                                      for s in sc]).contiguous()
+            frames = (_lib.FrustumFrame * F)(*[_frame_record(calibs[k], image_hw[k]) for k in frame_ids])
+            so = np.zeros(F + 1, dtype=np.int32)
+            np.cumsum([s.shape[0] for s in sc], out=so[1:])
+            N = int(so[-1])
+            job_box = np.array([box_record(jb["cut"]) for jb in jobs], dtype=np.dtype(_lib.RefineBox))
+            job_frame = np.array([fpos[jb["frame"]] for jb in jobs], dtype=np.int32)
+            gt_box = np.array([box_record(obj_array(o)) for o in gt_flat], dtype=np.dtype(_lib.RefineBox))
+            if mode == _lib.REFINE_GT:
+                job_ref = np.array([gt_base[jb["frame"]] + jb["gt"] for jb in jobs], dtype=np.int32)
+            elif mode == _lib.REFINE_MATCHED:
+                job_ref = np.arange(J, dtype=np.int32)                 # one job per detection
+            else:
+                job_ref = np.zeros(J, dtype=np.int32)
+            parts = [bytes(frames), job_box.tobytes(), so.tobytes(), job_frame.tobytes(), job_ref.tobytes(),
+                     gt_box.tobytes()]
+            D = P = 0
+            if mode == _lib.REFINE_MATCHED:
+                D = J
+                ngt = np.array([gt_off[f + 1] - gt_off[f] for f in job_frame], dtype=np.int64)
+                po = np.zeros(D + 1, dtype=np.int32)
+                np.cumsum(ngt, out=po[1:])
+                P = int(po[-1])
+                det_c = iou_corners(np.stack([jb["box"] for jb in jobs]))
+                gt_c = iou_corners(np.stack([obj_array(o) for o in gt_flat]))
+                parts += [det_c.tobytes(), gt_c.tobytes(), np.asarray(gt_off, np.int32).tobytes(), po.tobytes()]
+            nb = [len(p) for p in parts]
+            o = np.cumsum([0] + [(n + 255) // 256 * 256 for n in nb])
+            hbuf = np.zeros(int(o[-1]), dtype=np.uint8)
+            for p, start in zip(parts, o):
+                hbuf[start:start + len(p)] = np.frombuffer(p, dtype=np.uint8)
+            inp = torch.from_numpy(hbuf).to(dev)
+            ib = inp.data_ptr()
+            a = _lib.RefineExtractArgs()
+            a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, F, N, J, G
+            a.num_dets, a.num_pairs, a.iou_thresh = D, P, self.iou_thresh
+            a.scans = scan_dev.data_ptr() if N > 0 else None
+            a.frames, a.jobs, a.scan_offsets, a.job_frame, a.job_ref = (ib + int(v) for v in o[:5])
+            a.gt_boxes = ib + int(o[5]) if G > 0 else None
+            if mode == _lib.REFINE_MATCHED:
+                a.det_frame = a.job_frame
+                a.det_corners, a.gt_corners, a.gt_offsets, a.pair_offsets = (ib + int(v) for v in o[6:10])
+            a.host_scan_offsets = so.ctypes.data
+            nbytes = _lib.load().fcn_refine_extract_workspace_bytes(C.byref(a))
+            if nbytes < 0:
+                _lib.check(-1, "fcn_refine_extract_workspace_bytes")
+            ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
+            summary = torch.empty(4 + J, dtype=torch.int64, device=dev)   # info | job_points | job_gt (int32 each)
+            a.workspace, a.workspace_bytes = ws.data_ptr(), int(nbytes)
+            a.info, a.job_points, a.job_gt = summary.data_ptr(), summary.data_ptr() + 32, summary.data_ptr() + 32 + 4 * J
+            if timer is not None:
+                timer("start")
+            _lib.call("fcn_refine_extract_count", C.byref(a), stream.cuda_stream)
+            if timer is not None:
+                timer("count")
+            back = summary.cpu().numpy()                                       # the one host sync
+            K, M, bad = int(back[0]), int(back[1]), int(back[2])
+            if bad:
+                raise RuntimeError("fcn_refine_extract: %d jobs or pairs reference no frame or box" % bad)
+            if M >= 2 ** 31:
+                raise RuntimeError("fcn_refine_extract: %d frustum points do not fit int32 offsets" % M)
+            job_points = back[4:].view(np.int32)[:J]
+            job_gt = back[4:].view(np.int32)[J:2 * J]
+            kept = np.flatnonzero(job_points >= 0)
+            assert len(kept) == K and int(job_points[kept].sum()) == M
+            if mode == _lib.REFINE_MATCHED:
+                check_matched_extents(jobs, gt_flat, job_gt)
+            points = torch.empty((M, 4), dtype=torch.float32, device=dev)
+            offsets = torch.empty(K + 1, dtype=torch.int32, device=dev)
+            label = None if mode == _lib.REFINE_DET else torch.empty(M, dtype=torch.uint8, device=dev)
+            a.num_kept, a.num_out_points = K, M
+            a.points, a.offsets = points.data_ptr(), offsets.data_ptr()
+            a.labels = None if label is None else label.data_ptr()
+            if timer is not None:
+                timer("write_start")
+            _lib.call("fcn_refine_extract_write", C.byref(a), stream.cuda_stream)
+            if timer is not None:
+                timer("write")
+        return self._result(mode, points, offsets, label, job_points[kept].astype(np.int64), kept.astype(np.int64),
+                            job_gt[kept].astype(np.int64), jobs, gt_flat, calibs, stream)
+
+    @staticmethod
+    def _result(mode, points, offsets, label, counts, kept, kept_gt, jobs, gt_flat, calibs, stream):
+        L = {n: [] for n in ("id_list", "box2d_list", "type_list", "frustum_angle_list", "prob_list", "calib_list",
+                             "box3d_list", "heading_list", "size_list", "pred_box3d_list", "pred_box3d_size_list",
+                             "pred_box3d_angle_list")}
+        for j, g in zip(kept.tolist(), kept_gt.tolist()):
+            jb = jobs[j]
+            obj, cut = jb["obj"], jb["cut"]
+            L["id_list"].append(jb["frame"])
+            L["type_list"].append(obj.type)
+            L["frustum_angle_list"].append(frustum_angle(cut))
+            L["calib_list"].append(calibs[jb["frame"]])
+            L["pred_box3d_list"].append(compute_box_3d_obj_array(cut))
+            L["pred_box3d_size_list"].append(cut[3:6])
+            L["pred_box3d_angle_list"].append(cut[-1])
+            if mode == _lib.REFINE_DET:
+                L["box2d_list"].append(obj.box2d)
+                L["prob_list"].append(obj.score)
+            else:
+                gt = gt_flat[g]
+                L["box3d_list"].append(compute_box_3d_obj_array(obj_array(gt)))
+                L["heading_list"].append(gt.ry)
+                L["size_list"].append(np.array([gt.l, gt.w, gt.h]))
+                L["box2d_list"].append(gt.box2d)
+        if mode != _lib.REFINE_DET:
+            L["prob_list"] = None
+        else:
+            for n in ("box3d_list", "heading_list", "size_list"):
+                L[n] = None
+        return RefineFrustums(mode, points, offsets, label, counts, kept, L, stream)

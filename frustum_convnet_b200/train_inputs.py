@@ -245,22 +245,52 @@ class TrainBatchBuilder:
             if lists[n] is None or len(lists[n]) != F:
                 raise ValueError("kind=%r needs %s with one entry per frustum" % (self.kind, n))
         fr = frustum_table(self.kind, self.strides, self.max_depth, self.labels, classes, type_list, **lists)
+        pts = np.concatenate([np.asarray(p)[:, :3] for p in input_list]).astype(np.float64 if self.points_f64 else
+                                                                                  np.float32)
+        self._install(fr, counts, torch.from_numpy(np.ascontiguousarray(pts)).to(self.device), label_list)
+
+    @classmethod
+    def from_frustums(cls, fr, kind, strides, npoints, classes=None, **kw):
+        """The dataset of a refine_extract.RefineFrustums: its points stay on the device (the x, y, z columns are
+        copied there), the per-frustum constants come from its host lists.  The same batches as set_dataset on
+        fr's lists.  labels defaults to whether fr has ground truth."""
+        if kind != "refine":
+            raise ValueError("from_frustums builds the refinement provider's batches (kind='refine'), got %r" % kind)
+        kw.setdefault("labels", fr.has_labels)
+        tb = cls(kind, strides, npoints, **kw)
+        if tb.labels and not fr.has_labels:
+            raise ValueError("labels=True needs frustums with ground truth (from_ground_truth or "
+                             "from_matched_detections)")
+        if len(fr) == 0:
+            raise ValueError("empty dataset")
+        if fr.points.device.type != "cuda" or (tb.device.index is not None and fr.points.device != tb.device):
+            raise RuntimeError("the frustums live on %s, the builder on %s" % (fr.points.device, tb.device))
+        counts = np.asarray(fr.counts, dtype=np.int64)
+        fr.wait()                          # the points were written on the extraction's stream
+        names = ("box3d_list", "heading_list", "size_list", "prob_list", "pred_box3d_list", "pred_box3d_size_list",
+                 "pred_box3d_angle_list")
+        table = frustum_table(kind, tb.strides, tb.max_depth, tb.labels,
+                              KITTI_CLASSES if classes is None else classes, fr.type_list,
+                              **{n: getattr(fr, n) for n in names})
+        tb.points_f64 = False
+        tb._install(table, counts, fr.points[:, :3].contiguous(), None)
+        return tb
+
+    def _install(self, fr, counts, d_points, label_list):
         S = len(self.strides)
         self.T_of = fr["T"][:, :S].astype(np.int64)
         self.counts = counts
         dev = self.device
-        pts = np.concatenate([np.asarray(p)[:, :3] for p in input_list]).astype(np.float64 if self.points_f64 else
-                                                                                  np.float32)
-        self.d_points = torch.from_numpy(np.ascontiguousarray(pts)).to(dev)
+        self.d_points = d_points
         self.d_offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)).to(dev)
         self.d_frustums = torch.from_numpy(fr.view(np.uint8)).to(dev)
         self.d_seg = None
         if self._has_seg:
             seg = np.concatenate([np.asarray(s).astype(np.int64) for s in label_list])  # provider_sample.py:206
-            if len(seg) != len(pts) or (np.abs(seg) >= 2 ** 31).any():
+            if len(seg) != len(d_points) or (np.abs(seg) >= 2 ** 31).any():
                 raise ValueError("label_list must hold one int32-range label per point")
             self.d_seg = torch.from_numpy(seg.astype(np.int32)).to(dev)
-        self.num_frustums = F
+        self.num_frustums = len(counts)
         self.B_cap = 0                     # output buffers follow the dataset (T capacity)
 
     # ------------------------------------------------------------------ per step

@@ -797,6 +797,74 @@ FCN_API long long fcn_frustum_extract_workspace_bytes(const fcn_frustum_extract_
 FCN_API int fcn_frustum_extract_count(const fcn_frustum_extract_args *args, fcn_stream_t stream);
 FCN_API int fcn_frustum_extract_write(const fcn_frustum_extract_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (16) KITTI refinement frustums on the device: extract_frustum_data, extract_frustum_det_data and
+ *      extract_frustum_data_rgb_detection of kitti/prepare_data_refine.py:239-773 for several frames and all their
+ *      3-D boxes at once.
+ *
+ *      The frames' in-image points are those of section (15) (same projection, same test, scan order).  A job is one
+ *      3-D box that cuts points out of its frame (job_frame[j]): the enlarged (and perhaps perturbed) box jobs[j].
+ *      Every box is tested in float64 in its own frame: p in box <=> |cs dx - sn dz| <= half[0], |dy| <= half[1] and
+ *      |sn dx + cs dz| <= half[2], with (dx, dy, dz) = p - center and every product and sum rounded separately.  The
+ *      label box of a job (the points of the job that are also in it are labelled 1):
+ *        FCN_REFINE_GT       gt_boxes[job_ref[j]]; the job is dropped when no point is labelled;
+ *        FCN_REFINE_MATCHED  the ground truth matched to detection job_ref[j]: the first maximum of the 3-D IoU (the
+ *                            reference's rbbox_iou_3d, float64, with its standup-box pre-filter at 0) of its corners
+ *                            det_corners[d] against gt_corners[g] for the ground truths g in [gt_offsets[f],
+ *                            gt_offsets[f + 1]) of its frame f = det_frame[d]; none when that maximum is below
+ *                            iou_thresh.  The job is dropped without a match or when no point is labelled;
+ *        FCN_REFINE_DET      none; the job is dropped when it has no point.
+ *      num_pairs = sum over the detections of their frame's ground-truth count; pair_offsets is its exclusive sum.
+ *
+ *      Two calls in order on one stream, sharing the caller's workspace (fcn_refine_extract_workspace_bytes: needs the
+ *      device, -1 on invalid arguments), no host sync, no allocation:
+ *        fcn_refine_extract_count : writes job_points (DEVICE, num_jobs: the job's point count when kept, -1 when
+ *                                   dropped or when an index is out of range), job_gt (DEVICE, num_jobs: the label
+ *                                   box's index in gt_boxes, -1 for none) and info (DEVICE int64[4]: kept jobs K, their
+ *                                   points M, jobs or detections with an out-of-range index, 0);
+ *        fcn_refine_extract_write : needs num_kept = K and num_out_points = M as read by the host; writes the kept jobs
+ *                                   in job order: points (M, 4) float32 rect x, y, z and intensity in scan order,
+ *                                   labels (M) uint8 (not written in FCN_REFINE_DET mode; may be NULL) and offsets (K + 1)
+ *                                   int32.  The k-th kept job is the k-th j with job_points[j] >= 0.
+ *      With num_frames == 0 or num_jobs == 0 both calls return 0 and do nothing (K = M = 0; info is not written).
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_REFINE_GT 0
+#define FCN_REFINE_MATCHED 1
+#define FCN_REFINE_DET 2
+typedef struct {
+    double center[3];   /* cx, cy - h / 2, cz (rect camera coordinates) */
+    double half[3];     /* l / 2, h / 2, w / 2 */
+    double cs, sn;      /* cos(ry), sin(ry) */
+} fcn_refine_box;
+typedef struct {
+    int mode, num_frames, num_points, num_jobs, num_gt, num_dets, num_pairs, num_kept;
+    long long num_out_points;
+    double iou_thresh;
+    const float *scans;                 /* DEVICE (num_points, 4), 16-byte aligned */
+    const int32_t *scan_offsets;        /* DEVICE (num_frames + 1) */
+    const int32_t *host_scan_offsets;   /* HOST copy: starts at 0, never decreases, ends at num_points */
+    const fcn_frustum_frame *frames;    /* DEVICE (num_frames) */
+    const fcn_refine_box *jobs;         /* DEVICE (num_jobs) */
+    const int32_t *job_frame;           /* DEVICE (num_jobs) */
+    const int32_t *job_ref;             /* DEVICE (num_jobs): ground-truth index (GT), detection index (MATCHED) */
+    const fcn_refine_box *gt_boxes;     /* DEVICE (num_gt) */
+    const double *gt_corners;           /* DEVICE (num_gt, 8, 3), MATCHED only */
+    const double *det_corners;          /* DEVICE (num_dets, 8, 3), MATCHED only */
+    const int32_t *det_frame;           /* DEVICE (num_dets), MATCHED only */
+    const int32_t *gt_offsets;          /* DEVICE (num_frames + 1), MATCHED only */
+    const int32_t *pair_offsets;        /* DEVICE (num_dets + 1), MATCHED only */
+    void *workspace;
+    long long workspace_bytes;
+    long long *info;                    /* DEVICE int64[4] */
+    int32_t *job_points, *job_gt;       /* DEVICE (num_jobs) each */
+    float *points;                      /* fcn_refine_extract_write outputs (DEVICE) */
+    uint8_t *labels;
+    int32_t *offsets;
+} fcn_refine_extract_args;
+FCN_API long long fcn_refine_extract_workspace_bytes(const fcn_refine_extract_args *args);
+FCN_API int fcn_refine_extract_count(const fcn_refine_extract_args *args, fcn_stream_t stream);
+FCN_API int fcn_refine_extract_write(const fcn_refine_extract_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

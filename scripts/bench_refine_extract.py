@@ -1,0 +1,112 @@
+#!/usr/bin/env python
+"""Time of the KITTI refinement extractor (frustum_convnet_b200/refine_extract.py, csrc/refine_extract.cu) per frame.
+
+    python scripts/bench_refine_extract.py [--frames 64] [--points 120000] [--boxes 8] [--calls 20] [--warmup 3]
+
+The scenes are synthetic (oracle/kitti_refine_synth.large_scene, seed 0): KITTI-sized scans (~120k points) with 8
+ground-truth objects a frame and their detections, 64 frames per call, whitelist Car.  Modes: train
+(from_ground_truth, perturb, augment = 5: the refinement training set), matched (from_matched_detections,
+remove_diff) and det (from_detections).  Reported per frame and mode, medians over ``--calls`` calls after
+``--warmup``:
+  count_us / write_us  CUDA events around the two device entries, scans already on the device;
+  e2e_us               host wall time of a whole call from scans in pinned host memory: the H2D copy, the host job
+                       table (perturbation included), both passes and the one read back, until the outputs are complete;
+  oracle_us            oracle/refine_extract.extract (numpy, half-space test) on the host, one run.
+Prints one JSON line with the card name and its power limit.  Writes nothing to the tree."""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "scripts"))
+
+WHITELIST = ("Car",)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=64)
+    ap.add_argument("--points", type=int, default=120000)
+    ap.add_argument("--boxes", type=int, default=8)
+    ap.add_argument("--calls", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    args = ap.parse_args()
+
+    import torch
+    from bench_detect import gpu_identity
+    from frustum_convnet_b200.refine_extract import RefineFrustumExtractor
+    from oracle import kitti_refine_synth as krs
+    from oracle import refine_extract as orx
+    assert torch.cuda.is_available(), "bench_refine_extract.py needs a CUDA device; there is no CPU fallback"
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scans, calibs, hw, labels, results = krs.large_scene(0, args.frames, args.points, args.boxes)
+    keys = sorted(scans)
+    gt, dets = krs.objects(labels), krs.objects(results)
+    pinned = torch.from_numpy(np.concatenate([scans[k] for k in keys])).pin_memory()
+    off = np.concatenate([[0], np.cumsum([len(scans[k]) for k in keys])])
+    dev_scans = {k: torch.from_numpy(scans[k]).to(dev) for k in keys}
+    ex = RefineFrustumExtractor(WHITELIST, dev)
+    stream = torch.cuda.current_stream(dev)
+    calls = {
+        "train": lambda s, t: ex.from_ground_truth(s, calibs, hw, keys, gt, perturb=True, augment=5,
+                                                   rng=np.random.RandomState(1), timer=t),
+        "matched": lambda s, t: ex.from_matched_detections(s, calibs, hw, keys, dets, gt, remove_diff=True, timer=t),
+        "det": lambda s, t: ex.from_detections(s, calibs, hw, keys, dets, timer=t),
+    }
+    oracle = {
+        "train": lambda: orx.extract("gt", scans, calibs, hw, keys, None, gt, WHITELIST, False, True, 5,
+                                     np.random.RandomState(1)),
+        "matched": lambda: orx.extract("matched", scans, calibs, hw, keys, dets, gt, WHITELIST, True),
+        "det": lambda: orx.extract("det", scans, calibs, hw, keys, dets, None, WHITELIST),
+    }
+    out = {"bench": "refine_extract", "frames": args.frames, "scan_points": int(off[-1]), "calls": args.calls}
+    for mode, call in calls.items():
+        rec = {"count": [], "write": [], "e2e": []}
+        fr = None
+        for it in range(args.warmup + args.calls):
+            marks = {}
+
+            def timer(name):
+                e = torch.cuda.Event(enable_timing=True)
+                e.record(stream)
+                marks[name] = e
+
+            torch.cuda.synchronize()
+            fr = call(dev_scans, timer)
+            torch.cuda.synchronize()
+            t_count = marks["start"].elapsed_time(marks["count"])
+            t_write = marks["write_start"].elapsed_time(marks["write"])
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            flat = pinned.to(dev, non_blocking=True)
+            call({k: flat[off[i]:off[i + 1]] for i, k in enumerate(keys)}, None)
+            torch.cuda.synchronize()
+            wall = time.perf_counter() - t0
+            if it < args.warmup:
+                continue
+            rec["count"].append(t_count * 1e3 / args.frames)
+            rec["write"].append(t_write * 1e3 / args.frames)
+            rec["e2e"].append(wall * 1e6 / args.frames)
+        t0 = time.perf_counter()
+        ref = oracle[mode]()
+        t_oracle = time.perf_counter() - t0
+        assert ref["id_list"] == fr.id_list and fr.counts.tolist() == [len(p) for p in ref["input_list"]], \
+            "device and oracle disagree (%s)" % mode
+        out[mode] = {"frustums": len(fr), "frustum_points": int(fr.counts.sum()),
+                     **{k + "_us_per_frame": float(np.median(v)) for k, v in rec.items()},
+                     "oracle_us_per_frame": t_oracle * 1e6 / args.frames}
+    out.update(gpu_identity(dev))
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
