@@ -41,6 +41,56 @@ inline int cuda_fail(const char *fn, cudaError_t e) {
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// Host copy of CSR offsets o[0..n] (records split per image, class or frame): they start at 0, never decrease and
+// end at total.
+inline bool offsets_ok(const int32_t *o, int n, int total) {
+    if (o[0] != 0 || o[n] != total) return false;
+    for (int i = 0; i < n; ++i)
+        if (o[i + 1] < o[i]) return false;
+    return true;
+}
+
+// Workspace of a two-phase entry family (fcn_*_workspace_bytes, then entries that share the caller's workspace).
+// The family's layout function takes pieces in a fixed order from a Carve: with a null base it only sizes them, so
+// the size query and every entry read one layout.  Each piece is rounded up to 256 bytes.
+struct Carve {
+    char *base;
+    size_t off;
+    char *take(size_t bytes) {
+        char *p = base ? base + off : nullptr;
+        off += (bytes + 255) & ~(size_t)255;
+        return p;
+    }
+};
+
+// fcn_<family>_workspace_bytes: the bytes `layout(Carve &)` takes, or -1 when a cub size query in it fails.
+template <typename Layout>
+inline long long workspace_size(const char *fn, Layout &&layout) {
+    Carve c{nullptr, 0};
+    const cudaError_t e = layout(c);
+    if (e != cudaSuccess) {
+        cuda_fail(fn, e);
+        return -1;
+    }
+    return (long long)c.off;
+}
+
+// The prepare step of every entry of a family: size the layout, check the caller's workspace against it, carve it.
+template <typename Layout>
+inline int carve_workspace(const char *fn, const char *family, void *workspace, long long workspace_bytes,
+                           Layout &&layout) {
+    const long long need = workspace_size(fn, layout);
+    if (need < 0) return FCN_ERR_CUDA;
+    if (workspace_bytes < need) {
+        char msg[96];
+        snprintf(msg, sizeof(msg), "workspace smaller than fcn_%s_workspace_bytes()", family);
+        return invalid(fn, msg);
+    }
+    Carve c{(char *)workspace, 0};
+    const cudaError_t e = layout(c);
+    return e != cudaSuccess ? cuda_fail(fn, e) : FCN_OK;
+}
+
 int sm_count();
 
 // Programmatic dependent launch (PDL): every kernel of the forward chain is launched with the

@@ -326,13 +326,11 @@ struct DetWs {
     float *corners, *cube;
     unsigned *removed;
     void *temp;
-    size_t temp_bytes, total;
+    size_t temp_bytes;
 };
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-// carve (base == nullptr: sizes only); returns a CUDA error of the cub size queries
-static cudaError_t det_layout(int capacity, int S, char *base, DetWs &w) {
+// returns a CUDA error of the cub size queries
+static cudaError_t det_layout(int capacity, int S, Carve &c, DetWs &w) {
     const size_t C = (size_t)capacity;
     size_t t_sort = 0, t_scan32 = 0, t_scan64 = 0;
     cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (unsigned long long *)nullptr,
@@ -344,25 +342,22 @@ static cudaError_t det_layout(int capacity, int S, char *base, DetWs &w) {
     e = cub::DeviceScan::ExclusiveSum(nullptr, t_scan64, (long long *)nullptr, (long long *)nullptr, S + 1);
     if (e != cudaSuccess) return e;
     w.temp_bytes = std::max(t_sort, std::max(t_scan32, t_scan64));
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += align256(bytes); return p; };
-    w.keys_a = (unsigned long long *)take(C * 8);
-    w.keys_b = (unsigned long long *)take(C * 8);
-    w.vals_a = (int *)take(C * 4);
-    w.vals_b = (int *)take(C * 4);
-    w.sorted = (fcn_det_record *)take(C * sizeof(fcn_det_record));
-    w.seg_cnt = (int *)take((size_t)(S + 1) * 4);
-    w.mask_w = (long long *)take((size_t)(S + 1) * 8);
-    w.tiles = (long long *)take((size_t)(S + 1) * 8);
-    w.mask_off = (long long *)take((size_t)(S + 1) * 8);
-    w.tile_off = (long long *)take((size_t)(S + 1) * 8);
-    w.rank_idx = (int *)take(C * 4);
-    w.keep = (int *)take(C * 4);
-    w.corners = (float *)take(C * 24 * 4);
-    w.cube = (float *)take(C * 6 * 4);
-    w.removed = (unsigned *)take((C / 32 + (size_t)S + 2) * 4);
-    w.temp = take(w.temp_bytes);
-    w.total = off;
+    w.keys_a = (unsigned long long *)c.take(C * 8);
+    w.keys_b = (unsigned long long *)c.take(C * 8);
+    w.vals_a = (int *)c.take(C * 4);
+    w.vals_b = (int *)c.take(C * 4);
+    w.sorted = (fcn_det_record *)c.take(C * sizeof(fcn_det_record));
+    w.seg_cnt = (int *)c.take((size_t)(S + 1) * 4);
+    w.mask_w = (long long *)c.take((size_t)(S + 1) * 8);
+    w.tiles = (long long *)c.take((size_t)(S + 1) * 8);
+    w.mask_off = (long long *)c.take((size_t)(S + 1) * 8);
+    w.tile_off = (long long *)c.take((size_t)(S + 1) * 8);
+    w.rank_idx = (int *)c.take(C * 4);
+    w.keep = (int *)c.take(C * 4);
+    w.corners = (float *)c.take(C * 24 * 4);
+    w.cube = (float *)c.take(C * 6 * 4);
+    w.removed = (unsigned *)c.take((C / 32 + (size_t)S + 2) * 4);
+    w.temp = c.take(w.temp_bytes);
     return cudaSuccess;
 }
 
@@ -398,12 +393,7 @@ extern "C" long long fcn_det_workspace_bytes(int capacity, int num_segments) {
         return -1;
     }
     DetWs w;
-    const cudaError_t e = det_layout(std::max(capacity, 1), num_segments, nullptr, w);
-    if (e != cudaSuccess) {
-        cuda_fail(__func__, e);
-        return -1;
-    }
-    return (long long)w.total;
+    return workspace_size(__func__, [&](Carve &c) { return det_layout(std::max(capacity, 1), num_segments, c, w); });
 }
 
 static int det_check_finalize(const fcn_det_finalize_args *a, const char *fn) {
@@ -421,14 +411,14 @@ static int det_check_finalize(const fcn_det_finalize_args *a, const char *fn) {
 }
 
 extern "C" int fcn_det_prepare(const fcn_det_finalize_args *a, fcn_stream_t stream) {
-    const int st = det_check_finalize(a, __func__);
+    int st = det_check_finalize(a, __func__);
     if (st != FCN_OK) return st;
     const int C = std::max(a->capacity, 1), S = a->num_segments, nms = a->method == FCN_DET_NMS;
     cudaStream_t s = (cudaStream_t)stream;
     DetWs w;
-    FCN_CUDA(det_layout(C, S, nullptr, w));
-    FCN_REQUIRE(a->workspace_bytes >= (long long)w.total, "workspace smaller than fcn_det_workspace_bytes()");
-    FCN_CUDA(det_layout(C, S, (char *)a->workspace, w));
+    st = carve_workspace(__func__, "det", a->workspace, a->workspace_bytes,
+                         [&](Carve &c) { return det_layout(C, S, c, w); });
+    if (st != FCN_OK) return st;
     FCN_CUDA(cudaMemsetAsync(w.seg_cnt, 0, (size_t)(S + 1) * 4, s));
     const int g = det_grid(C, DET_FIN_THREADS);
     det_keys_kernel<<<g, DET_FIN_THREADS, 0, s>>>(a->capacity, a->counter, a->records, w.keys_a, w.vals_a, w.seg_cnt);
@@ -458,7 +448,7 @@ extern "C" int fcn_det_prepare(const fcn_det_finalize_args *a, fcn_stream_t stre
 }
 
 extern "C" int fcn_det_select(const fcn_det_finalize_args *a, fcn_stream_t stream) {
-    const int st = det_check_finalize(a, __func__);
+    int st = det_check_finalize(a, __func__);
     if (st != FCN_OK) return st;
     if (a->n_counted < 0 || a->n_counted > a->capacity) {
         snprintf(g_err, sizeof(g_err),
@@ -469,9 +459,9 @@ extern "C" int fcn_det_select(const fcn_det_finalize_args *a, fcn_stream_t strea
     const int C = std::max(a->capacity, 1), S = a->num_segments, n = a->n_counted, nms = a->method == FCN_DET_NMS;
     cudaStream_t s = (cudaStream_t)stream;
     DetWs w;
-    FCN_CUDA(det_layout(C, S, nullptr, w));
-    FCN_REQUIRE(a->workspace_bytes >= (long long)w.total, "workspace smaller than fcn_det_workspace_bytes()");
-    FCN_CUDA(det_layout(C, S, (char *)a->workspace, w));
+    st = carve_workspace(__func__, "det", a->workspace, a->workspace_bytes,
+                         [&](Carve &c) { return det_layout(C, S, c, w); });
+    if (st != FCN_OK) return st;
     FCN_REQUIRE(!nms || a->mask_words >= 0, "bad mask_words");
     FCN_REQUIRE(!nms || a->mask_words == 0 || a->mask, "NULL mask");
     if (n > 0 && nms) {

@@ -146,12 +146,10 @@ struct FxWs {
     float4 *fov_pts;
     double *fov_u, *fov_v, *box, *angle;
     void *temp;
-    size_t temp_bytes, total;
+    size_t temp_bytes;
 };
 
-static size_t fx_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-static cudaError_t fx_layout(const fcn_frustum_extract_args *a, char *base, FxWs &w) {
+static cudaError_t fx_layout(const fcn_frustum_extract_args *a, Carve &c, FxWs &w) {
     const size_t N = (size_t)a->num_points, D = (size_t)a->num_dets;
     size_t t0 = 0, t1 = 0, t2 = 0;
     cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, t0, (const int32_t *)nullptr, (int32_t *)nullptr,
@@ -164,27 +162,23 @@ static cudaError_t fx_layout(const fcn_frustum_extract_args *a, char *base, FxWs
     if (e != cudaSuccess) return e;
     w.temp_bytes = t0 > t1 ? t0 : t1;
     w.temp_bytes = w.temp_bytes > t2 ? w.temp_bytes : t2;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += fx_align(bytes); return p; };
-    w.flags = (int32_t *)take((N + 1) * 4);
-    w.pos = (int32_t *)take((N + 1) * 4);
-    w.fov_pts = (float4 *)take(N * 16);
-    w.fov_u = (double *)take(N * 8);
-    w.fov_v = (double *)take(N * 8);
-    w.keep = (int32_t *)take((D + 1) * 4);
-    w.keep_pos = (int32_t *)take((D + 1) * 4);
-    w.cnt = (long long *)take((D + 1) * 8);
-    w.cnt_pos = (long long *)take((D + 1) * 8);
-    w.box = (double *)take(D * 32);
-    w.angle = (double *)take(D * 8);
-    w.bad = (int32_t *)take(4);
-    w.temp = take(w.temp_bytes);
-    w.total = off;
+    w.flags = (int32_t *)c.take((N + 1) * 4);
+    w.pos = (int32_t *)c.take((N + 1) * 4);
+    w.fov_pts = (float4 *)c.take(N * 16);
+    w.fov_u = (double *)c.take(N * 8);
+    w.fov_v = (double *)c.take(N * 8);
+    w.keep = (int32_t *)c.take((D + 1) * 4);
+    w.keep_pos = (int32_t *)c.take((D + 1) * 4);
+    w.cnt = (long long *)c.take((D + 1) * 8);
+    w.cnt_pos = (long long *)c.take((D + 1) * 8);
+    w.box = (double *)c.take(D * 32);
+    w.angle = (double *)c.take(D * 8);
+    w.bad = (int32_t *)c.take(4);
+    w.temp = c.take(w.temp_bytes);
     return cudaSuccess;
 }
 
-// Host-side checks shared by every entry: counts, pointers, the host copy of the scan offsets.  Sets *max_n to the
-// largest scan.
+// Host-side checks shared by every entry: counts, pointers, the scans.  Sets *max_n to the largest scan.
 static int fx_check(const fcn_frustum_extract_args *a, const char *fn, int *max_n) {
     if (a == nullptr) return invalid(fn, "NULL args");
     if (a->num_frames < 0 || a->num_points < 0 || a->num_dets < 0)
@@ -193,31 +187,17 @@ static int fx_check(const fcn_frustum_extract_args *a, const char *fn, int *max_
         return invalid(fn, "too large (num_frames <= 65535, num_points <= 2^30, num_dets <= 2^28)");
     *max_n = 0;
     if (a->num_frames == 0 || a->num_dets == 0) return FCN_OK;
-    if (!a->host_scan_offsets) return invalid(fn, "NULL host_scan_offsets");
     if (!a->scan_offsets || !a->frames || !a->boxes || !a->det_frame || (a->num_points > 0 && !a->scans))
         return invalid(fn, "NULL pointer");
-    if (((uintptr_t)a->scans & 15) != 0) return invalid(fn, "scans must be 16-byte aligned");
-    const int32_t *so = a->host_scan_offsets;
-    if (so[0] != 0 || so[a->num_frames] != a->num_points)
-        return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
-    for (int f = 0; f < a->num_frames; ++f) {
-        if (so[f + 1] < so[f]) return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
-        if (so[f + 1] - so[f] > *max_n) *max_n = so[f + 1] - so[f];
-    }
-    return FCN_OK;
+    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, max_n);
 }
 
 static int fx_prepare(const fcn_frustum_extract_args *a, const char *fn, FxWs &w, int *max_n) {
     const int st = fx_check(a, fn, max_n);
     if (st != FCN_OK || a->num_frames == 0 || a->num_dets == 0) return st;
     if (!a->workspace || !a->info || !a->det_points) return invalid(fn, "NULL workspace, info or det_points");
-    cudaError_t e = fx_layout(a, nullptr, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    if (a->workspace_bytes < (long long)w.total)
-        return invalid(fn, "workspace smaller than fcn_frustum_extract_workspace_bytes()");
-    e = fx_layout(a, (char *)a->workspace, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    return FCN_OK;
+    return carve_workspace(fn, "frustum_extract", a->workspace, a->workspace_bytes,
+                           [&](Carve &c) { return fx_layout(a, c, w); });
 }
 
 }  // namespace fcn
@@ -229,12 +209,7 @@ extern "C" long long fcn_frustum_extract_workspace_bytes(const fcn_frustum_extra
     if (fx_check(a, __func__, &max_n) != FCN_OK) return -1;
     if (a->num_frames == 0 || a->num_dets == 0) return 0;
     FxWs w;
-    const cudaError_t e = fx_layout(a, nullptr, w);
-    if (e != cudaSuccess) {
-        cuda_fail(__func__, e);
-        return -1;
-    }
-    return (long long)w.total;
+    return workspace_size(__func__, [&](Carve &c) { return fx_layout(a, c, w); });
 }
 
 extern "C" int fcn_frustum_extract_count(const fcn_frustum_extract_args *a, fcn_stream_t stream) {

@@ -80,4 +80,18 @@ __device__ __forceinline__ void fov_compact(const float4 *__restrict__ scans, co
     }
 }
 
+// Host check of the scans both extractors take: 16-byte-aligned float4 points and the host copy of the scan offsets
+// (num_frames + 1 entries).  Raises *max_n (0 on entry) to the largest scan, the x extent of the flag and compact
+// grids.
+inline int check_scans(const char *fn, const int32_t *host_so, int num_frames, int num_points, const void *scans,
+                       int *max_n) {
+    if (!host_so) return invalid(fn, "NULL host_scan_offsets");
+    if (((uintptr_t)scans & 15) != 0) return invalid(fn, "scans must be 16-byte aligned");
+    if (!offsets_ok(host_so, num_frames, num_points))
+        return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
+    for (int f = 0; f < num_frames; ++f)
+        if (host_so[f + 1] - host_so[f] > *max_n) *max_n = host_so[f + 1] - host_so[f];
+    return FCN_OK;
+}
+
 }  // namespace fcn

@@ -427,18 +427,16 @@ struct KeWs {
     int4 *part_cnt;
     unsigned *mask;
     void *temp;
-    size_t temp_bytes, total;
+    size_t temp_bytes;
 };
 
 struct KeSizes {
     long long num_pairs, mask_words;
 };
 
-static size_t ke_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
 static int ke_nblk(int num_images) { return std::max(1, ceil_div(num_images, KE_THREADS)); }
 
-static cudaError_t ke_layout(const fcn_kitti_eval_args *a, const KeSizes &sz, char *base, KeWs &w) {
+static cudaError_t ke_layout(const fcn_kitti_eval_args *a, const KeSizes &sz, Carve &c, KeWs &w) {
     const size_t N = (size_t)a->num_images, G = (size_t)a->num_gt;
     size_t t_sort = 0, t_scan32 = 0, t_scan64 = 0;
     const int items = (int)(KE_EVALS * G);
@@ -451,33 +449,30 @@ static cudaError_t ke_layout(const fcn_kitti_eval_args *a, const KeSizes &sz, ch
     e = cub::DeviceScan::ExclusiveSum(nullptr, t_scan64, (long long *)nullptr, (long long *)nullptr, (int)N + 1);
     if (e != cudaSuccess) return e;
     w.temp_bytes = std::max(t_sort, std::max(t_scan32, t_scan64));
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += ke_align(bytes); return p; };
     const size_t parts = (size_t)KE_EVALS * KE_PTS * ke_nblk(a->num_images);
-    w.flags = (int *)take(F_COUNT * 4);
-    w.pair_cnt = (long long *)take((N + 1) * 8);
-    w.pair_off = (long long *)take((N + 1) * 8);
-    w.word_cnt = (int32_t *)take((N + 1) * 4);
-    w.word_off = (int32_t *)take((N + 1) * 4);
-    w.ov = (double *)take(3 * (size_t)sz.num_pairs * 8);
-    w.tp_cnt = (int32_t *)take(KE_EVALS * N * 4);
-    w.ngt_cnt = (int32_t *)take(KE_EVALS * N * 4);
-    w.seg_off = (int32_t *)take((KE_EVALS + 1) * 4);
-    w.scores = (double *)take(KE_EVALS * G * 8);
-    w.sorted = (double *)take(KE_EVALS * G * 8);
-    w.thresholds = (double *)take(KE_EVALS * KE_PTS * 8);
-    w.n_thr = (int32_t *)take(KE_EVALS * 4);
-    w.n_gt = (int32_t *)take(KE_EVALS * 4);
-    w.mask = (unsigned *)take((size_t)KE_EVALS * KE_PTS * (size_t)sz.mask_words * 4);
-    w.part_cnt = (int4 *)take(parts * sizeof(int4));
-    w.part_sim = (double *)take(parts * 8);
-    w.temp = take(w.temp_bytes);
-    w.total = off;
+    w.flags = (int *)c.take(F_COUNT * 4);
+    w.pair_cnt = (long long *)c.take((N + 1) * 8);
+    w.pair_off = (long long *)c.take((N + 1) * 8);
+    w.word_cnt = (int32_t *)c.take((N + 1) * 4);
+    w.word_off = (int32_t *)c.take((N + 1) * 4);
+    w.ov = (double *)c.take(3 * (size_t)sz.num_pairs * 8);
+    w.tp_cnt = (int32_t *)c.take(KE_EVALS * N * 4);
+    w.ngt_cnt = (int32_t *)c.take(KE_EVALS * N * 4);
+    w.seg_off = (int32_t *)c.take((KE_EVALS + 1) * 4);
+    w.scores = (double *)c.take(KE_EVALS * G * 8);
+    w.sorted = (double *)c.take(KE_EVALS * G * 8);
+    w.thresholds = (double *)c.take(KE_EVALS * KE_PTS * 8);
+    w.n_thr = (int32_t *)c.take(KE_EVALS * 4);
+    w.n_gt = (int32_t *)c.take(KE_EVALS * 4);
+    w.mask = (unsigned *)c.take((size_t)KE_EVALS * KE_PTS * (size_t)sz.mask_words * 4);
+    w.part_cnt = (int4 *)c.take(parts * sizeof(int4));
+    w.part_sim = (double *)c.take(parts * 8);
+    w.temp = c.take(w.temp_bytes);
     return cudaSuccess;
 }
 
-// Host-side checks shared by every entry: counts, pointers and the host copies of the offsets (which must start at
-// 0, never decrease and end at the totals).  Fills the pair and mask-word totals.
+// Host-side checks shared by every entry: counts, pointers and the host copies of the offsets.  Fills the pair and
+// mask-word totals.
 static int ke_check(const fcn_kitti_eval_args *a, const char *fn, KeSizes &sz) {
     if (a == nullptr) return invalid(fn, "NULL args");
     if (a->num_images < 0 || a->num_gt < 0 || a->num_det < 0)
@@ -488,16 +483,14 @@ static int ke_check(const fcn_kitti_eval_args *a, const char *fn, KeSizes &sz) {
     if (!a->gt_offsets || !a->det_offsets || (a->num_gt > 0 && !a->gt) || (a->num_det > 0 && !a->det))
         return invalid(fn, "NULL pointer");
     const int32_t *go = a->host_gt_offsets, *dof = a->host_det_offsets;
-    if (go[0] != 0 || dof[0] != 0) return invalid(fn, "offsets must start at 0");
+    if (!offsets_ok(go, a->num_images, a->num_gt) || !offsets_ok(dof, a->num_images, a->num_det))
+        return invalid(fn, "offsets must start at 0, must not decrease and must end at num_gt and num_det");
     long long pairs = 0, words = 0;
     for (int i = 0; i < a->num_images; ++i) {
         const long long ng = (long long)go[i + 1] - go[i], nd = (long long)dof[i + 1] - dof[i];
-        if (ng < 0 || nd < 0) return invalid(fn, "offsets must not decrease");
         pairs += ng * nd;
         words += (nd + 31) / 32;
     }
-    if (go[a->num_images] != a->num_gt || dof[a->num_images] != a->num_det)
-        return invalid(fn, "the last offsets must equal num_gt and num_det");
     sz.num_pairs = pairs;
     sz.mask_words = words;
     return FCN_OK;
@@ -507,13 +500,8 @@ static int ke_prepare(const fcn_kitti_eval_args *a, const char *fn, KeWs &w, KeS
     const int st = ke_check(a, fn, sz);
     if (st != FCN_OK) return st;
     if (!a->workspace || !a->result) return invalid(fn, "NULL workspace or result");
-    cudaError_t e = ke_layout(a, sz, nullptr, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    if (a->workspace_bytes < (long long)w.total)
-        return invalid(fn, "workspace smaller than fcn_kitti_eval_workspace_bytes()");
-    e = ke_layout(a, sz, (char *)a->workspace, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    return FCN_OK;
+    return carve_workspace(fn, "kitti_eval", a->workspace, a->workspace_bytes,
+                           [&](Carve &c) { return ke_layout(a, sz, c, w); });
 }
 
 }  // namespace fcn
@@ -524,12 +512,7 @@ extern "C" long long fcn_kitti_eval_workspace_bytes(const fcn_kitti_eval_args *a
     KeSizes sz;
     if (ke_check(a, __func__, sz) != FCN_OK) return -1;
     KeWs w;
-    const cudaError_t e = ke_layout(a, sz, nullptr, w);
-    if (e != cudaSuccess) {
-        cuda_fail(__func__, e);
-        return -1;
-    }
-    return (long long)w.total;
+    return workspace_size(__func__, [&](Carve &c) { return ke_layout(a, sz, c, w); });
 }
 
 extern "C" int fcn_kitti_eval_overlaps(const fcn_kitti_eval_args *a, fcn_stream_t stream) {

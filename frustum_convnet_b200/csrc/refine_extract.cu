@@ -247,12 +247,10 @@ struct RxWs {
     float4 *fov_pts;
     double *iou;
     void *temp;
-    size_t temp_bytes, total;
+    size_t temp_bytes;
 };
 
-static size_t rx_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-static cudaError_t rx_layout(const fcn_refine_extract_args *a, char *base, RxWs &w) {
+static cudaError_t rx_layout(const fcn_refine_extract_args *a, Carve &c, RxWs &w) {
     const size_t N = (size_t)a->num_points, J = (size_t)a->num_jobs;
     const size_t D = a->mode == FCN_REFINE_MATCHED ? (size_t)a->num_dets : 0;
     const size_t P = a->mode == FCN_REFINE_MATCHED ? (size_t)a->num_pairs : 0;
@@ -267,27 +265,23 @@ static cudaError_t rx_layout(const fcn_refine_extract_args *a, char *base, RxWs 
     if (e != cudaSuccess) return e;
     w.temp_bytes = t0 > t1 ? t0 : t1;
     w.temp_bytes = w.temp_bytes > t2 ? w.temp_bytes : t2;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += rx_align(bytes); return p; };
-    w.flags = (int32_t *)take((N + 1) * 4);
-    w.pos = (int32_t *)take((N + 1) * 4);
-    w.fov_pts = (float4 *)take(N * 16);
-    w.keep = (int32_t *)take((J + 1) * 4);
-    w.keep_pos = (int32_t *)take((J + 1) * 4);
-    w.cnt = (long long *)take((J + 1) * 8);
-    w.cnt_pos = (long long *)take((J + 1) * 8);
-    w.iou = (double *)take(P * 8);
-    w.match = (int32_t *)take(D * 4);
-    w.bad = (int32_t *)take(4);
-    w.temp = take(w.temp_bytes);
-    w.total = off;
+    w.flags = (int32_t *)c.take((N + 1) * 4);
+    w.pos = (int32_t *)c.take((N + 1) * 4);
+    w.fov_pts = (float4 *)c.take(N * 16);
+    w.keep = (int32_t *)c.take((J + 1) * 4);
+    w.keep_pos = (int32_t *)c.take((J + 1) * 4);
+    w.cnt = (long long *)c.take((J + 1) * 8);
+    w.cnt_pos = (long long *)c.take((J + 1) * 8);
+    w.iou = (double *)c.take(P * 8);
+    w.match = (int32_t *)c.take(D * 4);
+    w.bad = (int32_t *)c.take(4);
+    w.temp = c.take(w.temp_bytes);
     return cudaSuccess;
 }
 
 static bool rx_empty(const fcn_refine_extract_args *a) { return a->num_frames == 0 || a->num_jobs == 0; }
 
-// Host-side checks shared by every entry: mode, counts, pointers, the host copy of the scan offsets.  Sets *max_n to
-// the largest scan.
+// Host-side checks shared by every entry: mode, counts, pointers, the scans.  Sets *max_n to the largest scan.
 static int rx_check(const fcn_refine_extract_args *a, const char *fn, int *max_n) {
     if (a == nullptr) return invalid(fn, "NULL args");
     if (a->mode != FCN_REFINE_GT && a->mode != FCN_REFINE_MATCHED && a->mode != FCN_REFINE_DET)
@@ -301,7 +295,6 @@ static int rx_check(const fcn_refine_extract_args *a, const char *fn, int *max_n
                            "num_dets <= 2^28)");
     *max_n = 0;
     if (rx_empty(a)) return FCN_OK;
-    if (!a->host_scan_offsets) return invalid(fn, "NULL host_scan_offsets");
     if (!a->scan_offsets || !a->frames || !a->jobs || !a->job_frame || (a->num_points > 0 && !a->scans))
         return invalid(fn, "NULL pointer");
     if (a->mode != FCN_REFINE_DET && (!a->job_ref || (a->num_gt > 0 && !a->gt_boxes)))
@@ -310,15 +303,7 @@ static int rx_check(const fcn_refine_extract_args *a, const char *fn, int *max_n
         (a->num_dets == 0 || !a->det_frame || !a->gt_offsets || !a->pair_offsets ||
          (a->num_pairs > 0 && (!a->gt_corners || !a->det_corners))))
         return invalid(fn, "matched mode needs num_dets > 0 and det_frame, gt_offsets, pair_offsets and corners");
-    if (((uintptr_t)a->scans & 15) != 0) return invalid(fn, "scans must be 16-byte aligned");
-    const int32_t *so = a->host_scan_offsets;
-    if (so[0] != 0 || so[a->num_frames] != a->num_points)
-        return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
-    for (int f = 0; f < a->num_frames; ++f) {
-        if (so[f + 1] < so[f]) return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
-        if (so[f + 1] - so[f] > *max_n) *max_n = so[f + 1] - so[f];
-    }
-    return FCN_OK;
+    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, max_n);
 }
 
 static int rx_prepare(const fcn_refine_extract_args *a, const char *fn, RxWs &w, int *max_n) {
@@ -326,13 +311,8 @@ static int rx_prepare(const fcn_refine_extract_args *a, const char *fn, RxWs &w,
     if (st != FCN_OK || rx_empty(a)) return st;
     if (!a->workspace || !a->info || !a->job_points || !a->job_gt)
         return invalid(fn, "NULL workspace, info, job_points or job_gt");
-    cudaError_t e = rx_layout(a, nullptr, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    if (a->workspace_bytes < (long long)w.total)
-        return invalid(fn, "workspace smaller than fcn_refine_extract_workspace_bytes()");
-    e = rx_layout(a, (char *)a->workspace, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    return FCN_OK;
+    return carve_workspace(fn, "refine_extract", a->workspace, a->workspace_bytes,
+                           [&](Carve &c) { return rx_layout(a, c, w); });
 }
 
 }  // namespace fcn
@@ -344,12 +324,7 @@ extern "C" long long fcn_refine_extract_workspace_bytes(const fcn_refine_extract
     if (rx_check(a, __func__, &max_n) != FCN_OK) return -1;
     if (rx_empty(a)) return 0;
     RxWs w;
-    const cudaError_t e = rx_layout(a, nullptr, w);
-    if (e != cudaSuccess) {
-        cuda_fail(__func__, e);
-        return -1;
-    }
-    return (long long)w.total;
+    return workspace_size(__func__, [&](Carve &c) { return rx_layout(a, c, w); });
 }
 
 extern "C" int fcn_refine_extract_count(const fcn_refine_extract_args *a, fcn_stream_t stream) {

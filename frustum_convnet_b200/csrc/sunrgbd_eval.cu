@@ -161,12 +161,10 @@ struct SeWs {
     int32_t *cand, *vals, *sorted_det, *first, *status;
     double *keys, *sorted_keys;
     void *temp;
-    size_t temp_bytes, total;
+    size_t temp_bytes;
 };
 
-static size_t se_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-static cudaError_t se_layout(const fcn_sunrgbd_eval_args *a, char *base, SeWs &w) {
+static cudaError_t se_layout(const fcn_sunrgbd_eval_args *a, Carve &c, SeWs &w) {
     const size_t D = (size_t)a->num_det, G = (size_t)a->num_gt, C = (size_t)a->num_classes;
     w.temp_bytes = 0;
     if (a->num_det > 0) {
@@ -175,25 +173,15 @@ static cudaError_t se_layout(const fcn_sunrgbd_eval_args *a, char *base, SeWs &w
             (int32_t *)nullptr, a->num_det, a->num_classes, (const int32_t *)nullptr, (const int32_t *)nullptr);
         if (e != cudaSuccess) return e;
     }
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += se_align(bytes); return p; };
-    w.cand = (int32_t *)take(D * 4);
-    w.vals = (int32_t *)take(D * 4);
-    w.sorted_det = (int32_t *)take(D * 4);
-    w.keys = (double *)take(D * 8);
-    w.sorted_keys = (double *)take(D * 8);
-    w.first = (int32_t *)take(G * 4);
-    w.status = (int32_t *)take(C * 4);
-    w.temp = take(w.temp_bytes);
-    w.total = off;
+    w.cand = (int32_t *)c.take(D * 4);
+    w.vals = (int32_t *)c.take(D * 4);
+    w.sorted_det = (int32_t *)c.take(D * 4);
+    w.keys = (double *)c.take(D * 8);
+    w.sorted_keys = (double *)c.take(D * 8);
+    w.first = (int32_t *)c.take(G * 4);
+    w.status = (int32_t *)c.take(C * 4);
+    w.temp = c.take(w.temp_bytes);
     return cudaSuccess;
-}
-
-static int se_offsets_ok(const int32_t *o, int n, int total) {
-    if (o[0] != 0) return 0;
-    for (int i = 0; i < n; ++i)
-        if (o[i + 1] < o[i]) return 0;
-    return o[n] == total;
 }
 
 // Host-side checks shared by every entry: counts, pointers and the host copies of the offsets.
@@ -211,8 +199,8 @@ static int se_check(const fcn_sunrgbd_eval_args *a, const char *fn) {
         (a->num_det > 0 && (!a->det_corners || !a->det_scores || !a->det_segments)))
         return invalid(fn, "NULL pointer");
     const int32_t *so = a->host_gt_segment_offsets, *gc = a->host_gt_class_offsets, *dc = a->host_det_class_offsets;
-    if (!se_offsets_ok(so, a->num_gt_segments, a->num_gt) || !se_offsets_ok(gc, a->num_classes, a->num_gt) ||
-        !se_offsets_ok(dc, a->num_classes, a->num_det))
+    if (!offsets_ok(so, a->num_gt_segments, a->num_gt) || !offsets_ok(gc, a->num_classes, a->num_gt) ||
+        !offsets_ok(dc, a->num_classes, a->num_det))
         return invalid(fn, "offsets must start at 0, never decrease and end at num_gt / num_det");
     for (int c = 0, s = 0; c <= a->num_classes; ++c) {          // every class boundary is a segment boundary
         while (s < a->num_gt_segments && so[s] < gc[c]) ++s;
@@ -226,13 +214,8 @@ static int se_prepare(const fcn_sunrgbd_eval_args *a, const char *fn, SeWs &w) {
     if (st != FCN_OK) return st;
     if (!a->workspace || !a->result || (a->num_det > 0 && (!a->rec || !a->prec)))
         return invalid(fn, "NULL workspace or output");
-    cudaError_t e = se_layout(a, nullptr, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    if (a->workspace_bytes < (long long)w.total)
-        return invalid(fn, "workspace smaller than fcn_sunrgbd_eval_workspace_bytes()");
-    e = se_layout(a, (char *)a->workspace, w);
-    if (e != cudaSuccess) return cuda_fail(fn, e);
-    return FCN_OK;
+    return carve_workspace(fn, "sunrgbd_eval", a->workspace, a->workspace_bytes,
+                           [&](Carve &c) { return se_layout(a, c, w); });
 }
 
 }  // namespace fcn
@@ -242,12 +225,7 @@ using namespace fcn;
 extern "C" long long fcn_sunrgbd_eval_workspace_bytes(const fcn_sunrgbd_eval_args *a) {
     if (se_check(a, __func__) != FCN_OK) return -1;
     SeWs w;
-    const cudaError_t e = se_layout(a, nullptr, w);
-    if (e != cudaSuccess) {
-        cuda_fail(__func__, e);
-        return -1;
-    }
-    return (long long)w.total;
+    return workspace_size(__func__, [&](Carve &c) { return se_layout(a, c, w); });
 }
 
 extern "C" int fcn_sunrgbd_eval_match(const fcn_sunrgbd_eval_args *a, fcn_stream_t stream) {

@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._host import cuda_device, workspace
 
 _DATASETS = {"KITTI": 0, "SUNRGBD": 1}
 _METHODS = {"nms": 0}          # every other cfg.TEST.METHOD behaves as 'top' (test_net_det.py:256-263)
@@ -36,9 +37,7 @@ class DetectionCollector:
         self.dataset, self.method = dataset, ("nms" if method == "nms" else "top")
         self.thresh, self.top_k = float(thresh), int(top_k)
         self.num_frustums = n
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        if self.device.type != "cuda":
-            raise RuntimeError("DetectionCollector: a CUDA device is required (there is no CPU fallback)")
+        self.device = cuda_device(device, "DetectionCollector")
         # segment table in the reference's dict order: images by first appearance, classes by first appearance
         # within the image (test_net_det.py:278-282)
         seg_of, self.segments = {}, []
@@ -120,10 +119,7 @@ class DetectionCollector:
                 cur.wait_stream(st)
         S = len(self.segments)
         with torch.cuda.device(dev):
-            nbytes = _lib.load().fcn_det_workspace_bytes(self.capacity, S)
-            if nbytes < 0:
-                _lib.check(-1, "fcn_det_workspace_bytes")
-            ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+            ws, nbytes = workspace("fcn_det_workspace_bytes", dev, self.capacity, S)
             info = torch.zeros(4, dtype=torch.int64, device=dev)
             off = torch.zeros(S + 1, dtype=torch.int32, device=dev)
             kc = torch.zeros(max(S, 1), dtype=torch.int32, device=dev)
@@ -133,7 +129,7 @@ class DetectionCollector:
             a.method, a.dataset = _METHODS.get(self.method, 1), _DATASETS[self.dataset]
             a.top_k, a.thresh = self.top_k, self.thresh
             a.counter, a.records, a.box2d = self.counter.data_ptr(), self.records.data_ptr(), self.box2d.data_ptr()
-            a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), int(nbytes), info.data_ptr()
+            a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), nbytes, info.data_ptr()
             a.seg_offsets, a.keep_count, a.rows = off.data_ptr(), kc.data_ptr(), rows.data_ptr()
             _lib.call("fcn_det_prepare", C.byref(a), cur.cuda_stream)
             n_counted, mask_words = (int(v) for v in info[:2].tolist())          # the one host sync

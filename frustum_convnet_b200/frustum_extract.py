@@ -24,6 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._host import csr_offsets, cuda_device, on_device, upload, workspace
 
 DET_ID2STR = {1: "Pedestrian", 2: "Car", 3: "Cyclist"}
 
@@ -62,13 +63,6 @@ class Frustums:
         return len(self.id_list)
 
 
-def on_device(t, dev):
-    """t is a CUDA tensor on dev ('cuda' without an index: the current device)."""
-    if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        return False
-    return t.device.index == (dev.index if dev.index is not None else torch.cuda.current_device())
-
-
 def _frame_record(calib, hw):
     f = _lib.FrustumFrame()
     for name, key, n in (("P", "P2", 12), ("V2C", "Tr_velo_to_cam", 12), ("R0", "R0_rect", 9)):
@@ -83,24 +77,54 @@ def _frame_record(calib, hw):
     return f
 
 
+def _scan(scan, dev, who):
+    if isinstance(scan, torch.Tensor):
+        if not on_device(scan, dev):
+            raise RuntimeError("%s: scans must be numpy arrays or CUDA tensors on %s" % (who, dev))
+        if scan.dtype != torch.float32 or scan.dim() != 2 or scan.shape[1] != 4:
+            raise ValueError("a scan must be an (n, 4) float32 array")
+        return scan
+    a = np.asarray(scan)
+    if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
+        raise ValueError("a scan must be an (n, 4) float32 array")
+    return a
+
+
+def scan_table(scans, calibs, image_hw, frame_ids, dev, who):
+    """The frames of both extractors (this module's and refine_extract's), in frame_ids order, checked on the host
+    -> (their scans, the fcn_frustum_frame array, the host scan offsets)."""
+    sc = [_scan(scans[k], dev, who) for k in frame_ids]
+    frames = (_lib.FrustumFrame * len(frame_ids))(*[_frame_record(calibs[k], image_hw[k]) for k in frame_ids])
+    return sc, frames, csr_offsets([s.shape[0] for s in sc])
+
+
+def upload_scans(sc, dev):
+    """scan_table's scans -> one (N, 4) float32 tensor on dev."""
+    if all(isinstance(s, np.ndarray) for s in sc):
+        return torch.from_numpy(np.concatenate(sc)).to(dev)
+    return torch.cat([s if isinstance(s, torch.Tensor) else torch.from_numpy(s).to(dev) for s in sc]).contiguous()
+
+
+def read_counts(summary, n, who, bad_what):
+    """The count pass's summary, read back once (the extraction's one host sync): int64 info (K kept records, M
+    points, bad references, -), then int32 words, the first n of them each record's point count (-1: dropped).
+    -> (K, M, the int32 words, the kept records)."""
+    back = summary.cpu().numpy()
+    K, M, bad = int(back[0]), int(back[1]), int(back[2])
+    if bad:
+        raise RuntimeError("%s: %d %s" % (who, bad, bad_what))
+    if M >= 2 ** 31:
+        raise RuntimeError("%s: %d frustum points do not fit int32 offsets" % (who, M))
+    words = back[4:].view(np.int32)
+    kept = np.flatnonzero(words[:n] >= 0)
+    assert len(kept) == K and int(words[kept].sum()) == M
+    return K, M, words, kept
+
+
 class FrustumExtractor:
     def __init__(self, type_whitelist=("Car",), device=None):
         self.type_whitelist = tuple(type_whitelist)
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        if self.device.type != "cuda":
-            raise RuntimeError("FrustumExtractor: a CUDA device is required (there is no CPU fallback)")
-
-    def _scan(self, scan):
-        if isinstance(scan, torch.Tensor):
-            if not on_device(scan, self.device):
-                raise RuntimeError("FrustumExtractor: scans must be numpy arrays or CUDA tensors on %s" % self.device)
-            if scan.dtype != torch.float32 or scan.dim() != 2 or scan.shape[1] != 4:
-                raise ValueError("a scan must be an (n, 4) float32 array")
-            return scan
-        a = np.asarray(scan)
-        if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
-            raise ValueError("a scan must be an (n, 4) float32 array")
-        return a
+        self.device = cuda_device(device, "FrustumExtractor")
 
     def extract(self, scans, calibs, image_hw, id_list, type_list, prob_list, box2d_list, stream=None, timer=None):
         """-> Frustums.  Runs on `stream` (default: the current stream of the extractor's device).  `timer(name)`
@@ -119,11 +143,8 @@ class FrustumExtractor:
         if not np.isfinite(boxes).all():
             raise ValueError("2-D boxes must be finite")
         det_frame = np.array([frame_of[id_list[i]] for i in lines], dtype=np.int32)
-        sc = [self._scan(scans[k]) for k in frame_ids]
-        frames = (_lib.FrustumFrame * len(frame_ids))(*[_frame_record(calibs[k], image_hw[k]) for k in frame_ids])
-        so = np.zeros(len(frame_ids) + 1, dtype=np.int32)
-        np.cumsum([s.shape[0] for s in sc], out=so[1:])
         dev = self.device
+        sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "FrustumExtractor")
         F, D, N = len(frame_ids), len(lines), int(so[-1])
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
@@ -132,47 +153,23 @@ class FrustumExtractor:
                                     torch.zeros(1, dtype=torch.int32, device=dev), *self._empty(dev),
                                     np.zeros(0, np.int64), [], id_list, type_list, prob_list, box2d_list, calibs,
                                     image_hw)
-            if all(isinstance(s, np.ndarray) for s in sc):
-                scan_dev = torch.from_numpy(np.concatenate(sc)).to(dev)
-            else:
-                scan_dev = torch.cat([s if isinstance(s, torch.Tensor) else torch.from_numpy(s).to(dev)
-                                      for s in sc]).contiguous()
-            # one host buffer: frames | boxes (D*4 f64) | scan offsets (F+1 i32) | det frames (D i32)
-            nb = [C.sizeof(frames), D * 32, (F + 1) * 4, D * 4]
-            o = np.cumsum([0] + nb)
-            hbuf = np.empty(int(o[-1]), dtype=np.uint8)
-            hbuf[o[0]:o[1]] = np.frombuffer(bytes(frames), dtype=np.uint8)
-            hbuf[o[1]:o[2]] = boxes.view(np.uint8).reshape(-1)
-            hbuf[o[2]:o[3]] = so.view(np.uint8)
-            hbuf[o[3]:o[4]] = det_frame.view(np.uint8)
-            inp = torch.from_numpy(hbuf).to(dev)
+            scan_dev = upload_scans(sc, dev)
+            inp, ptrs = upload([bytes(frames), boxes, so, det_frame], dev)
             a = _lib.FrustumExtractArgs()
             a.num_frames, a.num_points, a.num_dets = F, N, D
             a.scans = scan_dev.data_ptr() if N > 0 else None
-            ib = inp.data_ptr()
-            a.frames, a.boxes, a.scan_offsets, a.det_frame = (ib + int(v) for v in o[:4])
+            a.frames, a.boxes, a.scan_offsets, a.det_frame = ptrs
             a.host_scan_offsets = so.ctypes.data
-            nbytes = _lib.load().fcn_frustum_extract_workspace_bytes(C.byref(a))
-            if nbytes < 0:
-                _lib.check(-1, "fcn_frustum_extract_workspace_bytes")
-            ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
+            ws, nbytes = workspace("fcn_frustum_extract_workspace_bytes", dev, C.byref(a))
             summary = torch.empty(4 + (D + 1) // 2, dtype=torch.int64, device=dev)    # info | det_points
-            a.workspace, a.workspace_bytes = ws.data_ptr(), int(nbytes)
+            a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
             a.info, a.det_points = summary.data_ptr(), summary.data_ptr() + 32
             if timer is not None:
                 timer("start")
             _lib.call("fcn_frustum_extract_count", C.byref(a), stream.cuda_stream)
             if timer is not None:
                 timer("count")
-            back = summary.cpu().numpy()                                     # the one host sync
-            K, M, bad = int(back[0]), int(back[1]), int(back[2])
-            if bad:
-                raise RuntimeError("fcn_frustum_extract: %d detections reference no frame" % bad)
-            if M >= 2 ** 31:
-                raise RuntimeError("fcn_frustum_extract: %d frustum points do not fit int32 offsets" % M)
-            det_points = back[4:].view(np.int32)[:D]
-            kept = np.flatnonzero(det_points >= 0)
-            assert len(kept) == K and int(det_points[kept].sum()) == M
+            K, M, det_points, kept = read_counts(summary, D, "fcn_frustum_extract", "detections reference no frame")
             points = torch.empty((M, 4), dtype=torch.float32, device=dev)
             offsets = torch.empty(K + 1, dtype=torch.int32, device=dev)
             angle = torch.empty(K, dtype=torch.float64, device=dev)

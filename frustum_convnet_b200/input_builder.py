@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._host import on_device
 
 
 class FrustumBatchBuilder:
@@ -44,7 +45,6 @@ class FrustumBatchBuilder:
         round trip: points (M, 4 or 3) float32, offsets (B + 1) int32, frustum_angle (B) float64, box2d (B, 4) and
         P (B, 12) float64; cls_index (B) int32 (CUDA tensor or host values) or None.  Every frustum must hold at least
         one point (the extractor drops empty ones; this is not checked here, as that would need the host)."""
-        from .frustum_extract import on_device
         dev = self.device
         for name, t, dt, cols in (("points", points, torch.float32, (3, 4)), ("offsets", offsets, torch.int32, None),
                                   ("frustum_angle", frustum_angle, torch.float64, None),

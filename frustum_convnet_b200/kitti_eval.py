@@ -24,6 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._host import csr_offsets, cuda_device, workspace
 
 CLASS_NAMES = ("car", "pedestrian", "cyclist")
 METRICS = ("image", "ground", "3d")
@@ -92,12 +93,6 @@ def detection_records(dets, class_type):
     return out
 
 
-def _offsets(counts):
-    off = np.zeros(len(counts) + 1, dtype=np.int32)
-    np.cumsum(counts, out=off[1:])
-    return off
-
-
 class KittiGroundTruth:
     """label_2 records of a list of images, parsed once and kept on the device."""
 
@@ -107,12 +102,10 @@ class KittiGroundTruth:
             raise ValueError("image_ids must be unique")
         if len(records) != len(self.image_ids):
             raise ValueError("one record array per image is required")
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        if self.device.type != "cuda":
-            raise RuntimeError("KittiGroundTruth: a CUDA device is required (there is no CPU fallback)")
+        self.device = cuda_device(device, "KittiGroundTruth")
         self.records = [np.asarray(r, dtype=np.float64).reshape(-1, GT_COLS) for r in records]
         self.index = {idx: i for i, idx in enumerate(self.image_ids)}
-        self.host_offsets = _offsets([len(r) for r in self.records])
+        self.host_offsets = csr_offsets([len(r) for r in self.records])
         flat = np.concatenate(self.records) if self.records else np.zeros((0, GT_COLS))
         self.gt = torch.from_numpy(np.ascontiguousarray(flat)).to(self.device)
         self.offsets = torch.from_numpy(self.host_offsets).to(self.device)
@@ -211,7 +204,7 @@ class KittiEvaluator:
             raise ValueError("one detection record array per ground-truth image is required")
         dev = self.device
         det_records = [np.asarray(r, dtype=np.float64).reshape(-1, DET_COLS) for r in det_records]
-        host_det_off = _offsets([len(r) for r in det_records])
+        host_det_off = csr_offsets([len(r) for r in det_records])
         flat = np.concatenate(det_records) if det_records else np.zeros((0, DET_COLS))
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
@@ -223,12 +216,9 @@ class KittiEvaluator:
             a.gt_offsets, a.det_offsets = self.gt.offsets.data_ptr(), det_off.data_ptr()
             a.host_gt_offsets = self.gt.host_offsets.ctypes.data
             a.host_det_offsets = host_det_off.ctypes.data
-            nbytes = _lib.load().fcn_kitti_eval_workspace_bytes(C.byref(a))
-            if nbytes < 0:
-                _lib.check(-1, "fcn_kitti_eval_workspace_bytes")
-            ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+            ws, nbytes = workspace("fcn_kitti_eval_workspace_bytes", dev, C.byref(a))
             res = torch.zeros(C.sizeof(_lib.KittiEvalResult), dtype=torch.uint8, device=dev)   # + tail padding
-            a.workspace, a.workspace_bytes, a.result = ws.data_ptr(), int(nbytes), res.data_ptr()
+            a.workspace, a.workspace_bytes, a.result = ws.data_ptr(), nbytes, res.data_ptr()
             if timer is not None:
                 timer("start")
             for name in ("fcn_kitti_eval_overlaps", "fcn_kitti_eval_thresholds", "fcn_kitti_eval_statistics"):

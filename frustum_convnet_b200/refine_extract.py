@@ -44,7 +44,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .frustum_extract import _frame_record, on_device
+from ._host import csr_offsets, cuda_device, upload, workspace
+from .frustum_extract import read_counts, scan_table, upload_scans
 from .kitti_eval import detection_records
 
 RATIO = 1.2                # the enlargement of every box that cuts points (prepare_data_refine.py:319, :489, :724)
@@ -307,9 +308,7 @@ class RefineFrustums:
 class RefineFrustumExtractor:
     def __init__(self, type_whitelist=("Car",), device=None):
         self.type_whitelist = tuple(type_whitelist)
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        if self.device.type != "cuda":
-            raise RuntimeError("RefineFrustumExtractor: a CUDA device is required (there is no CPU fallback)")
+        self.device = cuda_device(device, "RefineFrustumExtractor")
 
     # ------------------------------------------------------------------ public modes
     def from_ground_truth(self, scans, calibs, image_hw, image_ids, gt, perturb=False, augment=1, rng=np.random,
@@ -349,19 +348,6 @@ class RefineFrustumExtractor:
             dets = objects_from_detections(dets)
         return {int(i): list(dets.get(int(i), [])) for i in image_ids}
 
-    def _scan(self, scan):
-        if isinstance(scan, torch.Tensor):
-            if not on_device(scan, self.device):
-                raise RuntimeError("RefineFrustumExtractor: scans must be numpy arrays or CUDA tensors on %s"
-                                   % self.device)
-            if scan.dtype != torch.float32 or scan.dim() != 2 or scan.shape[1] != 4:
-                raise ValueError("a scan must be an (n, 4) float32 array")
-            return scan
-        a = np.asarray(scan)
-        if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
-            raise ValueError("a scan must be an (n, 4) float32 array")
-        return a
-
     # ------------------------------------------------------------------ device call
     def _run(self, mode, scans, calibs, image_hw, jobs, gts, stream, timer):
         dev = self.device
@@ -384,16 +370,8 @@ class RefineFrustumExtractor:
                                     None if mode == _lib.REFINE_DET else torch.zeros(0, dtype=torch.uint8, device=dev),
                                     np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, np.int64), jobs,
                                     gt_flat, calibs, stream)
-            sc = [self._scan(scans[k]) for k in frame_ids]
-            if all(isinstance(s, np.ndarray) for s in sc):
-                scan_dev = torch.from_numpy(np.concatenate(sc)).to(dev)
-            else:
-                scan_dev = torch.cat([s if isinstance(s, torch.Tensor) else torch.from_numpy(s).to(dev)
-                                      for s in sc]).contiguous()
-            frames = (_lib.FrustumFrame * F)(*[_frame_record(calibs[k], image_hw[k]) for k in frame_ids])
-            so = np.zeros(F + 1, dtype=np.int32)
-            np.cumsum([s.shape[0] for s in sc], out=so[1:])
-            N = int(so[-1])
+            sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "RefineFrustumExtractor")
+            scan_dev, N = upload_scans(sc, dev), int(so[-1])
             job_box = np.array([box_record(jb["cut"]) for jb in jobs], dtype=np.dtype(_lib.RefineBox))
             job_frame = np.array([fpos[jb["frame"]] for jb in jobs], dtype=np.int32)
             gt_box = np.array([box_record(obj_array(o)) for o in gt_flat], dtype=np.dtype(_lib.RefineBox))
@@ -403,57 +381,38 @@ class RefineFrustumExtractor:
                 job_ref = np.arange(J, dtype=np.int32)                 # one job per detection
             else:
                 job_ref = np.zeros(J, dtype=np.int32)
-            parts = [bytes(frames), job_box.tobytes(), so.tobytes(), job_frame.tobytes(), job_ref.tobytes(),
-                     gt_box.tobytes()]
+            parts = [bytes(frames), job_box, so, job_frame, job_ref, gt_box]
             D = P = 0
             if mode == _lib.REFINE_MATCHED:
                 D = J
-                ngt = np.array([gt_off[f + 1] - gt_off[f] for f in job_frame], dtype=np.int64)
-                po = np.zeros(D + 1, dtype=np.int32)
-                np.cumsum(ngt, out=po[1:])
+                po = csr_offsets([gt_off[f + 1] - gt_off[f] for f in job_frame])
                 P = int(po[-1])
                 det_c = iou_corners(np.stack([jb["box"] for jb in jobs]))
                 gt_c = iou_corners(np.stack([obj_array(o) for o in gt_flat]))
-                parts += [det_c.tobytes(), gt_c.tobytes(), np.asarray(gt_off, np.int32).tobytes(), po.tobytes()]
-            nb = [len(p) for p in parts]
-            o = np.cumsum([0] + [(n + 255) // 256 * 256 for n in nb])
-            hbuf = np.zeros(int(o[-1]), dtype=np.uint8)
-            for p, start in zip(parts, o):
-                hbuf[start:start + len(p)] = np.frombuffer(p, dtype=np.uint8)
-            inp = torch.from_numpy(hbuf).to(dev)
-            ib = inp.data_ptr()
+                parts += [det_c, gt_c, np.asarray(gt_off, np.int32), po]
+            inp, ptrs = upload(parts, dev)
             a = _lib.RefineExtractArgs()
             a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, F, N, J, G
             a.num_dets, a.num_pairs, a.iou_thresh = D, P, self.iou_thresh
             a.scans = scan_dev.data_ptr() if N > 0 else None
-            a.frames, a.jobs, a.scan_offsets, a.job_frame, a.job_ref = (ib + int(v) for v in o[:5])
-            a.gt_boxes = ib + int(o[5]) if G > 0 else None
+            a.frames, a.jobs, a.scan_offsets, a.job_frame, a.job_ref = ptrs[:5]
+            a.gt_boxes = ptrs[5] if G > 0 else None
             if mode == _lib.REFINE_MATCHED:
                 a.det_frame = a.job_frame
-                a.det_corners, a.gt_corners, a.gt_offsets, a.pair_offsets = (ib + int(v) for v in o[6:10])
+                a.det_corners, a.gt_corners, a.gt_offsets, a.pair_offsets = ptrs[6:10]
             a.host_scan_offsets = so.ctypes.data
-            nbytes = _lib.load().fcn_refine_extract_workspace_bytes(C.byref(a))
-            if nbytes < 0:
-                _lib.check(-1, "fcn_refine_extract_workspace_bytes")
-            ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
+            ws, nbytes = workspace("fcn_refine_extract_workspace_bytes", dev, C.byref(a))
             summary = torch.empty(4 + J, dtype=torch.int64, device=dev)   # info | job_points | job_gt (int32 each)
-            a.workspace, a.workspace_bytes = ws.data_ptr(), int(nbytes)
+            a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
             a.info, a.job_points, a.job_gt = summary.data_ptr(), summary.data_ptr() + 32, summary.data_ptr() + 32 + 4 * J
             if timer is not None:
                 timer("start")
             _lib.call("fcn_refine_extract_count", C.byref(a), stream.cuda_stream)
             if timer is not None:
                 timer("count")
-            back = summary.cpu().numpy()                                       # the one host sync
-            K, M, bad = int(back[0]), int(back[1]), int(back[2])
-            if bad:
-                raise RuntimeError("fcn_refine_extract: %d jobs or pairs reference no frame or box" % bad)
-            if M >= 2 ** 31:
-                raise RuntimeError("fcn_refine_extract: %d frustum points do not fit int32 offsets" % M)
-            job_points = back[4:].view(np.int32)[:J]
-            job_gt = back[4:].view(np.int32)[J:2 * J]
-            kept = np.flatnonzero(job_points >= 0)
-            assert len(kept) == K and int(job_points[kept].sum()) == M
+            K, M, words, kept = read_counts(summary, J, "fcn_refine_extract",
+                                            "jobs or pairs reference no frame or box")
+            job_points, job_gt = words[:J], words[J:2 * J]
             if mode == _lib.REFINE_MATCHED:
                 check_matched_extents(jobs, gt_flat, job_gt)
             points = torch.empty((M, 4), dtype=torch.float32, device=dev)

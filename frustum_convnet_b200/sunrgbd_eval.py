@@ -35,6 +35,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._host import csr_offsets, cuda_device, upload, workspace
 
 CLASS_NAMES = ("bed", "table", "sofa", "chair", "toilet", "desk", "dresser", "night_stand", "bookshelf", "bathtub")
 _RES = C.sizeof(_lib.SunrgbdEvalResult)
@@ -100,12 +101,6 @@ def det_corners(rows):
     return out
 
 
-def _offsets(counts):
-    off = np.zeros(len(counts) + 1, dtype=np.int32)
-    np.cumsum(counts, out=off[1:])
-    return off
-
-
 class SunrgbdGroundTruth:
     """The ground truth of every class, converted once and kept on the device: rows grouped per class, and within a
     class per image (in file order, so the first of two equal overlaps wins as in the reference).
@@ -115,9 +110,7 @@ class SunrgbdGroundTruth:
     nor in the ground truth raises KeyError (a mismatched id map); without it every integral id is accepted."""
 
     def __init__(self, gt, image_ids=None, device=None):
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        if self.device.type != "cuda":
-            raise RuntimeError("SunrgbdGroundTruth: a CUDA device is required (there is no CPU fallback)")
+        self.device = cuda_device(device, "SunrgbdGroundTruth")
         self.classes = tuple(gt)
         if len(self.classes) > _lib.SUNRGBD_MAX_CLASSES:
             raise ValueError("at most %d classes" % _lib.SUNRGBD_MAX_CLASSES)
@@ -142,8 +135,8 @@ class SunrgbdGroundTruth:
             cls_counts.append(len(cor))
         self.known_images = (None if image_ids is None else
                              {k for (_, k) in self.segment_of} | {image_key(i) for i in image_ids})
-        self.host_segment_offsets = _offsets(seg_counts)
-        self.host_class_offsets = _offsets(cls_counts)
+        self.host_segment_offsets = csr_offsets(seg_counts)
+        self.host_class_offsets = csr_offsets(cls_counts)
         self.num_gt = int(self.host_class_offsets[-1])
         self.num_segments = len(seg_counts)
         flat = np.concatenate(corners) if corners else np.zeros((0, 8, 3))
@@ -243,36 +236,25 @@ class SunrgbdEvaluator:
             raise ValueError("detection corners must be finite")
         gt, dev = self.gt, self.device
         D, Cn = len(scores), len(gt.classes)
-        det_off = _offsets(counts)
-        # one host buffer: corners (D*24 f64) | scores (D f64) | segments (D i32) | class offsets (Cn+1 i32)
-        nb = [D * 192, D * 8, D * 4, (Cn + 1) * 4]
-        host = np.empty(sum(nb), dtype=np.uint8)
-        o = np.cumsum([0] + nb)
-        host[o[0]:o[1]] = np.ascontiguousarray(corners, dtype=np.float64).reshape(-1).view(np.uint8)
-        host[o[1]:o[2]] = np.ascontiguousarray(scores, dtype=np.float64).view(np.uint8)
-        host[o[2]:o[3]] = np.ascontiguousarray(seg, dtype=np.int32).view(np.uint8)
-        host[o[3]:o[4]] = det_off.view(np.uint8)
+        det_off = csr_offsets(counts)
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
-            buf = torch.from_numpy(host).to(dev)
-            base = buf.data_ptr()
+            buf, ptrs = upload([np.asarray(corners, np.float64), np.asarray(scores, np.float64),
+                                np.asarray(seg, np.int32), det_off], dev)
             a = _lib.SunrgbdEvalArgs()
             a.num_classes, a.num_gt, a.num_gt_segments, a.num_det = Cn, gt.num_gt, gt.num_segments, D
             a.ovthresh = float(ovthresh)
             a.gt_corners, a.gt_segment_offsets, a.gt_class_offsets = (gt.corners.data_ptr(),
                                                                       gt.segment_offsets.data_ptr(),
                                                                       gt.class_offsets.data_ptr())
-            a.det_corners, a.det_scores, a.det_segments, a.det_class_offsets = (base + int(v) for v in o[:4])
+            a.det_corners, a.det_scores, a.det_segments, a.det_class_offsets = ptrs
             a.host_gt_segment_offsets = gt.host_segment_offsets.ctypes.data
             a.host_gt_class_offsets = gt.host_class_offsets.ctypes.data
             a.host_det_class_offsets = det_off.ctypes.data
-            nbytes = _lib.load().fcn_sunrgbd_eval_workspace_bytes(C.byref(a))
-            if nbytes < 0:
-                _lib.check(-1, "fcn_sunrgbd_eval_workspace_bytes")
-            ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
+            ws, nbytes = workspace("fcn_sunrgbd_eval_workspace_bytes", dev, C.byref(a))
             out = torch.zeros(Cn * _RES + 16 * D, dtype=torch.uint8, device=dev)     # results | rec | prec
             ob = out.data_ptr()
-            a.workspace, a.workspace_bytes = ws.data_ptr(), int(nbytes)
+            a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
             a.result, a.rec, a.prec = ob, ob + Cn * _RES, ob + Cn * _RES + 8 * D
             if timer is not None:
                 timer("start")
