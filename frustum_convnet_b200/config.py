@@ -18,6 +18,7 @@ from __future__ import annotations
 import ast
 import copy
 import os
+from typing import List, NamedTuple
 
 import numpy as np
 import yaml
@@ -152,22 +153,51 @@ DATASET_INFO = {"KITTI": _Category(_KITTI_CLASSES, _KITTI_MEAN),
 class ArchSpec:
     """Static shape description of one PointNetDet variant."""
 
-    def __init__(self, name, nsample, mlps, block1_out, reg_in):
+    def __init__(self, name, nsample, mlps, block1_out, reg_in, block_widths=(), deconv_out=256):
         self.name = name
         self.nsample = tuple(nsample)       # K per scale
         self.mlps = tuple(tuple(m) for m in mlps)  # (C1,C2,C3) per scale
         self.num_scales = len(nsample)
         self.block1_out = block1_out        # ConvFeatNet block1_conv1 width
         self.reg_in = reg_in                # channels entering the heads
+        self.block_widths = tuple(block_widths)   # ConvFeatNet blocks 2..S: conv1 / conv2 / merge width
+        self.deconv_out = deconv_out        # width of every transposed conv = its slice of the heads' concat
 
 
 ARCH_KITTI = ArchSpec("kitti", (32, 64, 64, 128),
                       ((64, 64, 128), (64, 64, 128), (128, 128, 256), (256, 256, 512)),
-                      128, 768)
+                      128, 768, (128, 256, 512))
 ARCH_SUNRGBD = ArchSpec("sunrgbd", (128, 128, 256, 256, 256),
                         ((64, 64, 128), (64, 64, 128), (128, 128, 256), (256, 256, 512),
                          (256, 256, 512)),
-                        64, 1024)
+                        64, 1024, (128, 256, 512, 512))
+
+
+class FcnLayer(NamedTuple):
+    """One layer of ConvFeatNet + heads.  Every consumer reads the graph from these fields, never from a name."""
+    name: str       # state-dict name under ``conv_net.``; "heads" stands for cls_out + reg_out
+    kind: str       # "conv" (k=3, padding 1) | "merge" (1x1 over [block output, pooled feature]) | "deconv" | "heads"
+    srcs: tuple     # ((producer, channels), ...) in K order; a producer is a layer name or "feat<i>" (PointNet scale i)
+    Cout: int       # None for the heads: their width is set by the dataset's regression size
+    k: int
+    stride: int
+    level: int      # pyramid level (0-based scale) of the output positions; the concat and the heads are at level 1
+    c_off: int = 0  # deconv: first column of its output in the concat
+
+
+def fcn_layers(arch: ArchSpec, num_vec: int) -> List[FcnLayer]:
+    """ConvFeatNet + heads in reference order (det_base.py:167-183,196-224,367-368; det_base_sunrgbd.py:178-200)."""
+    S, V, D = arch.num_scales, num_vec, arch.deconv_out
+    L = [FcnLayer("block1_conv1", "conv", (("feat1", arch.mlps[0][2] + V),), arch.block1_out, 3, 1, 0)]
+    for i, w in enumerate(arch.block_widths, 2):
+        c1, c2 = "block%d_conv1" % i, "block%d_conv2" % i
+        L += [FcnLayer(c1, "conv", ((L[-1].name, L[-1].Cout),), w, 3, 2, i - 1),
+              FcnLayer(c2, "conv", ((c1, w),), w, 3, 1, i - 1),
+              FcnLayer("block%d_merge" % i, "merge", ((c2, w), ("feat%d" % i, arch.mlps[i - 1][2] + V)), w, 1, 1, i - 1)]
+    merges = [m for m in L if m.kind == "merge"]
+    deconvs = [FcnLayer("block%d_deconv" % (j + 2), "deconv", ((m.name, m.Cout),), D, 2 ** j, 2 ** j, 1, D * j)
+               for j, m in enumerate(merges)]
+    return L + deconvs + [FcnLayer("heads", "heads", tuple((d.name, D) for d in deconvs), None, 1, 1, 1)]
 
 
 # Named workloads of BASELINE.json `configs` -> (yaml, dataset, num_vec, arch)

@@ -25,8 +25,8 @@ import torch
 
 from . import _lib
 from . import mega as _mega
-from .config import DATASET_INFO, ArchSpec
-from .synth import fcn_layer_table, reg_out_size
+from .config import DATASET_INFO, ArchSpec, fcn_layers
+from .synth import reg_out_size
 
 BN_EPS = 1e-5
 
@@ -64,13 +64,18 @@ def _fold_bn(sd, prefix) -> Tuple[torch.Tensor, torch.Tensor]:
     return s, b - m * s
 
 
+def _out_map(L) -> str:
+    """Activation map an FCN layer writes: its own, the concat (transposed convs) or the logits (heads)."""
+    return {"deconv": "cat", "heads": "logits"}.get(L.kind, L.name)
+
+
 class _ConvLayer:
     """One fcn_conv_gemm call: packed weights + symbolic segment/output description.
     `wt` / `bias` arrive as HOST tensors (BN folded in float64 on the CPU: one upload per operand instead of
     ~900 tiny device launches per pack); the device copies are made here."""
 
-    def __init__(self, name, segs, K_pad, n_cols, Cout, up, relu, wt, bias, out, c_off, device):
-        self.name, self.segs, self.K_pad, self.n_cols = name, segs, K_pad, n_cols
+    def __init__(self, name, kind, segs, K_pad, n_cols, Cout, up, relu, wt, bias, out, c_off, device):
+        self.name, self.kind, self.segs, self.K_pad, self.n_cols = name, kind, segs, K_pad, n_cols
         self.Cout, self.up, self.relu = Cout, up, relu
         self.out, self.c_off, self.device = out, c_off, device
         if K_pad % 64:   # tensor-core stages are 64 K elements wide: one extra all-zero K block
@@ -161,74 +166,45 @@ class FrustumEngine:
                 if self.precision == 1 and j >= 2:
                     lay["w%d_tc" % j] = pack_sw128(wf, min(c2, 128) if j == 2 else 128).to(dev)
             self.pn.append(lay)
-        S, V = self.arch.num_scales, self.num_vec
-        widths = (128, 256, 512, 512)[: S - 1]
         if not self.has_fcn:
             return
-
-        def padded(c):
-            return _round_up(c, 32)
-
-        def conv3(name, src, ci, co, stride, out):
-            w = sd["conv_net.%s.0.weight" % name].double()                      # (Co,Ci,3)
-            s, sh = _fold_bn(sd, "conv_net.%s.1" % name)
-            cp, ncols = padded(ci), _round_up(co, 64)
-            wt = torch.zeros(3 * cp, ncols, dtype=torch.float64, device=cpu)
-            for j in range(3):
-                wt[j * cp: j * cp + ci, :co] = (w[:, :, j] * s[:, None]).t()
-            bias = torch.zeros(ncols, dtype=torch.float64, device=cpu)
-            bias[:co] = sh
-            segs = [(src, ci, j - 1, stride) for j in range(3)]
-            self.layers.append(_ConvLayer(name, segs, 3 * cp, ncols, co, 1, 1, wt.to(f32).contiguous(),
-                                          bias.to(f32).contiguous(), out, 0, dev))
-
-        def merge(name, src_a, ca, src_b, cb, co, out):
-            w = sd["conv_net.%s.0.weight" % name].double()[:, :, 0]            # (Co, ca+cb)
-            s, sh = _fold_bn(sd, "conv_net.%s.1" % name)
-            pa, pb, ncols = padded(ca), padded(cb), _round_up(co, 64)
-            wt = torch.zeros(pa + pb, ncols, dtype=torch.float64, device=cpu)
-            wt[:ca, :co] = (w[:, :ca] * s[:, None]).t()
-            wt[pa: pa + cb, :co] = (w[:, ca:] * s[:, None]).t()
-            bias = torch.zeros(ncols, dtype=torch.float64, device=cpu)
-            bias[:co] = sh
-            segs = [(src_a, ca, 0, 1), (src_b, cb, 0, 1)]
-            self.layers.append(_ConvLayer(name, segs, pa + pb, ncols, co, 1, 1, wt.to(f32).contiguous(),
-                                          bias.to(f32).contiguous(), out, 0, dev))
-
-        def deconv(name, src, ci, co, k, c_off):
-            w = sd["conv_net.%s.0.weight" % name].double()                      # (Ci,Co,k)
-            s, sh = _fold_bn(sd, "conv_net.%s.1" % name)
-            ncols = _round_up(k * co, 64)
-            wt = torch.zeros(padded(ci), ncols, dtype=torch.float64, device=cpu)
-            bias = torch.zeros(ncols, dtype=torch.float64, device=cpu)
-            for j in range(k):
-                wt[:ci, j * co:(j + 1) * co] = w[:, :, j] * s[None, :]
-                bias[j * co:(j + 1) * co] = sh
-            self.layers.append(_ConvLayer(name, [(src, ci, 0, 1)], padded(ci), ncols, co, k, 1,
-                                          wt.to(f32).contiguous(), bias.to(f32).contiguous(), "cat", c_off, dev))
-
-        conv3("block1_conv1", "feat1", self.c3[0] + V, self.arch.block1_out, 1, "x1")
-        prev, prev_c = "x1", self.arch.block1_out
-        for i in range(2, S + 1):
-            w = widths[i - 2]
-            conv3("block%d_conv1" % i, prev, prev_c, w, 2, "a%d" % i)
-            conv3("block%d_conv2" % i, "a%d" % i, w, w, 1, "b%d" % i)
-            merge("block%d_merge" % i, "b%d" % i, w, "feat%d" % i, self.c3[i - 1] + V, w, "m%d" % i)
-            prev, prev_c = "m%d" % i, w
-        for i in range(2, S + 1):
-            deconv("block%d_deconv" % i, "m%d" % i, widths[i - 2], 256, 2 ** (i - 2), 256 * (i - 2))
-        if not self.has_heads:
-            return
-        # heads: columns [cls0, cls1, reg...] zero-padded to ld_logit (det_base.py:250-251,367-368)
-        cin = self.arch.reg_in
-        wt = torch.zeros(_round_up(cin, 32), self.ld_logit, dtype=torch.float32, device=cpu)
-        bias = torch.zeros(self.ld_logit, dtype=torch.float32, device=cpu)
-        wt[:cin, 0:2] = sd["cls_out.weight"][:, :, 0].t()
-        wt[:cin, 2:2 + self.out_size] = sd["reg_out.weight"][:, :, 0].t()
-        bias[0:2] = sd["cls_out.bias"]
-        bias[2:2 + self.out_size] = sd["reg_out.bias"]
-        self.layers.append(_ConvLayer("heads", [("cat", cin, 0, 1)], _round_up(cin, 32), self.ld_logit,
-                                      self.ld_logit, 1, 0, wt.contiguous(), bias.contiguous(), "logits", 0, dev))
+        for L in fcn_layers(self.arch, self.num_vec):
+            if L.kind == "heads" and not self.has_heads:
+                return
+            ci = sum(c for _, c in L.srcs)
+            if L.kind == "heads":          # one K segment over the concat; columns [cls0, cls1, reg...]
+                segs, n_cols, co, up = [("cat", ci, 0, 1)], self.ld_logit, self.ld_logit, 1
+            elif L.kind == "deconv":       # taps laid out along N: column j * Cout + c is output position t * k + j
+                segs, n_cols, co, up = [(L.srcs[0][0], ci, 0, 1)], _round_up(L.k * L.Cout, 64), L.Cout, L.k
+            else:                          # conv taps (tap-major) and merge sources laid out along K
+                segs = [(src, c, j - L.k // 2, L.stride) for j in range(L.k) for src, c in L.srcs]
+                n_cols, co, up = _round_up(L.Cout, 64), L.Cout, 1
+            k_off = np.cumsum([0] + [_round_up(c, 32) for _, c, _, _ in segs]).tolist()
+            wt = torch.zeros(k_off[-1], n_cols, dtype=torch.float64, device=cpu)
+            bias = torch.zeros(n_cols, dtype=torch.float64, device=cpu)
+            if L.kind == "heads":          # det_base.py:250-251,367-368
+                osz = self.out_size
+                wt[:ci, 0:2] = sd["cls_out.weight"][:, :, 0].double().t()
+                wt[:ci, 2:2 + osz] = sd["reg_out.weight"][:, :, 0].double().t()
+                bias[0:2], bias[2:2 + osz] = sd["cls_out.bias"].double(), sd["reg_out.bias"].double()
+            else:
+                w = sd["conv_net.%s.0.weight" % L.name].double()     # conv / merge (Co,Ci,k), deconv (Ci,Co,k)
+                s, sh = _fold_bn(sd, "conv_net.%s.1" % L.name)
+                if L.kind == "deconv":
+                    for j in range(L.k):
+                        wt[:ci, j * co:(j + 1) * co] = w[:, :, j] * s[None, :]
+                        bias[j * co:(j + 1) * co] = sh
+                else:
+                    n = 0
+                    for j in range(L.k):
+                        c0 = 0
+                        for _, c in L.srcs:
+                            wt[k_off[n]: k_off[n] + c, :co] = (w[:, c0:c0 + c, j] * s[:, None]).t()
+                            c0, n = c0 + c, n + 1
+                    bias[:co] = sh
+            self.layers.append(_ConvLayer(L.name, L.kind, segs, k_off[-1], n_cols, co, up, int(L.kind != "heads"),
+                                          wt.to(f32).contiguous(), bias.to(f32).contiguous(), _out_map(L), L.c_off,
+                                          dev))
 
     # ------------------------------------------------------------------ shape plans
     def plan(self, B: int, N: int, T: Sequence[int]) -> "_Plan":
@@ -260,7 +236,7 @@ class FrustumEngine:
 
     @torch.no_grad()
     def conv_feat_net(self, feats_bct: Sequence[torch.Tensor]):
-        """ConvFeatNet.forward on channel-first inputs -> (B, 256*(S-1), T2)."""
+        """ConvFeatNet.forward on channel-first inputs -> (B, arch.reg_in, T2)."""
         B = feats_bct[0].shape[0]
         p = self.plan(B, 1, [f.shape[2] for f in feats_bct])
         return p.run_fcn_bct(feats_bct)
@@ -315,17 +291,14 @@ class _Plan:
             self.tiles.append(torch.empty((max(mt, 1), 4), dtype=torch.int32, device=dev))
             self.buf["feat%d" % (s + 1)] = torch.zeros((B, P[s], eng.ld_feat[s]), dtype=f32, device=dev)
         self.ntiles = torch.zeros(_lib.MAX_SCALES, dtype=torch.int32, device=dev)
-        widths = (128, 256, 512, 512)[: S - 1]
-        self.buf["x1"] = torch.zeros((B, P[0], arch.block1_out), dtype=f32, device=dev)
-        self.valid_T = {"x1": T[0], "cat": T[1], "logits": T[1]}
-        for i in range(2, S + 1):
-            for nm in ("a", "b", "m"):
-                self.buf["%s%d" % (nm, i)] = torch.zeros((B, P[i - 1], widths[i - 2]), dtype=f32, device=dev)
-                self.valid_T["%s%d" % (nm, i)] = T[i - 1]
-        for s in range(S):
-            self.valid_T["feat%d" % (s + 1)] = T[s]
-        self.buf["cat"] = torch.zeros((B, P[1], 256 * (S - 1)), dtype=f32, device=dev)
-        self.buf["logits"] = torch.zeros((B, P[1], eng.ld_logit), dtype=f32, device=dev)
+        self.valid_T = {"feat%d" % (s + 1): T[s] for s in range(S)}
+        # one map per conv / merge layer; the transposed convs share the concat, the heads write the logits
+        for L in fcn_layers(arch, eng.num_vec):
+            name = _out_map(L)
+            if name not in self.buf:
+                C = {"cat": arch.reg_in, "logits": eng.ld_logit}.get(name, L.Cout)
+                self.buf[name] = torch.zeros((B, P[L.level], C), dtype=f32, device=dev)
+                self.valid_T[name] = T[L.level]
         T2 = T[1]
         # the six outputs of det_base.py:411 are views into one flat block (single all-gather / D2H)
         widths_out = (2, 3, 1, 3, eng.num_bins, eng.num_size)
@@ -391,17 +364,19 @@ class _Plan:
             a.out = _ptr(self.buf["feat%d" % (s + 1)])
             a.feat_pitch = self.P[s]
             self.pn_args.append(a)
+        # GEMM geometry of every layer: (output positions T_out, row pitch P_m of the M space, N tile width)
+        self.geom = []
+        for L in eng.layers:
+            src, _, _, stride = L.segs[0]
+            T_in = self.valid_T[src]
+            self.geom.append((T_in if stride == 1 else (T_in + 1) // 2, self.buf[src].shape[1] // stride,
+                              128 if L.n_cols % 128 == 0 else 64))
         self.conv_args = []
         self._tmaps = []
-        for L in eng.layers:
+        for L, (T_out, P_m, nt) in zip(eng.layers, self.geom):
             a = _lib.ConvArgs()
             out = self.buf[L.out]
-            src0 = L.segs[0][0]
-            stride = L.segs[0][3]
-            a.B = self.B
-            T_in, P_in = self.valid_T[src0], self.buf[src0].shape[1]
-            a.T_out = T_in if stride == 1 else (T_in + 1) // 2
-            a.P_m = P_in // stride
+            a.B, a.T_out, a.P_m = self.B, T_out, P_m
             a.n_seg = len(L.segs)
             for j, (src, c, tap, st) in enumerate(L.segs):
                 t = self.buf[src]
@@ -413,7 +388,6 @@ class _Plan:
             if eng.precision == 1 and L.Cout % 32 == 0:
                 # The A operand feed is the limit, so the wider N tile (2x the MMA work per A byte) is used
                 # whenever the layer has >= 128 columns.
-                nt = 128 if L.n_cols % 128 == 0 else 64
                 a.w_tc = _ptr(L.tc_image(nt))
                 if eng.use_tma:
                     # fully TMA-fed variant: one 128-byte tensor map per A segment (host memory, kept alive here)
@@ -427,7 +401,7 @@ class _Plan:
                     a.precision = 3 if nt == 128 else 4
                 else:
                     a.precision = 1 if nt == 128 else 2
-            a.round_out = 1 if (eng.precision == 1 and L.name != "heads") else 0
+            a.round_out = 1 if (eng.precision == 1 and L.kind != "heads") else 0
             a.wt, a.bias = _ptr(L.wt), _ptr(L.bias)
             a.out, a.ld_out, a.T_store, a.c_off = _ptr(out), out.shape[2], self.valid_T[L.out], L.c_off
             a.P_store = out.shape[1]
@@ -444,23 +418,18 @@ class _Plan:
 
         def build(wide):
             descs = []
-            for L in eng.layers:
-                src0, stride = L.segs[0][0], L.segs[0][3]
-                T_in, P_in = self.valid_T[src0], self.buf[src0].shape[1]
-                T_out = T_in if stride == 1 else (T_in + 1) // 2
-                P_m = P_in // stride
+            for L, (T_out, P_m, nt) in zip(eng.layers, self.geom):
                 out = self.buf[L.out]
-                nt = 128 if L.n_cols % 128 == 0 else 64
-                if wide and L.n_cols % 256 == 0 and L.name != "heads":
+                if wide and L.n_cols % 256 == 0 and L.kind != "heads":
                     nt = 256
-                descs.append(_mega.LayerDesc(L.name, L.segs, L.K_pad, L.n_cols, L.Cout, L.up, L.relu, L.out, L.c_off, nt,
-                                             1 if L.name != "heads" else 0, P_m, T_out, self.B * P_m, out.shape[2],
-                                             out.shape[1], self.valid_T[L.out]))
+                descs.append(_mega.LayerDesc(L.name, L.kind, L.segs, L.K_pad, L.n_cols, L.Cout, L.up, L.relu, L.out,
+                                             L.c_off, nt, int(L.kind != "heads"), P_m, T_out, self.B * P_m,
+                                             out.shape[2], out.shape[1], self.valid_T[L.out]))
             return descs
 
         if eng.mega_nt256 == "auto":
             descs = build(True)
-            if min(d.m_tiles * d.n_tiles for d in descs if not d.name.endswith("_deconv") and d.name != "heads") >= 24:
+            if _mega.chain_tiles(descs) >= 24:
                 return descs
             return build(False)
         return build(bool(eng.mega_nt256))
@@ -487,8 +456,7 @@ class _Plan:
         m = _lib.MegaArgs()
         grid = eng.mega_grid
         if grid <= 0:
-            chain = [d.m_tiles * d.n_tiles for d in descs if not d.name.endswith("_deconv") and d.name != "heads"]
-            grid = max(4, min(48, (2 * min(chain)) // 3))
+            grid = max(4, min(48, (2 * _mega.chain_tiles(descs)) // 3))
         self.mega_grid = grid
         m.n_layers, m.n_jobs, m.n_flags, m.grid = len(descs), len(jobs), nflags, grid
         m.tmaps, m.n_maps = C.addressof(maps), len(map_keys)
@@ -583,32 +551,30 @@ class _Plan:
         """Main chain on the current stream; the transposed convs of all but the last block only
         feed the final concat, so they run on a side stream next to the following block."""
         main = torch.cuda.current_stream()
-        names = [L.name for L in self.eng.layers]
-        deconvs = [n for n in names if n.endswith("_deconv")]
-        side_set = set(deconvs[:-1])
-        side = self._side_streams(1)[0] if side_set else None
+        layers = self.eng.layers
+        deconvs = [i for i, L in enumerate(layers) if L.kind == "deconv"][:-1]
+        side_of = {layers[i].segs[0][0]: self.conv_args[i] for i in deconvs}   # map read -> side deconv
+        side = self._side_streams(1)[0] if side_of else None
         joins = []
-        for a, L in zip(self.conv_args, self.eng.layers):
-            if L.name in side_set:
+        for i, (a, L) in enumerate(zip(self.conv_args, layers)):
+            if i in deconvs:
                 continue
-            if L.name == "heads":
+            if L.kind == "heads":
                 for ev in joins:
                     main.wait_event(ev)
+                joins = []
             _lib.call("fcn_conv_gemm", C.byref(a), main.cuda_stream)
-            if L.name.endswith("_merge"):
-                dn = L.name.replace("_merge", "_deconv")
-                if dn in side_set:
-                    ev = torch.cuda.Event()
-                    ev.record(main)
-                    side.wait_event(ev)
-                    da = self.conv_args[names.index(dn)]
-                    _lib.call("fcn_conv_gemm", C.byref(da), side.cuda_stream)
-                    ev2 = torch.cuda.Event()
-                    ev2.record(side)
-                    joins.append(ev2)
-        if "heads" not in names:
-            for ev in joins:
-                main.wait_event(ev)
+            da = side_of.get(L.out)
+            if da is not None:
+                ev = torch.cuda.Event()
+                ev.record(main)
+                side.wait_event(ev)
+                _lib.call("fcn_conv_gemm", C.byref(da), side.cuda_stream)
+                ev2 = torch.cuda.Event()
+                ev2.record(side)
+                joins.append(ev2)
+        for ev in joins:
+            main.wait_event(ev)
 
     def _launch_decode(self, center_ref2):
         eng = self.eng
@@ -770,7 +736,7 @@ class _Plan:
                           _ptr(self.buf["feat%d" % (s + 1)]), _stream())
             st = _stream()
             for a, L in zip(self.conv_args, eng.layers):
-                if L.name == "heads":
+                if L.kind == "heads":
                     continue
                 _lib.call("fcn_conv_gemm", C.byref(a), st)
             cat = self.buf["cat"]
@@ -857,7 +823,7 @@ class _Plan:
         fcn_gf = []
         for j, (L, a) in enumerate(zip(eng.layers, self.conv_args)):
             kreal = sum(sg[1] for sg in L.segs)
-            nreal = (2 + eng.out_size) if L.name == "heads" else L.up * L.Cout
+            nreal = (2 + eng.out_size) if L.kind == "heads" else L.up * L.Cout
             fcn_gf.append(2e-9 * a.B * a.T_out * kreal * nreal)
         if mega:
             kern.append(dict(name="fcn_mega", ms=float(acc[1 + S]), executed_gflop=sum(fcn_gf), nominal_gflop=sum(fcn_gf)))

@@ -25,9 +25,9 @@ EPI_WARPS = 8          # completion counts per finished tile (one per consumer w
 class LayerDesc:
     """Shape-level description of one GEMM layer (no pointers): what ``build_tables`` needs."""
 
-    def __init__(self, name, segs, K_pad, n_cols, Cout, up, relu, out, c_off, NT, round_out,
+    def __init__(self, name, kind, segs, K_pad, n_cols, Cout, up, relu, out, c_off, NT, round_out,
                  P_m, T_out, n_rows, ld_out, P_store, T_store):
-        self.name, self.segs, self.K_pad, self.n_cols = name, segs, K_pad, n_cols
+        self.name, self.kind, self.segs, self.K_pad, self.n_cols = name, kind, segs, K_pad, n_cols
         self.Cout, self.up, self.relu, self.out, self.c_off = Cout, up, relu, out, c_off
         self.NT, self.round_out = NT, round_out
         self.P_m, self.T_out, self.n_rows = P_m, T_out, n_rows
@@ -37,23 +37,22 @@ class LayerDesc:
         self.k_atoms = 1 if NT == 256 else 2       # 32-wide K atoms per shared-memory stage (stage = 64 KB at most)
 
 
+def chain_tiles(layers: Sequence[LayerDesc]) -> int:
+    """Fewest output tiles of a main-chain layer (the conv and merge layers)."""
+    return min(L.m_tiles * L.n_tiles for L in layers if L.kind in ("conv", "merge"))
+
+
 def job_order(layers: Sequence[LayerDesc]) -> List[int]:
-    """Layer order of the job table: main chain in network order; every side transposed conv right after its
-    merge layer.  (eng.layers lists the deconvs after all blocks; moving them up keeps the order topological -
+    """Layer order of the job table: main chain in network order; every side transposed conv right after the
+    layer it reads.  (eng.layers lists the deconvs after all blocks; moving them up keeps the order topological -
     a deconv only reads its own block's merge output - and lets them overlap the next block.)"""
-    names = [L.name for L in layers]
     order = []
-    for i, n in enumerate(names):
-        if n.endswith("_deconv") or n == "heads":
-            continue
-        order.append(i)
-        if n.endswith("_merge"):
-            dn = n.replace("_merge", "_deconv")
-            if dn in names:
-                order.append(names.index(dn))
-    if "heads" in names:
-        order.append(names.index("heads"))
-    assert sorted(order) == list(range(len(names)))
+    for i, L in enumerate(layers):
+        if L.kind in ("conv", "merge"):
+            order.append(i)
+            order += [j for j, D in enumerate(layers) if D.kind == "deconv" and D.segs[0][0] == L.out]
+    order += [i for i, L in enumerate(layers) if L.kind == "heads"]
+    assert sorted(order) == list(range(len(layers)))
     return order
 
 
@@ -79,7 +78,7 @@ def build_tables(layers: Sequence[LayerDesc], interleave: bool = True):
                 map_keys.append(key)
             segs.append(dict(map_idx=map_idx[key], kblocks=(c + 31) // 32, tap=tap, stride=st))
         okey = ("store", L.out, L.up)
-        if L.name != "heads" and okey not in map_idx:
+        if L.kind != "heads" and okey not in map_idx:
             map_idx[okey] = len(map_keys)
             map_keys.append(okey)
         rows.append(dict(segs=segs, flag_base=flag_base[i], out_map=map_idx.get(okey, 0)))
@@ -103,7 +102,6 @@ def build_tables(layers: Sequence[LayerDesc], interleave: bool = True):
         return out
 
     order = job_order(layers)
-    names = [L.name for L in layers]
     jobs = []
 
     def emit(li):
@@ -113,7 +111,7 @@ def build_tables(layers: Sequence[LayerDesc], interleave: bool = True):
     k = 0
     while k < len(order):
         li = order[k]
-        if interleave and names[li].endswith("_deconv") and k + 1 < len(order) and names[order[k + 1]] != "heads":
+        if interleave and layers[li].kind == "deconv" and k + 1 < len(order) and layers[order[k + 1]].kind != "heads":
             # deconv of block i  x  first conv of block i+1: both only read merge_i -> interleave their tiles
             a, b = emit(li), emit(order[k + 1])
             na, nb = len(a), len(b)
@@ -156,7 +154,7 @@ def to_ctypes(layers: Sequence[LayerDesc], rows, jobs, ptrs):
         a.relu, a.round_out, a.up, a.Cout = L.relu, L.round_out, L.up, L.Cout
         a.P_m, a.T_out, a.n_rows = L.P_m, L.T_out, L.n_rows
         a.ld_out, a.P_store, a.T_store, a.c_off = L.ld_out, L.P_store, L.T_store, L.c_off
-        a.is_heads, a.flag_base, a.out_map = (1 if L.name == "heads" else 0), row["flag_base"], row["out_map"]
+        a.is_heads, a.flag_base, a.out_map = int(L.kind == "heads"), row["flag_base"], row["out_map"]
         a.w_tc, a.bias, a.out = ptrs[i]
     JA = (_lib.MegaJob * max(len(jobs), 1))()
     for j, jb in enumerate(jobs):

@@ -17,7 +17,7 @@ from collections import OrderedDict
 
 import numpy as np
 
-from .config import DATASET_INFO, WORKLOADS, ArchSpec
+from .config import DATASET_INFO, WORKLOADS, ArchSpec, fcn_layers
 
 _PRESETS = {
     # name: (N, strides, max_depth, z0 range, sigma, kind)
@@ -110,26 +110,6 @@ def make_frustums(workload: str, B: int, seed: int = 1234, max_depth=None, N=Non
 # --------------------------------------------------------------------------
 # parameters
 # --------------------------------------------------------------------------
-def fcn_layer_table(arch: ArchSpec, num_vec: int):
-    """Layer list of ConvFeatNet in reference order (det_base.py:167-183,
-    det_base_sunrgbd.py:178-200).  Each entry: (name, kind, Cin, Cout, k, stride)."""
-    S = arch.num_scales
-    widths = (128, 256, 512, 512)[: S - 1]
-    c3 = [m[2] for m in arch.mlps]
-    L = [("block1_conv1", "conv", c3[0] + num_vec, arch.block1_out, 3, 1)]
-    prev = arch.block1_out
-    for i in range(2, S + 1):
-        w = widths[i - 2]
-        L.append(("block%d_conv1" % i, "conv", prev, w, 3, 2))
-        L.append(("block%d_conv2" % i, "conv", w, w, 3, 1))
-        L.append(("block%d_merge" % i, "conv", w + c3[i - 1] + num_vec, w, 1, 1))
-        prev = w
-    for i in range(2, S + 1):
-        k = 2 ** (i - 2)
-        L.append(("block%d_deconv" % i, "deconv", widths[i - 2], 256, k, k))
-    return L
-
-
 def reg_out_size(dataset: str, num_bins: int = 12) -> int:
     return 3 + num_bins * 2 + DATASET_INFO[dataset].NUM_SIZE_CLUSTER * 4
 
@@ -156,12 +136,14 @@ def make_state_dict(arch: ArchSpec, num_vec: int, dataset: str, seed: int = 7,
             sd[p + ".0.weight"] = rng.normal(0, np.sqrt(2.0 / cin), size=(co, cin, 1, 1)).astype(np.float32)
             bn(p + ".1", co)
             cin = co
-    for name, kind, ci, co, k, s in fcn_layer_table(arch, num_vec):
-        p = "conv_net." + name
-        if kind == "conv":
-            sd[p + ".0.weight"] = rng.normal(0, np.sqrt(2.0 / (ci * k)), size=(co, ci, k)).astype(np.float32)
-        else:
+    for L in fcn_layers(arch, num_vec):
+        if L.kind == "heads":       # drawn below, under their own names
+            continue
+        ci, co, k, p = sum(c for _, c in L.srcs), L.Cout, L.k, "conv_net." + L.name
+        if L.kind == "deconv":
             sd[p + ".0.weight"] = rng.normal(0, np.sqrt(2.0 / (co * k)), size=(ci, co, k)).astype(np.float32)
+        else:
+            sd[p + ".0.weight"] = rng.normal(0, np.sqrt(2.0 / (ci * k)), size=(co, ci, k)).astype(np.float32)
         bn(p + ".1", co)
     osz = reg_out_size(dataset, num_bins)
     bound = np.sqrt(6.0 / arch.reg_in)

@@ -18,10 +18,11 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, List, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
-from .synth import fcn_layer_table
+from .config import fcn_layers
 
 
 def _ptr(t):
@@ -210,52 +211,33 @@ class TrainEngine:
             P.feat, P.argmax, P.dfeat, P.dA = _ptr(fa["Y"]), _ptr(argmax), _ptr(fa["dA"]), _ptr(last["dA"])
             self.pools.append(P)
         self.n_pn_layers = len(self.layers)
-        # ---- ConvFeatNet
-        cn = model.conv_net
-        c3s = [m[2] for m in arch.mlps]
-        widths = (128, 256, 512, 512)[: S - 1]
-        Tl = list(T)
+        # ---- ConvFeatNet + heads.  Weight index of (co, ci, tap j): conv / merge co * Ci * k + ci * k + j,
+        # transposed conv ci * Cout * k + co * k + j
         for i in range(1, S):
-            assert Tl[i] == (Tl[i - 1] + 1) // 2, "section counts are not a /2 pyramid"
-
-        def conv3(name, src, ci, co, stride, T_in):
-            blk = getattr(cn, name)
-            T_out = T_in if stride == 1 else (T_in + 1) // 2
-            new_act(name, B * T_out, co, T_out, bn=blk[1])
-            segs = [(src, ci, j - 1, stride, 3, j) for j in range(3)]
-            add_layer(name, name, segs, blk[0], blk[1], co, co, 1, ci * 3, 0, T_out)
-            return T_out
-
-        conv3("block1_conv1", "feat1", c3s[0] + self.V, arch.block1_out, 1, Tl[0])
-        prev, pc = "block1_conv1", arch.block1_out
-        for i in range(2, S + 1):
-            w = widths[i - 2]
-            conv3("block%d_conv1" % i, prev, pc, w, 2, Tl[i - 2])
-            conv3("block%d_conv2" % i, "block%d_conv1" % i, w, w, 1, Tl[i - 1])
-            nm = "block%d_merge" % i
-            blk = getattr(cn, nm)
-            cb = c3s[i - 1] + self.V
-            new_act(nm, B * Tl[i - 1], w, Tl[i - 1], bn=blk[1])
-            add_layer(nm, nm, [("block%d_conv2" % i, w, 0, 1, 1, 0), ("feat%d" % i, cb, 0, 1, 1, w)], blk[0], blk[1],
-                      w, w, 1, w + cb, 0, Tl[i - 1])
-            prev, pc = nm, w
-        for i in range(2, S + 1):
-            nm = "block%d_deconv" % i
-            blk = getattr(cn, nm)
-            k = 2 ** (i - 2)
-            ci = widths[i - 2]
-            new_act(nm, B * Tl[i - 1], k * 256, Tl[i - 1], up=k, cout=256, bn=blk[1])
-            add_layer(nm, nm, [("block%d_merge" % i, ci, 0, 1, 256 * k, 0)], blk[0], blk[1], k * 256, 256, k, k, 1,
-                      Tl[i - 1])
-        # ---- heads on the cropped concat of the three (four) transposed-conv outputs (det_base.py:222-224,367-368)
-        T2 = Tl[1]
-        cin = 256 * (S - 1)
-        hsegs = [("block%d_deconv" % i, 256, 0, 1, 1, 256 * (i - 2)) for i in range(2, S + 1)]
-        for nm, conv in (("cls_out", model.cls_out), ("reg_out", model.reg_out)):
-            co = conv.weight.shape[0]
-            new_act(nm, B * T2, co, T2, bn=None)
-            add_layer(nm, nm, hsegs, conv, None, co, co, 1, cin, 0, T2, bias=conv.bias)
-        self.T2 = T2
+            assert T[i] == (T[i - 1] + 1) // 2, "section counts are not a /2 pyramid"
+        table = {L.name: L for L in fcn_layers(arch, self.V)}
+        for L in table.values():
+            ci = sum(c for _, c in L.srcs)
+            if L.kind == "heads":     # on the cropped concat of the transposed-conv outputs (det_base.py:222-224,367-368)
+                segs = [(src, c, 0, 1, 1, table[src].c_off) for src, c in L.srcs]
+                for nm, conv in (("cls_out", model.cls_out), ("reg_out", model.reg_out)):
+                    co = conv.weight.shape[0]
+                    new_act(nm, B * T[L.level], co, T[L.level], bn=None)
+                    add_layer(nm, nm, segs, conv, None, co, co, 1, ci, 0, T[L.level], bias=conv.bias)
+                continue
+            blk = getattr(model.conv_net, L.name)
+            if L.kind == "deconv":    # one row per input position, k output positions per row
+                src, Tin = L.srcs[0][0], self.act[L.srcs[0][0]]["T"]
+                new_act(L.name, B * Tin, L.k * L.Cout, Tin, up=L.k, cout=L.Cout, bn=blk[1])
+                add_layer(L.name, L.name, [(src, ci, 0, 1, L.Cout * L.k, 0)], blk[0], blk[1], L.k * L.Cout, L.Cout,
+                          L.k, L.k, 1, Tin)
+            else:
+                c0 = np.cumsum([0] + [c for _, c in L.srcs]).tolist()
+                segs = [(src, c, j - L.k // 2, L.stride, L.k, c0[n] * L.k + j)
+                        for j in range(L.k) for n, (src, c) in enumerate(L.srcs)]
+                new_act(L.name, B * T[L.level], L.Cout, T[L.level], bn=blk[1])
+                add_layer(L.name, L.name, segs, blk[0], blk[1], L.Cout, L.Cout, 1, ci * L.k, 0, T[L.level])
+        self.T2 = T[1]
         # device copy of the layer table for the end-of-step kernel
         arr = (_lib.TrainLayer * len(self.layers))(*self.layers)
         self._table_host = arr

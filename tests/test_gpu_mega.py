@@ -151,7 +151,7 @@ def _compare_buffers(monkeypatch, w, sd, cfg, data):
     b0 = _buffers(p0)
     _, p1, o1, _, _ = _forward(monkeypatch, True, w, sd, cfg, d, shape=shape)
     b1 = _buffers(p1)
-    assert set(b0) == set(b1) and {"x1", "cat", "logits"} <= set(b0)
+    assert set(b0) == set(b1) and {"block1_conv1", "cat", "logits"} <= set(b0)
     for k in b0:
         assert torch.equal(b0[k], b1[k]), "buffer %s differs between the persistent and per-layer paths" % k
     _assert_pads_zero(p0, b0, "per-layer")
@@ -163,7 +163,7 @@ def _compare_buffers(monkeypatch, w, sd, cfg, data):
 
 @pytest.mark.parametrize("name", ["car_full_b1", "sunrgbd_full_b2", "people_small_b2"])
 def test_mega_intermediate_buffers_bit_exact(name, monkeypatch):
-    """Every activation buffer of the plan (x1, a_i, b_i, m_i, cat, logits), not just the six outputs."""
+    """Every activation buffer of the plan (one per conv / merge layer, cat, logits), not just the six outputs."""
     g, data, sd, w, cfg = load_golden(name)
     _compare_buffers(monkeypatch, w, sd, cfg, data)
 

@@ -171,9 +171,14 @@ def test_roofline_denominators_follow_from_the_architecture(wl):
     arch, V = w["arch"], w["num_vec"]
     T, K, N = list(synth.section_counts(wl)), arch.nsample, synth._PRESETS[wl]["N"]
     mac = sum(t * k * (3 * c1 + c1 * c2 + c2 * c3) for (c1, c2, c3), t, k in zip(arch.mlps, T, K))
-    for name, kind, ci, co, k, s in synth.fcn_layer_table(arch, V):
-        i = 1 if name == "block1_conv1" else int(name[5])
-        mac += T[i - 1] * ci * co * k          # conv: per output position; transposed conv: per input position
+    level = {}
+    for L in config.fcn_layers(arch, V):
+        level[L.name] = L.level
+        if L.kind == "heads":
+            continue
+        ci = sum(c for _, c in L.srcs)
+        lv = level[L.srcs[0][0]] if L.kind == "deconv" else L.level
+        mac += T[lv] * ci * L.Cout * L.k       # conv: per output position; transposed conv: per input position
     n_reg = 39 if arch.num_scales == 4 else 67   # det_base.py:248 / det_base_sunrgbd.py
     mac += T[1] * arch.reg_in * (2 + n_reg)
     n_size = 3 if arch.num_scales == 4 else 10
