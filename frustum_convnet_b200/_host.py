@@ -1,6 +1,6 @@
-"""Host side of the two-phase device entries (detect, kitti_eval, sunrgbd_eval, frustum_extract, refine_extract):
-check the device, build the host CSR offsets, upload the packed inputs in one copy, query and allocate the
-workspace.  Every entry of those modules takes its inputs the same way, so the rules live here once."""
+"""Host side of the two-phase device entries (detect, kitti_eval, sunrgbd_eval, frustum_extract, refine_extract,
+gt_extract): check the device, build the host CSR offsets, upload the packed inputs in one copy, query and allocate
+the workspace.  Every entry of those modules takes its inputs the same way, so the rules live here once."""
 from __future__ import annotations
 
 import numpy as np

@@ -295,6 +295,20 @@ class RefineExtractArgs(C.Structure):
                [(n, C.c_void_p) for n in ("info", "job_points", "job_gt", "points", "labels", "offsets")]
 
 
+class GtJob(C.Structure):
+    _fields_ = [("box", C.c_double * 4), ("frame", C.c_int32), ("label", C.c_int32)]
+
+
+class GtExtractArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("num_frames", "num_points", "num_jobs", "num_labels", "num_kept",
+                                       "reserved")] + \
+               [("num_out_points", C.c_longlong)] + \
+               [(n, C.c_void_p) for n in ("scans", "scan_offsets", "host_scan_offsets", "frames", "jobs",
+                                          "label_boxes", "workspace")] + \
+               [("workspace_bytes", C.c_longlong)] + \
+               [(n, C.c_void_p) for n in ("info", "job_points", "points", "labels", "offsets")]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -347,6 +361,9 @@ SIGNATURES = {
     "fcn_refine_extract_workspace_bytes": (C.c_longlong, [C.POINTER(RefineExtractArgs)]),
     "fcn_refine_extract_count": (_I, [C.POINTER(RefineExtractArgs), _P]),
     "fcn_refine_extract_write": (_I, [C.POINTER(RefineExtractArgs), _P]),
+    "fcn_gt_extract_workspace_bytes": (C.c_longlong, [C.POINTER(GtExtractArgs)]),
+    "fcn_gt_extract_count": (_I, [C.POINTER(GtExtractArgs), _P]),
+    "fcn_gt_extract_write": (_I, [C.POINTER(GtExtractArgs), _P]),
 }
 
 _lib = None

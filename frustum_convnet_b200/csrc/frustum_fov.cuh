@@ -1,7 +1,8 @@
-// The in-image point stage shared by the KITTI frustum extractors (csrc/frustum_extract.cu, section (15), and
-// csrc/refine_extract.cu, section (16)): each scan point projected velo -> rect -> image once in float64 and tested
-// against the image (get_lidar_in_image_fov, draw_util.py:15-18), then the in-image points of every frame compacted in
-// scan order.  The kernels of both files call these bodies, so both extract exactly the same points.
+// The in-image point stage shared by the KITTI frustum extractors (csrc/frustum_extract.cu, section (15),
+// csrc/refine_extract.cu, section (16), and csrc/gt_extract.cu, section (17)): each scan point projected velo -> rect
+// -> image once in float64 and tested against the image (get_lidar_in_image_fov, draw_util.py:15-18), then the
+// in-image points of every frame compacted in scan order.  The kernels of all three files call these bodies, so they
+// extract exactly the same points.
 #pragma once
 
 #include "common.cuh"

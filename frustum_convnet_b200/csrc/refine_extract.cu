@@ -21,6 +21,7 @@
 
 #include <cmath>
 
+#include "box_contains.cuh"
 #include "box_iou.cuh"
 #include "common.cuh"
 #include "frustum_fov.cuh"
@@ -38,17 +39,6 @@ rx_compact_kernel(const float4 *__restrict__ scans, const int32_t *__restrict__ 
                   const fcn_frustum_frame *__restrict__ frames, const int32_t *__restrict__ pos,
                   float4 *__restrict__ fov_pts) {
     fov_compact<false>(scans, so, frames, pos, fov_pts, nullptr, nullptr);
-}
-
-// The half-space test of oracle/refine_extract.py (in_box): the point in the box's own frame, in float64, every
-// product and sum rounded separately.  Substitutes for scipy's Delaunay(corners).find_simplex >= 0.
-__device__ __forceinline__ bool rx_in_box(const fcn_refine_box &b, float4 p) {
-    const double dx = __dsub_rn((double)p.x, b.center[0]);
-    const double dy = __dsub_rn((double)p.y, b.center[1]);
-    const double dz = __dsub_rn((double)p.z, b.center[2]);
-    const double lx = __dsub_rn(__dmul_rn(b.cs, dx), __dmul_rn(b.sn, dz));
-    const double lz = __dadd_rn(__dmul_rn(b.sn, dx), __dmul_rn(b.cs, dz));
-    return fabs(lx) <= b.half[0] && fabs(dy) <= b.half[1] && fabs(lz) <= b.half[2];
 }
 
 // bbox_overlaps_3d (ops/pybind11/rbbox_iou.py:62-96) of the two boxes' axis-aligned standup boxes, in its order
@@ -175,9 +165,9 @@ rx_count_kernel(int mode, int num_frames, int num_gt, int num_dets, const int32_
     int c = 0, l = 0;
     for (int i = p0 + threadIdx.x; i < p1; i += FX_THREADS) {
         const float4 p = fov_pts[i];
-        if (rx_in_box(box, p)) {
+        if (box3d_contains(box, p)) {
             ++c;
-            if (g >= 0) l += rx_in_box(lab, p);
+            if (g >= 0) l += box3d_contains(lab, p);
         }
     }
     c = Reduce(tmp).Sum(c);
@@ -228,12 +218,12 @@ rx_write_kernel(int num_kept, long long num_out, const int32_t *__restrict__ so,
         const int i = i0 + threadIdx.x;
         float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
         if (i < p1) p = fov_pts[i];
-        const int flag = i < p1 && rx_in_box(box, p);
+        const int flag = i < p1 && box3d_contains(box, p);
         int off, total;
         Scan(tmp).ExclusiveSum(flag, off, total);
         if (flag) {
             points[base + run + off] = p;
-            if (with_labels) labels[base + run + off] = rx_in_box(lab, p) ? 1 : 0;
+            if (with_labels) labels[base + run + off] = box3d_contains(lab, p) ? 1 : 0;
         }
         run += total;
         __syncthreads();

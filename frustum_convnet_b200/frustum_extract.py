@@ -91,8 +91,8 @@ def _scan(scan, dev, who):
 
 
 def scan_table(scans, calibs, image_hw, frame_ids, dev, who):
-    """The frames of both extractors (this module's and refine_extract's), in frame_ids order, checked on the host
-    -> (their scans, the fcn_frustum_frame array, the host scan offsets)."""
+    """The frames of every extractor (this module's, refine_extract's and gt_extract's), in frame_ids order, checked
+    on the host -> (their scans, the fcn_frustum_frame array, the host scan offsets)."""
     sc = [_scan(scans[k], dev, who) for k in frame_ids]
     frames = (_lib.FrustumFrame * len(frame_ids))(*[_frame_record(calibs[k], image_hw[k]) for k in frame_ids])
     return sc, frames, csr_offsets([s.shape[0] for s in sc])

@@ -251,10 +251,16 @@ class TrainBatchBuilder:
 
     @classmethod
     def from_frustums(cls, fr, kind, strides, npoints, classes=None, **kw):
-        """The dataset of a refine_extract.RefineFrustums: its points stay on the device (the x, y, z columns are
-        copied there), the per-frustum constants come from its host lists.  The same batches as set_dataset on
-        fr's lists.  labels defaults to whether fr has ground truth."""
-        if kind != "refine":
+        """The dataset of a refine_extract.RefineFrustums (kind="refine") or a gt_extract.GtFrustums (kind="det"): its
+        points stay on the device (the x, y, z columns are copied there; a GtFrustums' uint8 labels are cast to the
+        int32 seg labels there), the per-frustum constants come from its host lists.  The same batches as
+        set_dataset on fr's lists.  labels defaults to whether fr has ground truth."""
+        from .gt_extract import GtFrustums
+        gt = isinstance(fr, GtFrustums)
+        if gt and kind != "det":
+            raise ValueError("from_frustums builds the detection provider's batches (kind='det') from GtFrustums, "
+                             "got %r" % kind)
+        if not gt and kind != "refine":
             raise ValueError("from_frustums builds the refinement provider's batches (kind='refine'), got %r" % kind)
         kw.setdefault("labels", fr.has_labels)
         tb = cls(kind, strides, npoints, **kw)
@@ -266,17 +272,18 @@ class TrainBatchBuilder:
         if fr.points.device.type != "cuda" or (tb.device.index is not None and fr.points.device != tb.device):
             raise RuntimeError("the frustums live on %s, the builder on %s" % (fr.points.device, tb.device))
         counts = np.asarray(fr.counts, dtype=np.int64)
-        fr.wait()                          # the points were written on the extraction's stream
-        names = ("box3d_list", "heading_list", "size_list", "prob_list", "pred_box3d_list", "pred_box3d_size_list",
-                 "pred_box3d_angle_list")
+        fr.wait()                          # the points and labels were written on the extraction's stream
+        names = ("box3d_list", "heading_list", "size_list") + (
+            ("frustum_angle_list", "box2d_list", "calib_list") if gt else
+            ("prob_list", "pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list"))
         table = frustum_table(kind, tb.strides, tb.max_depth, tb.labels,
                               KITTI_CLASSES if classes is None else classes, fr.type_list,
                               **{n: getattr(fr, n) for n in names})
         tb.points_f64 = False
-        tb._install(table, counts, fr.points[:, :3].contiguous(), None)
+        tb._install(table, counts, fr.points[:, :3].contiguous(), None, fr.label.to(torch.int32) if gt else None)
         return tb
 
-    def _install(self, fr, counts, d_points, label_list):
+    def _install(self, fr, counts, d_points, label_list, d_seg=None):
         S = len(self.strides)
         self.T_of = fr["T"][:, :S].astype(np.int64)
         self.counts = counts
@@ -284,8 +291,8 @@ class TrainBatchBuilder:
         self.d_points = d_points
         self.d_offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)).to(dev)
         self.d_frustums = torch.from_numpy(fr.view(np.uint8)).to(dev)
-        self.d_seg = None
-        if self._has_seg:
+        self.d_seg = d_seg
+        if self._has_seg and d_seg is None:
             seg = np.concatenate([np.asarray(s).astype(np.int64) for s in label_list])  # provider_sample.py:206
             if len(seg) != len(d_points) or (np.abs(seg) >= 2 ** 31).any():
                 raise ValueError("label_list must hold one int32-range label per point")

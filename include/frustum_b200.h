@@ -865,6 +865,56 @@ FCN_API long long fcn_refine_extract_workspace_bytes(const fcn_refine_extract_ar
 FCN_API int fcn_refine_extract_count(const fcn_refine_extract_args *args, fcn_stream_t stream);
 FCN_API int fcn_refine_extract_write(const fcn_refine_extract_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (17) KITTI first-stage training frustums on the device: the point work of extract_frustum_data and
+ *      extract_frustum_det_data of kitti/prepare_data.py:102-391 (--gen_train, --gen_val and the _det extension) for
+ *      several frames and all their jobs at once.
+ *
+ *      The frames' in-image points and their float64 image coordinates u, v are those of section (15) (same
+ *      projection, same test, scan order).  A job j (jobs[j]) is one cutting 2-D box in frame jobs[j].frame and one
+ *      label 3-D box label_boxes[jobs[j].label] (fcn_refine_box of section (16): centre (tx, ty - h/2, tz), half extents
+ *      (l/2, h/2, w/2), ry; the corners of kitti_util.compute_box_3d).  The job's points are the frame's in-image
+ *      points with u < xmax, u >= xmin, v < ymax and v >= ymin for the box as given (not clipped); a point is labelled
+ *      1 when the section (16) half-space test puts it in the label box.  The job is dropped when no point is labelled.
+ *      The perturbation, the 2-D matching and the 25-px rule are the caller's: pass only the jobs to cut.
+ *
+ *      Two calls in order on one stream, sharing the caller's workspace (fcn_gt_extract_workspace_bytes: needs the
+ *      device, -1 on invalid arguments), no host sync, no allocation:
+ *        fcn_gt_extract_count : writes job_points (DEVICE, num_jobs: the job's point count when kept, -1 when dropped
+ *                               or when its frame or label index is out of range) and info (DEVICE int64[4]: kept jobs
+ *                               K, their points M, jobs with an out-of-range index, 0);
+ *        fcn_gt_extract_write : needs num_kept = K and num_out_points = M as read by the host; writes the kept jobs in
+ *                               job order: points (M, 4) float32 rect x, y, z and intensity in scan order, labels (M)
+ *                               uint8 and offsets (K + 1) int32.  The k-th kept job is the k-th j with
+ *                               job_points[j] >= 0.
+ *      With num_frames == 0 or num_jobs == 0 both calls return 0 and do nothing (K = M = 0; info is not written).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+    double box[4];      /* cutting box xmin, ymin, xmax, ymax */
+    int32_t frame;      /* index into frames */
+    int32_t label;      /* index into label_boxes */
+} fcn_gt_job;
+typedef struct {
+    int num_frames, num_points, num_jobs, num_labels, num_kept, reserved;
+    long long num_out_points;
+    const float *scans;                 /* DEVICE (num_points, 4), 16-byte aligned */
+    const int32_t *scan_offsets;        /* DEVICE (num_frames + 1) */
+    const int32_t *host_scan_offsets;   /* HOST copy: starts at 0, never decreases, ends at num_points */
+    const fcn_frustum_frame *frames;    /* DEVICE (num_frames) */
+    const fcn_gt_job *jobs;             /* DEVICE (num_jobs) */
+    const fcn_refine_box *label_boxes;  /* DEVICE (num_labels) */
+    void *workspace;
+    long long workspace_bytes;
+    long long *info;                    /* DEVICE int64[4] */
+    int32_t *job_points;                /* DEVICE (num_jobs) */
+    float *points;                      /* fcn_gt_extract_write outputs (DEVICE) */
+    uint8_t *labels;
+    int32_t *offsets;
+} fcn_gt_extract_args;
+FCN_API long long fcn_gt_extract_workspace_bytes(const fcn_gt_extract_args *args);
+FCN_API int fcn_gt_extract_count(const fcn_gt_extract_args *args, fcn_stream_t stream);
+FCN_API int fcn_gt_extract_write(const fcn_gt_extract_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
