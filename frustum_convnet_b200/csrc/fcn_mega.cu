@@ -13,13 +13,15 @@
 //     CTA whose dependencies are complete - no grid-wide barrier, no co-residency requirement, late CTAs
 //     (several forwards are in flight on other streams) simply pick up what is left;
 //   * layer-to-layer dependencies are per row tile: the epilogue of a tile publishes a counter
-//     (release, gpu scope); the TMA producer of a consumer tile acquires the counters of the (<= 4) source
-//     tiles it reads (taps +-1, stride 2, pixel-shuffled transposed convs), then crosses to the async proxy;
-//   * inside a CTA the same warp-specialised pipeline as conv_gemm_tma.cu, made continuous across jobs: warp 8 =
-//     scheduler + TMA producer (A boxes by cp.async.bulk.tensor with the conv taps / stride in the coordinates,
-//     weight stage images by bulk copies), warps 0-7 = two consumer warpgroups (wgmma, 64 rows each, N = NT =
-//     256 | 128 | 64) that also run the epilogue; the smem stage ring runs across job boundaries (the next job's
-//     operands stream while the current one is still multiplied or stored);
+//     (release, gpu scope); the scheduler warp acquires the counters of the (<= 4) source tiles a job reads
+//     (taps +-1, stride 2, pixel-shuffled transposed convs) one job ahead, the TMA producer then crosses to the
+//     async proxy;
+//   * inside a CTA the same warp-specialised pipeline as conv_gemm_tma.cu, made continuous across jobs: warp 9 =
+//     scheduler (job fetch, descriptor, dependency polling), warp 8 = TMA producer (A boxes by cp.async.bulk.tensor
+//     with the conv taps / stride in the coordinates, weight atoms by bulk copies), warps 0-7 = two consumer
+//     warpgroups (wgmma, 64 rows each, N = NT = 256 | 128 | 64) that also run the epilogue; the smem stage ring of
+//     32-wide K atoms runs across job boundaries (the next job's operands stream while the current one is still
+//     multiplied or stored);
 //   * the heads tile (NT = 64: all 2 + 39 logits of a position) stores the logits row and decodes it
 //     (decode.cuh - the same function the stand-alone decode kernel uses), writing the 6-tuple to the local
 //     result block AND to the peers' gather buffers over NVLink (multi-GPU: no NCCL all-gather, no extra
@@ -35,17 +37,25 @@ namespace fcn {
 using namespace gmma;
 
 constexpr int MG_ROWS = 128;
-constexpr int MG_MMA_WARPS = 8;      // warps 0-7: two consumer warpgroups (MMA + epilogue); warp 8: scheduler + TMA
-constexpr int MG_THREADS = (MG_MMA_WARPS + 1) * 32;
-constexpr int MG_NSTAGE = 3;         // stage slot: 2 x 16 KB of A + 32 KB of W (NT <= 128: 64-wide K; NT = 256: 32-wide)
-constexpr int MG_A_ATOM = MG_ROWS * 128, MG_A_STAGE = 2 * MG_A_ATOM;
-constexpr int MG_W_STAGE = 2 * 128 * 128;                     // two [128 x 32] atoms or one [256 x 32] atom
-__host__ __device__ constexpr int mg_k_atoms(int NT) { return NT == 256 ? 1 : 2; }   // 32-wide K atoms per stage
-constexpr int MG_OFF_W = MG_NSTAGE * MG_A_STAGE;
-constexpr int MG_OFF_BAR = MG_OFF_W + MG_NSTAGE * MG_W_STAGE;
+constexpr int MG_MMA_WARPS = 8;      // warps 0-7: two consumer warpgroups (MMA + epilogue)
+constexpr int MG_TMA_WARP = MG_MMA_WARPS, MG_SCHED_WARP = MG_MMA_WARPS + 1;
+constexpr int MG_THREADS = (MG_MMA_WARPS + 2) * 32;
+// Stage ring: every stage carries ONE 32-wide K atom, a slot = [128 x 32] A box + [NT x 32] W image of the table's
+// widest tile, and the ring holds as many slots as fit in MG_RING_BYTES (NT <= 128: 6 x 32 KB, NT = 256: 4 x 48 KB).
+// Fine-grained slots keep more K ahead of the MMAs: the consumers hold two slots (the stage being multiplied and
+// the one whose wgmma group has not retired yet), the producer fills the rest.
+constexpr int MG_A_ATOM = MG_ROWS * 128;
+constexpr int MG_RING_BYTES = 192 * 1024, MG_MAX_SLOTS = 8;
+__host__ __device__ constexpr int mg_slot_bytes(int nt_max) { return MG_A_ATOM + nt_max * 128; }
+__host__ __device__ constexpr int mg_slots(int nt_max) {
+    return MG_RING_BYTES / mg_slot_bytes(nt_max) < MG_MAX_SLOTS ? MG_RING_BYTES / mg_slot_bytes(nt_max) : MG_MAX_SLOTS;
+}
+static_assert(mg_slots(256) >= 3, "the widest tile needs a ring of at least three slots");
+__host__ __device__ constexpr int mg_k_atoms(int NT) { return NT == 256 ? 1 : 2; }   // per stage of the weight image
+constexpr int MG_OFF_BAR = MG_RING_BYTES;
 constexpr int MG_JOBQ = 4;                                    // job descriptors in flight inside a CTA
-constexpr int MG_NBAR = 2 * MG_NSTAGE + 2 * MG_JOBQ;          // full/empty, job_full/job_empty
-constexpr int MG_OFF_JOBQ = MG_OFF_BAR + MG_NBAR * 8;         // fcn_mega_job[MG_JOBQ] (64 B each)
+constexpr int MG_NBAR = 2 * MG_MAX_SLOTS + 2 * MG_JOBQ + 1;   // full/empty, job_full/job_empty, taken
+constexpr int MG_OFF_JOBQ = MG_OFF_BAR + ((MG_NBAR * 8 + 63) & ~63);   // fcn_mega_job[MG_JOBQ] (64 B each)
 constexpr int MG_MAX_LAYERS = 24, MG_MAX_MAPS = 48;
 constexpr int MG_BYTES = MG_OFF_JOBQ + MG_JOBQ * (int)sizeof(fcn_mega_job) + 1024;
 static_assert(MG_BYTES <= 232448, "exceeds the 227 KB shared-memory limit per CTA");
@@ -57,6 +67,7 @@ struct alignas(64) MegaParams {
     CUtensorMap maps[MG_MAX_MAPS];
     fcn_mega_layer layers[MG_MAX_LAYERS];
     fcn_mega_args a;
+    int n_slot, slot_bytes;          // stage ring geometry (mg_slots / mg_slot_bytes of the widest tile)
 };
 static_assert(sizeof(MegaParams) <= 32000, "kernel parameter space");
 
@@ -79,53 +90,82 @@ __device__ __forceinline__ void red_release_gpu_add(int *p, int v) {
 // generic-proxy writes of other SMs (observed through the acquire above) -> subsequent async-proxy (TMA) reads
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;\n" ::: "memory"); }
 
-// One job of a consumer warpgroup: the K loop of its 64 rows x NT columns over the stage ring (`stage` runs on
-// across jobs), then the epilogue.  A stage is handed back when the wgmma group that read it has retired.
+// Phase timeline (off unless fcn_mega_args.dbg_clocks is set): one row of 16 clock64 values per job, for the first
+// MG_DBG_JOBS jobs of every CTA, at dbg_clocks[(blockIdx.x * MG_DBG_JOBS + q) * 16]:
+//   [0] TMA lane took the job  [1] job index  [2] scheduler fetched it  [3] its dependencies were met
+//   [4] TMA lane issued its last box  [5] TMA clocks spent in `empty` waits
+//   [6 + 4 wg] first `full` satisfied  [7 + 4 wg] clocks in `full` waits  [8 + 4 wg] last MMA retired
+//   [9 + 4 wg] epilogue done (warp 0 of consumer warpgroup wg)  [14] layer  [15] SM id
+// Clocks are per SM: compare them within a row or a CTA only.
+constexpr int MG_DBG_JOBS = 64;
+__device__ __forceinline__ long long *mg_dbg_row(const fcn_mega_args &p, uint32_t q) {
+    return (p.dbg_clocks != nullptr && q < MG_DBG_JOBS) ? p.dbg_clocks + 16 * ((size_t)blockIdx.x * MG_DBG_JOBS + q)
+                                                        : nullptr;
+}
+__device__ __forceinline__ int smid() {
+    int v;
+    asm volatile("mov.u32 %0, %%smid;\n" : "=r"(v));
+    return v;
+}
+
+// column groups whose bias pairs the epilogue loads together (NT = 256: the accumulator leaves room for two)
+__host__ __device__ constexpr int mg_epi_batch(int NT) { return NT == 256 ? 2 : 8; }
+
+// One job of a consumer warpgroup: the K loop of its 64 rows x NT columns over the stage ring (ring position
+// `st`, phase `ph` run on across jobs), then the epilogue.  A stage is handed back when the wgmma group that read
+// it has retired.
 template <int NT>
 __device__ __forceinline__ void mg_job(const MegaParams &P, const fcn_mega_layer &L, int m_tile, int n_tile,
-                                       uint32_t &stage, uint8_t *sA, uint8_t *sW, uint64_t *full, uint64_t *empty,
-                                       int *flags) {
+                                       uint32_t &st, uint32_t &ph, uint8_t *ring, uint64_t *full, uint64_t *empty,
+                                       int *flags, long long *dbg) {
     const fcn_mega_args &p = P.a;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3, t = tid & 127;
-    // 32-wide K atoms per stage (the layer table's k_atoms, checked on the host): a compile-time count keeps every
-    // wgmma of a stage in straight-line code
-    constexpr int KA = mg_k_atoms(NT);
-    const int NS = L.n_stage;
-    const uint32_t w_atom16 = (uint32_t)(NT * 128) >> 4;              // second 32-wide K atom of a W stage
-    const uint64_t adesc0 = make_desc_sw128(smem_u32(sA) + wg * (64 * 128));
-    const uint64_t bdesc0 = make_desc_sw128(smem_u32(sW));
+    const int NS = L.n_stage * L.k_atoms;                              // 32-wide K stages of this tile
+    const uint32_t n_slot = (uint32_t)P.n_slot, slot16 = (uint32_t)P.slot_bytes >> 4;
+    const uint64_t adesc0 = make_desc_sw128(smem_u32(ring) + wg * (64 * 128));
+    const uint64_t bdesc0 = make_desc_sw128(smem_u32(ring) + MG_A_ATOM);
     float acc[NT / 2];
 #pragma unroll
     for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
     int prev = -1;
-    for (int s = 0; s < NS; ++s, ++stage) {
-        const uint32_t st = stage % MG_NSTAGE, ph = (stage / MG_NSTAGE) & 1;
+    long long t_first = 0, t_full = 0;                                 // timeline (dbg != nullptr only)
+    for (int s = 0; s < NS; ++s) {
+        const long long t0 = dbg ? clock64() : 0;
         mbar_wait(&full[st], ph);
-        const uint64_t ad = adesc0 + (uint64_t)(st * (MG_A_STAGE >> 4));
-        const uint64_t bd = bdesc0 + (uint64_t)(st * (MG_W_STAGE >> 4));
+        if (dbg) {
+            const long long t1 = clock64();
+            t_full += t1 - t0;
+            if (s == 0) t_first = t1;
+        }
+        const uint64_t ad = adesc0 + (uint64_t)(st * slot16);
+        const uint64_t bd = bdesc0 + (uint64_t)(st * slot16);
         wgmma_fence();
         fence_acc(acc);
 #pragma unroll
-        for (int a = 0; a < KA; ++a)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                wgmma_tf32<NT>(acc, ad + (uint64_t)(a * (MG_A_ATOM >> 4) + 2 * k), bd + (uint64_t)(a * w_atom16 + 2 * k),
-                               (s | a | k) != 0);
+        for (int k = 0; k < 4; ++k) wgmma_tf32<NT>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (s | k) != 0);
         wgmma_commit();
         fence_acc(acc);
         wgmma_wait<1>();
         if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
         prev = (int)st;
+        if (++st == n_slot) { st = 0; ph ^= 1; }
     }
     wgmma_wait<0>();
     fence_acc(acc);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+    if (dbg && lane == 0) { dbg[0] = t_first; dbg[1] = t_full; dbg[2] = clock64(); }
 
     const int rbase = m_tile * MG_ROWS + 64 * wg;                     // first flattened GEMM row of this warpgroup
     if (!L.is_heads) {
         // +bias (+ReLU, TF32 rounding) -> the output map.  One GEMM row holds `up` consecutive output positions
         // (pixel shuffle of the transposed convs): row r, column n = jj*Cout + co -> out[r][jj][c_off + co].
         // Pad positions (past T_out / T_store) are written as zeros: the next layer's taps read them.
+        // The bias pairs of mg_epi_batch(NT) column groups are loaded together, unconditionally (clamped to a valid
+        // column), ahead of their stores: a load behind each store's conditions serialised the epilogue on the
+        // load latency.
+        constexpr int EB = mg_epi_batch(NT);
+        const float *bias = L.bias;
+        const int ncols = L.up * L.Cout;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
             const int r = rbase + 16 * wq + (lane >> 2) + 8 * half;
@@ -133,24 +173,34 @@ __device__ __forceinline__ void mg_job(const MegaParams &P, const fcn_mega_layer
             const int rt = r % L.P_m;
             float *orow = L.out + (size_t)r * L.up * L.ld_out + L.c_off;
 #pragma unroll
-            for (int j = 0; j < NT / 8; ++j) {
-                const int n = n_tile * NT + 8 * j + 2 * (lane & 3);   // even; the pair never crosses a Cout boundary
-                if (n >= L.up * L.Cout) continue;
-                const int jj = n / L.Cout, co = n - jj * L.Cout;
-                float2 o = make_float2(0.f, 0.f);
-                if (rt < L.T_out && rt * L.up + jj < L.T_store) {
-                    const float2 bb = __ldg((const float2 *)(L.bias + n));
-                    o = make_float2(acc[4 * j + 2 * half] + bb.x, acc[4 * j + 2 * half + 1] + bb.y);
-                    if (L.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
-                    if (L.round_out) { o.x = to_tf32(o.x); o.y = to_tf32(o.y); }
+            for (int j0 = 0; j0 < NT / 8; j0 += EB) {
+                float2 bb[EB];
+#pragma unroll
+                for (int u = 0; u < EB; ++u) {
+                    const int n = n_tile * NT + 8 * (j0 + u) + 2 * (lane & 3);
+                    bb[u] = __ldg((const float2 *)(bias + min(n, ncols - 2)));
                 }
-                *(float2 *)(orow + jj * L.ld_out + co) = o;
+#pragma unroll
+                for (int u = 0; u < EB; ++u) {
+                    const int j = j0 + u;
+                    const int n = n_tile * NT + 8 * j + 2 * (lane & 3);   // even; a pair never crosses a Cout boundary
+                    if (n >= ncols) continue;
+                    const int jj = n / L.Cout, co = n - jj * L.Cout;
+                    float2 o = make_float2(0.f, 0.f);
+                    if (rt < L.T_out && rt * L.up + jj < L.T_store) {
+                        o = make_float2(acc[4 * j + 2 * half] + bb[u].x, acc[4 * j + 2 * half + 1] + bb[u].y);
+                        if (L.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                        if (L.round_out) { o.x = to_tf32(o.x); o.y = to_tf32(o.y); }
+                    }
+                    *(float2 *)(orow + jj * L.ld_out + co) = o;
+                }
             }
         }
         // publish: one count per consumer warp once its stores are visible at gpu scope
         __threadfence();
         __syncwarp();
         if (lane == 0) red_release_gpu_add(flags + L.flag_base + m_tile, 1);
+        if (dbg && lane == 0) dbg[3] = clock64();
         return;
     }
     // heads (NT = 64): store the logits rows, then thread t < 64 of the warpgroup decodes row rbase + t into the
@@ -221,6 +271,7 @@ __device__ __forceinline__ void mg_job(const MegaParams &P, const fcn_mega_layer
     __threadfence();
     __syncwarp();
     if (lane == 0) red_release_gpu_add(flags + L.flag_base + m_tile, 1);
+    if (dbg && lane == 0) dbg[3] = clock64();
 }
 
 __global__ void __launch_bounds__(MG_THREADS, 1)
@@ -228,17 +279,19 @@ fcn_mega_kernel(const __grid_constant__ MegaParams P) {
     const fcn_mega_args &p = P.a;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t *smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-    uint8_t *sA = smem, *sW = smem + MG_OFF_W;
+    uint8_t *ring = smem;
     uint64_t *bars = (uint64_t *)(smem + MG_OFF_BAR);
-    uint64_t *full = bars, *empty = bars + MG_NSTAGE;
-    uint64_t *job_full = bars + 2 * MG_NSTAGE, *job_empty = job_full + MG_JOBQ;
+    uint64_t *full = bars, *empty = bars + MG_MAX_SLOTS;
+    uint64_t *job_full = bars + 2 * MG_MAX_SLOTS, *job_empty = job_full + MG_JOBQ, *taken = job_empty + MG_JOBQ;
     fcn_mega_job *jobq = (fcn_mega_job *)(smem + MG_OFF_JOBQ);
     const fcn_mega_layer *s_layers = P.layers;      // kernel parameters (constant bank)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
-        for (int i = 0; i < MG_NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], MG_MMA_WARPS); }
-        for (int i = 0; i < MG_JOBQ; ++i) { mbar_init(&job_full[i], 1); mbar_init(&job_empty[i], MG_MMA_WARPS); }
+        for (int i = 0; i < MG_MAX_SLOTS; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], MG_MMA_WARPS); }
+        // a queue entry is read by the 8 consumer warps and the TMA lane
+        for (int i = 0; i < MG_JOBQ; ++i) { mbar_init(&job_full[i], 1); mbar_init(&job_empty[i], MG_MMA_WARPS + 1); }
+        mbar_init(taken, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -247,98 +300,92 @@ fcn_mega_kernel(const __grid_constant__ MegaParams P) {
 
     int *job_counter = p.sync, *done_ctas = p.sync + 1, *epoch = p.sync + 2, *flags = p.sync + 4;
 
-    if (warp == MG_MMA_WARPS) {
-        // ================= scheduler + TMA producer (one lane) =================
+    if (warp == MG_SCHED_WARP) {
+        // ================= scheduler: fetches job q+1 and waits for its producer tiles while job q streams ========
+        // A job enters the queue only once its dependencies are met, so the TMA lane never waits on other CTAs.
+        // Job q+1 is taken (atomicAdd) only after the TMA lane has started job q: the CTA holds at most one job that
+        // nobody works on yet, and later CTAs find the rest.  Deadlock-free as before: the jobs of a CTA are taken in
+        // table order and each waits only on earlier jobs, which are running or done.
+        for (uint32_t q = 0;; ++q) {
+            if (q > 0) mbar_wait(taken, (q - 1) & 1);
+            int j = 0;
+            if (lane == 0) j = atomicAdd(job_counter, 1);
+            j = __shfl_sync(0xffffffffu, j, 0);
+            long long *dbg = mg_dbg_row(p, q);
+            if (dbg && lane == 0) { dbg[1] = j; dbg[2] = clock64(); }
+            const uint32_t slot = q % MG_JOBQ;
+            mbar_wait(&job_empty[slot], ((q / MG_JOBQ) & 1) ^ 1);
+            int4 *dst = (int4 *)&jobq[slot];
+            if (j < p.n_jobs) {
+                if (lane < 4) dst[lane] = __ldg((const int4 *)(p.jobs + j) + lane);
+            } else if (lane == 0) {
+                dst[0] = make_int4(-1, 0, 0, 0);
+            }
+            __syncwarp();
+            if (j < p.n_jobs) {
+                // all counters of the producer tiles at once: lane i polls counters i, i+32, ... of each dependency
+                const fcn_mega_job &job = jobq[slot];
+                uint32_t spins = 0;
+                bool ready;
+                do {
+                    ready = true;
+                    for (int d = 0; d < job.n_dep; ++d)
+                        for (int i = lane; i < job.dep[d].count; i += 32)
+                            if (ld_acquire_gpu(flags + job.dep[d].first + i) < job.dep[d].target) ready = false;
+                    if (++spins > (1u << 24)) __trap();   // protocol bug -> launch failure, not a hang
+                } while (!__all_sync(0xffffffffu, ready));
+            }
+            if (dbg && lane == 0) dbg[3] = clock64();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&job_full[slot]);     // release: descriptor + the acquired counters
+            if (j >= p.n_jobs) break;
+        }
+    } else if (warp == MG_TMA_WARP) {
+        // ================= TMA producer (one lane): waits only on the ring and the job queue =================
         if (lane == 0) {
-            uint32_t stage = 0;                       // running K-stage counter across jobs
-            // The job index comes from ONE atomicAdd; index and descriptor of job q+1 are fetched while the first
-            // K stages of job q are in flight (the fetch chain is two dependent L2 round trips, ~1.8 k clk: issued
-            // at the top of a job it left the tensor pipe idle between jobs).
-            auto publish = [&](uint32_t q, int j) -> int {     // descriptor -> queue slot q; returns the layer (-1: end)
+            const uint32_t n_slot = (uint32_t)P.n_slot, slot_bytes = (uint32_t)P.slot_bytes;
+            uint32_t st = 0, ph = 0;                 // ring position and phase, running across jobs
+            for (uint32_t q = 0;; ++q) {
                 const uint32_t slot = q % MG_JOBQ;
-                mbar_wait(&job_empty[slot], ((q / MG_JOBQ) & 1) ^ 1);
-                int4 *dst = (int4 *)&jobq[slot];
-                int layer = -1;
-                if (j < p.n_jobs) {
-                    const int4 *src = (const int4 *)(p.jobs + j);
-                    const int4 a0 = __ldg(src), a1 = __ldg(src + 1), a2 = __ldg(src + 2), a3 = __ldg(src + 3);
-                    dst[0] = a0; dst[1] = a1; dst[2] = a2; dst[3] = a3;
-                    layer = a0.x;
-                } else {
-                    dst[0] = make_int4(-1, 0, 0, 0);
-                }
-                mbar_arrive(&job_full[slot]);         // release: the queue entry is visible to the waiters
-                return layer;
-            };
-            int jcur = atomicAdd(job_counter, 1);
-            int layer = publish(0, jcur);
-            for (uint32_t q = 0; layer >= 0; ++q) {
-                const fcn_mega_job &job = jobq[q % MG_JOBQ];   // own copy in shared memory (slot is reused only
-                                                               // after MG_JOBQ more jobs were published)
+                mbar_wait(&job_full[slot], (q / MG_JOBQ) & 1);
+                const int layer = jobq[slot].layer, m_tile = jobq[slot].m_tile, n_tile = jobq[slot].n_tile;
+                const int n_dep = jobq[slot].n_dep;
+                mbar_arrive(&job_empty[slot]);
+                mbar_arrive(taken);                  // the scheduler may fetch the next job
+                if (layer < 0) break;
+                long long *dbg = mg_dbg_row(p, q);
+                long long t_empty = 0;
+                if (dbg) { dbg[0] = clock64(); dbg[14] = layer; dbg[15] = smid(); }
                 const fcn_mega_layer &L = s_layers[layer];
-                long long *dbg = (p.dbg_clocks != nullptr && blockIdx.x == 0 && q < 64) ? p.dbg_clocks + 16 * q : nullptr;
-                if (dbg) { dbg[0] = clock64(); dbg[1] = jcur; }
-                const int r0 = job.m_tile * MG_ROWS;
-                const int NS = L.n_stage;
-                const int ka = mg_k_atoms(L.NT);
-                const uint32_t w_bytes = (uint32_t)(L.NT * 128 * ka);    // [NT rows x 32 tf32] per atom
-                const uint32_t a_bytes = (uint32_t)(ka * MG_A_ATOM);
-                const uint8_t *wsrc = (const uint8_t *)L.w_tc + (size_t)job.n_tile * NS * w_bytes;
-                // weights do not depend on other tiles: the first ring-full of weight stages streams WHILE this
-                // tile's dependencies are awaited (only the A boxes wait for the producer tiles).  (Issuing every
-                // stage's A boxes individually behind a non-blocking dependency probe is not done.)
-                const int npre = NS < MG_NSTAGE ? NS : MG_NSTAGE;
-                for (int s = 0; s < npre; ++s) {
-                    const uint32_t sg = stage + s, st = sg % MG_NSTAGE, ph = (sg / MG_NSTAGE) & 1;
-                    mbar_wait(&empty[st], ph ^ 1);
-                    mbar_arrive_expect_tx(&full[st], a_bytes + w_bytes);
-                    bulk_g2s(sW + st * MG_W_STAGE, wsrc + (size_t)s * w_bytes, w_bytes, &full[st]);
-                }
-                const int jnext = atomicAdd(job_counter, 1);   // in flight during the dependency wait below
-                // dependencies: the row tiles of the producing layers this tile reads
-                const int n_dep = job.n_dep;
-                for (int d = 0; d < n_dep; ++d) {
-                    const int first = job.dep[d].first, cnt = job.dep[d].count, target = job.dep[d].target;
-                    for (int i = 0; i < cnt; ++i) {
-                        uint32_t spins = 0;
-                        while (ld_acquire_gpu(flags + first + i) < target) {
-                            if (++spins > (1u << 24)) __trap();   // protocol bug -> launch failure, not a hang
-                        }
-                    }
-                }
-                if (dbg) dbg[2] = clock64();
+                const int r0 = m_tile * MG_ROWS;
+                const int NS = L.n_stage * L.k_atoms;
+                const uint32_t w_bytes = (uint32_t)(L.NT * 128);          // one [NT rows x 32 tf32] atom
+                const uint8_t *wsrc = (const uint8_t *)L.w_tc + (size_t)n_tile * NS * w_bytes;
+                // the scheduler acquired the producer tiles' counters (generic proxy): order them before the TMA reads
                 if (n_dep > 0) fence_proxy_async_global();
-                if (dbg) dbg[3] = clock64();
                 int seg = 0, kbi = 0;                 // running (segment, 32-channel block inside the segment)
-                int next_layer = -1;
-                for (int s = 0; s < NS; ++s, ++stage) {
-                    const uint32_t st = stage % MG_NSTAGE, ph = (stage / MG_NSTAGE) & 1;
-                    if (s == npre) next_layer = publish(q + 1, jnext);   // first ring-full issued: fetch the next job
-                    if (s >= npre) {
-                        mbar_wait(&empty[st], ph ^ 1);
-                        mbar_arrive_expect_tx(&full[st], a_bytes + w_bytes);
-                        bulk_g2s(sW + st * MG_W_STAGE, wsrc + (size_t)s * w_bytes, w_bytes, &full[st]);
+                for (int s = 0; s < NS; ++s) {
+                    const long long t0 = dbg ? clock64() : 0;
+                    mbar_wait(&empty[st], ph ^ 1);
+                    if (dbg) t_empty += clock64() - t0;
+                    uint8_t *sl = ring + st * slot_bytes;
+                    mbar_arrive_expect_tx(&full[st], MG_A_ATOM + w_bytes);
+                    bulk_g2s(sl + MG_A_ATOM, wsrc + (size_t)s * w_bytes, w_bytes, &full[st]);
+                    if (seg < L.n_seg) {
+                        const fcn_mega_seg &sgm = L.seg[seg];
+                        mg_tma_load_3d(smem_u32(sl), &P.maps[sgm.map_idx], kbi * 32, r0 * sgm.stride + sgm.tap, 0, &full[st]);
+                        if (++kbi >= sgm.kblocks) { kbi = 0; ++seg; }
+                    } else {   // K padding block: a box fully outside the channel range -> zeros
+                        mg_tma_load_3d(smem_u32(sl), &P.maps[L.seg[0].map_idx], 1 << 20, 0, 0, &full[st]);
                     }
-                    for (int a = 0; a < ka; ++a) {
-                        const uint32_t dst = smem_u32(sA) + st * MG_A_STAGE + a * MG_A_ATOM;
-                        if (seg < L.n_seg) {
-                            const fcn_mega_seg &sgm = L.seg[seg];
-                            mg_tma_load_3d(dst, &P.maps[sgm.map_idx], kbi * 32, r0 * sgm.stride + sgm.tap, 0, &full[st]);
-                            if (++kbi >= sgm.kblocks) { kbi = 0; ++seg; }
-                        } else {   // K padding block: a box fully outside the channel range -> zeros
-                            mg_tma_load_3d(dst, &P.maps[L.seg[0].map_idx], 1 << 20, 0, 0, &full[st]);
-                        }
-                    }
+                    if (++st == n_slot) { st = 0; ph ^= 1; }
                 }
-                if (NS <= npre) next_layer = publish(q + 1, jnext);
-                if (dbg) dbg[4] = clock64();
-                layer = next_layer;
-                jcur = jnext;
+                if (dbg) { dbg[4] = clock64(); dbg[5] = t_empty; }
             }
         }
     } else {
         // ================= consumer warpgroups: MMA + epilogue of every job, 64 rows each =================
-        uint32_t stage = 0;
+        uint32_t st = 0, ph = 0;
         for (uint32_t q = 0;; ++q) {
             const uint32_t slot = q % MG_JOBQ;
             mbar_wait(&job_full[slot], (q / MG_JOBQ) & 1);
@@ -347,9 +394,11 @@ fcn_mega_kernel(const __grid_constant__ MegaParams P) {
             if (lane == 0) mbar_arrive(&job_empty[slot]);
             if (layer < 0) break;
             const fcn_mega_layer &L = s_layers[layer];
-            if (L.NT == 256) mg_job<256>(P, L, m_tile, n_tile, stage, sA, sW, full, empty, flags);
-            else if (L.NT == 128) mg_job<128>(P, L, m_tile, n_tile, stage, sA, sW, full, empty, flags);
-            else mg_job<64>(P, L, m_tile, n_tile, stage, sA, sW, full, empty, flags);
+            long long *dbg = (warp & 3) == 0 ? mg_dbg_row(p, q) : nullptr;   // warp 0 of each warpgroup
+            if (dbg) dbg += 6 + 4 * (warp >> 2);
+            if (L.NT == 256) mg_job<256>(P, L, m_tile, n_tile, st, ph, ring, full, empty, flags, dbg);
+            else if (L.NT == 128) mg_job<128>(P, L, m_tile, n_tile, st, ph, ring, full, empty, flags, dbg);
+            else mg_job<64>(P, L, m_tile, n_tile, st, ph, ring, full, empty, flags, dbg);
         }
     }
     if (p.n_out > 1) __threadfence_system();      // this thread's remote (NVLink) result stores, if any
@@ -392,10 +441,12 @@ extern "C" int fcn_mega_forward(const fcn_mega_args *args, fcn_stream_t stream) 
     FCN_REQUIRE(a.n_out >= 0 && a.n_out <= FCN_MAX_PEERS && a.n_flag_out >= 0 && a.n_flag_out <= FCN_MAX_PEERS,
                 "too many output sets");
     FCN_REQUIRE(a.NH >= 1 && a.NH <= DEC_MAX_BINS && a.NS >= 1 && a.NS <= DEC_MAX_BINS, "bad decode sizes");
+    int nt_max = 0;
     for (int i = 0; i < a.n_layers; ++i) {
         const fcn_mega_layer &L = a.layers[i];
         FCN_REQUIRE((L.NT == 64 || L.NT == 128 || L.NT == 256) && L.k_atoms == mg_k_atoms(L.NT),
                     "layer tile width must be 64, 128 or 256, with k_atoms = 1 for 256 and 2 otherwise");
+        nt_max = L.NT > nt_max ? L.NT : nt_max;
     }
     if (a.n_jobs == 0) return FCN_OK;
     static_assert(sizeof(DecodeOut) == sizeof(fcn_decode_out), "decode output block layout");
@@ -407,6 +458,8 @@ extern "C" int fcn_mega_forward(const fcn_mega_args *args, fcn_stream_t stream) 
     memcpy(P.maps, a.tmaps, sizeof(CUtensorMap) * a.n_maps);   // HOST arrays -> kernel parameters
     memcpy(P.layers, a.layers, sizeof(fcn_mega_layer) * a.n_layers);
     P.a = a;
+    P.n_slot = mg_slots(nt_max);              // every accepted tile width fits (static_assert on mg_slots(256))
+    P.slot_bytes = mg_slot_bytes(nt_max);
     static const int prio = env_priority("FCN_PRIO_CONV");
     FCN_CUDA(launch_pdl_prio(prio, fcn_mega_kernel, dim3(grid), dim3(MG_THREADS), (size_t)MG_BYTES, (cudaStream_t)stream, P));
     return FCN_OK;

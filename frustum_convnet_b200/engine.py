@@ -120,7 +120,7 @@ class FrustumEngine:
         # persistent CTAs per forward.  A CTA that waits for a producer tile holds its SM idle: FEW CTAs per forward
         # and several forwards in flight favour throughput; FCN_MEGA_GRID=<SM count> favours the latency of a single
         # forward instead.  0 = adaptive: 2/3 of the smallest per-layer tile count of the main chain, within [4, 48]
-        # (car B=32: 24, people: 48, SUN-RGBD: 6)
+        # (B=32: car 24, people 30, SUN-RGBD 6)
         self.mega_grid = int(os.environ.get("FCN_MEGA_GRID", "0"))
         # 256-wide N tiles for the layers with >= 256 output columns: less shared-memory traffic per MAC (the A box
         # feeds twice as many MMA columns) but half as many jobs per layer.  "auto" uses them when every main-chain

@@ -34,7 +34,7 @@ class LayerDesc:
         self.ld_out, self.P_store, self.T_store = ld_out, P_store, T_store
         self.m_tiles = (n_rows + ROWS - 1) // ROWS
         self.n_tiles = n_cols // NT
-        self.k_atoms = 1 if NT == 256 else 2       # 32-wide K atoms per shared-memory stage (stage = 64 KB at most)
+        self.k_atoms = 1 if NT == 256 else 2       # 32-wide K atoms per stage of the packed weight image
 
 
 def chain_tiles(layers: Sequence[LayerDesc]) -> int:

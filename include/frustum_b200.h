@@ -210,14 +210,15 @@ typedef struct {
 typedef struct {
     int n_seg;
     fcn_mega_seg seg[FCN_MAX_SEGS];
-    int n_stage;                 /* K stages per tile: K_pad / (32 * k_atoms) */
+    int n_stage;                 /* weight-image stages per tile: K_pad / (32 * k_atoms) */
     int NT, n_tiles_n;           /* N tile (256 | 128 | 64) and their number */
     int relu, round_out, up, Cout;
     int P_m, T_out, n_rows;      /* GEMM row space: row r = b*P_m + t, valid iff t < T_out; n_rows = B*P_m */
     int ld_out, P_store, T_store, c_off;
     int is_heads, flag_base;
     int out_map;                 /* tensor map of the epilogue's TMA store (fcn_encode_store_map); unused for heads */
-    int k_atoms;                 /* 32-wide K atoms per stage: 2 (NT <= 128) or 1 (NT = 256); 0 reads as 2 */
+    int k_atoms;                 /* 32-wide K atoms per weight-image stage: 2 (NT <= 128) or 1 (NT = 256); the kernel
+                                    streams n_stage * k_atoms stages of one atom each */
     const void *w_tc;            /* packed stage images, N-tile major */
     const float *bias;
     float *out;
@@ -238,7 +239,8 @@ typedef struct {
     int n_out, n_flag_out;
     fcn_decode_out outs[FCN_MAX_PEERS];
     int32_t *flag_out[FCN_MAX_PEERS];
-    long long *dbg_clocks;                 /* optional (NULL): CTA 0 dumps 16 timestamps per job (first 64 jobs) */
+    long long *dbg_clocks;                 /* optional (NULL): phase timeline, 16 clocks per job for the first 64
+                                              jobs of every CTA (grid x 64 x 16 values; fcn_mega.cu) */
 } fcn_mega_args;
 FCN_API int fcn_mega_forward(const fcn_mega_args *args, fcn_stream_t stream);
 
