@@ -2,9 +2,10 @@
 // kitti/prepare_data.py:462-568 for several frames and all their 2-D detections in one pair of calls.
 //
 // The reference re-masks the whole scan for every detection and projects every scan twice.  Here:
-//   fcn_frustum_extract_count  flags    one thread per scan point: velo -> rect -> image in float64 (every product and
-//                                       sum rounded separately, kitti_util.py:172-210) and the image test of
-//                                       get_lidar_in_image_fov (draw_util.py:15-18);
+//   fcn_frustum_extract_count  flags    (csrc/frustum_fov.cu, as the scans and compact below) one thread per scan
+//                                       point: velo -> rect -> image in float64 (every product and sum rounded
+//                                       separately, kitti_util.py:172-210) and the image test of get_lidar_in_image_fov
+//                                       (draw_util.py:15-18);
 //                              scan     exclusive sum of the flags over all frames (frames stay contiguous, scan order
 //                                       is kept): the position of every in-image point;
 //                              compact  the in-image points, recomputed, stored at those positions: float32 rect and
@@ -15,8 +16,6 @@
 //                              scans    exclusive sums over the kept detections and their point counts, then info;
 //   fcn_frustum_extract_write  write    one CTA per kept detection: the box test again, a block scan for stable
 //                                       positions, the points scattered in scan order, and the per-detection values.
-#include <cub/cub.cuh>
-
 #include <cmath>
 
 #include "common.cuh"
@@ -24,19 +23,6 @@
 #include "input_builder.cuh"
 
 namespace fcn {
-
-__global__ void __launch_bounds__(FX_THREADS)
-fx_flag_kernel(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
-               const fcn_frustum_frame *__restrict__ frames, int32_t *__restrict__ flags) {
-    fov_flag(scans, so, frames, flags);
-}
-
-__global__ void __launch_bounds__(FX_THREADS)
-fx_compact_kernel(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
-                  const fcn_frustum_frame *__restrict__ frames, const int32_t *__restrict__ pos,
-                  float4 *__restrict__ fov_pts, double *__restrict__ fov_u, double *__restrict__ fov_v) {
-    fov_compact<true>(scans, so, frames, pos, fov_pts, fov_u, fov_v);
-}
 
 // np.clip(a, 0, hi): NaN stays NaN
 __device__ __forceinline__ double fx_clip(double a, double hi) {
@@ -54,14 +40,10 @@ fx_count_kernel(int num_frames, const int32_t *__restrict__ so, const fcn_frustu
                 const int32_t *__restrict__ pos, const double *__restrict__ fov_u, const double *__restrict__ fov_v,
                 int32_t *__restrict__ det_points, int32_t *__restrict__ keep, long long *__restrict__ cnt,
                 double *__restrict__ box_ws, double *__restrict__ angle_ws, int32_t *__restrict__ bad) {
-    using Reduce = cub::BlockReduce<int, FX_THREADS>;
-    __shared__ typename Reduce::TempStorage tmp;
     const int d = blockIdx.x, f = det_frame[d];
     if (f < 0 || f >= num_frames) {
         if (threadIdx.x == 0) {
-            det_points[d] = -1;
-            keep[d] = 0;
-            cnt[d] = 0;
+            job_words(d, true, 0, det_points, keep, cnt);
             atomicAdd(bad, 1);
         }
         return;
@@ -73,14 +55,10 @@ fx_count_kernel(int num_frames, const int32_t *__restrict__ so, const fcn_frustu
     b[2] = fx_clip(boxes[4 * d + 2], (double)(fr->width - 1));
     b[3] = fx_clip(boxes[4 * d + 3], (double)(fr->height - 1));
     const int p0 = pos[so[f]], p1 = pos[so[f + 1]];
-    int c = 0;
-    for (int i = p0 + threadIdx.x; i < p1; i += FX_THREADS) c += fx_in_box(fov_u[i], fov_v[i], b);
-    c = Reduce(tmp).Sum(c);
+    int c, l;
+    job_count<false>(p0, p1, c, l, [&](int i, int &n, int &) { n += fx_in_box(fov_u[i], fov_v[i], b); });
     if (threadIdx.x == 0) {
-        const bool drop = b[3] - b[1] < 5.0 || b[2] - b[0] < 1.0 || c < 1;
-        det_points[d] = drop ? -1 : c;
-        keep[d] = drop ? 0 : 1;
-        cnt[d] = drop ? 0 : c;
+        job_words(d, b[3] - b[1] < 5.0 || b[2] - b[0] < 1.0 || c < 1, c, det_points, keep, cnt);
         const RectProjection rp(b, fr->P);
         double x, y;
         rp.at(20.0, &x, &y);
@@ -88,15 +66,6 @@ fx_count_kernel(int num_frames, const int32_t *__restrict__ so, const fcn_frustu
 #pragma unroll
         for (int j = 0; j < 4; ++j) box_ws[4 * d + j] = b[j];
     }
-}
-
-__global__ void fx_info_kernel(int num_dets, const int32_t *__restrict__ keep_pos,
-                               const long long *__restrict__ cnt_pos, const int32_t *__restrict__ bad,
-                               long long *__restrict__ info) {
-    info[0] = keep_pos[num_dets];
-    info[1] = cnt_pos[num_dets];
-    info[2] = *bad;
-    info[3] = 0;
 }
 
 __global__ void __launch_bounds__(FX_THREADS)
@@ -109,13 +78,13 @@ fx_write_kernel(int num_kept, long long num_out, const int32_t *__restrict__ so,
                 const double *__restrict__ fov_v, float4 *__restrict__ points, int32_t *__restrict__ offsets,
                 double *__restrict__ angle, double *__restrict__ box2d, double *__restrict__ P,
                 int32_t *__restrict__ det_index) {
-    using Scan = cub::BlockScan<int, FX_THREADS>;
-    __shared__ typename Scan::TempStorage tmp;
+    // kept_slot's guard spelled out: offsets[k + 1] is written with the per-detection values, where this kernel has
+    // always written it (kept_slot's earlier store changes its instruction schedule)
     const int d = blockIdx.x, c = det_points[d];
     if (c < 0) return;
     const int k = keep_pos[d];
     const long long base = cnt_pos[d];
-    if (k >= num_kept || base + c > num_out) return;     // sizes read by the host disagree with the count pass
+    if (k >= num_kept || base + c > num_out) return;
     const int f = det_frame[d];
     const double *b = box_ws + 4 * d;
     if (threadIdx.x < 12) P[12 * k + threadIdx.x] = frames[f].P[threadIdx.x];
@@ -126,56 +95,20 @@ fx_write_kernel(int num_kept, long long num_out, const int32_t *__restrict__ so,
         det_index[k] = d;
     }
     const double bb[4] = {b[0], b[1], b[2], b[3]};
-    const int p0 = pos[so[f]], p1 = pos[so[f + 1]];
-    int run = 0;
-    for (int i0 = p0; i0 < p1 && run < c; i0 += FX_THREADS) {
-        const int i = i0 + threadIdx.x;
-        const int flag = i < p1 && fx_in_box(fov_u[i], fov_v[i], bb);
-        int off, total;
-        Scan(tmp).ExclusiveSum(flag, off, total);
-        if (flag) points[base + run + off] = fov_pts[i];
-        run += total;
-        __syncthreads();
-    }
+    job_scatter(pos[so[f]], pos[so[f + 1]], c, base, [&](int i) { return fx_in_box(fov_u[i], fov_v[i], bb); },
+                [&](long long o, int i) { points[o] = fov_pts[i]; });
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-struct FxWs {
-    int32_t *flags, *pos, *keep, *keep_pos, *bad;
-    long long *cnt, *cnt_pos;
-    float4 *fov_pts;
-    double *fov_u, *fov_v, *box, *angle;
-    void *temp;
-    size_t temp_bytes;
+struct FxWs : FovWs {
+    double *box, *angle;
 };
 
 static cudaError_t fx_layout(const fcn_frustum_extract_args *a, Carve &c, FxWs &w) {
-    const size_t N = (size_t)a->num_points, D = (size_t)a->num_dets;
-    size_t t0 = 0, t1 = 0, t2 = 0;
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, t0, (const int32_t *)nullptr, (int32_t *)nullptr,
-                                                  a->num_points + 1);
-    if (e != cudaSuccess) return e;
-    e = cub::DeviceScan::ExclusiveSum(nullptr, t1, (const int32_t *)nullptr, (int32_t *)nullptr, a->num_dets + 1);
-    if (e != cudaSuccess) return e;
-    e = cub::DeviceScan::ExclusiveSum(nullptr, t2, (const long long *)nullptr, (long long *)nullptr,
-                                      a->num_dets + 1);
-    if (e != cudaSuccess) return e;
-    w.temp_bytes = t0 > t1 ? t0 : t1;
-    w.temp_bytes = w.temp_bytes > t2 ? w.temp_bytes : t2;
-    w.flags = (int32_t *)c.take((N + 1) * 4);
-    w.pos = (int32_t *)c.take((N + 1) * 4);
-    w.fov_pts = (float4 *)c.take(N * 16);
-    w.fov_u = (double *)c.take(N * 8);
-    w.fov_v = (double *)c.take(N * 8);
-    w.keep = (int32_t *)c.take((D + 1) * 4);
-    w.keep_pos = (int32_t *)c.take((D + 1) * 4);
-    w.cnt = (long long *)c.take((D + 1) * 8);
-    w.cnt_pos = (long long *)c.take((D + 1) * 8);
-    w.box = (double *)c.take(D * 32);
-    w.angle = (double *)c.take(D * 8);
-    w.bad = (int32_t *)c.take(4);
-    w.temp = c.take(w.temp_bytes);
-    return cudaSuccess;
+    const cudaError_t e = fov_carve(c, a->num_points, a->num_dets, true, w);
+    w.box = (double *)c.take((size_t)a->num_dets * 32);
+    w.angle = (double *)c.take((size_t)a->num_dets * 8);
+    return e;
 }
 
 // Host-side checks shared by every entry: counts, pointers, the scans.  Sets *max_n to the largest scan.
@@ -218,30 +151,12 @@ extern "C" int fcn_frustum_extract_count(const fcn_frustum_extract_args *a, fcn_
     const int st = fx_prepare(a, __func__, w, &max_n);
     if (st != FCN_OK || a->num_frames == 0 || a->num_dets == 0) return st;
     cudaStream_t s = (cudaStream_t)stream;
-    const int N = a->num_points, D = a->num_dets, F = a->num_frames;
-    const float4 *scans = (const float4 *)a->scans;
-    FCN_CUDA(cudaMemsetAsync(w.flags + N, 0, 4, s));
-    FCN_CUDA(cudaMemsetAsync(w.keep + D, 0, 4, s));
-    FCN_CUDA(cudaMemsetAsync(w.cnt + D, 0, 8, s));
-    FCN_CUDA(cudaMemsetAsync(w.bad, 0, 4, s));
-    const dim3 grid(ceil_div(max_n, FX_THREADS), F);
-    if (max_n > 0) {
-        fx_flag_kernel<<<grid, FX_THREADS, 0, s>>>(scans, a->scan_offsets, a->frames, w.flags);
-        FCN_LAUNCH_CHECK();
-    }
-    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.flags, w.pos, N + 1, s));
-    if (max_n > 0) {
-        fx_compact_kernel<<<grid, FX_THREADS, 0, s>>>(scans, a->scan_offsets, a->frames, w.pos, w.fov_pts, w.fov_u,
-                                                      w.fov_v);
-        FCN_LAUNCH_CHECK();
-    }
+    const int D = a->num_dets, F = a->num_frames;
+    FCN_CUDA(fov_stage(w, a->num_points, D, F, max_n, a->scans, a->scan_offsets, a->frames, s));
     fx_count_kernel<<<D, FX_THREADS, 0, s>>>(F, a->scan_offsets, a->frames, a->boxes, a->det_frame, w.pos, w.fov_u,
                                              w.fov_v, a->det_points, w.keep, w.cnt, w.box, w.angle, w.bad);
     FCN_LAUNCH_CHECK();
-    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.keep, w.keep_pos, D + 1, s));
-    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.cnt, w.cnt_pos, D + 1, s));
-    fx_info_kernel<<<1, 1, 0, s>>>(D, w.keep_pos, w.cnt_pos, w.bad, a->info);
-    FCN_LAUNCH_CHECK();
+    FCN_CUDA(job_totals(w, D, a->info, s));
     return FCN_OK;
 }
 

@@ -1,87 +1,101 @@
-// The in-image point stage shared by the KITTI frustum extractors (csrc/frustum_extract.cu, section (15),
-// csrc/refine_extract.cu, section (16), and csrc/gt_extract.cu, section (17)): each scan point projected velo -> rect
-// -> image once in float64 and tested against the image (get_lidar_in_image_fov, draw_util.py:15-18), then the
-// in-image points of every frame compacted in scan order.  The kernels of all three files call these bodies, so they
-// extract exactly the same points.
+// The stages shared by the KITTI frustum extractors (csrc/frustum_extract.cu, section (15), csrc/refine_extract.cu,
+// section (16), and csrc/gt_extract.cu, section (17)).  Each extractor's count entry runs
+//   fov_stage    flag the in-image points, scan the flags, compact the in-image points (csrc/frustum_fov.cu);
+//   its own count kernel, one CTA per job over the job's frame's in-image points (job_count, job_words here);
+//   job_totals   scan the kept flags and the point counts, then the info words;
+// and its write entry one CTA per kept job (kept_slot, job_scatter here).  The extractors differ only in their job
+// tests, drop rules and per-frustum extras, so they extract exactly the same in-image points.
 #pragma once
 
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
+
 #include "common.cuh"
-#include "input_builder.cuh"
 
 namespace fcn {
 
 constexpr int FX_THREADS = 256;
-constexpr int FX_FRAME_DOUBLES = 33;     // P (12), V2C (12), R0 (9) of fcn_frustum_frame
 
-// velo (x, y, z) -> float32 rect and float64 image coordinates; true when the point is in the image.  The order of the
-// operations is restated by oracle/frustum_extract.py.
-__device__ __forceinline__ bool fx_project(const double *__restrict__ m, int height, int width, float4 s, float4 *rect,
-                                           double *u, double *v) {
-    const double *P = m, *V = m + 12, *R = m + 24;
-    const double x = s.x, y = s.y, z = s.z;
-    double ref[3], r[3], img[3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-        ref[i] = dadd<true>(dadd<true>(dadd<true>(dmul<true>(V[4 * i], x), dmul<true>(V[4 * i + 1], y)),
-                                       dmul<true>(V[4 * i + 2], z)), V[4 * i + 3]);
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-        r[i] = dadd<true>(dadd<true>(dmul<true>(R[3 * i], ref[0]), dmul<true>(R[3 * i + 1], ref[1])),
-                          dmul<true>(R[3 * i + 2], ref[2]));
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-        img[i] = dadd<true>(dadd<true>(dadd<true>(dmul<true>(P[4 * i], r[0]), dmul<true>(P[4 * i + 1], r[1])),
-                                       dmul<true>(P[4 * i + 2], r[2])), P[4 * i + 3]);
-    *u = __ddiv_rn(img[0], img[2]);
-    *v = __ddiv_rn(img[1], img[2]);
-    *rect = make_float4((float)r[0], (float)r[1], (float)r[2], s.w);
-    return *u >= 0.0 && *u < (double)width && *v >= 0.0 && *v < (double)height && s.x > 2.0f;
-}
+// Workspace pieces every extractor has; each family carves its own pieces after these.
+struct FovWs {
+    int32_t *flags, *pos, *keep, *keep_pos, *bad;
+    long long *cnt, *cnt_pos;
+    float4 *fov_pts;
+    double *fov_u, *fov_v;      // float64 image coordinates of the in-image points (null unless uv)
+    void *temp;
+    size_t temp_bytes;
+};
 
-// one frame per blockIdx.y; the frame's matrices in shared memory
-__device__ __forceinline__ void fx_load_frame(const fcn_frustum_frame *__restrict__ frames, int f, double *m) {
-    if (threadIdx.x < FX_FRAME_DOUBLES) m[threadIdx.x] = frames[f].P[threadIdx.x];   // P, V2C, R0 are contiguous
-    __syncthreads();
-}
+// Takes the shared pieces for num_points scan points and num_jobs jobs from c (fov_u, fov_v only when uv).
+cudaError_t fov_carve(Carve &c, int num_points, int num_jobs, bool uv, FovWs &w);
 
-// Body of a flag kernel: grid (points of the largest frame / FX_THREADS, frames), flags[i] = point i is in the image.
-__device__ __forceinline__ void fov_flag(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
-                                         const fcn_frustum_frame *__restrict__ frames, int32_t *__restrict__ flags) {
-    __shared__ double m[FX_FRAME_DOUBLES];
-    const int f = blockIdx.y;
-    fx_load_frame(frames, f, m);
-    const int i = so[f] + blockIdx.x * FX_THREADS + threadIdx.x;
-    if (i >= so[f + 1]) return;
-    float4 rect;
-    double u, v;
-    flags[i] = fx_project(m, frames[f].height, frames[f].width, scans[i], &rect, &u, &v) ? 1 : 0;
-}
+// The in-image stage of a count entry on stream s: clears the scan tails and the bad counter, then flags every scan
+// point, scans the flags into pos and compacts the in-image points of each frame, in scan order, to fov_pts (and
+// fov_u, fov_v).  max_n is the largest scan (check_scans), the x extent of the flag and compact grids.
+cudaError_t fov_stage(const FovWs &w, int num_points, int num_jobs, int num_frames, int max_n, const void *scans,
+                      const int32_t *scan_offsets, const fcn_frustum_frame *frames, cudaStream_t s);
 
-// Body of a compact kernel (same grid): every in-image point, recomputed, stored at its exclusive-sum position pos[i]
-// as float32 rect x, y, z and intensity, with its float64 image coordinates when kUV.
-template <bool kUV>
-__device__ __forceinline__ void fov_compact(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
-                                            const fcn_frustum_frame *__restrict__ frames,
-                                            const int32_t *__restrict__ pos, float4 *__restrict__ fov_pts,
-                                            double *__restrict__ fov_u, double *__restrict__ fov_v) {
-    __shared__ double m[FX_FRAME_DOUBLES];
-    const int f = blockIdx.y;
-    fx_load_frame(frames, f, m);
-    const int i = so[f] + blockIdx.x * FX_THREADS + threadIdx.x;
-    if (i >= so[f + 1]) return;
-    float4 rect;
-    double u, v;
-    if (fx_project(m, frames[f].height, frames[f].width, scans[i], &rect, &u, &v)) {
-        const int k = pos[i];
-        fov_pts[k] = rect;
-        if (kUV) {
-            fov_u[k] = u;
-            fov_v[k] = v;
-        }
+// After the count kernel: exclusive sums over keep and cnt, then info = (kept jobs, their points, bad, 0).
+cudaError_t job_totals(const FovWs &w, int num_jobs, long long *info, cudaStream_t s);
+
+// One job's count over its frame's in-image points [p0, p1): visit(i, c, l) adds in-image point i to the thread's
+// count c and, with kLabels, to its labelled count l.  The block's c and l end up on thread 0.
+template <bool kLabels, typename Visit>
+__device__ __forceinline__ void job_count(int p0, int p1, int &c, int &l, Visit visit) {
+    using Reduce = cub::BlockReduce<int, FX_THREADS>;
+    __shared__ typename Reduce::TempStorage tmp;
+    c = 0;
+    l = 0;
+    for (int i = p0 + threadIdx.x; i < p1; i += FX_THREADS) visit(i, c, l);
+    c = Reduce(tmp).Sum(c);
+    if (kLabels) {
+        __syncthreads();
+        l = Reduce(tmp).Sum(l);
     }
 }
 
-// Host check of the scans both extractors take: 16-byte-aligned float4 points and the host copy of the scan offsets
+// A count kernel's words for job j (thread 0): its point count c, kept, or -1 and not kept when dropped.
+__device__ __forceinline__ void job_words(int j, bool drop, int c, int32_t *__restrict__ job_points,
+                                          int32_t *__restrict__ keep, long long *__restrict__ cnt) {
+    job_points[j] = drop ? -1 : c;
+    keep[j] = drop ? 0 : 1;
+    cnt[j] = drop ? 0 : c;
+}
+
+// The write kernel's guard for job j: false when the job was dropped (c < 0) or the sizes the host read disagree
+// with the count pass; else its slot *k and first output position *base, with offsets[*k + 1] written.
+__device__ __forceinline__ bool kept_slot(int j, int c, int num_kept, long long num_out,
+                                          const int32_t *__restrict__ keep_pos, const long long *__restrict__ cnt_pos,
+                                          int32_t *__restrict__ offsets, int *k, long long *base) {
+    if (c < 0) return false;
+    const int kj = keep_pos[j];
+    const long long bj = cnt_pos[j];
+    if (kj >= num_kept || bj + c > num_out) return false;
+    if (threadIdx.x == 0) offsets[kj + 1] = (int32_t)(bj + c);
+    *k = kj;
+    *base = bj;
+    return true;
+}
+
+// A write kernel's stable scatter: the in-image points i of [p0, p1) with in(i), in scan order, handed to put(o, i)
+// at the output positions o = base, base + 1, ...; stops once the job's c points are placed.
+template <typename In, typename Put>
+__device__ __forceinline__ void job_scatter(int p0, int p1, int c, long long base, In in, Put put) {
+    using Scan = cub::BlockScan<int, FX_THREADS>;
+    __shared__ typename Scan::TempStorage tmp;
+    int run = 0;
+    for (int i0 = p0; i0 < p1 && run < c; i0 += FX_THREADS) {
+        const int i = i0 + threadIdx.x;
+        const int flag = i < p1 && in(i);
+        int off, total;
+        Scan(tmp).ExclusiveSum(flag, off, total);
+        if (flag) put(base + run + off, i);
+        run += total;
+        __syncthreads();
+    }
+}
+
+// Host check of the scans every extractor takes: 16-byte-aligned float4 points and the host copy of the scan offsets
 // (num_frames + 1 entries).  Raises *max_n (0 on entry) to the largest scan, the x extent of the flag and compact
 // grids.
 inline int check_scans(const char *fn, const int32_t *host_so, int num_frames, int num_points, const void *scans,

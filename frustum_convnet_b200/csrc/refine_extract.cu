@@ -4,7 +4,7 @@
 //
 // The reference re-reads and re-projects every scan and runs one scipy Delaunay per box and augmentation.  Here the
 // per-box constants (enlargement, perturbation, corners, angles) come from the host, and:
-//   fcn_refine_extract_count  flags    the in-image test of every scan point (frustum_fov.cuh, as section (15));
+//   fcn_refine_extract_count  flags    the in-image test of every scan point (frustum_fov.cu, as section (15));
 //                             scan     exclusive sum of the flags over all frames: the position of every in-image point;
 //                             compact  the in-image points as float32 rect x, y, z and intensity, in scan order;
 //                             iou      matched mode: one thread per (detection, ground truth) pair of a frame, the
@@ -17,8 +17,6 @@
 //   fcn_refine_extract_write  write    one CTA per kept job: the box tests again, a block scan for stable positions,
 //                                      the points and their labels scattered in scan order.  Which job each kept
 //                                      frustum is follows from job_points (the kept jobs in job order); the host has it.
-#include <cub/cub.cuh>
-
 #include <cmath>
 
 #include "box_contains.cuh"
@@ -27,19 +25,6 @@
 #include "frustum_fov.cuh"
 
 namespace fcn {
-
-__global__ void __launch_bounds__(FX_THREADS)
-rx_flag_kernel(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
-               const fcn_frustum_frame *__restrict__ frames, int32_t *__restrict__ flags) {
-    fov_flag(scans, so, frames, flags);
-}
-
-__global__ void __launch_bounds__(FX_THREADS)
-rx_compact_kernel(const float4 *__restrict__ scans, const int32_t *__restrict__ so,
-                  const fcn_frustum_frame *__restrict__ frames, const int32_t *__restrict__ pos,
-                  float4 *__restrict__ fov_pts) {
-    fov_compact<false>(scans, so, frames, pos, fov_pts, nullptr, nullptr);
-}
 
 // bbox_overlaps_3d (ops/pybind11/rbbox_iou.py:62-96) of the two boxes' axis-aligned standup boxes, in its order
 __device__ double rx_standup_iou(const double *__restrict__ c, const double *__restrict__ q) {
@@ -128,6 +113,8 @@ rx_match_kernel(int num_dets, int num_frames, double thresh, const int32_t *__re
     match[d] = (arg < 0 || best < thresh) ? -1 : gt_offsets[f] + arg;
 }
 
+// rx_count_kernel and rx_write_kernel keep their own loops and guards rather than job_count, job_words, kept_slot and
+// job_scatter of frustum_fov.cuh: with those, ptxas schedules these two kernels differently.
 __global__ void __launch_bounds__(FX_THREADS)
 rx_count_kernel(int mode, int num_frames, int num_gt, int num_dets, const int32_t *__restrict__ so,
                 const fcn_refine_box *__restrict__ jobs, const int32_t *__restrict__ job_frame,
@@ -182,15 +169,6 @@ rx_count_kernel(int mode, int num_frames, int num_gt, int num_dets, const int32_
     }
 }
 
-__global__ void rx_info_kernel(int num_jobs, const int32_t *__restrict__ keep_pos,
-                               const long long *__restrict__ cnt_pos, const int32_t *__restrict__ bad,
-                               long long *__restrict__ info) {
-    info[0] = keep_pos[num_jobs];
-    info[1] = cnt_pos[num_jobs];
-    info[2] = *bad;
-    info[3] = 0;
-}
-
 __global__ void __launch_bounds__(FX_THREADS)
 rx_write_kernel(int num_kept, long long num_out, const int32_t *__restrict__ so,
                 const fcn_refine_box *__restrict__ jobs, const int32_t *__restrict__ job_frame,
@@ -231,42 +209,17 @@ rx_write_kernel(int num_kept, long long num_out, const int32_t *__restrict__ so,
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-struct RxWs {
-    int32_t *flags, *pos, *keep, *keep_pos, *match, *bad;
-    long long *cnt, *cnt_pos;
-    float4 *fov_pts;
+struct RxWs : FovWs {
     double *iou;
-    void *temp;
-    size_t temp_bytes;
+    int32_t *match;
 };
 
 static cudaError_t rx_layout(const fcn_refine_extract_args *a, Carve &c, RxWs &w) {
-    const size_t N = (size_t)a->num_points, J = (size_t)a->num_jobs;
-    const size_t D = a->mode == FCN_REFINE_MATCHED ? (size_t)a->num_dets : 0;
-    const size_t P = a->mode == FCN_REFINE_MATCHED ? (size_t)a->num_pairs : 0;
-    size_t t0 = 0, t1 = 0, t2 = 0;
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, t0, (const int32_t *)nullptr, (int32_t *)nullptr,
-                                                  a->num_points + 1);
-    if (e != cudaSuccess) return e;
-    e = cub::DeviceScan::ExclusiveSum(nullptr, t1, (const int32_t *)nullptr, (int32_t *)nullptr, a->num_jobs + 1);
-    if (e != cudaSuccess) return e;
-    e = cub::DeviceScan::ExclusiveSum(nullptr, t2, (const long long *)nullptr, (long long *)nullptr,
-                                      a->num_jobs + 1);
-    if (e != cudaSuccess) return e;
-    w.temp_bytes = t0 > t1 ? t0 : t1;
-    w.temp_bytes = w.temp_bytes > t2 ? w.temp_bytes : t2;
-    w.flags = (int32_t *)c.take((N + 1) * 4);
-    w.pos = (int32_t *)c.take((N + 1) * 4);
-    w.fov_pts = (float4 *)c.take(N * 16);
-    w.keep = (int32_t *)c.take((J + 1) * 4);
-    w.keep_pos = (int32_t *)c.take((J + 1) * 4);
-    w.cnt = (long long *)c.take((J + 1) * 8);
-    w.cnt_pos = (long long *)c.take((J + 1) * 8);
-    w.iou = (double *)c.take(P * 8);
-    w.match = (int32_t *)c.take(D * 4);
-    w.bad = (int32_t *)c.take(4);
-    w.temp = c.take(w.temp_bytes);
-    return cudaSuccess;
+    const cudaError_t e = fov_carve(c, a->num_points, a->num_jobs, false, w);
+    const bool matched = a->mode == FCN_REFINE_MATCHED;
+    w.iou = (double *)c.take(matched ? (size_t)a->num_pairs * 8 : 0);
+    w.match = (int32_t *)c.take(matched ? (size_t)a->num_dets * 4 : 0);
+    return e;
 }
 
 static bool rx_empty(const fcn_refine_extract_args *a) { return a->num_frames == 0 || a->num_jobs == 0; }
@@ -323,22 +276,8 @@ extern "C" int fcn_refine_extract_count(const fcn_refine_extract_args *a, fcn_st
     const int st = rx_prepare(a, __func__, w, &max_n);
     if (st != FCN_OK || rx_empty(a)) return st;
     cudaStream_t s = (cudaStream_t)stream;
-    const int N = a->num_points, J = a->num_jobs, F = a->num_frames;
-    const float4 *scans = (const float4 *)a->scans;
-    FCN_CUDA(cudaMemsetAsync(w.flags + N, 0, 4, s));
-    FCN_CUDA(cudaMemsetAsync(w.keep + J, 0, 4, s));
-    FCN_CUDA(cudaMemsetAsync(w.cnt + J, 0, 8, s));
-    FCN_CUDA(cudaMemsetAsync(w.bad, 0, 4, s));
-    const dim3 grid(ceil_div(max_n, FX_THREADS), F);
-    if (max_n > 0) {
-        rx_flag_kernel<<<grid, FX_THREADS, 0, s>>>(scans, a->scan_offsets, a->frames, w.flags);
-        FCN_LAUNCH_CHECK();
-    }
-    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.flags, w.pos, N + 1, s));
-    if (max_n > 0) {
-        rx_compact_kernel<<<grid, FX_THREADS, 0, s>>>(scans, a->scan_offsets, a->frames, w.pos, w.fov_pts);
-        FCN_LAUNCH_CHECK();
-    }
+    const int J = a->num_jobs, F = a->num_frames;
+    FCN_CUDA(fov_stage(w, a->num_points, J, F, max_n, a->scans, a->scan_offsets, a->frames, s));
     if (a->mode == FCN_REFINE_MATCHED) {
         if (a->num_pairs > 0) {
             rx_iou_kernel<<<ceil_div(a->num_pairs, FX_THREADS), FX_THREADS, 0, s>>>(
@@ -354,10 +293,7 @@ extern "C" int fcn_refine_extract_count(const fcn_refine_extract_args *a, fcn_st
                                              a->job_frame, a->job_ref, a->gt_boxes, w.match, w.pos, w.fov_pts,
                                              a->job_points, a->job_gt, w.keep, w.cnt, w.bad);
     FCN_LAUNCH_CHECK();
-    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.keep, w.keep_pos, J + 1, s));
-    FCN_CUDA(cub::DeviceScan::ExclusiveSum(w.temp, w.temp_bytes, w.cnt, w.cnt_pos, J + 1, s));
-    rx_info_kernel<<<1, 1, 0, s>>>(J, w.keep_pos, w.cnt_pos, w.bad, a->info);
-    FCN_LAUNCH_CHECK();
+    FCN_CUDA(job_totals(w, J, a->info, s));
     return FCN_OK;
 }
 

@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import pickle
 
 import numpy as np
 import torch
@@ -105,6 +106,14 @@ def upload_scans(sc, dev):
     return torch.cat([s if isinstance(s, torch.Tensor) else torch.from_numpy(s).to(dev) for s in sc]).contiguous()
 
 
+def frame_order(frames):
+    """Frame ids (one per job, several jobs a frame) -> (the distinct ids in first-appearance order, {id: position})."""
+    pos = {}
+    for k in frames:
+        pos.setdefault(k, len(pos))
+    return list(pos), pos
+
+
 def read_counts(summary, n, who, bad_what):
     """The count pass's summary, read back once (the extraction's one host sync): int64 info (K kept records, M
     points, bad references, -), then int32 words, the first n of them each record's point count (-1: dropped).
@@ -121,6 +130,91 @@ def read_counts(summary, n, who, bad_what):
     return K, M, words, kept
 
 
+def run_extract(family, a, sc, so, n, word_fields, outputs, dev, stream, timer, bad_what):
+    """The two device calls of an extractor family ('frustum_extract', 'refine_extract', 'gt_extract') on the current
+    stream `stream`.  a: the family's args struct with its counts and inputs filled; sc, so: scan_table's scans and
+    host scan offsets.  Uploads the scans, queries the workspace, runs fcn_<family>_count into one summary (info, then
+    the per-job int32 words: n of them for each args field of word_fields), reads it back once (read_counts, naming
+    bad_what), then runs fcn_<family>_write into new points, offsets and the tensors of outputs(K, M, words), a dict
+    {args field: tensor or None}.  `timer(name)` (optional) marks "start", "count", "write_start" and "write".
+    -> (the int32 words, the kept jobs, {args field: output tensor}, points and offsets included)."""
+    scan_dev = upload_scans(sc, dev)            # like so and the caller's upload, alive until the write is enqueued
+    a.scans = scan_dev.data_ptr() if int(so[-1]) > 0 else None
+    a.host_scan_offsets = so.ctypes.data
+    ws, nbytes = workspace("fcn_%s_workspace_bytes" % family, dev, C.byref(a))
+    summary = torch.empty(4 + (len(word_fields) * n + 1) // 2, dtype=torch.int64, device=dev)
+    a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), nbytes, summary.data_ptr()
+    for k, field in enumerate(word_fields):
+        setattr(a, field, summary.data_ptr() + 32 + 4 * n * k)
+    if timer is not None:
+        timer("start")
+    _lib.call("fcn_%s_count" % family, C.byref(a), stream.cuda_stream)
+    if timer is not None:
+        timer("count")
+    K, M, words, kept = read_counts(summary, n, "fcn_" + family, bad_what)
+    out = {"points": torch.empty((M, 4), dtype=torch.float32, device=dev),
+           "offsets": torch.empty(K + 1, dtype=torch.int32, device=dev), **outputs(K, M, words)}
+    a.num_kept, a.num_out_points = K, M
+    for field, t in out.items():
+        setattr(a, field, None if t is None else t.data_ptr())
+    if timer is not None:
+        timer("write_start")
+    _lib.call("fcn_%s_write" % family, C.byref(a), stream.cuda_stream)
+    if timer is not None:
+        timer("write")
+    return words, kept, out
+
+
+class LabelledFrustums:
+    """The result of refine_extract's and gt_extract's extractors: K kept frustums and their M points.  Device:
+    points (M, 4) float32, offsets (K + 1) int32, label (M) uint8 (None without labels), written on the extraction's
+    stream.  Host: counts (K,) and job_index (K,) (the job, i.e. box and augmentation, of each frustum), int64, and
+    the provider's lists.  input_list(), label_list() and TrainBatchBuilder.from_frustums make the current stream wait
+    for that stream first (wait()); other readers of the tensors on another stream call wait() themselves."""
+
+    has_labels = True
+    pickle_names = ()          # the lists in the order the reference pickles them
+
+    def __init__(self, points, offsets, label, counts, job_index, stream):
+        self.points, self.offsets, self.label = points, offsets, label
+        self.stream = stream
+        self.counts = counts
+        self.job_index = job_index
+
+    def __len__(self):
+        return len(self.id_list)
+
+    def _split(self, t):
+        off = np.concatenate([[0], np.cumsum(self.counts)])
+        return [t[off[k]:off[k + 1]] for k in range(len(self))]
+
+    def wait(self):
+        """Make the current stream of the tensors' device wait for the extraction's stream."""
+        if self.stream is not None:
+            torch.cuda.current_stream(self.points.device).wait_stream(self.stream)
+
+    def input_list(self):
+        """The per-frustum (n, 4) float32 point arrays, copied to the host."""
+        self.wait()
+        return self._split(self.points.cpu().numpy())
+
+    def label_list(self):
+        """The per-frustum (n,) float64 labels (1 inside the ground-truth box), copied to the host."""
+        if not self.has_labels:
+            raise ValueError("frustums from detections have no labels")
+        self.wait()
+        return self._split(self.label.cpu().numpy().astype(np.float64))
+
+    def to_pickle(self, path):
+        """The lists in the order the reference's function pickles them (readable by the reference's provider)."""
+        values = {"input_list": self.input_list()}
+        if self.has_labels:
+            values["label_list"] = self.label_list()
+        with open(path, "wb") as fp:
+            for n in self.pickle_names:
+                pickle.dump(values[n] if n in values else getattr(self, n), fp, -1)
+
+
 class FrustumExtractor:
     def __init__(self, type_whitelist=("Car",), device=None):
         self.type_whitelist = tuple(type_whitelist)
@@ -133,11 +227,7 @@ class FrustumExtractor:
         if len(type_list) != n or len(prob_list) != n or len(box2d_list) != n:
             raise ValueError("id_list, type_list, prob_list and box2d_list must have the same length")
         lines = [i for i in range(n) if type_list[i] in self.type_whitelist]
-        frame_of, frame_ids = {}, []
-        for i in lines:
-            if id_list[i] not in frame_of:
-                frame_of[id_list[i]] = len(frame_ids)
-                frame_ids.append(id_list[i])
+        frame_ids, frame_of = frame_order(id_list[i] for i in lines)
         boxes = np.array([np.asarray(box2d_list[i], dtype=np.float64).reshape(4) for i in lines],
                          dtype=np.float64).reshape(-1, 4)
         if not np.isfinite(boxes).all():
@@ -153,40 +243,21 @@ class FrustumExtractor:
                                     torch.zeros(1, dtype=torch.int32, device=dev), *self._empty(dev),
                                     np.zeros(0, np.int64), [], id_list, type_list, prob_list, box2d_list, calibs,
                                     image_hw)
-            scan_dev = upload_scans(sc, dev)
             inp, ptrs = upload([bytes(frames), boxes, so, det_frame], dev)
             a = _lib.FrustumExtractArgs()
             a.num_frames, a.num_points, a.num_dets = F, N, D
-            a.scans = scan_dev.data_ptr() if N > 0 else None
             a.frames, a.boxes, a.scan_offsets, a.det_frame = ptrs
-            a.host_scan_offsets = so.ctypes.data
-            ws, nbytes = workspace("fcn_frustum_extract_workspace_bytes", dev, C.byref(a))
-            summary = torch.empty(4 + (D + 1) // 2, dtype=torch.int64, device=dev)    # info | det_points
-            a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
-            a.info, a.det_points = summary.data_ptr(), summary.data_ptr() + 32
-            if timer is not None:
-                timer("start")
-            _lib.call("fcn_frustum_extract_count", C.byref(a), stream.cuda_stream)
-            if timer is not None:
-                timer("count")
-            K, M, det_points, kept = read_counts(summary, D, "fcn_frustum_extract", "detections reference no frame")
-            points = torch.empty((M, 4), dtype=torch.float32, device=dev)
-            offsets = torch.empty(K + 1, dtype=torch.int32, device=dev)
-            angle = torch.empty(K, dtype=torch.float64, device=dev)
-            box2d = torch.empty((K, 4), dtype=torch.float64, device=dev)
-            P = torch.empty((K, 12), dtype=torch.float64, device=dev)
-            det_index = torch.empty(K, dtype=torch.int32, device=dev)
-            a.num_kept, a.num_out_points = K, M
-            a.points, a.offsets, a.frustum_angle = points.data_ptr(), offsets.data_ptr(), angle.data_ptr()
-            a.box2d, a.P, a.det_index = box2d.data_ptr(), P.data_ptr(), det_index.data_ptr()
-            if timer is not None:
-                timer("write_start")
-            _lib.call("fcn_frustum_extract_write", C.byref(a), stream.cuda_stream)
-            if timer is not None:
-                timer("write")
+            det_points, kept, out = run_extract(
+                "frustum_extract", a, sc, so, D, ("det_points",),
+                lambda K, M, words: {"frustum_angle": torch.empty(K, dtype=torch.float64, device=dev),
+                                     "box2d": torch.empty((K, 4), dtype=torch.float64, device=dev),
+                                     "P": torch.empty((K, 12), dtype=torch.float64, device=dev),
+                                     "det_index": torch.empty(K, dtype=torch.int32, device=dev)},
+                dev, stream, timer, "detections reference no frame")
         line_idx = np.asarray(lines, dtype=np.int64)[kept]
-        return self._result(points, offsets, angle, box2d, P, det_points[kept].astype(np.int64), line_idx, id_list,
-                            type_list, prob_list, box2d_list, calibs, image_hw)
+        return self._result(out["points"], out["offsets"], out["frustum_angle"], out["box2d"], out["P"],
+                            det_points[kept].astype(np.int64), line_idx, id_list, type_list, prob_list, box2d_list,
+                            calibs, image_hw)
 
     @staticmethod
     def _empty(dev):

@@ -33,17 +33,13 @@ reference's own numpy expressions; nothing random runs on the device.  One host 
 frustums and their points.  No CPU fallback: CPU tensors and devices raise."""
 from __future__ import annotations
 
-import ctypes as C
-import os
-import pickle
-
 import numpy as np
 import torch
 
 from . import _lib
-from ._host import cuda_device, upload, workspace
-from .frustum_extract import read_counts, scan_table, upload_scans
-from .refine_extract import _check_box, box_record, obj_array, read_label_dir
+from ._host import cuda_device, upload
+from .frustum_extract import LabelledFrustums, frame_order, run_extract, scan_table
+from .refine_extract import _check_box, box_record, iou_thresh, obj_array, objects_of
 
 SHIFT_RATIO = 0.1          # random_shift_box2d(box2d, H, W, 0.1) of the training sets (prepare_data.py:187, :321)
 MIN_HEIGHT = 25            # a ground truth whose 2-D box is shorter is rejected (:220, :354)
@@ -208,52 +204,17 @@ def job_lists(jobs, calibs):
 
 
 # ------------------------------------------------------------------------------ result
-class GtFrustums:
-    """One extraction: K kept frustums and their M points.  Device: points (M, 4) float32, offsets (K + 1) int32,
-    label (M) uint8, written on the extraction's stream.  Host: counts (K,), job_index (K,) (the job, i.e. box and
-    augmentation, of each frustum) and the provider's lists (datasets/provider_sample.py:97-108).  input_list(),
-    label_list() and TrainBatchBuilder.from_frustums make the current stream wait for that stream first (wait());
-    other readers of the tensors on another stream call wait() themselves."""
+class GtFrustums(LabelledFrustums):
+    """One extraction (LabelledFrustums), always labelled; the lists are the provider's
+    (datasets/provider_sample.py:97-108)."""
 
-    has_labels = True
+    pickle_names = NAMES
 
     def __init__(self, points, offsets, label, counts, job_index, lists, stream=None):
-        self.points, self.offsets, self.label = points, offsets, label
-        self.stream = stream
-        self.counts = counts                  # (K,) host int64
-        self.job_index = job_index            # (K,) host int64
+        super().__init__(points, offsets, label, counts, job_index, stream)
         for n in NAMES:
             if n not in ("input_list", "label_list"):
                 setattr(self, n, lists[n])
-
-    def __len__(self):
-        return len(self.id_list)
-
-    def _split(self, t):
-        off = np.concatenate([[0], np.cumsum(self.counts)])
-        return [t[off[k]:off[k + 1]] for k in range(len(self))]
-
-    def wait(self):
-        """Make the current stream of the tensors' device wait for the extraction's stream."""
-        if self.stream is not None:
-            torch.cuda.current_stream(self.points.device).wait_stream(self.stream)
-
-    def input_list(self):
-        """The per-frustum (n, 4) float32 point arrays, copied to the host."""
-        self.wait()
-        return self._split(self.points.cpu().numpy())
-
-    def label_list(self):
-        """The per-frustum (n,) float64 labels (1 inside the ground-truth box), copied to the host."""
-        self.wait()
-        return self._split(self.label.cpu().numpy().astype(np.float64))
-
-    def to_pickle(self, path):
-        """The lists in the order the reference's function pickles them (readable by the reference's provider)."""
-        values = {"input_list": self.input_list(), "label_list": self.label_list()}
-        with open(path, "wb") as fp:
-            for n in NAMES:
-                pickle.dump(values[n] if n in values else getattr(self, n), fp, -1)
 
 
 class GtFrustumExtractor:
@@ -263,12 +224,12 @@ class GtFrustumExtractor:
 
     @property
     def iou_thresh(self):
-        return 0.5 if "Car" in self.type_whitelist else 0.25          # prepare_data.py:141
+        return iou_thresh(self.type_whitelist)
 
     def from_ground_truth(self, scans, calibs, image_hw, image_ids, gt, perturb=False, augment=1, rng=np.random,
                           stream=None, timer=None):
         """gt: a label_2 directory or {idx: [KittiObject]}.  rng: the np.random module or a RandomState."""
-        gt = self._objects(gt, image_ids)
+        gt = objects_of(gt, image_ids)
         jobs = job_table(image_ids, gt, self.type_whitelist, image_hw, perturb, int(augment), rng)
         return self._run(scans, calibs, image_hw, jobs, stream, timer)
 
@@ -276,28 +237,20 @@ class GtFrustumExtractor:
                                 gt, perturb=False, augment=1, rng=np.random, stream=None, timer=None):
         """id_list ... box2d_list: read_rgb_detections' four lists; gt as for from_ground_truth."""
         dets = detection_table(id_list, type_list, prob_list, box2d_list)
-        gt = self._objects(gt, image_ids)
+        gt = objects_of(gt, image_ids)
         jobs = job_table(image_ids, gt, self.type_whitelist, image_hw, perturb, int(augment), rng, dets,
                          self.iou_thresh)
         return self._run(scans, calibs, image_hw, jobs, stream, timer)
 
-    @staticmethod
-    def _objects(gt, image_ids):
-        if isinstance(gt, (str, os.PathLike)):
-            return read_label_dir(gt, image_ids)
-        return {int(k): v for k, v in gt.items()}
-
     # ------------------------------------------------------------------ device call
     def _run(self, scans, calibs, image_hw, jobs, stream, timer):
         dev = self.device
-        frame_ids, labels, label_of = [], [], {}
+        frame_ids, fpos = frame_order(jb["frame"] for jb in jobs)
+        labels, label_of = [], {}
         for jb in jobs:
-            if not frame_ids or frame_ids[-1] != jb["frame"]:
-                frame_ids.append(jb["frame"])
             if id(jb["obj"]) not in label_of:
                 label_of[id(jb["obj"])] = len(labels)
                 labels.append(jb["obj"])
-        fpos = {k: f for f, k in enumerate(frame_ids)}
         J, F = len(jobs), len(frame_ids)
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
@@ -307,7 +260,6 @@ class GtFrustumExtractor:
                                   torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.int64),
                                   np.zeros(0, np.int64), job_lists([], calibs), stream)
             sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "GtFrustumExtractor")
-            scan_dev, N = upload_scans(sc, dev), int(so[-1])
             job_rec = np.zeros(J, dtype=np.dtype(_lib.GtJob))
             job_rec["box"] = np.stack([jb["cut"] for jb in jobs])
             job_rec["frame"] = [fpos[jb["frame"]] for jb in jobs]
@@ -315,29 +267,11 @@ class GtFrustumExtractor:
             label_box = np.array([box_record(obj_array(o)) for o in labels], dtype=np.dtype(_lib.RefineBox))
             inp, ptrs = upload([bytes(frames), job_rec, label_box, so], dev)
             a = _lib.GtExtractArgs()
-            a.num_frames, a.num_points, a.num_jobs, a.num_labels = F, N, J, len(labels)
-            a.scans = scan_dev.data_ptr() if N > 0 else None
+            a.num_frames, a.num_points, a.num_jobs, a.num_labels = F, int(so[-1]), J, len(labels)
             a.frames, a.jobs, a.label_boxes, a.scan_offsets = ptrs
-            a.host_scan_offsets = so.ctypes.data
-            ws, nbytes = workspace("fcn_gt_extract_workspace_bytes", dev, C.byref(a))
-            summary = torch.empty(4 + (J + 1) // 2, dtype=torch.int64, device=dev)    # info | job_points
-            a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
-            a.info, a.job_points = summary.data_ptr(), summary.data_ptr() + 32
-            if timer is not None:
-                timer("start")
-            _lib.call("fcn_gt_extract_count", C.byref(a), stream.cuda_stream)
-            if timer is not None:
-                timer("count")
-            K, M, job_points, kept = read_counts(summary, J, "fcn_gt_extract", "jobs reference no frame or label box")
-            points = torch.empty((M, 4), dtype=torch.float32, device=dev)
-            offsets = torch.empty(K + 1, dtype=torch.int32, device=dev)
-            label = torch.empty(M, dtype=torch.uint8, device=dev)
-            a.num_kept, a.num_out_points = K, M
-            a.points, a.offsets, a.labels = points.data_ptr(), offsets.data_ptr(), label.data_ptr()
-            if timer is not None:
-                timer("write_start")
-            _lib.call("fcn_gt_extract_write", C.byref(a), stream.cuda_stream)
-            if timer is not None:
-                timer("write")
-        return GtFrustums(points, offsets, label, job_points[kept].astype(np.int64), kept.astype(np.int64),
-                          job_lists([jobs[j] for j in kept.tolist()], calibs), stream)
+            job_points, kept, out = run_extract(
+                "gt_extract", a, sc, so, J, ("job_points",),
+                lambda K, M, words: {"labels": torch.empty(M, dtype=torch.uint8, device=dev)},
+                dev, stream, timer, "jobs reference no frame or label box")
+        return GtFrustums(out["points"], out["offsets"], out["labels"], job_points[kept].astype(np.int64),
+                          kept.astype(np.int64), job_lists([jobs[j] for j in kept.tolist()], calibs), stream)

@@ -36,16 +36,14 @@ themselves (read_result_dir).  Ground truth is a label_2 directory (or a {idx: [
 per call, to learn the kept frustums and their points.  No CPU fallback: CPU tensors and devices raise."""
 from __future__ import annotations
 
-import ctypes as C
 import os
-import pickle
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._host import csr_offsets, cuda_device, upload, workspace
-from .frustum_extract import read_counts, scan_table, upload_scans
+from ._host import csr_offsets, cuda_device, upload
+from .frustum_extract import LabelledFrustums, frame_order, run_extract, scan_table
 from .kitti_eval import detection_records
 
 RATIO = 1.2                # the enlargement of every box that cuts points (prepare_data_refine.py:319, :489, :724)
@@ -78,6 +76,18 @@ def read_objects(path):
 
 def read_label_dir(label_dir, image_ids):
     return {int(i): read_objects(os.path.join(label_dir, "%06d.txt" % int(i))) for i in image_ids}
+
+
+def objects_of(gt, image_ids):
+    """Ground truth as the extractors take it, a label_2 directory or {idx: [KittiObject]} -> {int idx: objects}."""
+    if isinstance(gt, (str, os.PathLike)):
+        return read_label_dir(gt, image_ids)
+    return {int(k): v for k, v in gt.items()}
+
+
+def iou_thresh(type_whitelist):
+    """The matching threshold of matched detections (prepare_data.py:141, prepare_data_refine.py:447)."""
+    return 0.5 if "Car" in type_whitelist else 0.25
 
 
 def read_result_dir(result_dir, image_ids):
@@ -252,57 +262,19 @@ _DET_NAMES = ("id_list", "box2d_list", "input_list", "type_list", "frustum_angle
               "pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list")
 
 
-class RefineFrustums:
-    """One extraction: K kept frustums and their M points.  Device: points (M, 4) float32, offsets (K + 1) int32,
-    label (M) uint8 (None for detections), written on the extraction's stream.  Host: the provider's lists
-    (datasets/provider_sample_refine.py:85-117).  input_list(), label_list() and TrainBatchBuilder.from_frustums make
-    the current stream wait for that stream first (wait()); other readers of the tensors on another stream call
-    wait() themselves."""
+class RefineFrustums(LabelledFrustums):
+    """One extraction (LabelledFrustums) in `mode`, without labels (label None) for detections; the lists are the
+    provider's (datasets/provider_sample_refine.py:85-117)."""
 
     def __init__(self, mode, points, offsets, label, counts, job_index, lists, stream=None):
-        self.mode, self.points, self.offsets, self.label = mode, points, offsets, label
-        self.stream = stream
-        self.counts = counts                  # (K,) host int64
-        self.job_index = job_index            # (K,) host int64: the job (box, augmentation) of each frustum
+        super().__init__(points, offsets, label, counts, job_index, stream)
+        self.mode = mode
         self.has_labels = mode != _lib.REFINE_DET
+        self.pickle_names = _GT_NAMES if self.has_labels else _DET_NAMES
         for n in ("id_list", "box2d_list", "type_list", "frustum_angle_list", "prob_list", "calib_list",
                   "box3d_list", "heading_list", "size_list", "pred_box3d_list", "pred_box3d_size_list",
                   "pred_box3d_angle_list"):
             setattr(self, n, lists.get(n))
-
-    def __len__(self):
-        return len(self.id_list)
-
-    def _split(self, t):
-        off = np.concatenate([[0], np.cumsum(self.counts)])
-        return [t[off[k]:off[k + 1]] for k in range(len(self))]
-
-    def wait(self):
-        """Make the current stream of the tensors' device wait for the extraction's stream."""
-        if self.stream is not None:
-            torch.cuda.current_stream(self.points.device).wait_stream(self.stream)
-
-    def input_list(self):
-        """The per-frustum (n, 4) float32 point arrays, copied to the host."""
-        self.wait()
-        return self._split(self.points.cpu().numpy())
-
-    def label_list(self):
-        """The per-frustum (n,) float64 labels (1 inside the ground-truth box), copied to the host."""
-        if not self.has_labels:
-            raise ValueError("frustums from detections have no labels")
-        self.wait()
-        return self._split(self.label.cpu().numpy().astype(np.float64))
-
-    def to_pickle(self, path):
-        """The lists in the order the reference's function pickles them (readable by the reference's provider)."""
-        names = _GT_NAMES if self.has_labels else _DET_NAMES
-        values = {"input_list": self.input_list()}
-        if self.has_labels:
-            values["label_list"] = self.label_list()
-        with open(path, "wb") as fp:
-            for n in names:
-                pickle.dump(values[n] if n in values else getattr(self, n), fp, -1)
 
 
 class RefineFrustumExtractor:
@@ -314,7 +286,7 @@ class RefineFrustumExtractor:
     def from_ground_truth(self, scans, calibs, image_hw, image_ids, gt, perturb=False, augment=1, rng=np.random,
                           remove_diff=False, stream=None, timer=None):
         """gt: a label_2 directory or {idx: [KittiObject]}.  rng: the np.random module or a RandomState."""
-        gt = self._objects(gt, image_ids)
+        gt = objects_of(gt, image_ids)
         jobs, gts = job_table(_lib.REFINE_GT, image_ids, None, gt, self.type_whitelist, remove_diff, perturb,
                               int(augment), rng)
         return self._run(_lib.REFINE_GT, scans, calibs, image_hw, jobs, gts, stream, timer)
@@ -322,7 +294,7 @@ class RefineFrustumExtractor:
     def from_matched_detections(self, scans, calibs, image_hw, image_ids, dets, gt, remove_diff=False, stream=None,
                                 timer=None):
         """dets: the collector's dict or {idx: [KittiObject]} (read_result_dir); gt as for from_ground_truth."""
-        dets, gt = self._dets(dets, image_ids), self._objects(gt, image_ids)
+        dets, gt = self._dets(dets, image_ids), objects_of(gt, image_ids)
         jobs, gts = job_table(_lib.REFINE_MATCHED, image_ids, dets, gt, self.type_whitelist, remove_diff)
         return self._run(_lib.REFINE_MATCHED, scans, calibs, image_hw, jobs, gts, stream, timer)
 
@@ -333,13 +305,7 @@ class RefineFrustumExtractor:
 
     @property
     def iou_thresh(self):
-        return 0.5 if "Car" in self.type_whitelist else 0.25          # prepare_data_refine.py:447
-
-    @staticmethod
-    def _objects(gt, image_ids):
-        if isinstance(gt, (str, os.PathLike)):
-            return read_label_dir(gt, image_ids)
-        return {int(k): v for k, v in gt.items()}
+        return iou_thresh(self.type_whitelist)
 
     @staticmethod
     def _dets(dets, image_ids):
@@ -351,11 +317,7 @@ class RefineFrustumExtractor:
     # ------------------------------------------------------------------ device call
     def _run(self, mode, scans, calibs, image_hw, jobs, gts, stream, timer):
         dev = self.device
-        frame_ids = []
-        for jb in jobs:
-            if not frame_ids or frame_ids[-1] != jb["frame"]:
-                frame_ids.append(jb["frame"])
-        fpos = {k: f for f, k in enumerate(frame_ids)}
+        frame_ids, fpos = frame_order(jb["frame"] for jb in jobs)
         gt_flat, gt_off = [], [0]
         for k in frame_ids:
             gt_flat += gts.get(k, [])
@@ -371,7 +333,6 @@ class RefineFrustumExtractor:
                                     np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, np.int64), jobs,
                                     gt_flat, calibs, stream)
             sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "RefineFrustumExtractor")
-            scan_dev, N = upload_scans(sc, dev), int(so[-1])
             job_box = np.array([box_record(jb["cut"]) for jb in jobs], dtype=np.dtype(_lib.RefineBox))
             job_frame = np.array([fpos[jb["frame"]] for jb in jobs], dtype=np.int32)
             gt_box = np.array([box_record(obj_array(o)) for o in gt_flat], dtype=np.dtype(_lib.RefineBox))
@@ -392,42 +353,24 @@ class RefineFrustumExtractor:
                 parts += [det_c, gt_c, np.asarray(gt_off, np.int32), po]
             inp, ptrs = upload(parts, dev)
             a = _lib.RefineExtractArgs()
-            a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, F, N, J, G
+            a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, F, int(so[-1]), J, G
             a.num_dets, a.num_pairs, a.iou_thresh = D, P, self.iou_thresh
-            a.scans = scan_dev.data_ptr() if N > 0 else None
             a.frames, a.jobs, a.scan_offsets, a.job_frame, a.job_ref = ptrs[:5]
             a.gt_boxes = ptrs[5] if G > 0 else None
             if mode == _lib.REFINE_MATCHED:
                 a.det_frame = a.job_frame
                 a.det_corners, a.gt_corners, a.gt_offsets, a.pair_offsets = ptrs[6:10]
-            a.host_scan_offsets = so.ctypes.data
-            ws, nbytes = workspace("fcn_refine_extract_workspace_bytes", dev, C.byref(a))
-            summary = torch.empty(4 + J, dtype=torch.int64, device=dev)   # info | job_points | job_gt (int32 each)
-            a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
-            a.info, a.job_points, a.job_gt = summary.data_ptr(), summary.data_ptr() + 32, summary.data_ptr() + 32 + 4 * J
-            if timer is not None:
-                timer("start")
-            _lib.call("fcn_refine_extract_count", C.byref(a), stream.cuda_stream)
-            if timer is not None:
-                timer("count")
-            K, M, words, kept = read_counts(summary, J, "fcn_refine_extract",
-                                            "jobs or pairs reference no frame or box")
-            job_points, job_gt = words[:J], words[J:2 * J]
-            if mode == _lib.REFINE_MATCHED:
-                check_matched_extents(jobs, gt_flat, job_gt)
-            points = torch.empty((M, 4), dtype=torch.float32, device=dev)
-            offsets = torch.empty(K + 1, dtype=torch.int32, device=dev)
-            label = None if mode == _lib.REFINE_DET else torch.empty(M, dtype=torch.uint8, device=dev)
-            a.num_kept, a.num_out_points = K, M
-            a.points, a.offsets = points.data_ptr(), offsets.data_ptr()
-            a.labels = None if label is None else label.data_ptr()
-            if timer is not None:
-                timer("write_start")
-            _lib.call("fcn_refine_extract_write", C.byref(a), stream.cuda_stream)
-            if timer is not None:
-                timer("write")
-        return self._result(mode, points, offsets, label, job_points[kept].astype(np.int64), kept.astype(np.int64),
-                            job_gt[kept].astype(np.int64), jobs, gt_flat, calibs, stream)
+
+            def outputs(K, M, words):
+                if mode == _lib.REFINE_MATCHED:
+                    check_matched_extents(jobs, gt_flat, words[J:2 * J])
+                return {"labels": None if mode == _lib.REFINE_DET else torch.empty(M, dtype=torch.uint8, device=dev)}
+
+            words, kept, out = run_extract("refine_extract", a, sc, so, J, ("job_points", "job_gt"), outputs, dev,
+                                           stream, timer, "jobs or pairs reference no frame or box")
+        job_points, job_gt = words[:J], words[J:2 * J]
+        return self._result(mode, out["points"], out["offsets"], out["labels"], job_points[kept].astype(np.int64),
+                            kept.astype(np.int64), job_gt[kept].astype(np.int64), jobs, gt_flat, calibs, stream)
 
     @staticmethod
     def _result(mode, points, offsets, label, counts, kept, kept_gt, jobs, gt_flat, calibs, stream):

@@ -162,25 +162,38 @@ def test_wrappers_reject_cpu_tensors_and_mismatched_lists():
                                torch.zeros(1, 12, dtype=torch.float64))
 
 
-def test_kernels_compile_without_spills(tmp_path):
+def test_detection_extraction_kernels_compile_without_spills(tmp_path):
+    """The detection extractor's own kernels (csrc/frustum_extract.cu) and the stage it shares with the other
+    extractors (csrc/frustum_fov.cu, the family's only CUB device scans) compile for sm_90a without spills."""
     from frustum_convnet_b200 import build
     try:
         nvcc = build._nvcc()
     except RuntimeError:
         pytest.skip("nvcc is not installed")
-    r = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, "frustum_extract.cu"),
-                        "-o", str(tmp_path / "fx.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    reports, name = {}, None
-    for ln in (r.stdout + r.stderr).splitlines():
-        m = re.search(r"Compiling entry function '(\S+)'", ln)
-        if m:
-            name = m.group(1)
-            reports[name] = ""
-        elif name is not None:
-            reports[name] += ln + "\n"
-    fx = {k: v for k, v in reports.items() if "fx_" in k}
-    assert len(fx) == 5, sorted(fx)
-    for k, text in reports.items():
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", text)
-        assert m and (int(m.group(1)), int(m.group(2))) == (0, 0), k + "\n" + text
+    reports = {}
+    for src in ("frustum_extract", "frustum_fov"):
+        r = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, src + ".cu"),
+                            "-o", str(tmp_path / (src + ".o"))], capture_output=True, text=True)
+        assert r.returncode == 0, r.stdout + r.stderr
+        reports[src], name = {}, None
+        for ln in (r.stdout + r.stderr).splitlines():
+            m = re.search(r"Compiling entry function '(\S+)'", ln)
+            if m:
+                name = m.group(1)
+                reports[src][name] = ""
+            elif name is not None:
+                reports[src][name] += ln + "\n"
+
+    def named(src, *parts):
+        return sorted(p for p in parts if any(p in k for k in reports[src]))
+
+    own = ("fx_count_kernel", "fx_write_kernel")
+    shared = ("fov_flag_kernel", "fov_compact_kernelILb0", "fov_compact_kernelILb1", "job_info_kernel")
+    assert named("frustum_extract", *own) == sorted(own) and len(reports["frustum_extract"]) == 2, \
+        sorted(reports["frustum_extract"])
+    assert named("frustum_fov", *shared) == sorted(shared), sorted(reports["frustum_fov"])
+    assert any("DeviceScanKernel" in k for k in reports["frustum_fov"]), sorted(reports["frustum_fov"])
+    for src in reports:
+        for k, text in reports[src].items():
+            m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", text)
+            assert m and (int(m.group(1)), int(m.group(2))) == (0, 0), k + "\n" + text

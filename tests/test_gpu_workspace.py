@@ -1,7 +1,7 @@
-"""GPU: every two-phase entry family (detect, kitti_eval, sunrgbd_eval, frustum_extract, refine_extract) checks the
-caller's workspace against its fcn_*_workspace_bytes() size.  Each family runs through its public class on a small
-valid input; every entry call that takes a workspace is first replayed one byte short, which must be refused with
-the size function's name before any device work, and then runs with exactly the queried size."""
+"""GPU: every two-phase entry family (detect, kitti_eval, sunrgbd_eval, frustum_extract, refine_extract, gt_extract)
+checks the caller's workspace against its fcn_*_workspace_bytes() size.  Each family runs through its public class on
+a small valid input; every entry call that takes a workspace is first replayed one byte short, which must be refused
+with the size function's name before any device work, and then runs with exactly the queried size."""
 import ctypes
 
 import numpy as np
@@ -15,6 +15,7 @@ ENTRIES = {
     "sunrgbd_eval": ("fcn_sunrgbd_eval_match", "fcn_sunrgbd_eval_curves"),
     "frustum_extract": ("fcn_frustum_extract_count", "fcn_frustum_extract_write"),
     "refine_extract": ("fcn_refine_extract_count", "fcn_refine_extract_write"),
+    "gt_extract": ("fcn_gt_extract_count", "fcn_gt_extract_write"),
 }
 
 
@@ -56,8 +57,15 @@ def _refine_extract():
     assert len(_run("matched", scans, calibs, hws, z["frame_ids"].tolist(), labels, results))
 
 
+def _gt_extract():
+    from test_gpu_gt_extract import _run, scenes
+    z, scans, calibs, hws, labels, dets = scenes()
+    assert len(_run("car_matched", scans, calibs, hws, z["frame_ids"].tolist(), labels, dets,
+                    np.random.RandomState(1)))
+
+
 RUN = {"det": _detect, "kitti_eval": _kitti_eval, "sunrgbd_eval": _sunrgbd_eval, "frustum_extract": _frustum_extract,
-       "refine_extract": _refine_extract}
+       "refine_extract": _refine_extract, "gt_extract": _gt_extract}
 
 
 @pytest.mark.parametrize("family", sorted(ENTRIES))
