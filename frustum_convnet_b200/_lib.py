@@ -309,6 +309,24 @@ class GtExtractArgs(C.Structure):
                [(n, C.c_void_p) for n in ("info", "job_points", "points", "labels", "offsets")]
 
 
+SUNRGBD_MAX_POINTS = 2048
+
+
+class SunrgbdFrame(C.Structure):
+    _fields_ = [("Rtilt", C.c_double * 9), ("K", C.c_double * 9)]
+
+
+class SunrgbdExtractArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("num_frames", "num_points", "num_jobs", "num_labels", "num_choices",
+                                       "labelled", "job_begin", "job_end", "num_kept", "reserved")] + \
+               [("num_out_points", C.c_longlong)] + \
+               [(n, C.c_void_p) for n in ("scans", "scan_offsets", "host_scan_offsets", "frames", "jobs",
+                                          "label_boxes", "job_choice", "choice_ranks", "choice_slots",
+                                          "workspace")] + \
+               [("workspace_bytes", C.c_longlong)] + \
+               [(n, C.c_void_p) for n in ("info", "job_points", "job_labelled", "points", "labels", "offsets")]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check every symbol of the header
 _I, _F, _P = C.c_int, C.c_float, C.c_void_p
 SIGNATURES = {
@@ -364,6 +382,11 @@ SIGNATURES = {
     "fcn_gt_extract_workspace_bytes": (C.c_longlong, [C.POINTER(GtExtractArgs)]),
     "fcn_gt_extract_count": (_I, [C.POINTER(GtExtractArgs), _P]),
     "fcn_gt_extract_write": (_I, [C.POINTER(GtExtractArgs), _P]),
+    "fcn_sunrgbd_extract_workspace_bytes": (C.c_longlong, [C.POINTER(SunrgbdExtractArgs)]),
+    "fcn_sunrgbd_extract_project": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
+    "fcn_sunrgbd_extract_count": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
+    "fcn_sunrgbd_extract_select": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
+    "fcn_sunrgbd_extract_write": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
 }
 
 _lib = None

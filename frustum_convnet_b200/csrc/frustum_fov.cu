@@ -90,23 +90,16 @@ __global__ void job_info_kernel(int num_jobs, const int32_t *__restrict__ keep_p
     info[3] = 0;
 }
 
-cudaError_t fov_carve(Carve &c, int num_points, int num_jobs, bool uv, FovWs &w) {
-    const size_t N = (size_t)num_points, J = (size_t)num_jobs;
-    size_t t0 = 0, t1 = 0, t2 = 0;
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, t0, (const int32_t *)nullptr, (int32_t *)nullptr,
-                                                  num_points + 1);
-    if (e != cudaSuccess) return e;
-    e = cub::DeviceScan::ExclusiveSum(nullptr, t1, (const int32_t *)nullptr, (int32_t *)nullptr, num_jobs + 1);
+cudaError_t job_carve(Carve &c, int num_jobs, size_t min_temp_bytes, JobWs &w) {
+    const size_t J = (size_t)num_jobs;
+    size_t t1 = 0, t2 = 0;
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, t1, (const int32_t *)nullptr, (int32_t *)nullptr,
+                                                  num_jobs + 1);
     if (e != cudaSuccess) return e;
     e = cub::DeviceScan::ExclusiveSum(nullptr, t2, (const long long *)nullptr, (long long *)nullptr, num_jobs + 1);
     if (e != cudaSuccess) return e;
-    w.temp_bytes = t0 > t1 ? t0 : t1;
+    w.temp_bytes = min_temp_bytes > t1 ? min_temp_bytes : t1;
     w.temp_bytes = w.temp_bytes > t2 ? w.temp_bytes : t2;
-    w.flags = (int32_t *)c.take((N + 1) * 4);
-    w.pos = (int32_t *)c.take((N + 1) * 4);
-    w.fov_pts = (float4 *)c.take(N * 16);
-    w.fov_u = uv ? (double *)c.take(N * 8) : nullptr;
-    w.fov_v = uv ? (double *)c.take(N * 8) : nullptr;
     w.keep = (int32_t *)c.take((J + 1) * 4);
     w.keep_pos = (int32_t *)c.take((J + 1) * 4);
     w.cnt = (long long *)c.take((J + 1) * 8);
@@ -114,6 +107,20 @@ cudaError_t fov_carve(Carve &c, int num_points, int num_jobs, bool uv, FovWs &w)
     w.bad = (int32_t *)c.take(4);
     w.temp = c.take(w.temp_bytes);
     return cudaSuccess;
+}
+
+cudaError_t fov_carve(Carve &c, int num_points, int num_jobs, bool uv, FovWs &w) {
+    const size_t N = (size_t)num_points;
+    size_t t0 = 0;
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, t0, (const int32_t *)nullptr, (int32_t *)nullptr,
+                                                  num_points + 1);
+    if (e != cudaSuccess) return e;
+    w.flags = (int32_t *)c.take((N + 1) * 4);
+    w.pos = (int32_t *)c.take((N + 1) * 4);
+    w.fov_pts = (float4 *)c.take(N * 16);
+    w.fov_u = uv ? (double *)c.take(N * 8) : nullptr;
+    w.fov_v = uv ? (double *)c.take(N * 8) : nullptr;
+    return job_carve(c, num_jobs, t0, w);
 }
 
 cudaError_t fov_stage(const FovWs &w, int num_points, int num_jobs, int num_frames, int max_n, const void *scans,
@@ -142,7 +149,7 @@ cudaError_t fov_stage(const FovWs &w, int num_points, int num_jobs, int num_fram
     return cudaGetLastError();
 }
 
-cudaError_t job_totals(const FovWs &w, int num_jobs, long long *info, cudaStream_t s) {
+cudaError_t job_totals(const JobWs &w, int num_jobs, long long *info, cudaStream_t s) {
     size_t temp_bytes = w.temp_bytes;
     cudaError_t e = cub::DeviceScan::ExclusiveSum(w.temp, temp_bytes, w.keep, w.keep_pos, num_jobs + 1, s);
     if (e != cudaSuccess) return e;

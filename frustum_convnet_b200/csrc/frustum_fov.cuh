@@ -16,15 +16,24 @@ namespace fcn {
 
 constexpr int FX_THREADS = 256;
 
-// Workspace pieces every extractor has; each family carves its own pieces after these.
-struct FovWs {
-    int32_t *flags, *pos, *keep, *keep_pos, *bad;
+// Workspace pieces of the job pass (kept flags, point counts, their scans and the bad-reference counter), which
+// every extractor has, the SUN-RGBD one (csrc/sunrgbd_extract.cu, section (18)) included.
+struct JobWs {
+    int32_t *keep, *keep_pos, *bad;
     long long *cnt, *cnt_pos;
-    float4 *fov_pts;
-    double *fov_u, *fov_v;      // float64 image coordinates of the in-image points (null unless uv)
     void *temp;
     size_t temp_bytes;
 };
+
+// Plus the in-image stage's pieces of the KITTI extractors; each family carves its own pieces after these.
+struct FovWs : JobWs {
+    int32_t *flags, *pos;
+    float4 *fov_pts;
+    double *fov_u, *fov_v;      // float64 image coordinates of the in-image points (null unless uv)
+};
+
+// Takes the job pieces for num_jobs jobs from c, with room in temp for at least min_temp_bytes.
+cudaError_t job_carve(Carve &c, int num_jobs, size_t min_temp_bytes, JobWs &w);
 
 // Takes the shared pieces for num_points scan points and num_jobs jobs from c (fov_u, fov_v only when uv).
 cudaError_t fov_carve(Carve &c, int num_points, int num_jobs, bool uv, FovWs &w);
@@ -36,7 +45,7 @@ cudaError_t fov_stage(const FovWs &w, int num_points, int num_jobs, int num_fram
                       const int32_t *scan_offsets, const fcn_frustum_frame *frames, cudaStream_t s);
 
 // After the count kernel: exclusive sums over keep and cnt, then info = (kept jobs, their points, bad, 0).
-cudaError_t job_totals(const FovWs &w, int num_jobs, long long *info, cudaStream_t s);
+cudaError_t job_totals(const JobWs &w, int num_jobs, long long *info, cudaStream_t s);
 
 // One job's count over its frame's in-image points [p0, p1): visit(i, c, l) adds in-image point i to the thread's
 // count c and, with kLabels, to its labelled count l.  The block's c and l end up on thread 0.

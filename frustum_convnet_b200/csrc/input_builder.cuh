@@ -19,6 +19,16 @@ __device__ __forceinline__ double dadd(double a, double b) {
     else return a + b;
 }
 
+// x . y over k = 0, 1, 2 as OpenBLAS's dgemm accumulates it (numpy's np.dot of float64 matrices): a0 b0 rounded,
+// then one FMA per further term.  Used by the SUN-RGBD training inputs (train_inputs.cu) and the SUN-RGBD frustum
+// projection (sunrgbd_extract.cu).
+__device__ __forceinline__ double dot_fma(double a0, double b0, double a1, double b1) {
+    return __fma_rn(a1, b1, __dmul_rn(a0, b0));
+}
+__device__ __forceinline__ double dot_fma(double a0, double b0, double a1, double b1, double a2, double b2) {
+    return __fma_rn(a2, b2, dot_fma(a0, b0, a1, b1));
+}
+
 // rot_angle = np.pi / 2.0 + frustum_angle  (provider_sample.py:330-333) and its sine / cosine
 __device__ __forceinline__ double centre_view_angle(double frustum_angle, double *sn, double *cs) {
     const double rot = 1.5707963267948966 + frustum_angle;

@@ -23,13 +23,6 @@ constexpr double kPi = 3.141592653589793;
 __device__ __forceinline__ double dsub(double a, double b) { return __dadd_rn(a, -b); }
 __device__ __forceinline__ double clip(double v, double lo, double hi) { return fmin(fmax(v, lo), hi); }
 
-// x . y over k = 0, 1, 2 as OpenBLAS's dgemm accumulates it: a0 b0 rounded, then one FMA per further term
-__device__ __forceinline__ double dot_fma(double a0, double b0, double a1, double b1) {
-    return __fma_rn(a1, b1, __dmul_rn(a0, b0));
-}
-__device__ __forceinline__ double dot_fma(double a0, double b0, double a1, double b1, double a2, double b2) {
-    return __fma_rn(a2, b2, dot_fma(a0, b0, a1, b1));
-}
 // rotate_pc_along_y's np.dot(pc[:, [0, 2]], rotmat.T) in that order: x' = x c + z (-s), z' = x s + z c
 __device__ __forceinline__ void rotate_y_fma(double x, double z, double cs, double sn, double *xo, double *zo) {
     *xo = dot_fma(x, cs, z, -sn);

@@ -78,16 +78,16 @@ def _frame_record(calib, hw):
     return f
 
 
-def _scan(scan, dev, who):
+def _scan(scan, dev, who, cols=4):
     if isinstance(scan, torch.Tensor):
         if not on_device(scan, dev):
             raise RuntimeError("%s: scans must be numpy arrays or CUDA tensors on %s" % (who, dev))
-        if scan.dtype != torch.float32 or scan.dim() != 2 or scan.shape[1] != 4:
-            raise ValueError("a scan must be an (n, 4) float32 array")
+        if scan.dtype != torch.float32 or scan.dim() != 2 or scan.shape[1] != cols:
+            raise ValueError("a scan must be an (n, %d) float32 array" % cols)
         return scan
     a = np.asarray(scan)
-    if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
-        raise ValueError("a scan must be an (n, 4) float32 array")
+    if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != cols:
+        raise ValueError("a scan must be an (n, %d) float32 array" % cols)
     return a
 
 
@@ -100,7 +100,7 @@ def scan_table(scans, calibs, image_hw, frame_ids, dev, who):
 
 
 def upload_scans(sc, dev):
-    """scan_table's scans -> one (N, 4) float32 tensor on dev."""
+    """scan_table's scans -> one (N, 4) float32 tensor on dev (N, 6 for SUN-RGBD clouds)."""
     if all(isinstance(s, np.ndarray) for s in sc):
         return torch.from_numpy(np.concatenate(sc)).to(dev)
     return torch.cat([s if isinstance(s, torch.Tensor) else torch.from_numpy(s).to(dev) for s in sc]).contiguous()
@@ -166,8 +166,8 @@ def run_extract(family, a, sc, so, n, word_fields, outputs, dev, stream, timer, 
 
 
 class LabelledFrustums:
-    """The result of refine_extract's and gt_extract's extractors: K kept frustums and their M points.  Device:
-    points (M, 4) float32, offsets (K + 1) int32, label (M) uint8 (None without labels), written on the extraction's
+    """The result of refine_extract's, gt_extract's and sunrgbd_extract's extractors: K kept frustums and their M
+    points.  Device: points (M, 4) float32 ((M, 6) for SUN-RGBD), offsets (K + 1) int32, label (M) uint8 (None without labels), written on the extraction's
     stream.  Host: counts (K,) and job_index (K,) (the job, i.e. box and augmentation, of each frustum), int64, and
     the provider's lists.  input_list(), label_list() and TrainBatchBuilder.from_frustums make the current stream wait
     for that stream first (wait()); other readers of the tensors on another stream call wait() themselves."""
@@ -194,7 +194,7 @@ class LabelledFrustums:
             torch.cuda.current_stream(self.points.device).wait_stream(self.stream)
 
     def input_list(self):
-        """The per-frustum (n, 4) float32 point arrays, copied to the host."""
+        """The per-frustum (n, 4) (SUN-RGBD: (n, 6)) float32 point arrays, copied to the host."""
         self.wait()
         return self._split(self.points.cpu().numpy())
 

@@ -251,11 +251,18 @@ class TrainBatchBuilder:
 
     @classmethod
     def from_frustums(cls, fr, kind, strides, npoints, classes=None, **kw):
-        """The dataset of a refine_extract.RefineFrustums (kind="refine") or a gt_extract.GtFrustums (kind="det"): its
-        points stay on the device (the x, y, z columns are copied there; a GtFrustums' uint8 labels are cast to the
-        int32 seg labels there), the per-frustum constants come from its host lists.  The same batches as
-        set_dataset on fr's lists.  labels defaults to whether fr has ground truth."""
+        """The dataset of a refine_extract.RefineFrustums (kind="refine"), a gt_extract.GtFrustums (kind="det") or a
+        sunrgbd_extract.SunrgbdFrustums (kind="sunrgbd"): its points stay on the device (the x, y, z columns are
+        copied there; uint8 labels are cast to the int32 seg labels there), the per-frustum constants come from its
+        host lists.  The same batches as set_dataset on fr's lists.  labels defaults to whether fr has ground truth;
+        classes to the kind's dataset."""
         from .gt_extract import GtFrustums
+        from .sunrgbd_extract import SunrgbdFrustums
+        if isinstance(fr, SunrgbdFrustums):
+            if kind != "sunrgbd":
+                raise ValueError("from_frustums builds the SUN-RGBD provider's batches (kind='sunrgbd') from "
+                                 "SunrgbdFrustums, got %r" % kind)
+            return cls._from_sunrgbd(fr, strides, npoints, classes, **kw)
         gt = isinstance(fr, GtFrustums)
         if gt and kind != "det":
             raise ValueError("from_frustums builds the detection provider's batches (kind='det') from GtFrustums, "
@@ -281,6 +288,27 @@ class TrainBatchBuilder:
                               **{n: getattr(fr, n) for n in names})
         tb.points_f64 = False
         tb._install(table, counts, fr.points[:, :3].contiguous(), None, fr.label.to(torch.int32) if gt else None)
+        return tb
+
+    @classmethod
+    def _from_sunrgbd(cls, fr, strides, npoints, classes, **kw):
+        kw.setdefault("labels", fr.has_labels)
+        tb = cls("sunrgbd", strides, npoints, **kw)
+        if tb.labels and not fr.has_labels:
+            raise ValueError("labels=True needs frustums with ground truth (from_ground_truth)")
+        if len(fr) == 0:
+            raise ValueError("empty dataset")
+        if fr.points.device.type != "cuda" or (tb.device.index is not None and fr.points.device != tb.device):
+            raise RuntimeError("the frustums live on %s, the builder on %s" % (fr.points.device, tb.device))
+        fr.wait()                          # the points and labels were written on the extraction's stream
+        names = ("frustum_angle_list", "box2d_list", "calib_K_list", "calib_R_list") + (
+            ("box3d_list", "heading_list", "size_list") if tb.labels else ("prob_list",))
+        table = frustum_table("sunrgbd", tb.strides, tb.max_depth, tb.labels,
+                              SUNRGBD_CLASSES if classes is None else classes, fr.type_list,
+                              **{n: getattr(fr, n) for n in names})
+        tb.points_f64 = False
+        tb._install(table, np.asarray(fr.counts, dtype=np.int64), fr.points[:, :3].contiguous(), None,
+                    fr.label.to(torch.int32) if tb.labels else None)
         return tb
 
     def _install(self, fr, counts, d_points, label_list, d_seg=None):

@@ -917,6 +917,76 @@ FCN_API long long fcn_gt_extract_workspace_bytes(const fcn_gt_extract_args *args
 FCN_API int fcn_gt_extract_count(const fcn_gt_extract_args *args, fcn_stream_t stream);
 FCN_API int fcn_gt_extract_write(const fcn_gt_extract_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (18) SUN-RGBD frustums on the device: the point work of extract_frustum_data and
+ *      extract_frustum_data_from_rgb_detection of sunrgbd/prepare_data.py:132-381 (--gen_train, --gen_val,
+ *      --gen_val_rgb_detection) for several frames and all their jobs at once.
+ *
+ *      Scans are (n, 6) float32 rows x, y, z, r, g, b in upright depth coordinates.  Every scan point is a candidate
+ *      (no image-bounds test): its float64 image coordinates are project_upright_depth_to_image's, each np.dot
+ *      accumulated as OpenBLAS's dgemm does (the first product rounded, then one FMA per further term) and the two
+ *      divisions IEEE.  A job j (jobs[j], fcn_gt_job of section (17)) is one cutting 2-D box in frame jobs[j].frame
+ *      and, when jobs[j].label >= 0, one label 3-D box label_boxes[jobs[j].label] (fcn_refine_box: centre
+ *      (cx, -cz, cy), half extents (l, h, w), cs = cos(heading_angle), sn = sin(heading_angle), the corners of
+ *      sunrgbd_utils.compute_box_3d flipped to upright camera coordinates).  Its in-box points are the frame's points
+ *      with u < xmax, u >= xmin, v < ymax and v >= ymin, in scan order; a point is labelled 1 when the section (16)
+ *      half-space test puts its upright camera coordinates (x, -z, y) in the label box.  labelled = 1 for the ground
+ *      truth sets (all jobs have a label box), 0 for detections (no job has one).
+ *
+ *      Four calls in order on one stream, sharing the caller's workspace (fcn_sunrgbd_extract_workspace_bytes: needs
+ *      the device, -1 on invalid arguments), no host sync, no allocation:
+ *        fcn_sunrgbd_extract_project : u, v of every scan point into the workspace;
+ *        fcn_sunrgbd_extract_count   : for the jobs [job_begin, job_end) (may run several times; the jobs of a
+ *                                      range are uploaded before it, a later call overwrites a job's words):
+ *                                      job_points (DEVICE, num_jobs: the in-box count n, -1 when the frame or
+ *                                      label index is out of range) and job_labelled (DEVICE, num_jobs: its
+ *                                      labelled points);
+ *        fcn_sunrgbd_extract_select  : after every job is counted and the subsample draws uploaded: job_choice
+ *                                      (DEVICE, num_jobs: c for the c-th job with n > 2048, -1 for the others),
+ *                                      choice_ranks (DEVICE, num_choices x 2048: the in-box ranks np.random.choice
+ *                                      chose, sorted) and choice_slots (DEVICE, same shape: the output row of each).
+ *                                      A job keeps min(n, 2048) points; it is dropped when fewer than 5 of them are
+ *                                      labelled (labelled = 1) or when n < 5 (labelled = 0).  Overwrites job_points
+ *                                      with the kept count (-1 when dropped) and writes info (DEVICE
+ *                                      int64[4]: kept jobs K, their points M, jobs with an out-of-range index, 0);
+ *        fcn_sunrgbd_extract_write   : needs num_kept = K and num_out_points = M as read by the host; writes the kept
+ *                                      jobs in job order: points (M, 6) float32 (x, -z, y, r, g, b), in scan order or,
+ *                                      for a job with n > 2048, in choice order; labels (M) uint8 (labelled = 1
+ *                                      only) and offsets (K + 1) int32.
+ *      With num_frames == 0 or num_jobs == 0 every call returns 0 and does nothing (K = M = 0; info is not written).
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_SUNRGBD_MAX_POINTS 2048
+typedef struct {
+    double Rtilt[9];    /* row-major */
+    double K[9];        /* row-major */
+} fcn_sunrgbd_frame;
+typedef struct {
+    int num_frames, num_points, num_jobs, num_labels, num_choices, labelled;
+    int job_begin, job_end, num_kept, reserved;
+    long long num_out_points;
+    const float *scans;                 /* DEVICE (num_points, 6) */
+    const int32_t *scan_offsets;        /* DEVICE (num_frames + 1) */
+    const int32_t *host_scan_offsets;   /* HOST copy: starts at 0, never decreases, ends at num_points */
+    const fcn_sunrgbd_frame *frames;    /* DEVICE (num_frames) */
+    const fcn_gt_job *jobs;             /* DEVICE (num_jobs) */
+    const fcn_refine_box *label_boxes;  /* DEVICE (num_labels) */
+    const int32_t *job_choice;          /* DEVICE (num_jobs), select */
+    const int32_t *choice_ranks;        /* DEVICE (num_choices, 2048), select and write */
+    const int32_t *choice_slots;        /* DEVICE (num_choices, 2048), write */
+    void *workspace;
+    long long workspace_bytes;
+    long long *info;                    /* DEVICE int64[4] */
+    int32_t *job_points, *job_labelled; /* DEVICE (num_jobs) each */
+    float *points;                      /* fcn_sunrgbd_extract_write outputs (DEVICE) */
+    uint8_t *labels;
+    int32_t *offsets;
+} fcn_sunrgbd_extract_args;
+FCN_API long long fcn_sunrgbd_extract_workspace_bytes(const fcn_sunrgbd_extract_args *args);
+FCN_API int fcn_sunrgbd_extract_project(const fcn_sunrgbd_extract_args *args, fcn_stream_t stream);
+FCN_API int fcn_sunrgbd_extract_count(const fcn_sunrgbd_extract_args *args, fcn_stream_t stream);
+FCN_API int fcn_sunrgbd_extract_select(const fcn_sunrgbd_extract_args *args, fcn_stream_t stream);
+FCN_API int fcn_sunrgbd_extract_write(const fcn_sunrgbd_extract_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
