@@ -45,11 +45,16 @@ __device__ __forceinline__ BnCoef bn_coef(const double *sums, const float *gamma
     return r;
 }
 
-// operand element: post-activation value of source `s` at (frustum b, position p, channel c); 0 outside [0, T*up)
-__device__ __forceinline__ float src_act(const fcn_train_src &s, int b, int p, int c, float scale, float shift) {
-    if (p < 0 || p >= s.T * s.up) return 0.f;
-    const int row = b * s.T + p / s.up, col = s.c0 + (p % s.up) * s.cup + c;
-    float x = s.raw[(size_t)row * s.ld + col];
+// (scale, shift) with which a consumer applies source `s`'s BN to its channel c: identity without statistics or for a
+// channel past the segment (!in_range)
+__device__ __forceinline__ float2 src_coef(const fcn_train_src &s, int c, bool in_range) {
+    if (s.sums == nullptr || !in_range) return make_float2(1.f, 0.f);
+    const BnCoef b = bn_coef(s.sums, s.gamma, s.beta, s.Cstat, (s.coff + c) % s.Cstat, 1.0 / s.count);
+    return make_float2(b.scale, b.shift);
+}
+
+// the producer's BN + ReLU applied to a raw element of source `s` (raw value without statistics)
+__device__ __forceinline__ float src_bn_relu(const fcn_train_src &s, float x, float scale, float shift) {
     if (s.sums != nullptr) {
         x = fmaf(x, scale, shift);
         if (s.relu) x = fmaxf(x, 0.f);
@@ -57,12 +62,20 @@ __device__ __forceinline__ float src_act(const fcn_train_src &s, int b, int p, i
     return x;
 }
 
-// gradient element dY(r, n) of a layer (BN backward applied on the fly; plain layers: dY = dA)
-struct DyCtx {
-    float scale, m1, m2, mean, invstd, shift;
+// operand element: post-activation value of source `s` at (frustum b, position p, channel c); 0 outside [0, T*up)
+__device__ __forceinline__ float src_act(const fcn_train_src &s, int b, int p, int c, float scale, float shift) {
+    if (p < 0 || p >= s.T * s.up) return 0.f;
+    const int row = b * s.T + p / s.up, col = s.c0 + (p % s.up) * s.cup + c;
+    return src_bn_relu(s, s.raw[(size_t)row * s.ld + col], scale, shift);
+}
+
+// gradient element dY(r, n) of a layer (BN backward applied on the fly; plain layers: dY = dA).  Output column n's
+// coefficients: BN scale / shift / mean / invstd and m1 = mean(dz), m2 = mean(dz * xh); identity without BN.
+struct DyCoef {
+    float scale, shift, mean, invstd, m1, m2;
 };
-__device__ __forceinline__ DyCtx dy_ctx(const fcn_train_layer &L, int n) {
-    DyCtx c;
+__device__ __forceinline__ DyCoef dy_coef(const fcn_train_layer &L, int n) {
+    DyCoef c;
     if (!L.has_bn) { c.scale = 1.f; c.m1 = c.m2 = c.mean = c.shift = 0.f; c.invstd = 1.f; return c; }
     const int co = n % L.Cout;
     const double inv = 1.0 / ((double)L.B * L.T_out * L.up);
@@ -72,13 +85,46 @@ __device__ __forceinline__ DyCtx dy_ctx(const fcn_train_layer &L, int n) {
     c.m2 = (float)(L.dsums[L.Cout + co] * inv);
     return c;
 }
-__device__ __forceinline__ float dy_elem(const fcn_train_layer &L, const DyCtx &c, int r, int n) {
+__device__ __forceinline__ float dy_apply(const DyCoef &c, float da, float y, bool relu) {
+    const float dz = (relu && fmaf(y, c.scale, c.shift) <= 0.f) ? 0.f : da;
+    return c.scale * (dz - c.m1 - (y - c.mean) * c.invstd * c.m2);
+}
+// no BN: dA itself (dy_apply with identity coefficients would turn an inf / NaN in Y into NaN)
+__device__ __forceinline__ float dy_elem(const fcn_train_layer &L, const DyCoef &c, int r, int n) {
     const float da = L.dA[(size_t)r * L.N + n];
     if (!L.has_bn) return da;
-    const float y = L.Y[(size_t)r * L.N + n];
-    const float dz = (L.relu && fmaf(y, c.scale, c.shift) <= 0.f) ? 0.f : da;
-    const float xh = (y - c.mean) * c.invstd;
-    return c.scale * (dz - c.m1 - xh * c.m2);
+    return dy_apply(c, da, L.Y[(size_t)r * L.N + n], L.relu);
+}
+
+// one TG_BK step of the generic kernels' 4 x 4 micro-tile (rows ty*4.., columns tx*4..)
+__device__ __forceinline__ void tile_fma_4x4(float (&acc)[4][4], const float (&As)[TG_BK][TG_BM + 4],
+                                             const float (&Bs)[TG_BK][TG_BN + 4], int tx, int ty) {
+#pragma unroll
+    for (int kk = 0; kk < TG_BK; ++kk) {
+        float a[4], bq[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) bq[j] = Bs[kk][tx * 4 + j];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bq[j], acc[i][j]);
+    }
+}
+
+// Block = 32 columns (nl) x 8 row lanes (rl): each column's two partial sums a1, a2 added over the lanes in lane
+// order.  Every thread calls it (barrier).  Returns `lead` (a thread of lane 0); where true, a1 and a2 hold the sums.
+__device__ __forceinline__ bool column_pair_sum(float &a1, float &a2, int nl, int rl, bool lead) {
+    __shared__ float s1[8][33], s2[8][33];
+    s1[rl][nl] = a1; s2[rl][nl] = a2;
+    __syncthreads();
+    if (lead) {
+        a1 = a2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { a1 += s1[i][nl]; a2 += s2[i][nl]; }
+    }
+    return lead;
 }
 
 // weight element (segment channel c, output column n) in the parameter layout
@@ -114,7 +160,7 @@ train_fwd_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ 
         for (int t = t_lo; t < t_hi; ++t) {
             const int k0 = t * TG_BK;
             __syncthreads();
-            if (tid < TG_BK) {
+            if (tid < TG_BK) {          // src_coef, with the inverse count hoisted out of the tile loop
                 const int c = k0 + tid;
                 float sc = 1.f, sh = 0.f;
                 if (s.sums != nullptr && c < g.C) {
@@ -142,18 +188,7 @@ train_fwd_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ 
                 Bs[kk][nn] = (c < g.C && n < L.N) ? L.W[w_index(L, g, c, n)] : 0.f;
             }
             __syncthreads();
-#pragma unroll
-            for (int kk = 0; kk < TG_BK; ++kk) {
-                float a[4], bq[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) bq[j] = Bs[kk][tx * 4 + j];
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bq[j], acc[i][j]);
-            }
+            tile_fma_4x4(acc, As, Bs, tx, ty);
         }
     }
     if (gridDim.z > 1) {                                     // partial sums of this K slice
@@ -209,7 +244,6 @@ train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *
     const int n = blockIdx.x * 32 + nl;
     const int M = L.B * L.T_out;
     const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
-    __shared__ float s1[8][33], s2[8][33];
     float a1 = 0.f, a2 = 0.f;
     if (n < L.N) {
         const float bias = L.bias != nullptr ? L.bias[n] : 0.f;
@@ -221,15 +255,10 @@ train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *
         }
     }
     if (!L.has_bn) return;
-    s1[rl][nl] = a1; s2[rl][nl] = a2;
-    __syncthreads();
-    if (rl == 0 && n < L.N) {
-        float t1 = 0.f, t2 = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { t1 += s1[i][nl]; t2 += s2[i][nl]; }
+    if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
         const int co = n % L.Cout;
-        atomicAdd(&L.sums[co], (double)t1);
-        atomicAdd(&L.sums[L.Cout + co], (double)t2);
+        atomicAdd(&L.sums[co], (double)a1);
+        atomicAdd(&L.sums[L.Cout + co], (double)a2);
     }
 }
 
@@ -241,7 +270,6 @@ train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bloc
     const int n = blockIdx.x * 32 + nl;
     const int M = L.B * L.T_out;
     const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
-    __shared__ float s1[8][33], s2[8][33];
     float a1 = 0.f, a2 = 0.f;
     if (n < L.N) {
         BnCoef b = {1.f, 0.f, 0.f, 1.f};
@@ -255,16 +283,11 @@ train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bloc
             a2 += dz * ((y - b.mean) * b.invstd);
         }
     }
-    s1[rl][nl] = a1; s2[rl][nl] = a2;
-    __syncthreads();
-    if (rl == 0 && n < L.N) {
-        float t1 = 0.f, t2 = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { t1 += s1[i][nl]; t2 += s2[i][nl]; }
+    if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
         const int co = L.has_bn ? n % L.Cout : n;
         const int C = L.has_bn ? L.Cout : L.N;
-        atomicAdd(&L.dsums[co], (double)t1);
-        if (L.has_bn) atomicAdd(&L.dsums[C + co], (double)t2);
+        atomicAdd(&L.dsums[co], (double)a1);
+        if (L.has_bn) atomicAdd(&L.dsums[C + co], (double)a2);
     }
 }
 
@@ -273,7 +296,7 @@ __global__ void __launch_bounds__(TG_THREADS)
 train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows_per_block) {
     __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[row][k-channel], Bs[row][n]
     __shared__ float s_scale[TG_BM], s_shift[TG_BM];
-    __shared__ DyCtx s_dy[TG_BN];
+    __shared__ DyCoef s_dy[TG_BN];
     const fcn_train_seg &g = L.seg[seg_idx];
     const fcn_train_src &s = g.src;
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
@@ -281,15 +304,10 @@ train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows
     const int M = L.B * L.T_out;
     const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
     if (tid < TG_BM) {
-        const int c = c0 + tid;
-        float sc = 1.f, sh = 0.f;
-        if (s.sums != nullptr && c < g.C) {
-            const BnCoef b = bn_coef(s.sums, s.gamma, s.beta, s.Cstat, (s.coff + c) % s.Cstat, 1.0 / s.count);
-            sc = b.scale; sh = b.shift;
-        }
-        s_scale[tid] = sc; s_shift[tid] = sh;
+        const float2 k = src_coef(s, c0 + tid, c0 + tid < g.C);
+        s_scale[tid] = k.x; s_shift[tid] = k.y;
     }
-    if (tid < TG_BN) s_dy[tid] = dy_ctx(L, min(n0 + tid, L.N - 1));
+    if (tid < TG_BN) s_dy[tid] = dy_coef(L, min(n0 + tid, L.N - 1));
     float acc[4][4] = {};
     for (int rr0 = rb; rr0 < re; rr0 += TG_BK) {
         __syncthreads();
@@ -311,18 +329,7 @@ train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows
             Bs[rr][nn] = (r < re && n < L.N) ? dy_elem(L, s_dy[nn], r, n) : 0.f;
         }
         __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < TG_BK; ++kk) {
-            float a[4], bq[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) bq[j] = Bs[kk][tx * 4 + j];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bq[j], acc[i][j]);
-        }
+        tile_fma_4x4(acc, As, Bs, tx, ty);
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -340,7 +347,7 @@ train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows
 __global__ void __launch_bounds__(TG_THREADS)
 train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_per_slice) {
     __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[n][row], Bs[n][channel]
-    __shared__ DyCtx s_dy[TG_BK];
+    __shared__ DyCoef s_dy[TG_BK];
     const fcn_train_seg &g = L.seg[seg_idx];
     const fcn_train_src &s = g.src;
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
@@ -350,7 +357,7 @@ train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_pe
     const int n_lo = blockIdx.z * n_per_slice, n_hi = min(L.N, n_lo + n_per_slice);
     for (int nn0 = n_lo; nn0 < n_hi; nn0 += TG_BK) {
         __syncthreads();
-        if (tid < TG_BK) s_dy[tid] = dy_ctx(L, min(nn0 + tid, L.N - 1));
+        if (tid < TG_BK) s_dy[tid] = dy_coef(L, min(nn0 + tid, L.N - 1));
         __syncthreads();
 #pragma unroll
         for (int i = 0; i < 4; ++i) {       // dY tile: 64 rows x 16 columns (consecutive threads -> consecutive n)
@@ -363,18 +370,7 @@ train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_pe
             Bs[kk][cc] = (n < n_hi && c < g.C) ? L.W[w_index(L, g, c, n)] : 0.f;
         }
         __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < TG_BK; ++kk) {
-            float a[4], bq[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) bq[j] = Bs[kk][tx * 4 + j];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bq[j], acc[i][j]);
-        }
+        tile_fma_4x4(acc, As, Bs, tx, ty);
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -460,26 +456,26 @@ __global__ void train_adam_kernel(float *__restrict__ p, const float *__restrict
 
 // =====================================================================================================
 // Fast path for the PointNet layers 2/3 (97 % of the step's FLOPs): single source, 1x1 conv, rows map 1:1
-// (tap 0, stride 1, no pixel shuffle), channels and columns multiples of 16 / 64.  128 x 64 x 16 tiles,
-// 8 x 4 micro-tiles, float4 global loads along the contiguous axis, register prefetch of the next tile.
-// Same arithmetic (fp32 FMA, same on-the-fly BN / ReLU forward and backward) as the generic kernels above.
+// (tap 0, stride 1, no pixel shuffle), channels and columns multiples of 64 up to 512 (host_plain states the rule).
+// 128 x 64 x 16 tiles, 8 x 4 micro-tiles, float4 global loads along the contiguous axis, register prefetch of the
+// next tile.  Same arithmetic (fp32 FMA, same on-the-fly BN / ReLU forward and backward) as the generic kernels above.
 // =====================================================================================================
 constexpr int FP_BM = 128, FP_BN = 64, FP_BK = 16, FP_THREADS = 256;
 
-#define FP_COMPUTE(As_, Bs_)                                                                        \
-    _Pragma("unroll") for (int kk = 0; kk < FP_BK; ++kk) {                                          \
-        const float4 a0 = *(const float4 *)&As_[kk][ty * 8], a1 = *(const float4 *)&As_[kk][ty * 8 + 4]; \
-        const float4 b0 = *(const float4 *)&Bs_[kk][tx * 4];                                        \
-        const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};                       \
-        const float b[4] = {b0.x, b0.y, b0.z, b0.w};                                                \
-        _Pragma("unroll") for (int i = 0; i < 8; ++i)                                               \
-            _Pragma("unroll") for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);  \
+// one FP_BK step of the plain kernels' 8 x 4 micro-tile (rows ty*8.., columns tx*4..), float4 shared loads
+__device__ __forceinline__ void tile_fma_8x4(float (&acc)[8][4], const float (&As)[FP_BK][FP_BM + 4],
+                                             const float (&Bs)[FP_BK][FP_BN + 4], int tx, int ty) {
+#pragma unroll
+    for (int kk = 0; kk < FP_BK; ++kk) {
+        const float4 a0 = *(const float4 *)&As[kk][ty * 8], a1 = *(const float4 *)&As[kk][ty * 8 + 4];
+        const float4 b0 = *(const float4 *)&Bs[kk][tx * 4];
+        const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+        const float b[4] = {b0.x, b0.y, b0.z, b0.w};
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
     }
-
-__device__ __forceinline__ bool plain_layer(const fcn_train_layer &L) {
-    const fcn_train_seg &g = L.seg[0];
-    return L.n_seg == 1 && g.tap == 0 && g.stride == 1 && g.src.up == 1 && L.up == 1 && g.src.T == L.T_out &&
-           g.s_ci == 1 && g.C % FP_BK == 0 && L.N % FP_BN == 0 && g.src.c0 == 0 && g.src.ld % 4 == 0;
 }
 
 // Y[M,N] = act(X[M,K]) * W^T   (W in parameter layout (N,K): both operands contiguous along K)
@@ -494,16 +490,11 @@ train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
     const int r0 = blockIdx.x * FP_BM, n0 = blockIdx.y * FP_BN;
     const int M = L.B * L.T_out, K = g.C;
     for (int c = tid; c < K; c += FP_THREADS) {
-        float sc = 1.f, sh = 0.f;
-        if (s.sums != nullptr) {
-            const BnCoef b = bn_coef(s.sums, s.gamma, s.beta, s.Cstat, (s.coff + c) % s.Cstat, 1.0 / s.count);
-            sc = b.scale; sh = b.shift;
-        }
-        s_scale[c] = sc; s_shift[c] = sh;
+        const float2 k = src_coef(s, c, true);
+        s_scale[c] = k.x; s_shift[c] = k.y;
     }
     if (tid < FP_BN) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
     __syncthreads();
-    const bool act = s.sums != nullptr, relu = s.relu != 0;
     // A: 128 rows x 16 k = 512 float4 (2 per thread); B: 64 n x 16 k = 256 float4 (1 per thread)
     const int arow = tid / 4, akq = (tid % 4) * 4;
     const int bn = tid / 4, bkq = (tid % 4) * 4;
@@ -523,11 +514,7 @@ train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
             const bool ok = r0 + arow + 64 * h < M;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                float x = v[i];
-                if (act) {
-                    x = fmaf(x, s_scale[k0 + akq + i], s_shift[k0 + akq + i]);
-                    if (relu) x = fmaxf(x, 0.f);
-                }
+                const float x = src_bn_relu(s, v[i], s_scale[k0 + akq + i], s_shift[k0 + akq + i]);
                 As[akq + i][arow + 64 * h] = ok ? x : 0.f;
             }
         }
@@ -540,7 +527,7 @@ train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
         sstore(k0);
         __syncthreads();
         if (k0 + FP_BK < K) gload(k0 + FP_BK);
-        FP_COMPUTE(As, Bs)
+        tile_fma_8x4(acc, As, Bs, tx, ty);
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -565,15 +552,6 @@ train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
     }
 }
 
-// dY(m, n) for 4 consecutive n (BN/ReLU backward on the fly), coefficient arrays in shared memory
-struct DyCoef {
-    float scale, shift, mean, invstd, m1, m2;
-};
-__device__ __forceinline__ float dy_apply(const DyCoef &c, float da, float y, bool relu) {
-    const float dz = (relu && fmaf(y, c.scale, c.shift) <= 0.f) ? 0.f : da;
-    return c.scale * (dz - c.m1 - (y - c.mean) * c.invstd * c.m2);
-}
-
 // dX[M,K] += dY[M,N] * W   (W (N,K): contiguous along K).  One CTA owns each element and there is no N split, so
 // the accumulation into the source gradient (shared with its other consumers) is a plain read-add-store.
 __global__ void __launch_bounds__(FP_THREADS)
@@ -585,10 +563,7 @@ train_dx_plain_kernel(const __grid_constant__ fcn_train_layer L) {
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
     const int r0 = blockIdx.x * FP_BM, c0 = blockIdx.y * FP_BN;
     const int M = L.B * L.T_out, N = L.N;
-    for (int n = tid; n < N; n += FP_THREADS) {
-        const DyCtx c = dy_ctx(L, n);
-        s_c[n] = {c.scale, c.shift, c.mean, c.invstd, c.m1, c.m2};
-    }
+    for (int n = tid; n < N; n += FP_THREADS) s_c[n] = dy_coef(L, n);
     __syncthreads();
     const bool relu = L.relu != 0;
     const int arow = tid / 4, anq = (tid % 4) * 4;          // dY tile: 128 rows x 16 n
@@ -625,7 +600,7 @@ train_dx_plain_kernel(const __grid_constant__ fcn_train_layer L) {
         sstore(n0);
         __syncthreads();
         if (n0 + FP_BK < N) gload(n0 + FP_BK);
-        FP_COMPUTE(As, Bs)
+        tile_fma_8x4(acc, As, Bs, tx, ty);
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -650,21 +625,13 @@ train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bl
     const int n0 = blockIdx.x * FP_BM, c0 = blockIdx.y * FP_BN;
     const int M = L.B * L.T_out, N = L.N;
     const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
-    if (tid < FP_BM) {
-        const int n = min(n0 + tid, N - 1);
-        const DyCtx c = dy_ctx(L, n);
-        s_c[tid] = {c.scale, c.shift, c.mean, c.invstd, c.m1, c.m2};
-    }
+    if (tid < FP_BM) s_c[tid] = dy_coef(L, min(n0 + tid, N - 1));
     if (tid < FP_BN) {
-        float sc = 1.f, sh = 0.f;
-        if (s.sums != nullptr) {
-            const BnCoef b = bn_coef(s.sums, s.gamma, s.beta, s.Cstat, (s.coff + c0 + tid) % s.Cstat, 1.0 / s.count);
-            sc = b.scale; sh = b.shift;
-        }
-        s_scale[tid] = sc; s_shift[tid] = sh;
+        const float2 k = src_coef(s, c0 + tid, true);
+        s_scale[tid] = k.x; s_shift[tid] = k.y;
     }
     __syncthreads();
-    const bool relu = L.relu != 0, act = s.sums != nullptr, srelu = s.relu != 0;
+    const bool relu = L.relu != 0;
     // dY tile: 16 rows x 128 n = 512 float4 (2 per thread); X tile: 16 rows x 64 k = 256 float4 (1 per thread)
     const int ar = tid / 32, anq = (tid % 32) * 4;
     const int br = tid / 16, bkq = (tid % 16) * 4;
@@ -699,10 +666,7 @@ train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bl
         float x[4] = {px.x, px.y, px.z, px.w};
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            if (act) {
-                x[i] = fmaf(x[i], s_scale[bkq + i], s_shift[bkq + i]);
-                if (srelu) x[i] = fmaxf(x[i], 0.f);
-            }
+            x[i] = src_bn_relu(s, x[i], s_scale[bkq + i], s_shift[bkq + i]);
             if (!ok) x[i] = 0.f;
         }
         *(float4 *)&Bs[br][bkq] = make_float4(x[0], x[1], x[2], x[3]);
@@ -714,7 +678,7 @@ train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bl
         sstore(m0);
         __syncthreads();
         if (m0 + FP_BK < re) gload(m0 + FP_BK);
-        FP_COMPUTE(As, Bs)
+        tile_fma_8x4(acc, As, Bs, tx, ty);
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -739,19 +703,23 @@ static int check_layer(const fcn_train_layer &L) {
     return FCN_OK;
 }
 
-static bool host_plain(const fcn_train_layer &L, bool need_src_grad_layout) {
+// the layer takes the plain kernels (shared-memory tables: C, N <= 512; float4 loads: 16-byte aligned rows)
+static bool host_plain(const fcn_train_layer &L) {
     const fcn_train_seg &g = L.seg[0];
-    const bool ok = L.n_seg == 1 && g.tap == 0 && g.stride == 1 && g.src.up == 1 && L.up == 1 && g.src.T == L.T_out &&
-                    g.s_ci == 1 && g.C % 64 == 0 && g.C <= 512 && L.N % 64 == 0 && L.N <= 512 && g.src.c0 == 0 &&
-                    g.src.ld % 4 == 0 && g.w_off % 4 == 0 && L.s_co % 4 == 0 && L.has_bn && L.bias == nullptr &&
-                    L.Cout == L.N;
-    (void)need_src_grad_layout;
-    return ok;
+    return L.n_seg == 1 && g.tap == 0 && g.stride == 1 && g.src.up == 1 && L.up == 1 && g.src.T == L.T_out &&
+           g.s_ci == 1 && g.C % 64 == 0 && g.C <= 512 && L.N % 64 == 0 && L.N <= 512 && g.src.c0 == 0 &&
+           g.src.ld % 4 == 0 && g.w_off % 4 == 0 && L.s_co % 4 == 0 && L.has_bn && L.bias == nullptr &&
+           L.Cout == L.N;
 }
 
 }  // namespace fcn
 
 using namespace fcn;
+
+// The generic kernels split their reduction until about this many CTAs exist: 2 per SM of the 148-SM GPU the splits
+// were tuned for, not the H100's 132.  Kept because the forward's K split decides the order in which its partial
+// sums add up, so another value changes the bits of Y.
+constexpr int SPLIT_CTAS = 2 * 148;
 
 // K slices of the generic forward GEMM for this layer (1 = no split); `workspace_floats` bounds the partial sums
 static int fwd_slices(const fcn_train_layer &L, long long workspace_floats, int *tiles_per_slice) {
@@ -759,7 +727,7 @@ static int fwd_slices(const fcn_train_layer &L, long long workspace_floats, int 
     int tiles = 0;
     for (int i = 0; i < L.n_seg; ++i) tiles += ceil_div(L.seg[i].C, TG_BK);
     const int ctas = ceil_div(M, TG_BM) * ceil_div(L.N, TG_BN);
-    int want = ceil_div(2 * 148, ctas);                      // ~2 CTAs per SM in total
+    int want = ceil_div(SPLIT_CTAS, ctas);
     if (want > tiles / 2) want = tiles / 2;                  // at least two K tiles per slice
     const long long fit = workspace_floats / ((long long)M * L.N);
     if (want > fit) want = (int)fit;
@@ -768,8 +736,16 @@ static int fwd_slices(const fcn_train_layer &L, long long workspace_floats, int 
     return ceil_div(tiles, *tiles_per_slice);
 }
 
+// Rows (dW) or columns (dX) per CTA of a backward reduction of length `len` over `ctas` output tiles: about
+// SPLIT_CTAS CTAs in all, a multiple of TG_BK and at least two tiles.  The layers are skinny, and a handful of CTAs
+// with long serial loops would be the bottleneck (the outputs are atomic accumulations).
+static int split_len(int len, int ctas) {
+    const int per = ceil_div(ceil_div(len, ceil_div(SPLIT_CTAS, ctas)), TG_BK) * TG_BK;
+    return per < 2 * TG_BK ? 2 * TG_BK : per;
+}
+
 extern "C" long long fcn_train_workspace_floats(const fcn_train_layer *L) {
-    // enough for the split the launcher would like to use: 2*148 CTAs' worth of partial tiles, at most K/32 slices
+    // enough for the split the launcher would like to use: SPLIT_CTAS CTAs' worth of partial tiles, at most K/32 slices
     if (L == nullptr) return 0;
     int tps = 0;
     const int n = fwd_slices(*L, (long long)1 << 40, &tps);
@@ -782,7 +758,7 @@ extern "C" int fcn_train_forward(const fcn_train_layer *L, float *workspace, lon
     if (int rc = check_layer(*L)) return rc;
     const int M = L->B * L->T_out;
     cudaStream_t st = (cudaStream_t)stream;
-    if (host_plain(*L, false)) {
+    if (host_plain(*L)) {
         dim3 grid(ceil_div(M, FP_BM), L->N / FP_BN);
         train_fwd_plain_kernel<<<grid, FP_THREADS, 0, st>>>(*L);
         FCN_LAUNCH_CHECK();
@@ -814,7 +790,7 @@ extern "C" int fcn_train_backward(const fcn_train_layer *L, int need_dx_mask, fc
         train_reduce_kernel<<<grid, 256, 0, st>>>(*L, rpb);
         FCN_LAUNCH_CHECK();
     }
-    if (host_plain(*L, true)) {
+    if (host_plain(*L)) {
         const int rpb = 1024;
         dim3 grid(ceil_div(L->N, FP_BM), L->seg[0].C / FP_BN, ceil_div(M, rpb));
         train_dw_plain_kernel<<<grid, FP_THREADS, 0, st>>>(*L, rpb);
@@ -827,20 +803,12 @@ extern "C" int fcn_train_backward(const fcn_train_layer *L, int need_dx_mask, fc
         return FCN_OK;
     }
     for (int sg = 0; sg < L->n_seg; ++sg) {
-        // split the reduction (rows for dW, columns for dX) until ~2 CTAs per SM exist: the layers are skinny and
-        // a handful of CTAs with long serial loops would be the bottleneck (outputs are atomic accumulations)
-        const int cw = ceil_div(L->seg[sg].C, TG_BM) * ceil_div(L->N, TG_BN);
-        int zs = ceil_div(2 * 148, cw);
-        int rpb = ceil_div(ceil_div(M, zs), TG_BK) * TG_BK;
-        if (rpb < 2 * TG_BK) rpb = 2 * TG_BK;
+        const int rpb = split_len(M, ceil_div(L->seg[sg].C, TG_BM) * ceil_div(L->N, TG_BN));
         dim3 grid(ceil_div(L->seg[sg].C, TG_BM), ceil_div(L->N, TG_BN), ceil_div(M, rpb));
         train_dw_kernel<<<grid, TG_THREADS, 0, st>>>(*L, sg, rpb);
         FCN_LAUNCH_CHECK();
         if (((need_dx_mask >> sg) & 1) && L->seg[sg].src.grad != nullptr) {
-            const int cx = ceil_div(M, TG_BM) * ceil_div(L->seg[sg].C, TG_BN);
-            int zx = ceil_div(2 * 148, cx);
-            int nps = ceil_div(ceil_div(L->N, zx), TG_BK) * TG_BK;
-            if (nps < 2 * TG_BK) nps = 2 * TG_BK;
+            const int nps = split_len(L->N, ceil_div(M, TG_BM) * ceil_div(L->seg[sg].C, TG_BN));
             dim3 gx(ceil_div(M, TG_BM), ceil_div(L->seg[sg].C, TG_BN), ceil_div(L->N, nps));
             train_dx_kernel<<<gx, TG_THREADS, 0, st>>>(*L, sg, nps);
             FCN_LAUNCH_CHECK();
