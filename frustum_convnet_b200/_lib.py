@@ -366,6 +366,7 @@ SIGNATURES = {
     "fcn_val_partials_floats": (C.c_longlong, [_I, _I]),
     "fcn_val_batch": (_I, [C.POINTER(ValBatchArgs), _P]),
     "fcn_val_finalize": (_I, [_P, _I, _P, _P, _P]),
+    "fcn_train_states_append": (_I, [_P, _I, _P, _I, _P, _P]),
     "fcn_kitti_eval_workspace_bytes": (C.c_longlong, [C.POINTER(KittiEvalArgs)]),
     "fcn_kitti_eval_overlaps": (_I, [C.POINTER(KittiEvalArgs), _P]),
     "fcn_kitti_eval_thresholds": (_I, [C.POINTER(KittiEvalArgs), _P]),

@@ -6,6 +6,7 @@
 //   val_final_kernel  : one warp sums the slots in CTA order, forms the 14 values with the reference's denominators
 //                       and appends one table row at the index taken from the device counter
 //   val_finalize_kernel: one thread per meter replays sum += val * n, count += n (count from 1e-14) in row order
+//   train_states_append_kernel: appends a training step's fcn_det_loss result block as one row of the same table
 // No float atomics anywhere, so a batch gives the same bits on every run, stream and graph replay.
 #include "loss_terms.cuh"
 
@@ -139,6 +140,28 @@ __global__ void __launch_bounds__(VAL_THREADS) val_rows_kernel(const __grid_cons
     }
 }
 
+// One row [14 values, B, nfg, nkeep, 0] at row index state[0]++ (one thread).  The first row without a foreground row
+// is recorded (the reference asserts there); rows at or past `capacity` are counted, flagged and not written.
+__device__ __forceinline__ void append_row(const float *vals, int B, float nfg_raw, float nkeep_raw, float *table,
+                                           int capacity, int32_t *state) {
+    const int row = atomicAdd(&state[0], 1);
+    if (nfg_raw == 0.f && !(state[1] & FCN_VAL_NO_FG)) {
+        state[2] = row;
+        state[1] |= FCN_VAL_NO_FG;
+    }
+    if (row >= capacity) {
+        state[1] |= FCN_VAL_OVERFLOW;
+        return;
+    }
+    float *dst = table + (size_t)row * FCN_VAL_ROW;
+#pragma unroll
+    for (int i = 0; i < FCN_VAL_VALUES; ++i) dst[i] = vals[i];
+    dst[FCN_VAL_VALUES + 0] = (float)B;
+    dst[FCN_VAL_VALUES + 1] = nfg_raw;
+    dst[FCN_VAL_VALUES + 2] = nkeep_raw;
+    dst[FCN_VAL_VALUES + 3] = 0.f;
+}
+
 __global__ void val_final_kernel(const __grid_constant__ fcn_val_batch_args a, int nblk) {
     __shared__ float acc[VAL_SLOT];
     if (threadIdx.x < VAL_SLOT) {
@@ -170,22 +193,13 @@ __global__ void val_final_kernel(const __grid_constant__ fcn_val_batch_args a, i
     out[11] = a.with_iou ? __fdiv_rn(acc[A_IOU2], nfg) : nan;
     out[12] = a.with_iou ? __fdiv_rn(acc[A_IOU3], nfg) : nan;
     out[13] = a.with_iou ? __fdiv_rn(acc[A_IOUGT], nfg) : nan;
-    const int row = atomicAdd(&a.state[0], 1);
-    if (nfg_raw == 0.f && !(a.state[1] & FCN_VAL_NO_FG)) {
-        a.state[2] = row;                                          // the first batch the reference would reject
-        a.state[1] |= FCN_VAL_NO_FG;
-    }
-    if (row >= a.capacity) {
-        a.state[1] |= FCN_VAL_OVERFLOW;
-        return;
-    }
-    float *dst = a.table + (size_t)row * FCN_VAL_ROW;
-#pragma unroll
-    for (int i = 0; i < FCN_VAL_VALUES; ++i) dst[i] = out[i];
-    dst[FCN_VAL_VALUES + 0] = (float)a.B;
-    dst[FCN_VAL_VALUES + 1] = nfg_raw;
-    dst[FCN_VAL_VALUES + 2] = nkeep_raw;
-    dst[FCN_VAL_VALUES + 3] = 0.f;
+    append_row(out, a.B, nfg_raw, nkeep_raw, a.table, a.capacity, a.state);
+}
+
+// fcn_train_states_append: `loss` is fcn_det_loss's result block (14 values, nfg, nkeep), read as it stands
+__global__ void train_states_append_kernel(const float *__restrict__ loss, int B, float *__restrict__ table,
+                                           int capacity, int32_t *__restrict__ state) {
+    append_row(loss, B, loss[FCN_VAL_VALUES], loss[FCN_VAL_VALUES + 1], table, capacity, state);
 }
 
 // AverageMeter.update (utils/utils.py:62-66) in float64, every product and sum rounded on its own as Python does
@@ -238,6 +252,16 @@ extern "C" int fcn_val_batch(const fcn_val_batch_args *args, fcn_stream_t stream
     val_rows_kernel<<<nblk, VAL_THREADS, 0, st>>>(a);
     FCN_LAUNCH_CHECK();
     val_final_kernel<<<1, 32, 0, st>>>(a, nblk);
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
+}
+
+extern "C" int fcn_train_states_append(const float *loss, int B, float *table, int capacity, int32_t *state,
+                                       fcn_stream_t stream) {
+    FCN_REQUIRE(loss != nullptr && table != nullptr && state != nullptr, "NULL pointer");
+    FCN_REQUIRE(capacity >= 1, "capacity must be >= 1");
+    FCN_REQUIRE(B >= 1, "B must be >= 1");
+    train_states_append_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(loss, B, table, capacity, state);
     FCN_LAUNCH_CHECK();
     return FCN_OK;
 }

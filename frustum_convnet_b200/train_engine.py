@@ -374,18 +374,131 @@ class TrainEngine:
         return n_fwd + n_bwd + 1      # + fused Adam
 
 
+class FlatAdam(torch.optim.Adam):
+    """``torch.optim.Adam`` over a model's parameters (one param group, FlatParams order) whose state is the flat
+    bucket: each parameter's ``exp_avg`` / ``exp_avg_sq`` are views of two flat buffers and the step count is shared,
+    so `state_dict` / `load_state_dict` speak torch's own format (the reference's checkpoints,
+    train_net_det.py:345-361,384-398) while `step` is ONE ``fcn_adam_step`` launch over the whole bucket.  `step`
+    reads lr, betas, eps and weight_decay from ``param_groups[0]`` on every call, where lr schedulers and the
+    reference's MIN_LR clamp write.  The per-parameter ``state[p]["step"]`` tensors are brought up to date by
+    `state_dict`; ``step_count`` is the live value."""
+
+    def __init__(self, model, flat, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
+        super().__init__(list(model.parameters()), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
+        self.model, self.flat = model, flat
+        self.exp_avg = torch.zeros_like(flat.param)
+        self.exp_avg_sq = torch.zeros_like(flat.param)
+        self.step_count = 0
+        self.grad_scale = 1.0          # multiplies the gradient first: 1/world after a summing all-reduce
+        self._bind()
+        self.register_state_dict_pre_hook(FlatAdam._sync_steps)
+        self.register_load_state_dict_pre_hook(FlatAdam._check_loaded)
+        self.register_load_state_dict_post_hook(FlatAdam._adopt_loaded)
+
+    def _views(self):
+        for p in self.param_groups[0]["params"]:
+            off, n = self.flat.offsets[id(p)], p.numel()
+            yield p, self.exp_avg[off: off + n].view(p.shape), self.exp_avg_sq[off: off + n].view(p.shape)
+
+    def _bind(self):
+        for p, m, v in self._views():
+            self.state[p] = {"step": torch.tensor(float(self.step_count)), "exp_avg": m, "exp_avg_sq": v}
+
+    @staticmethod
+    def _check_group(g):
+        bad = [k for k in ("amsgrad", "maximize", "decoupled_weight_decay") if g.get(k)]
+        if bad:
+            raise ValueError("TrainStep.optimizer: %s is set; the fused step (fcn_adam_step) is plain Adam with L2 "
+                             "weight decay" % " / ".join(bad))
+
+    @staticmethod
+    def _sync_steps(opt):
+        for p in opt.param_groups[0]["params"]:
+            opt.state[p]["step"] = torch.tensor(float(opt.step_count))
+
+    @staticmethod
+    def _check_loaded(opt, state_dict):
+        groups = state_dict["param_groups"]
+        if len(groups) != 1:
+            raise ValueError("TrainStep.optimizer: the loaded state has %d parameter groups; the fused step takes "
+                             "exactly one (all parameters of the model)" % len(groups))
+        FlatAdam._check_group(groups[0])
+        ids, params = groups[0]["params"], opt.param_groups[0]["params"]
+        if len(ids) != len(params):
+            raise ValueError("TrainStep.optimizer: the loaded state has %d parameters, the model has %d"
+                             % (len(ids), len(params)))
+        steps = set()
+        for i, (k, p) in enumerate(zip(ids, params)):
+            st = state_dict["state"].get(k)
+            if not st:
+                steps.add(0.0)
+                continue
+            for key in ("exp_avg", "exp_avg_sq"):
+                if key not in st:
+                    raise ValueError("TrainStep.optimizer: parameter %d: the loaded state has no %s (not an Adam "
+                                     "state)" % (i, key))
+                if tuple(st[key].shape) != tuple(p.shape):
+                    raise ValueError("TrainStep.optimizer: parameter %d: loaded %s has shape %s, the parameter %s"
+                                     % (i, key, tuple(st[key].shape), tuple(p.shape)))
+            steps.add(float(st["step"]))
+        if len(steps) > 1:
+            raise ValueError("TrainStep.optimizer: the loaded per-parameter step counts differ (%s); the fused step "
+                             "keeps one count for all parameters" % sorted(steps))
+
+    @staticmethod
+    @torch.no_grad()
+    def _adopt_loaded(opt):
+        step = 0
+        for p, m, v in opt._views():
+            st = opt.state.get(p)
+            if st:
+                m.copy_(st["exp_avg"])
+                v.copy_(st["exp_avg_sq"])
+                step = int(float(st["step"]))
+            else:
+                m.zero_()
+                v.zero_()
+        opt.step_count = step
+        opt._bind()
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        """One Adam step of every parameter from the gradient in the flat bucket (``TrainStep.forward_backward``
+        leaves it there)."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        g = self.param_groups[0]
+        FlatAdam._check_group(g)
+        b1, b2 = g["betas"]
+        self.step_count += 1
+        self.model.refresh()       # parameters change behind autograd's version counters: eval pack must rebuild
+        f = self.flat
+        _lib.call("fcn_adam_step", _ptr(f.param), _ptr(f.grad), _ptr(self.exp_avg), _ptr(self.exp_avg_sq), f.numel,
+                  float(g["lr"]), float(b1), float(b2), float(g["eps"]), float(g["weight_decay"]), self.step_count,
+                  float(self.grad_scale), _stream())
+        return loss
+
+
 class TrainStep:
     """One optimizer step of PointNetDet on the hand-written kernels: forward -> losses (PyTorch ops on the logits)
     -> backward kernels -> ONE all-reduce of the flat gradient bucket (when torch.distributed is initialised and
-    world > 1) -> fused Adam.  Mirrors train/train_net_det.py:121-128 (zero_grad / backward / step)."""
+    world > 1) -> fused Adam.  Mirrors train/train_net_det.py:121-134 (zero_grad / backward / step and the
+    TrainingStates update).  ``optimizer`` is a torch.optim.Adam (FlatAdam) for lr schedulers and checkpoints;
+    ``states`` (validate.TrainStates) collects every step's losses and metrics on the device."""
 
-    def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, comm_stream=None):
+    def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, comm_stream=None,
+                 states_capacity=None):
+        from .validate import TrainStates
         self.model = model
-        self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
         self.engines: Dict[tuple, TrainEngine] = {}
-        self.step_count = 0
-        self.flat = None
-        self.m = self.v = None
+        self.flat = getattr(model, "_flat_params", None)
+        if self.flat is None:
+            self.flat = model._flat_params = FlatParams(model)
+        self.optimizer = FlatAdam(model, self.flat, lr, betas, eps, weight_decay)
+        self.m, self.v = self.optimizer.exp_avg, self.optimizer.exp_avg_sq
+        self.states = TrainStates(self.flat.param.device, states_capacity)
         self._comm = None
         self._split = 0
         self._loss_graphs = {}
@@ -393,15 +506,35 @@ class TrainStep:
         # CUDA graph (train_path.LossGraph), "eager" = the reference-shaped PyTorch ops
         self.loss_impl = "kernel"
 
+    @property
+    def lr(self):
+        return self.optimizer.param_groups[0]["lr"]
+
+    @lr.setter
+    def lr(self, value):
+        self.optimizer.param_groups[0]["lr"] = value
+
+    @property
+    def betas(self):
+        return self.optimizer.param_groups[0]["betas"]
+
+    @property
+    def eps(self):
+        return self.optimizer.param_groups[0]["eps"]
+
+    @property
+    def wd(self):
+        return self.optimizer.param_groups[0]["weight_decay"]
+
+    @property
+    def step_count(self):
+        return self.optimizer.step_count
+
     def engine(self, B, N, T) -> TrainEngine:
         key = (int(B), int(N), tuple(int(t) for t in T))
         e = self.engines.get(key)
         if e is None:
             e = self.engines[key] = TrainEngine(self.model, *key)
-            if self.flat is None:
-                self.flat = e.flat
-                self.m = torch.zeros_like(self.flat.param)
-                self.v = torch.zeros_like(self.flat.param)
         return e
 
     def _losses(self, eng, cls, reg, center_ref2, data):
@@ -450,6 +583,7 @@ class TrainStep:
         self.flat.grad.zero_()
         cls, reg = eng.forward(pc, centers, data.get("one_hot"))
         losses, metrics, dcls, dreg = self._losses(eng, cls, reg, centers[1], data)
+        self.states.append(self._state_block(eng, losses, metrics, data), eng.B)
         if world > 1:
             if self._comm is None:
                 self._comm = torch.cuda.Stream(device=self.flat.grad.device)
@@ -471,9 +605,16 @@ class TrainStep:
             cur.wait_stream(self._comm)
         else:
             eng.backward(dcls, dreg)
-        self.step_count += 1
-        self.model.refresh()       # parameters change behind autograd's version counters: eval pack must rebuild
-        _lib.call("fcn_adam_step", _ptr(self.flat.param), _ptr(self.flat.grad), _ptr(self.m), _ptr(self.v),
-                  self.flat.numel, float(self.lr), float(self.betas[0]), float(self.betas[1]), float(self.eps),
-                  float(self.wd), int(self.step_count), 1.0 / world, _stream())
+        self.optimizer.grad_scale = 1.0 / world
+        self.optimizer.step()
         return losses, metrics
+
+    def _state_block(self, eng, losses, metrics, data):
+        """The step's 16-float block for ``states``: fcn_det_loss's result as it stands, or the same layout stacked
+        on the device from the PyTorch losses (loss_impl "graph" / "eager")."""
+        if self.loss_impl == "kernel":
+            return self._loss_graphs[("kernel", eng.B, eng.T2)].out
+        vals = {**losses, **metrics}
+        lab = data["cls_label"]
+        return torch.stack([vals[k].detach().reshape(()).float() for k in self.states.keys] +
+                           [(lab == 1).sum().float(), (lab != -1).sum().float()])

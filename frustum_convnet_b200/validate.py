@@ -7,6 +7,8 @@ of every batch from the fused forward's head logits, averaged over the epoch wit
     states = val.finalize()                      # == TrainingStates.get_states(avg=True) of the reference loop
     val.reset()
 
+`TrainStates` keeps the reference train() loop's per-step TrainingStates the same way (``TrainStep.states``).
+
 `add` stages the batch into the forward plan of its (B, N, T) shape, replays the plan's forward graph and runs
 ``fcn_val_batch`` (csrc/validate.cu) on the plan's pitched head logits; the batch's 14 values are appended to a
 device table.  `finalize` replays the reference's float64 AverageMeter over that table (``fcn_val_finalize``) and
@@ -25,6 +27,17 @@ from .config import get_cfg
 
 LOSS_KEYS = ("total_loss", "cls_loss", "center_loss", "head_cls_loss", "head_res_loss", "size_cls_loss",
              "size_res_loss", "corners_loss")
+
+
+def state_keys():
+    """The 14 names of the reference's TrainingStates in its order (det_base.py:505-523), IoU_<cfg.IOU_THRESH> last."""
+    return LOSS_KEYS + ("cls_acc", "head_acc", "size_acc", "IoU_2D", "IoU_3D", "IoU_" + str(get_cfg().IOU_THRESH))
+
+
+def _replay_meters(table, capacity, state, result, stream):
+    """fcn_val_finalize over a (capacity, VAL_ROW) table on `stream`, then one host read -> ValResult."""
+    _lib.call("fcn_val_finalize", table.data_ptr(), capacity, state.data_ptr(), result.data_ptr(), stream.cuda_stream)
+    return _lib.ValResult.from_buffer_copy(result.cpu().numpy().tobytes())
 
 
 class _PlanLabels:
@@ -76,8 +89,8 @@ class Validator:
         if self.capacity < 1:
             raise ValueError("capacity must be >= 1")
         cfg = get_cfg()
-        self.iou_key = "IoU_" + str(cfg.IOU_THRESH)
-        self.keys = LOSS_KEYS + ("cls_acc", "head_acc", "size_acc", "IoU_2D", "IoU_3D", self.iou_key)
+        self.keys = state_keys()
+        self.iou_key = self.keys[-1]
         L = cfg.LOSS
         self._weights = (float(L.BOX_LOSS_WEIGHT), float(L.HEAD_REG_WEIGHT), float(L.SIZE_REG_WEIGHT),
                          float(L.CORNER_LOSS_WEIGHT), float(cfg.IOU_THRESH))
@@ -161,11 +174,7 @@ class Validator:
         ``TrainingStates.get_states(avg=True)``; one host read.  Raises if a batch had no foreground row or the
         table overflowed."""
         with torch.cuda.device(self.device):
-            cur = self._join()
-            _lib.call("fcn_val_finalize", self.table.data_ptr(), self.capacity, self.state.data_ptr(),
-                      self._result.data_ptr(), cur.cuda_stream)
-            raw = self._result.cpu().numpy().tobytes()
-        r = _lib.ValResult.from_buffer_copy(raw)
+            r = _replay_meters(self.table, self.capacity, self.state, self._result, self._join())
         self.last_result = r
         if r.status & _lib.VAL_NO_FG:
             raise RuntimeError("Validator: batch %d of the epoch has no foreground row (cls_label == 1); the reference "
@@ -190,3 +199,100 @@ class Validator:
             n = min(int(self.state[0].item()), self.capacity)
             t = self.table[:n].cpu().numpy()
         return np.ascontiguousarray(t if full else t[:, :_lib.VAL_VALUES])
+
+
+class TrainStates:
+    """The training loop's TrainingStates (train/train_net_det.py:131-134) on the device: every optimizer step of
+    ``TrainStep.step`` appends its 14 losses and metrics and its batch size to a device table
+    (``fcn_train_states_append``, no host sync), and the epoch's averages are the same float64 AverageMeter replay as
+    `Validator.finalize` (``fcn_val_finalize``).  Appends, `reset` and the reads are ordered on the current stream.
+
+        ts.states.reset()                          # start of an epoch
+        for i, data in enumerate(loader):
+            ts.step(data)
+            if (i + 1) % cfg.disp == 0:
+                print(ts.states.last())            # training_states.get_states(avg=False); one sync
+        epoch = ts.states.finalize()               # training_states.get_states(avg=True)
+
+    `capacity` = steps one epoch may add (default 4096)."""
+
+    def __init__(self, device, capacity=None):
+        self.device = torch.device(device)
+        self.capacity = int(capacity) if capacity is not None else 4096
+        if self.capacity < 1:
+            raise ValueError("capacity must be >= 1")
+        self.keys = state_keys()
+        self.table = torch.zeros((self.capacity, _lib.VAL_ROW), dtype=torch.float32, device=self.device)
+        self.state = torch.zeros(4, dtype=torch.int32, device=self.device)
+        self._result = torch.zeros(C.sizeof(_lib.ValResult), dtype=torch.uint8, device=self.device)
+        self.last_result = None
+
+    def reset(self):
+        """Start a new epoch (stream-ordered: the counter is zeroed on the current stream)."""
+        with torch.cuda.device(self.device):
+            self.state.zero_()
+
+    def append(self, block, B):
+        """One step: `block` holds 16 device floats laid out as fcn_det_loss's result (the 14 values, #foreground,
+        #non-ignored rows); B is the step's batch size."""
+        if not (block.is_cuda and block.dtype == torch.float32 and block.numel() == 16 and block.is_contiguous()):
+            raise ValueError("TrainStates.append: block must be 16 contiguous float32 values on the device")
+        _lib.call("fcn_train_states_append", block.data_ptr(), int(B), self.table.data_ptr(), self.capacity,
+                  self.state.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _check(self, status, first_no_fg, added):
+        if status & _lib.VAL_NO_FG:
+            raise RuntimeError("TrainStates: step %d of the epoch has no foreground row (cls_label == 1); the reference "
+                               "train() rejects it (assert fg_idx.numel() != 0)" % first_no_fg)
+        if status & _lib.VAL_OVERFLOW:
+            raise RuntimeError("TrainStates: %d steps were added but the capacity is %d; construct "
+                               "TrainStep(..., states_capacity=%d) or more" % (added, self.capacity, added))
+
+    def last(self):
+        """-> OrderedDict of the last step's 14 values (``get_states(avg=False)``); one host read, meant for every
+        `cfg.disp` steps rather than every step."""
+        with torch.cuda.device(self.device):
+            idx = (self.state[:1].long() - 1).clamp_(0, self.capacity - 1)
+            raw = torch.cat([self.table.index_select(0, idx).view(-1), self.state.view(torch.float32)]).cpu().numpy()
+        row, state = raw[:_lib.VAL_ROW], raw[_lib.VAL_ROW:].view(np.int32)
+        if state[0] == 0:
+            raise RuntimeError("TrainStates.last: no step since the last reset()")
+        self._check(int(state[1]), int(state[2]), int(state[0]))
+        return OrderedDict((k, float(row[i])) for i, k in enumerate(self.keys))
+
+    def per_step(self, full=False):
+        """(n, 14) float32 values of the steps added so far; full=True returns the whole rows (n, 18) with B, nfg and
+        nkeep in columns 14-16."""
+        with torch.cuda.device(self.device):
+            n = min(int(self.state[0].item()), self.capacity)
+            t = self.table[:n].cpu().numpy()
+        return np.ascontiguousarray(t if full else t[:, :_lib.VAL_VALUES])
+
+    def _over_ranks(self, world):
+        """The table as the reference's DataParallel loop logs it: each step's values averaged over the replicas,
+        B / nfg / nkeep summed (the full batch), and the status bits of every rank; one all_reduce of the table."""
+        import torch.distributed as dist
+        table = self.table.clone()
+        dist.all_reduce(table)
+        table[:, :_lib.VAL_VALUES] /= world
+        s = self.state
+        no_fg = (s[1] & _lib.VAL_NO_FG) != 0
+        flags = torch.stack([s[1] & _lib.VAL_NO_FG, s[1] & _lib.VAL_OVERFLOW,
+                             torch.where(no_fg, -s[2], torch.full_like(s[2], -(2 ** 31 - 1)))])
+        dist.all_reduce(flags, op=dist.ReduceOp.MAX)        # OR of the bits, earliest step without a foreground row
+        state = torch.stack([s[0], flags[0] | flags[1], -flags[2], s[3]])
+        return table, state
+
+    def finalize(self):
+        """-> OrderedDict of the 14 epoch averages (``get_states(avg=True)``); one host read.  With torch.distributed
+        initialised and world > 1 every rank must call it (ranks step in lockstep, so row i is the same step on every
+        rank).  Raises, naming the step, if a step had no foreground row, and if more steps were added than
+        `capacity`, naming the capacity needed."""
+        import torch.distributed as dist
+        world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        with torch.cuda.device(self.device):
+            table, state = self._over_ranks(world) if world > 1 else (self.table, self.state)
+            r = _replay_meters(table, self.capacity, state, self._result, torch.cuda.current_stream(self.device))
+        self.last_result = r
+        self._check(r.status, r.first_no_fg, r.added)
+        return OrderedDict((k, float(r.avg[i])) for i, k in enumerate(self.keys))

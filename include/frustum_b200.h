@@ -600,6 +600,12 @@ FCN_API int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stream_
  *
  *      fcn_val_finalize (once per epoch): one thread per value replays sum += (double)val * B, count += B with
  *      count starting at 1e-14, in row order, and writes avg = sum / count with the row count and status.
+ *
+ *      fcn_train_states_append (once per training step; no host sync, no allocation, capturable): one launch that
+ *      appends a training step's losses and metrics to a table of the same layout, so the epoch's averages come
+ *      from the same fcn_val_finalize.  `loss` is fcn_det_loss's `out` block (16 floats: the 14 values, #foreground,
+ *      #non-ignored rows), B the step's batch size; the row is [14 values, B, nfg, nkeep, 0] at state[0]++, with
+ *      state's status bits set as fcn_val_batch sets them.  capacity >= 1.
  * ------------------------------------------------------------------------------------------ */
 #define FCN_VAL_VALUES 14
 #define FCN_VAL_ROW 18
@@ -625,6 +631,8 @@ FCN_API long long fcn_val_partials_floats(int B, int T2);
 FCN_API int fcn_val_batch(const fcn_val_batch_args *args, fcn_stream_t stream);
 FCN_API int fcn_val_finalize(const float *table, int capacity, const int32_t *state, fcn_val_result *result,
                              fcn_stream_t stream);
+FCN_API int fcn_train_states_append(const float *loss, int B, float *table, int capacity, int32_t *state,
+                                    fcn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * (13) KITTI object evaluation on the device: the offline evaluator train/kitti_eval/evaluate_object_3d_offline.cpp
