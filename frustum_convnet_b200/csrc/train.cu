@@ -4,7 +4,7 @@
 //   conv (1x1 / k3 / strided / transposed) + BatchNorm with BATCH statistics + ReLU      models/common.py:38-63
 //   PointNetModule / PointNetFeat (mask, max over K)                                      models/det_base.py:62-159
 //   ConvFeatNet (concats, crops) and the two heads                                        models/det_base.py:163-224,367-368
-//   the optimizer step                                                                    train/train_net_det.py:121-128,322-323
+//   the optimizer step (Adam or SGD)                                                      train/train_net_det.py:121-128,321-328
 // Batch-statistics BN breaks the eval fusions (the statistics of layer l must be complete before layer l+1 can
 // normalise its input), so the train step is a sequence of table-driven kernels over dense position-major fp32
 // tensors [rows, channels]:
@@ -453,6 +453,25 @@ __global__ void train_adam_kernel(float *__restrict__ p, const float *__restrict
     p[i] -= (lr / bc1) * (mi / denom);
 }
 
+// ------------------------------------------------------------------ fused SGD over the flat parameter bucket
+// torch.optim.SGD (train_net_det.py:324-326) as torch/optim/sgd.py::_single_tensor_sgd does it, one rounding per torch
+// op: d = g + wd * p (skipped at wd == 0, as torch skips it); buf = d on the first step, else buf * momentum + d;
+// p += -lr * (buf or d).  torch's CUDA add(x, y, alpha) computes x + alpha * y as one FMA, so those two steps are
+// __fmaf_rn; every rounding is an explicit intrinsic so that -fmad cannot change the result.
+__global__ void train_sgd_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ buf, size_t n,
+                                 float lr, float momentum, float wd, int first, float gscale) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float pi = p[i];
+    float d = __fmul_rn(g[i], gscale);
+    if (wd != 0.f) d = __fmaf_rn(wd, pi, d);                             // grad.add(param, alpha=wd)
+    if (momentum != 0.f) {
+        if (!first) d = __fadd_rn(__fmul_rn(buf[i], momentum), d);       // buf.mul_(momentum).add_(d)
+        buf[i] = d;
+    }
+    p[i] = __fmaf_rn(-lr, d, pi);                                        // param.add_(d, alpha=-lr)
+}
+
 
 // =====================================================================================================
 // Fast path for the PointNet layers 2/3 (97 % of the step's FLOPs): single source, 1x1 conv, rows map 1:1
@@ -850,6 +869,19 @@ extern "C" int fcn_adam_step(float *param, const float *grad, float *exp_avg, fl
     const int threads = 256;
     train_adam_kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, (cudaStream_t)stream>>>(
         param, grad, exp_avg, exp_avg_sq, (size_t)n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, grad_scale);
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
+}
+
+extern "C" int fcn_sgd_step(float *param, const float *grad, float *momentum_buffer, long long n, float lr,
+                            float momentum, float weight_decay, int first, float grad_scale, fcn_stream_t stream) {
+    FCN_REQUIRE(param && grad, "NULL param / grad");
+    FCN_REQUIRE(momentum == 0.f || momentum_buffer, "NULL momentum_buffer with momentum != 0");
+    FCN_REQUIRE(n >= 0, "n < 0");
+    if (n == 0) return FCN_OK;
+    const int threads = 256;
+    train_sgd_kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, (cudaStream_t)stream>>>(
+        param, grad, momentum_buffer, (size_t)n, lr, momentum, weight_decay, first, grad_scale);
     FCN_LAUNCH_CHECK();
     return FCN_OK;
 }

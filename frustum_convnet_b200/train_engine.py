@@ -10,7 +10,7 @@ tensors, executed by csrc/train.cu:
 The losses stay PyTorch ops on the (B*T2, 2+39) logits (SURVEY.md 8-a6; ~320 rows); their autograd gives dlogits,
 from which ``backward`` runs the hand-written backward kernels.  Parameters live in ONE flat fp32 buffer (every
 ``nn.Parameter`` is a view), gradients in ONE flat bucket written in the parameter layout by the kernels:
-one ``all_reduce`` per step (SURVEY.md 8(e)) and one fused Adam launch (``fcn_adam_step``).
+one ``all_reduce`` per step (SURVEY.md 8(e)) and one fused optimizer launch (``fcn_adam_step`` or ``fcn_sgd_step``).
 BatchNorm statistics are per rank (the reference's DataParallel semantics: per-replica BN, no SyncBN).
 """
 from __future__ import annotations
@@ -371,7 +371,21 @@ class TrainEngine:
     def kernel_launches_per_step(self):
         n_fwd = len(self.layers) + len(self.pools) + 2
         n_bwd = sum(1 + L.n_seg + bin(m).count("1") for L, m in zip(self.layers, self.dx_mask)) + len(self.pools) + 1
-        return n_fwd + n_bwd + 1      # + fused Adam
+        return n_fwd + n_bwd + 1      # + fused Adam or SGD
+
+
+def _one_group(opt, state_dict):
+    """-> (group, parameter ids, opt's parameters) of a loaded optimizer state that has the one parameter group over
+    all of the model's parameters that a fused step over the flat bucket takes; ValueError otherwise."""
+    groups = state_dict["param_groups"]
+    if len(groups) != 1:
+        raise ValueError("TrainStep.optimizer: the loaded state has %d parameter groups; the fused step takes "
+                         "exactly one (all parameters of the model)" % len(groups))
+    ids, params = groups[0]["params"], opt.param_groups[0]["params"]
+    if len(ids) != len(params):
+        raise ValueError("TrainStep.optimizer: the loaded state has %d parameters, the model has %d"
+                         % (len(ids), len(params)))
+    return groups[0], ids, params
 
 
 class FlatAdam(torch.optim.Adam):
@@ -418,15 +432,8 @@ class FlatAdam(torch.optim.Adam):
 
     @staticmethod
     def _check_loaded(opt, state_dict):
-        groups = state_dict["param_groups"]
-        if len(groups) != 1:
-            raise ValueError("TrainStep.optimizer: the loaded state has %d parameter groups; the fused step takes "
-                             "exactly one (all parameters of the model)" % len(groups))
-        FlatAdam._check_group(groups[0])
-        ids, params = groups[0]["params"], opt.param_groups[0]["params"]
-        if len(ids) != len(params):
-            raise ValueError("TrainStep.optimizer: the loaded state has %d parameters, the model has %d"
-                             % (len(ids), len(params)))
+        group, ids, params = _one_group(opt, state_dict)
+        FlatAdam._check_group(group)
         steps = set()
         for i, (k, p) in enumerate(zip(ids, params)):
             st = state_dict["state"].get(k)
@@ -481,23 +488,129 @@ class FlatAdam(torch.optim.Adam):
         return loss
 
 
+class FlatSGD(torch.optim.SGD):
+    """``torch.optim.SGD`` over a model's parameters (one param group, FlatParams order) whose state is the flat
+    bucket: each parameter's ``momentum_buffer`` is a view of one flat buffer, so `state_dict` / `load_state_dict`
+    speak torch's own format while `step` is ONE ``fcn_sgd_step`` launch over the whole bucket.  `step` reads lr,
+    momentum and weight_decay from ``param_groups[0]`` on every call.  torch creates a parameter's buffer on its first
+    step with momentum; the fused step keeps one flag for the bucket (``has_buffers``), so the state is empty before
+    that step and holds every parameter's buffer after it, as torch's does.  nesterov, dampening and maximize are
+    rejected (the reference uses none of them).  ``step_count`` counts the steps this object took; torch's SGD state
+    has no step count to restore it from."""
+
+    def __init__(self, model, flat, lr=1e-3, momentum=0.0, weight_decay=0.0):
+        super().__init__(list(model.parameters()), lr=lr, momentum=momentum, weight_decay=weight_decay)
+        self.model, self.flat = model, flat
+        self.momentum_buffer = torch.zeros_like(flat.param)
+        self.has_buffers = False
+        self.step_count = 0
+        self.grad_scale = 1.0          # multiplies the gradient first: 1/world after a summing all-reduce
+        self.register_load_state_dict_pre_hook(FlatSGD._check_loaded)
+        self.register_load_state_dict_post_hook(FlatSGD._adopt_loaded)
+
+    def _views(self):
+        for p in self.param_groups[0]["params"]:
+            off, n = self.flat.offsets[id(p)], p.numel()
+            yield p, self.momentum_buffer[off: off + n].view(p.shape)
+
+    def _bind(self):
+        self.state.clear()
+        if self.has_buffers:
+            for p, b in self._views():
+                self.state[p] = {"momentum_buffer": b}
+
+    @staticmethod
+    def _check_group(g):
+        if "momentum" not in g:
+            raise ValueError("TrainStep.optimizer: the parameter group has no momentum (not an SGD state)")
+        bad = [k for k in ("nesterov", "maximize") if g.get(k)] + (["dampening"] if g.get("dampening", 0) else [])
+        if bad:
+            raise ValueError("TrainStep.optimizer: %s is set; the fused step (fcn_sgd_step) is plain SGD with momentum "
+                             "and L2 weight decay" % " / ".join(bad))
+
+    @staticmethod
+    def _check_loaded(opt, state_dict):
+        group, ids, params = _one_group(opt, state_dict)
+        FlatSGD._check_group(group)
+        with_buffer = 0
+        for i, (k, p) in enumerate(zip(ids, params)):
+            st = state_dict["state"].get(k) or {}
+            other = sorted(set(st) - {"momentum_buffer"})
+            if other:
+                raise ValueError("TrainStep.optimizer: parameter %d: the loaded state has %s (not an SGD state)"
+                                 % (i, " / ".join(other)))
+            buf = st.get("momentum_buffer")      # torch < 2 wrote None when momentum was 0
+            if buf is None:
+                continue
+            if tuple(buf.shape) != tuple(p.shape):
+                raise ValueError("TrainStep.optimizer: parameter %d: loaded momentum_buffer has shape %s, the "
+                                 "parameter %s" % (i, tuple(buf.shape), tuple(p.shape)))
+            with_buffer += 1
+        if 0 < with_buffer < len(params):
+            raise ValueError("TrainStep.optimizer: the loaded state has momentum buffers on %d of %d parameters; the "
+                             "fused step keeps buffers for all parameters or none" % (with_buffer, len(params)))
+
+    @staticmethod
+    @torch.no_grad()
+    def _adopt_loaded(opt):
+        loaded = [opt.state.get(p, {}).get("momentum_buffer") for p in opt.param_groups[0]["params"]]
+        opt.has_buffers = loaded[0] is not None        # _check_loaded admits buffers on all parameters or on none
+        if opt.has_buffers:
+            # each source onto its own view: a source may BE that view (torch keeps a loaded tensor that already has
+            # the parameter's dtype and device, as in opt.load_state_dict(opt.state_dict())), so nothing is zeroed first
+            for (p, b), src in zip(opt._views(), loaded):
+                b.copy_(src)
+        else:
+            opt.momentum_buffer.zero_()
+        opt._bind()
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        """One SGD step of every parameter from the gradient in the flat bucket (``TrainStep.forward_backward``
+        leaves it there)."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        g = self.param_groups[0]
+        FlatSGD._check_group(g)
+        momentum = float(g["momentum"])
+        first = not self.has_buffers
+        self.model.refresh()       # parameters change behind autograd's version counters: eval pack must rebuild
+        f = self.flat
+        _lib.call("fcn_sgd_step", _ptr(f.param), _ptr(f.grad), _ptr(self.momentum_buffer), f.numel, float(g["lr"]),
+                  momentum, float(g["weight_decay"]), int(first), float(self.grad_scale), _stream())
+        self.step_count += 1
+        if momentum != 0 and first:
+            self.has_buffers = True
+            self._bind()
+        return loss
+
+
 class TrainStep:
     """One optimizer step of PointNetDet on the hand-written kernels: forward -> losses (PyTorch ops on the logits)
     -> backward kernels -> ONE all-reduce of the flat gradient bucket (when torch.distributed is initialised and
-    world > 1) -> fused Adam.  Mirrors train/train_net_det.py:121-134 (zero_grad / backward / step and the
-    TrainingStates update).  ``optimizer`` is a torch.optim.Adam (FlatAdam) for lr schedulers and checkpoints;
-    ``states`` (validate.TrainStates) collects every step's losses and metrics on the device."""
+    world > 1) -> fused Adam or SGD.  Mirrors train/train_net_det.py:121-134 (zero_grad / backward / step and the
+    TrainingStates update).  ``optimizer`` ("adam" or "sgd", the values of cfg.TRAIN.OPTIMIZER,
+    train_net_det.py:321-328) selects a torch.optim.Adam (FlatAdam) or torch.optim.SGD (FlatSGD, with ``momentum``)
+    for lr schedulers and checkpoints; ``states`` (validate.TrainStates) collects every step's losses and metrics on
+    the device."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, comm_stream=None,
-                 states_capacity=None):
+                 states_capacity=None, optimizer="adam", momentum=0.0):
         from .validate import TrainStates
+        if optimizer not in ("adam", "sgd"):
+            raise ValueError("TrainStep: optimizer %r is not supported; the fused steps are 'adam' and 'sgd'"
+                             % (optimizer,))
         self.model = model
         self.engines: Dict[tuple, TrainEngine] = {}
         self.flat = getattr(model, "_flat_params", None)
         if self.flat is None:
             self.flat = model._flat_params = FlatParams(model)
-        self.optimizer = FlatAdam(model, self.flat, lr, betas, eps, weight_decay)
-        self.m, self.v = self.optimizer.exp_avg, self.optimizer.exp_avg_sq
+        if optimizer == "adam":
+            self.optimizer = FlatAdam(model, self.flat, lr, betas, eps, weight_decay)
+        else:
+            self.optimizer = FlatSGD(model, self.flat, lr, momentum, weight_decay)
         self.states = TrainStates(self.flat.param.device, states_capacity)
         self._comm = None
         self._split = 0
@@ -514,13 +627,26 @@ class TrainStep:
     def lr(self, value):
         self.optimizer.param_groups[0]["lr"] = value
 
+    def _adam(self, name):
+        if not isinstance(self.optimizer, FlatAdam):
+            raise AttributeError("TrainStep.%s exists for Adam only; this TrainStep steps with SGD" % name)
+        return self.optimizer
+
+    @property
+    def m(self):
+        return self._adam("m").exp_avg
+
+    @property
+    def v(self):
+        return self._adam("v").exp_avg_sq
+
     @property
     def betas(self):
-        return self.optimizer.param_groups[0]["betas"]
+        return self._adam("betas").param_groups[0]["betas"]
 
     @property
     def eps(self):
-        return self.optimizer.param_groups[0]["eps"]
+        return self._adam("eps").param_groups[0]["eps"]
 
     @property
     def wd(self):
@@ -569,7 +695,7 @@ class TrainStep:
         return losses, metrics
 
     def step(self, data):
-        """forward + losses + backward + gradient all-reduce + Adam.  With world > 1 the flat bucket is reduced in
+        """forward + losses + backward + gradient all-reduce + Adam or SGD.  With world > 1 the flat bucket is reduced in
         TWO pieces on a communication stream: the FCN + heads part (92 % of the parameters, complete after the
         first ~15 % of the backward) overlaps the PointNet backward; the PointNet part follows."""
         import torch.distributed as dist

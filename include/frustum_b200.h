@@ -336,6 +336,15 @@ FCN_API int fcn_train_finalize(const fcn_train_layer *layers_dev, int n_layers, 
 FCN_API int fcn_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, long long n, float lr,
                           float beta1, float beta2, float eps, float weight_decay, int step, float grad_scale,
                           fcn_stream_t stream);
+/* fused SGD over one flat bucket (torch.optim.SGD with momentum and L2 weight decay; no nesterov, dampening or
+ * maximize), the operations and roundings of torch's single-tensor step: d = g*grad_scale (+ wd*p when wd != 0);
+ * with momentum != 0, momentum_buffer = d when `first` (torch's first step with momentum), else
+ * momentum_buffer*momentum + d, and d = momentum_buffer; then p += (-lr)*d.  The two "+ alpha*y" steps are single
+ * FMAs, as torch's CUDA add(x, y, alpha=) computes them.  grad_scale multiplies the gradient first (1/world after a
+ * sum all-reduce; exactly 1 on one rank).  n == 0 is a no-op.  momentum_buffer may be NULL when
+ * momentum == 0 (then it is neither read nor written). */
+FCN_API int fcn_sgd_step(float *param, const float *grad, float *momentum_buffer, long long n, float lr,
+                         float momentum, float weight_decay, int first, float grad_scale, fcn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * (7b) Fused detection losses + gradient w.r.t. the head logits (row 8(f)-2, train half): everything of
