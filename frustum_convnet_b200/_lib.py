@@ -347,6 +347,9 @@ SIGNATURES = {
     "fcn_train_forward": (_I, [C.POINTER(TrainLayer), _P, C.c_longlong, _P]),
     "fcn_train_workspace_floats": (C.c_longlong, [C.POINTER(TrainLayer)]),
     "fcn_train_backward": (_I, [C.POINTER(TrainLayer), _I, _P]),
+    "fcn_train_deterministic_workspace_floats": (C.c_longlong, [C.POINTER(TrainLayer)]),
+    "fcn_train_forward_deterministic": (_I, [C.POINTER(TrainLayer), _P, C.c_longlong, _P]),
+    "fcn_train_backward_deterministic": (_I, [C.POINTER(TrainLayer), _I, _P, C.c_longlong, _P]),
     "fcn_train_pool": (_I, [C.POINTER(TrainPool), _I, _P]),
     "fcn_train_finalize": (_I, [_P, _I, _I, _P]),
     "fcn_adam_step": (_I, [_P, _P, _P, _P, C.c_longlong, _F, _F, _F, _F, _F, _I, _F, _P]),
@@ -354,6 +357,8 @@ SIGNATURES = {
     "fcn_rotate_nms_3d": (_I, [_I, _P, _P, _F, _I, _P, _P, _I, _P]),
     "fcn_rotate_nms_3d_max_dets": (_I, []),
     "fcn_det_loss": (_I, [C.POINTER(LossArgs), _P]),
+    "fcn_det_loss_deterministic_scratch_floats": (C.c_longlong, [C.c_longlong]),
+    "fcn_det_loss_deterministic": (_I, [C.POINTER(LossArgs), _P]),
     "fcn_build_inputs": (_I, [C.POINTER(InputArgs), _P]),
     "fcn_ipc_export": (_I, [_P, _P, C.POINTER(C.c_longlong)]),
     "fcn_ipc_open": (_I, [_P, C.POINTER(C.c_void_p)]),

@@ -20,6 +20,8 @@
 //   * weights and gradients are addressed IN THE PARAMETER LAYOUT (Conv1d (Co,Ci,k), ConvTranspose1d (Ci,Co,k),
 //     Conv2d (Co,Ci,1,1)) through strides, so gradients land directly in one flat bucket (one all-reduce);
 //   * fp32 FMA arithmetic (parity with the fp32 reference fixture: losses 2e-4, gradients 2e-3).
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace fcn {
@@ -149,6 +151,8 @@ train_fwd_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ 
     const int M = L.B * L.T_out;
     const int q_lo = blockIdx.z * tiles_per_slice, q_hi = q_lo + tiles_per_slice;
     float acc[4][4] = {};
+    // this K loop and the partial-sum store below are repeated in fwd_k_tiles / fwd_store_partial (deterministic
+    // forward): change them together
     int q0 = 0;                                              // first linear K tile of the current segment
     for (int sg = 0; sg < L.n_seg; ++sg) {
         const fcn_train_seg &g = L.seg[sg];
@@ -236,15 +240,128 @@ train_fwd_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ 
     }
 }
 
-// Y = sum over K slices (fixed order) + bias; batch statistics.  Block = 32 columns x 8 row lanes.
-__global__ void __launch_bounds__(256)
-train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *__restrict__ partial, int nslice,
-                        int rows_per_block) {
-    const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
-    const int n = blockIdx.x * 32 + nl;
+// Deterministic forward, generic layers: the CTA's 64 x 64 output tile over the linear K tiles [q_lo, q_hi) of all
+// segments.  This is train_fwd_kernel's K loop and partial-sum store, and the two copies must stay in step:
+// train_fwd_kernel keeps its own, because calling these helpers there changes its register allocation (the default
+// path's code stays as it was).
+__device__ __forceinline__ void fwd_k_tiles(const fcn_train_layer &L, int tid, int tx, int ty, int M, int r0, int n0,
+                                            int q_lo, int q_hi, float (&acc)[4][4], float (&As)[TG_BK][TG_BM + 4],
+                                            float (&Bs)[TG_BK][TG_BN + 4], float (&s_scale)[TG_BK],
+                                            float (&s_shift)[TG_BK]) {
+    int q0 = 0;                                              // first linear K tile of the current segment
+    for (int sg = 0; sg < L.n_seg; ++sg) {
+        const fcn_train_seg &g = L.seg[sg];
+        const fcn_train_src &s = g.src;
+        const double inv = s.sums != nullptr ? 1.0 / s.count : 0.0;
+        const int nt = (g.C + TG_BK - 1) / TG_BK;
+        const int t_lo = max(q_lo - q0, 0), t_hi = min(q_hi - q0, nt);
+        q0 += nt;
+        for (int t = t_lo; t < t_hi; ++t) {
+            const int k0 = t * TG_BK;
+            __syncthreads();
+            if (tid < TG_BK) {          // src_coef, with the inverse count hoisted out of the tile loop
+                const int c = k0 + tid;
+                float sc = 1.f, sh = 0.f;
+                if (s.sums != nullptr && c < g.C) {
+                    const BnCoef b = bn_coef(s.sums, s.gamma, s.beta, s.Cstat, (s.coff + c) % s.Cstat, inv);
+                    sc = b.scale; sh = b.shift;
+                }
+                s_scale[tid] = sc; s_shift[tid] = sh;
+            }
+            __syncthreads();
+            // A tile: 64 rows x 16 channels (consecutive threads -> consecutive channels)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int rr = ty + 16 * i, r = r0 + rr, c = k0 + tx;
+                float v = 0.f;
+                if (r < M && c < g.C) {
+                    const int b = r / L.T_out, tt = r - b * L.T_out;
+                    v = src_act(s, b, tt * g.stride + g.tap, c, s_scale[tx], s_shift[tx]);
+                }
+                As[tx][rr] = v;
+            }
+            // B tile: 16 channels x 64 columns
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int kk = tid / 64 + 4 * i, nn = tid % 64, c = k0 + kk, n = n0 + nn;
+                Bs[kk][nn] = (c < g.C && n < L.N) ? L.W[w_index(L, g, c, n)] : 0.f;
+            }
+            __syncthreads();
+            tile_fma_4x4(acc, As, Bs, tx, ty);
+        }
+    }
+}
+
+// the tile's partial sums of K slice blockIdx.z: partial[z][M][N]
+__device__ __forceinline__ void fwd_store_partial(const fcn_train_layer &L, int M, int r0, int n0, float *partial,
+                                                  const float (&acc)[4][4]) {
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    float *dst = partial + (size_t)blockIdx.z * M * L.N;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int r = r0 + ty * 4 + i;
+        if (r >= M) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int n = n0 + tx * 4 + j;
+            if (n < L.N) dst[(size_t)r * L.N + n] = acc[i][j];
+        }
+    }
+}
+
+// Deterministic forward (fcn_train_forward_deterministic): gridDim.z > 1 stores the K slices' partial sums as
+// train_fwd_kernel does; gridDim.z == 1 stores Y (+bias) and, for a BN layer, this CTA's column sums Sum(y), Sum(y^2)
+// over its 64 rows (16 row groups added in group order) to slot blockIdx.x of `slots` [row block][2N], plain stores.
+__global__ void __launch_bounds__(TG_THREADS)
+train_fwd_det_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ partial, int tiles_per_slice,
+                     float *__restrict__ slots) {
+    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];
+    __shared__ float s_scale[TG_BK], s_shift[TG_BK];
+    __shared__ float s_ps[16][TG_BN + 1], s_pq[16][TG_BN + 1];
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int r0 = blockIdx.x * TG_BM, n0 = blockIdx.y * TG_BN;
     const int M = L.B * L.T_out;
-    const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
-    float a1 = 0.f, a2 = 0.f;
+    const int q_lo = blockIdx.z * tiles_per_slice, q_hi = q_lo + tiles_per_slice;
+    float acc[4][4] = {};
+    fwd_k_tiles(L, tid, tx, ty, M, r0, n0, q_lo, q_hi, acc, As, Bs, s_scale, s_shift);
+    if (gridDim.z > 1) {
+        fwd_store_partial(L, M, r0, n0, partial, acc);
+        return;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int n = n0 + tx * 4 + j;
+        float ps = 0.f, pq = 0.f;
+        if (n < L.N) {
+            const float bias = L.bias != nullptr ? L.bias[n] : 0.f;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int r = r0 + ty * 4 + i;
+                if (r < M) {
+                    const float y = acc[i][j] + bias;
+                    L.Y[(size_t)r * L.N + n] = y;
+                    ps += y; pq += y * y;
+                }
+            }
+        }
+        s_ps[ty][tx * 4 + j] = ps; s_pq[ty][tx * 4 + j] = pq;
+    }
+    if (!L.has_bn) return;
+    __syncthreads();
+    if (tid < TG_BN && n0 + tid < L.N) {
+        float a1 = 0.f, a2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) { a1 += s_ps[i][tid]; a2 += s_pq[i][tid]; }
+        float *slot = slots + (size_t)blockIdx.x * 2 * L.N;
+        slot[n0 + tid] = a1;
+        slot[L.N + n0 + tid] = a2;
+    }
+}
+
+// Y = sum over K slices (fixed order) + bias for column n, rows rb + rl, rb + rl + 8, ... < re; a1, a2 = Sum(y), Sum(y^2)
+// over those rows
+__device__ __forceinline__ void fwd_finish_rows(const fcn_train_layer &L, int M, const float *partial, int nslice,
+                                                int n, int rl, int rb, int re, float &a1, float &a2) {
     if (n < L.N) {
         const float bias = L.bias != nullptr ? L.bias[n] : 0.f;
         for (int r = rb + rl; r < re; r += 8) {
@@ -254,6 +371,18 @@ train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *
             a1 += y; a2 += y * y;
         }
     }
+}
+
+// Y = sum over K slices (fixed order) + bias; batch statistics.  Block = 32 columns x 8 row lanes.
+__global__ void __launch_bounds__(256)
+train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *__restrict__ partial, int nslice,
+                        int rows_per_block) {
+    const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
+    const int n = blockIdx.x * 32 + nl;
+    const int M = L.B * L.T_out;
+    const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
+    float a1 = 0.f, a2 = 0.f;
+    fwd_finish_rows(L, M, partial, nslice, n, rl, rb, re, a1, a2);
     if (!L.has_bn) return;
     if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
         const int co = n % L.Cout;
@@ -262,15 +391,57 @@ train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *
     }
 }
 
-// ------------------------------------------------------------------ backward: column reduction Sum(dz), Sum(dz*xh)
+// train_fwd_finish_kernel of the deterministic forward: the statistics of row block blockIdx.y go to its slot
+// [row block][2N] (plain stores)
 __global__ void __launch_bounds__(256)
-train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block) {
-    // block = 32 columns x 8 row lanes
+train_fwd_finish_det_kernel(const __grid_constant__ fcn_train_layer L, const float *__restrict__ partial, int nslice,
+                            int rows_per_block, float *__restrict__ slots) {
     const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
     const int n = blockIdx.x * 32 + nl;
     const int M = L.B * L.T_out;
     const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
     float a1 = 0.f, a2 = 0.f;
+    fwd_finish_rows(L, M, partial, nslice, n, rl, rb, re, a1, a2);
+    if (!L.has_bn) return;
+    if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
+        float *slot = slots + (size_t)blockIdx.y * 2 * L.N;
+        slot[n] = a1;
+        slot[L.N + n] = a2;
+    }
+}
+
+// Adds the slots [nrb][halves * N] of a deterministic column reduction into dst (fp64, accumulating):
+//   dst[h*C + c] += sum over row blocks rb and column groups j of slots[rb][h*N + j*C + c]     (h < halves)
+// (C = Cout: the up > 1 columns n = j*Cout + co of a transposed conv share channel co).  Block = 32 outputs x 8
+// lanes; lane l adds the row blocks l, l + 8, ... in order, then the lanes are added in lane order: a fixed order.
+__global__ void __launch_bounds__(256)
+train_slots_sum_kernel(double *__restrict__ dst, const float *__restrict__ slots, int nrb, int N, int C, int halves) {
+    __shared__ double s[8][33];
+    const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
+    const int o = blockIdx.x * 32 + nl;
+    double a = 0.0;
+    if (o < halves * C) {
+        const int h = o / C, c = o - h * C;
+        const float *col = slots + (size_t)h * N + c;
+        for (int rb = rl; rb < nrb; rb += 8) {
+            const float *row = col + (size_t)rb * halves * N;
+            for (int j = 0; j < N; j += C) a += (double)row[j];
+        }
+    }
+    s[rl][nl] = a;
+    __syncthreads();
+    if (rl == 0 && o < halves * C) {
+        double t = 0.0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) t += s[i][nl];
+        dst[o] += t;
+    }
+}
+
+// ------------------------------------------------------------------ backward: column reduction Sum(dz), Sum(dz*xh)
+// column n's sums over rows rb + rl, rb + rl + 8, ... < re
+__device__ __forceinline__ void reduce_rows(const fcn_train_layer &L, int M, int n, int rl, int rb, int re,
+                                            float &a1, float &a2) {
     if (n < L.N) {
         BnCoef b = {1.f, 0.f, 0.f, 1.f};
         if (L.has_bn) b = bn_coef(L.sums, L.gamma, L.beta, L.Cout, n % L.Cout, 1.0 / ((double)M * L.up));
@@ -283,6 +454,17 @@ train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bloc
             a2 += dz * ((y - b.mean) * b.invstd);
         }
     }
+}
+
+__global__ void __launch_bounds__(256)
+train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block) {
+    // block = 32 columns x 8 row lanes
+    const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
+    const int n = blockIdx.x * 32 + nl;
+    const int M = L.B * L.T_out;
+    const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
+    float a1 = 0.f, a2 = 0.f;
+    reduce_rows(L, M, n, rl, rb, re, a1, a2);
     if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
         const int co = L.has_bn ? n % L.Cout : n;
         const int C = L.has_bn ? L.Cout : L.N;
@@ -291,24 +473,37 @@ train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bloc
     }
 }
 
+// train_reduce_kernel of the deterministic backward: row block blockIdx.y's sums go to its slot [row block][h*N]
+// (h = 2 with BN: Sum(dz), Sum(dz*xh); h = 1 without: Sum(dA)), plain stores
+__global__ void __launch_bounds__(256)
+train_reduce_det_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block, float *__restrict__ slots) {
+    const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
+    const int n = blockIdx.x * 32 + nl;
+    const int M = L.B * L.T_out;
+    const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
+    float a1 = 0.f, a2 = 0.f;
+    reduce_rows(L, M, n, rl, rb, re, a1, a2);
+    if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
+        float *slot = slots + (size_t)blockIdx.y * (L.has_bn ? 2 : 1) * L.N;
+        slot[n] = a1;
+        if (L.has_bn) slot[L.N + n] = a2;
+    }
+}
+
 // ------------------------------------------------------------------ backward: dW += act(X)^T * dY
-__global__ void __launch_bounds__(TG_THREADS)
-train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows_per_block) {
-    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[row][k-channel], Bs[row][n]
-    __shared__ float s_scale[TG_BM], s_shift[TG_BM];
-    __shared__ DyCoef s_dy[TG_BN];
-    const fcn_train_seg &g = L.seg[seg_idx];
+// the CTA's 64 channels x 64 columns tile of act(X)^T * dY over rows [rb, re) of segment g
+__device__ __forceinline__ void dw_tile(const fcn_train_layer &L, const fcn_train_seg &g, int rb, int re,
+                                        float (&acc)[4][4], float (&As)[TG_BK][TG_BM + 4],
+                                        float (&Bs)[TG_BK][TG_BN + 4], float (&s_scale)[TG_BM],
+                                        float (&s_shift)[TG_BM], DyCoef (&s_dy)[TG_BN]) {
     const fcn_train_src &s = g.src;
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
     const int c0 = blockIdx.x * TG_BM, n0 = blockIdx.y * TG_BN;
-    const int M = L.B * L.T_out;
-    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
     if (tid < TG_BM) {
         const float2 k = src_coef(s, c0 + tid, c0 + tid < g.C);
         s_scale[tid] = k.x; s_shift[tid] = k.y;
     }
     if (tid < TG_BN) s_dy[tid] = dy_coef(L, min(n0 + tid, L.N - 1));
-    float acc[4][4] = {};
     for (int rr0 = rb; rr0 < re; rr0 += TG_BK) {
         __syncthreads();
         // A tile: 16 rows x 64 channels of this segment
@@ -331,6 +526,20 @@ train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows
         __syncthreads();
         tile_fma_4x4(acc, As, Bs, tx, ty);
     }
+}
+
+__global__ void __launch_bounds__(TG_THREADS)
+train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows_per_block) {
+    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[row][k-channel], Bs[row][n]
+    __shared__ float s_scale[TG_BM], s_shift[TG_BM];
+    __shared__ DyCoef s_dy[TG_BN];
+    const fcn_train_seg &g = L.seg[seg_idx];
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int c0 = blockIdx.x * TG_BM, n0 = blockIdx.y * TG_BN;
+    const int M = L.B * L.T_out;
+    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
+    float acc[4][4] = {};
+    dw_tile(L, g, rb, re, acc, As, Bs, s_scale, s_shift, s_dy);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int c = c0 + ty * 4 + i;
@@ -343,18 +552,55 @@ train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows
     }
 }
 
-// ------------------------------------------------------------------ backward: dX(seg) += dY * W^T
+// train_dw_kernel of the deterministic backward: row slice blockIdx.z's tile goes to part[z][C][N] (plain stores);
+// train_dw_sum_kernel adds the slices
 __global__ void __launch_bounds__(TG_THREADS)
-train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_per_slice) {
-    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[n][row], Bs[n][channel]
-    __shared__ DyCoef s_dy[TG_BK];
+train_dw_det_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows_per_block,
+                    float *__restrict__ part) {
+    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];
+    __shared__ float s_scale[TG_BM], s_shift[TG_BM];
+    __shared__ DyCoef s_dy[TG_BN];
     const fcn_train_seg &g = L.seg[seg_idx];
-    const fcn_train_src &s = g.src;
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int r0 = blockIdx.x * TG_BM, c0 = blockIdx.y * TG_BN;
+    const int c0 = blockIdx.x * TG_BM, n0 = blockIdx.y * TG_BN;
     const int M = L.B * L.T_out;
+    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
     float acc[4][4] = {};
-    const int n_lo = blockIdx.z * n_per_slice, n_hi = min(L.N, n_lo + n_per_slice);
+    dw_tile(L, g, rb, re, acc, As, Bs, s_scale, s_shift, s_dy);
+    float *dst = part + (size_t)blockIdx.z * g.C * L.N;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int c = c0 + ty * 4 + i;
+        if (c >= g.C) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int n = n0 + tx * 4 + j;
+            if (n < L.N) dst[(size_t)c * L.N + n] = acc[i][j];
+        }
+    }
+}
+
+// dW (parameter layout) += the sum over the nz row slices, in slice order, of the partial tiles in `part`:
+// [z][C][N] (generic kernel) or [z][N][C] (plain kernel, cn_layout = 0).  One read-add-store per weight: w_index is
+// injective within a segment and the segments of a layer run one after another.
+__global__ void train_dw_sum_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, const float *__restrict__ part,
+                                    int nz, int cn_layout) {
+    const fcn_train_seg &g = L.seg[seg_idx];
+    const size_t total = (size_t)g.C * L.N, i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int c = cn_layout ? (int)(i / L.N) : (int)(i % g.C), n = cn_layout ? (int)(i % L.N) : (int)(i / g.C);
+    float sum = 0.f;
+    for (int z = 0; z < nz; ++z) sum += part[(size_t)z * total + i];
+    float *w = L.dW + w_index(L, g, c, n);
+    *w += sum;
+}
+
+// ------------------------------------------------------------------ backward: dX(seg) += dY * W^T
+// the CTA's 64 rows x 64 channels tile of dY * W^T over the columns [n_lo, n_hi) of segment g
+__device__ __forceinline__ void dx_tile(const fcn_train_layer &L, const fcn_train_seg &g, int M, int r0, int c0,
+                                        int n_lo, int n_hi, float (&acc)[4][4], float (&As)[TG_BK][TG_BM + 4],
+                                        float (&Bs)[TG_BK][TG_BN + 4], DyCoef (&s_dy)[TG_BK]) {
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
     for (int nn0 = n_lo; nn0 < n_hi; nn0 += TG_BK) {
         __syncthreads();
         if (tid < TG_BK) s_dy[tid] = dy_coef(L, min(nn0 + tid, L.N - 1));
@@ -372,19 +618,88 @@ train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_pe
         __syncthreads();
         tile_fma_4x4(acc, As, Bs, tx, ty);
     }
+}
+
+// source position of output row r through segment g (the consumer's index map); false outside [0, T*up)
+__device__ __forceinline__ bool dx_target(const fcn_train_layer &L, const fcn_train_seg &g, int r, int &row,
+                                          int &colb) {
+    const fcn_train_src &s = g.src;
+    const int b = r / L.T_out, t = r - b * L.T_out, p = t * g.stride + g.tap;
+    if (p < 0 || p >= s.T * s.up) return false;
+    row = b * s.T + p / s.up;
+    colb = s.c0 + (p % s.up) * s.cup;
+    return true;
+}
+
+__global__ void __launch_bounds__(TG_THREADS)
+train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_per_slice) {
+    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[n][row], Bs[n][channel]
+    __shared__ DyCoef s_dy[TG_BK];
+    const fcn_train_seg &g = L.seg[seg_idx];
+    const fcn_train_src &s = g.src;
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int r0 = blockIdx.x * TG_BM, c0 = blockIdx.y * TG_BN;
+    const int M = L.B * L.T_out;
+    float acc[4][4] = {};
+    const int n_lo = blockIdx.z * n_per_slice, n_hi = min(L.N, n_lo + n_per_slice);
+    dx_tile(L, g, M, r0, c0, n_lo, n_hi, acc, As, Bs, s_dy);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int r = r0 + ty * 4 + i;
         if (r >= M) continue;
-        const int b = r / L.T_out, t = r - b * L.T_out, p = t * g.stride + g.tap;
-        if (p < 0 || p >= s.T * s.up) continue;
-        const int row = b * s.T + p / s.up, colb = s.c0 + (p % s.up) * s.cup;
+        int row, colb;
+        if (!dx_target(L, g, r, row, colb)) continue;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int c = c0 + tx * 4 + j;
             if (c < g.C) atomicAdd(&s.grad[(size_t)row * s.ld + colb + c], acc[i][j]);
         }
     }
+}
+
+// train_dx_kernel of the deterministic backward: column slice blockIdx.z's tile goes to part[z][M][C] (plain
+// stores); train_dx_sum_kernel adds the slices
+__global__ void __launch_bounds__(TG_THREADS)
+train_dx_det_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_per_slice,
+                    float *__restrict__ part) {
+    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];
+    __shared__ DyCoef s_dy[TG_BK];
+    const fcn_train_seg &g = L.seg[seg_idx];
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int r0 = blockIdx.x * TG_BM, c0 = blockIdx.y * TG_BN;
+    const int M = L.B * L.T_out;
+    float acc[4][4] = {};
+    const int n_lo = blockIdx.z * n_per_slice, n_hi = min(L.N, n_lo + n_per_slice);
+    dx_tile(L, g, M, r0, c0, n_lo, n_hi, acc, As, Bs, s_dy);
+    float *dst = part + (size_t)blockIdx.z * M * g.C;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int r = r0 + ty * 4 + i;
+        if (r >= M) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int c = c0 + tx * 4 + j;
+            if (c < g.C) dst[(size_t)r * g.C + c] = acc[i][j];
+        }
+    }
+}
+
+// src.grad += the sum over the nz column slices, in slice order, of part[z][M][C], through the index map of
+// train_dx_kernel: one read-add-store per element (the map is injective within a segment: distinct output rows reach
+// distinct source positions; the segments of a layer and the layers run one after another)
+__global__ void train_dx_sum_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, const float *__restrict__ part,
+                                    int nz) {
+    const fcn_train_seg &g = L.seg[seg_idx];
+    const int M = L.B * L.T_out;
+    const size_t total = (size_t)M * g.C, i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int r = (int)(i / g.C), c = (int)(i % g.C);
+    int row, colb;
+    if (!dx_target(L, g, r, row, colb)) return;
+    float sum = 0.f;
+    for (int z = 0; z < nz; ++z) sum += part[(size_t)z * total + i];
+    float *d = g.src.grad + (size_t)row * g.src.ld + colb + c;
+    *d += sum;
 }
 
 // ------------------------------------------------------------------ PointNet pooling (mask, max over K) fwd / bwd
@@ -497,23 +812,12 @@ __device__ __forceinline__ void tile_fma_8x4(float (&acc)[8][4], const float (&A
     }
 }
 
-// Y[M,N] = act(X[M,K]) * W^T   (W in parameter layout (N,K): both operands contiguous along K)
-__global__ void __launch_bounds__(FP_THREADS)
-train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
-    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
-    __shared__ float s_scale[512], s_shift[512];
-    __shared__ float s_sum[FP_BN], s_sq[FP_BN];
-    const fcn_train_seg &g = L.seg[0];
+// the plain forward's 128 x 64 output tile over all of K (s_scale / s_shift: the source's BN, staged for all K)
+__device__ __forceinline__ void fwd_plain_tiles(const fcn_train_layer &L, const fcn_train_seg &g, int tid, int tx,
+                                                int ty, int r0, int n0, int M, int K, float (&acc)[8][4],
+                                                float (&As)[FP_BK][FP_BM + 4], float (&Bs)[FP_BK][FP_BN + 4],
+                                                const float (&s_scale)[512], const float (&s_shift)[512]) {
     const fcn_train_src &s = g.src;
-    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int r0 = blockIdx.x * FP_BM, n0 = blockIdx.y * FP_BN;
-    const int M = L.B * L.T_out, K = g.C;
-    for (int c = tid; c < K; c += FP_THREADS) {
-        const float2 k = src_coef(s, c, true);
-        s_scale[c] = k.x; s_shift[c] = k.y;
-    }
-    if (tid < FP_BN) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
-    __syncthreads();
     // A: 128 rows x 16 k = 512 float4 (2 per thread); B: 64 n x 16 k = 256 float4 (1 per thread)
     const int arow = tid / 4, akq = (tid % 4) * 4;
     const int bn = tid / 4, bkq = (tid % 4) * 4;
@@ -539,7 +843,6 @@ train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
         }
         Bs[bkq + 0][bn] = pb.x; Bs[bkq + 1][bn] = pb.y; Bs[bkq + 2][bn] = pb.z; Bs[bkq + 3][bn] = pb.w;
     };
-    float acc[8][4] = {};
     gload(0);
     for (int k0 = 0; k0 < K; k0 += FP_BK) {
         __syncthreads();
@@ -548,6 +851,27 @@ train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
         if (k0 + FP_BK < K) gload(k0 + FP_BK);
         tile_fma_8x4(acc, As, Bs, tx, ty);
     }
+}
+
+// Y[M,N] = act(X[M,K]) * W^T   (W in parameter layout (N,K): both operands contiguous along K)
+__global__ void __launch_bounds__(FP_THREADS)
+train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
+    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
+    __shared__ float s_scale[512], s_shift[512];
+    __shared__ float s_sum[FP_BN], s_sq[FP_BN];
+    const fcn_train_seg &g = L.seg[0];
+    const fcn_train_src &s = g.src;
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int r0 = blockIdx.x * FP_BM, n0 = blockIdx.y * FP_BN;
+    const int M = L.B * L.T_out, K = g.C;
+    for (int c = tid; c < K; c += FP_THREADS) {
+        const float2 k = src_coef(s, c, true);
+        s_scale[c] = k.x; s_shift[c] = k.y;
+    }
+    if (tid < FP_BN) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
+    __syncthreads();
+    float acc[8][4] = {};
+    fwd_plain_tiles(L, g, tid, tx, ty, r0, n0, M, K, acc, As, Bs, s_scale, s_shift);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const int n = n0 + tx * 4 + j;
@@ -568,6 +892,50 @@ train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
     if (tid < FP_BN) {
         atomicAdd(&L.sums[n0 + tid], (double)s_sum[tid]);
         atomicAdd(&L.sums[L.Cout + n0 + tid], (double)s_sq[tid]);
+    }
+}
+
+// train_fwd_plain_kernel of the deterministic forward: this CTA's column sums over its 128 rows (16 row groups added
+// in group order) go to slot blockIdx.x of `slots` [row block][2N], plain stores
+__global__ void __launch_bounds__(FP_THREADS)
+train_fwd_plain_det_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ slots) {
+    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
+    __shared__ float s_scale[512], s_shift[512];
+    __shared__ float s_ps[16][FP_BN + 1], s_pq[16][FP_BN + 1];
+    const fcn_train_seg &g = L.seg[0];
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int r0 = blockIdx.x * FP_BM, n0 = blockIdx.y * FP_BN;
+    const int M = L.B * L.T_out, K = g.C;
+    for (int c = tid; c < K; c += FP_THREADS) {
+        const float2 k = src_coef(g.src, c, true);
+        s_scale[c] = k.x; s_shift[c] = k.y;
+    }
+    __syncthreads();
+    float acc[8][4] = {};
+    fwd_plain_tiles(L, g, tid, tx, ty, r0, n0, M, K, acc, As, Bs, s_scale, s_shift);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int n = n0 + tx * 4 + j;
+        float ps = 0.f, pq = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int r = r0 + ty * 8 + i;
+            if (r < M) {
+                const float y = acc[i][j];
+                L.Y[(size_t)r * L.N + n] = y;
+                ps += y; pq += y * y;
+            }
+        }
+        s_ps[ty][tx * 4 + j] = ps; s_pq[ty][tx * 4 + j] = pq;
+    }
+    __syncthreads();
+    if (tid < FP_BN) {
+        float a1 = 0.f, a2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) { a1 += s_ps[i][tid]; a2 += s_pq[i][tid]; }
+        float *slot = slots + (size_t)blockIdx.x * 2 * L.N;
+        slot[n0 + tid] = a1;
+        slot[L.N + n0 + tid] = a2;
     }
 }
 
@@ -632,18 +1000,14 @@ train_dx_plain_kernel(const __grid_constant__ fcn_train_layer L) {
     }
 }
 
-// dW[N,K] += dY[M,N]^T * act(X[M,K])   over the row slice [z*rows_per_block, ...): atomicAdd into the bucket
-__global__ void __launch_bounds__(FP_THREADS)
-train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block) {
-    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];   // As[row][n], Bs[row][k]
-    __shared__ DyCoef s_c[FP_BM];
-    __shared__ float s_scale[FP_BN], s_shift[FP_BN];
-    const fcn_train_seg &g = L.seg[0];
+// the plain dW's 128 columns x 64 channels tile of dY^T * act(X) over rows [rb, re)
+__device__ __forceinline__ void dw_plain_tiles(const fcn_train_layer &L, const fcn_train_seg &g, int tid, int n0,
+                                               int c0, int N, int rb, int re, float (&acc)[8][4],
+                                               float (&As)[FP_BK][FP_BM + 4], float (&Bs)[FP_BK][FP_BN + 4],
+                                               DyCoef (&s_c)[FP_BM], float (&s_scale)[FP_BN],
+                                               float (&s_shift)[FP_BN]) {
     const fcn_train_src &s = g.src;
-    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int n0 = blockIdx.x * FP_BM, c0 = blockIdx.y * FP_BN;
-    const int M = L.B * L.T_out, N = L.N;
-    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
+    const int tx = tid % 16, ty = tid / 16;
     if (tid < FP_BM) s_c[tid] = dy_coef(L, min(n0 + tid, N - 1));
     if (tid < FP_BN) {
         const float2 k = src_coef(s, c0 + tid, true);
@@ -690,7 +1054,6 @@ train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bl
         }
         *(float4 *)&Bs[br][bkq] = make_float4(x[0], x[1], x[2], x[3]);
     };
-    float acc[8][4] = {};
     gload(rb);
     for (int m0 = rb; m0 < re; m0 += FP_BK) {
         __syncthreads();
@@ -699,6 +1062,21 @@ train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bl
         if (m0 + FP_BK < re) gload(m0 + FP_BK);
         tile_fma_8x4(acc, As, Bs, tx, ty);
     }
+}
+
+// dW[N,K] += dY[M,N]^T * act(X[M,K])   over the row slice [z*rows_per_block, ...): atomicAdd into the bucket
+__global__ void __launch_bounds__(FP_THREADS)
+train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block) {
+    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];   // As[row][n], Bs[row][k]
+    __shared__ DyCoef s_c[FP_BM];
+    __shared__ float s_scale[FP_BN], s_shift[FP_BN];
+    const fcn_train_seg &g = L.seg[0];
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int n0 = blockIdx.x * FP_BM, c0 = blockIdx.y * FP_BN;
+    const int M = L.B * L.T_out, N = L.N;
+    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
+    float acc[8][4] = {};
+    dw_plain_tiles(L, g, tid, n0, c0, N, rb, re, acc, As, Bs, s_c, s_scale, s_shift);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int n = n0 + ty * 8 + i;
@@ -706,6 +1084,29 @@ train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bl
 #pragma unroll
         for (int j = 0; j < 4; ++j)
             atomicAdd(&L.dW[g.w_off + (size_t)n * L.s_co + c0 + tx * 4 + j], acc[i][j]);
+    }
+}
+
+// train_dw_plain_kernel of the deterministic backward: row slice blockIdx.z's tile goes to part[z][N][C] (plain
+// float4 stores); train_dw_sum_kernel adds the slices
+__global__ void __launch_bounds__(FP_THREADS)
+train_dw_plain_det_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block, float *__restrict__ part) {
+    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
+    __shared__ DyCoef s_c[FP_BM];
+    __shared__ float s_scale[FP_BN], s_shift[FP_BN];
+    const fcn_train_seg &g = L.seg[0];
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int n0 = blockIdx.x * FP_BM, c0 = blockIdx.y * FP_BN;
+    const int M = L.B * L.T_out, N = L.N, C = g.C;
+    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
+    float acc[8][4] = {};
+    dw_plain_tiles(L, g, tid, n0, c0, N, rb, re, acc, As, Bs, s_c, s_scale, s_shift);
+    float *dst = part + (size_t)blockIdx.z * N * C;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int n = n0 + ty * 8 + i;
+        if (n < N)
+            *(float4 *)(dst + (size_t)n * C + c0 + tx * 4) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
     }
 }
 
@@ -830,6 +1231,156 @@ extern "C" int fcn_train_backward(const fcn_train_layer *L, int need_dx_mask, fc
             const int nps = split_len(L->N, ceil_div(M, TG_BM) * ceil_div(L->seg[sg].C, TG_BN));
             dim3 gx(ceil_div(M, TG_BM), ceil_div(L->seg[sg].C, TG_BN), ceil_div(L->N, nps));
             train_dx_kernel<<<gx, TG_THREADS, 0, st>>>(*L, sg, nps);
+            FCN_LAUNCH_CHECK();
+        }
+    }
+    return FCN_OK;
+}
+
+// ------------------------------------------------------------------ deterministic mode
+// The same GEMMs with every float atomic replaced by plain stores of partial results into the workspace and ordered
+// sums of those partials: per-row-block column sums (slots) for Sum(y), Sum(y^2), Sum(dz), Sum(dz*xh), row-slice
+// tiles for dW and column-slice tiles for dX.  Every split depends on the layer's shape only: the forward's K split
+// is the one fwd_slices picks for an unbounded workspace, the backward's splits are fcn_train_backward's.
+constexpr int DET_FINISH_RPB = 32;     // rows per block of train_fwd_finish_det_kernel
+constexpr int PLAIN_DW_RPB = 1024;     // rows per row slice of the plain dW kernels
+
+static int reduce_rpb(int M) { return M >= 4096 ? 256 : 32; }
+
+// sizes, in floats, of what the deterministic forward keeps in the workspace: K-split partials, then the slots
+struct DetFwdPlan {
+    int nslice, tiles_per_slice, nrb;
+    long long partial, slots;
+};
+static DetFwdPlan det_fwd_plan(const fcn_train_layer &L) {
+    const int M = L.B * L.T_out;
+    DetFwdPlan p{1, 0, 0, 0, 0};
+    if (host_plain(L)) {
+        p.nrb = ceil_div(M, FP_BM);
+    } else {
+        p.nslice = fwd_slices(L, (long long)1 << 40, &p.tiles_per_slice);
+        p.partial = p.nslice > 1 ? (long long)p.nslice * M * L.N : 0;
+        p.nrb = ceil_div(M, p.nslice > 1 ? DET_FINISH_RPB : TG_BM);
+    }
+    p.slots = L.has_bn ? (long long)p.nrb * 2 * L.N : 0;
+    return p;
+}
+
+// the largest piece the deterministic backward keeps in the workspace (its launches use it one after another)
+static long long det_bwd_floats(const fcn_train_layer &L) {
+    const int M = L.B * L.T_out;
+    long long need = (long long)ceil_div(M, reduce_rpb(M)) * (L.has_bn ? 2 : 1) * L.N;
+    if (host_plain(L)) return std::max(need, (long long)ceil_div(M, PLAIN_DW_RPB) * L.N * L.seg[0].C);
+    for (int sg = 0; sg < L.n_seg; ++sg) {
+        const int C = L.seg[sg].C;
+        const int rpb = split_len(M, ceil_div(C, TG_BM) * ceil_div(L.N, TG_BN));
+        const int nps = split_len(L.N, ceil_div(M, TG_BM) * ceil_div(C, TG_BN));
+        need = std::max(need, (long long)ceil_div(M, rpb) * C * L.N);
+        need = std::max(need, (long long)ceil_div(L.N, nps) * M * C);
+    }
+    return need;
+}
+
+static bool shape_ok(const fcn_train_layer &L) {
+    if (L.B < 1 || L.T_out < 1 || L.N < 1 || L.Cout < 1 || L.up < 1 || L.n_seg < 1 || L.n_seg > FCN_MAX_SEGS)
+        return false;
+    for (int i = 0; i < L.n_seg; ++i)
+        if (L.seg[i].C < 1) return false;
+    return true;
+}
+
+static long long det_floats(const fcn_train_layer &L) {
+    const DetFwdPlan f = det_fwd_plan(L);
+    return std::max(f.partial + f.slots, det_bwd_floats(L));
+}
+
+static int det_workspace_check(const fcn_train_layer &L, const float *ws, long long ws_floats) {
+    FCN_REQUIRE(ws != nullptr, "NULL workspace (the deterministic kernels need fcn_train_deterministic_workspace_floats)");
+    FCN_REQUIRE(ws_floats >= det_floats(L), "workspace smaller than fcn_train_deterministic_workspace_floats(layer)");
+    return FCN_OK;
+}
+
+static int launch_slots_sum(double *dst, const float *slots, int nrb, int N, int C, int halves, cudaStream_t st) {
+    train_slots_sum_kernel<<<ceil_div(halves * C, 32), 256, 0, st>>>(dst, slots, nrb, N, C, halves);
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
+}
+
+extern "C" long long fcn_train_deterministic_workspace_floats(const fcn_train_layer *L) {
+    if (L == nullptr || !shape_ok(*L)) return 0;
+    return det_floats(*L);
+}
+
+extern "C" int fcn_train_forward_deterministic(const fcn_train_layer *L, float *workspace, long long workspace_floats,
+                                               fcn_stream_t stream) {
+    FCN_REQUIRE(L != nullptr, "NULL layer");
+    if (int rc = check_layer(*L)) return rc;
+    if (int rc = det_workspace_check(*L, workspace, workspace_floats)) return rc;
+    const int M = L->B * L->T_out;
+    cudaStream_t st = (cudaStream_t)stream;
+    const DetFwdPlan p = det_fwd_plan(*L);
+    float *slots = workspace + p.partial;
+    if (host_plain(*L)) {
+        dim3 grid(p.nrb, L->N / FP_BN);
+        train_fwd_plain_det_kernel<<<grid, FP_THREADS, 0, st>>>(*L, slots);
+        FCN_LAUNCH_CHECK();
+    } else {
+        dim3 grid(ceil_div(M, TG_BM), ceil_div(L->N, TG_BN), p.nslice);
+        train_fwd_det_kernel<<<grid, TG_THREADS, 0, st>>>(*L, workspace, p.tiles_per_slice, slots);
+        FCN_LAUNCH_CHECK();
+        if (p.nslice > 1) {
+            dim3 gf(ceil_div(L->N, 32), p.nrb);
+            train_fwd_finish_det_kernel<<<gf, 256, 0, st>>>(*L, workspace, p.nslice, DET_FINISH_RPB, slots);
+            FCN_LAUNCH_CHECK();
+        }
+    }
+    if (L->has_bn) return launch_slots_sum(L->sums, slots, p.nrb, L->N, L->Cout, 2, st);
+    return FCN_OK;
+}
+
+extern "C" int fcn_train_backward_deterministic(const fcn_train_layer *L, int need_dx_mask, float *workspace,
+                                                long long workspace_floats, fcn_stream_t stream) {
+    FCN_REQUIRE(L != nullptr, "NULL layer");
+    if (int rc = check_layer(*L)) return rc;
+    FCN_REQUIRE(L->dA && L->dW && L->dsums, "NULL gradient buffers");
+    if (int rc = det_workspace_check(*L, workspace, workspace_floats)) return rc;
+    const int M = L->B * L->T_out;
+    cudaStream_t st = (cudaStream_t)stream;
+    {   // Sum(dz), Sum(dz * xh) per channel
+        const int rpb = reduce_rpb(M), nrb = ceil_div(M, rpb);
+        train_reduce_det_kernel<<<dim3(ceil_div(L->N, 32), nrb), 256, 0, st>>>(*L, rpb, workspace);
+        FCN_LAUNCH_CHECK();
+        if (int rc = launch_slots_sum(L->dsums, workspace, nrb, L->N, L->has_bn ? L->Cout : L->N, L->has_bn ? 2 : 1, st))
+            return rc;
+    }
+    if (host_plain(*L)) {
+        const int C = L->seg[0].C, nz = ceil_div(M, PLAIN_DW_RPB);
+        dim3 grid(ceil_div(L->N, FP_BM), C / FP_BN, nz);
+        train_dw_plain_det_kernel<<<grid, FP_THREADS, 0, st>>>(*L, PLAIN_DW_RPB, workspace);
+        FCN_LAUNCH_CHECK();
+        train_dw_sum_kernel<<<ceil_div(C * L->N, 256), 256, 0, st>>>(*L, 0, workspace, nz, 0);
+        FCN_LAUNCH_CHECK();
+        if ((need_dx_mask & 1) && L->seg[0].src.grad != nullptr) {     // one CTA per element, no split: order-free
+            dim3 gx(ceil_div(M, FP_BM), C / FP_BN);
+            train_dx_plain_kernel<<<gx, FP_THREADS, 0, st>>>(*L);
+            FCN_LAUNCH_CHECK();
+        }
+        return FCN_OK;
+    }
+    for (int sg = 0; sg < L->n_seg; ++sg) {
+        const int C = L->seg[sg].C;
+        const int rpb = split_len(M, ceil_div(C, TG_BM) * ceil_div(L->N, TG_BN)), nz = ceil_div(M, rpb);
+        dim3 grid(ceil_div(C, TG_BM), ceil_div(L->N, TG_BN), nz);
+        train_dw_det_kernel<<<grid, TG_THREADS, 0, st>>>(*L, sg, rpb, workspace);
+        FCN_LAUNCH_CHECK();
+        train_dw_sum_kernel<<<ceil_div(C * L->N, 256), 256, 0, st>>>(*L, sg, workspace, nz, 1);
+        FCN_LAUNCH_CHECK();
+        if (((need_dx_mask >> sg) & 1) && L->seg[sg].src.grad != nullptr) {
+            const int nps = split_len(L->N, ceil_div(M, TG_BM) * ceil_div(C, TG_BN)), nzx = ceil_div(L->N, nps);
+            dim3 gx(ceil_div(M, TG_BM), ceil_div(C, TG_BN), nzx);
+            train_dx_det_kernel<<<gx, TG_THREADS, 0, st>>>(*L, sg, nps, workspace);
+            FCN_LAUNCH_CHECK();
+            train_dx_sum_kernel<<<(unsigned)(((long long)M * C + 255) / 256), 256, 0, st>>>(*L, sg, workspace, nzx);
             FCN_LAUNCH_CHECK();
         }
     }

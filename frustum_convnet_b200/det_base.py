@@ -282,6 +282,8 @@ class PointNetDet(_EngineOwner):
         self.use_cuda_graph = default_cuda_graph()   # replay one CUDA graph per input shape (FCN_CUDA_GRAPH)
         self.copy_outputs = True      # False: return views of the engine's output block (zero-copy)
         self.train_kernels = os.environ.get("FCN_TRAIN_KERNELS", "1") != "0"   # train(): csrc/train.cu, else autograd
+        # train() kernels in their bit-reproducible mode: True / False, or None = torch.are_deterministic_algorithms_enabled()
+        self.deterministic = None
 
     def _engine_spec(self):
         return self.ARCH, self.num_vec, self.dataset_name, self.feat_net.dists, self.num_bins, ""

@@ -88,10 +88,12 @@ class LogitsFn(torch.autograd.Function):
 
 
 class TrainEngine:
-    """Kernel tables + workspaces of one PointNetDet for one input shape (B, N, T...)."""
+    """Kernel tables + workspaces of one PointNetDet for one input shape (B, N, T...).  ``deterministic``: the
+    layers run on ``fcn_train_forward_deterministic`` / ``fcn_train_backward_deterministic`` (bit-reproducible)."""
 
-    def __init__(self, model, B: int, N: int, T: Sequence[int]):
+    def __init__(self, model, B: int, N: int, T: Sequence[int], deterministic: bool = False):
         self.model = model
+        self.deterministic = bool(deterministic)
         arch = model.ARCH
         S = arch.num_scales
         assert len(T) == S
@@ -253,8 +255,10 @@ class TrainEngine:
         self._graphs = {}
         self.use_graph = True
         lib = _lib.load()
-        need = max([int(lib.fcn_train_workspace_floats(C.byref(L))) for L in self.layers] + [1])
-        self.workspace = torch.empty(need, dtype=f32, device=dev)   # K-split partial sums of the skinny FCN layers
+        query = lib.fcn_train_deterministic_workspace_floats if self.deterministic else lib.fcn_train_workspace_floats
+        need = max([int(query(C.byref(L))) for L in self.layers] + [1])
+        # K-split partial sums of the skinny FCN layers; deterministic mode: also the slots and slices of its sums
+        self.workspace = torch.empty(need, dtype=f32, device=dev)
 
     # ------------------------------------------------------------------
     def _group_args(self):
@@ -279,6 +283,20 @@ class TrainEngine:
         return g
 
     # ---- launch sequences (all pointers are static: the step is CUDA-graph capturable)
+    def _layer_forward(self, li, st):
+        if self.deterministic:
+            _lib.call("fcn_train_forward_deterministic", C.byref(self.layers[li]), _ptr(self.workspace),
+                      self.workspace.numel(), st)
+        else:
+            _lib.call("fcn_train_forward", C.byref(self.layers[li]), _ptr(self.workspace), self.workspace.numel(), st)
+
+    def _layer_backward(self, li, st):
+        if self.deterministic:
+            _lib.call("fcn_train_backward_deterministic", C.byref(self.layers[li]), self.dx_mask[li],
+                      _ptr(self.workspace), self.workspace.numel(), st)
+        else:
+            _lib.call("fcn_train_backward", C.byref(self.layers[li]), self.dx_mask[li], st)
+
     def _seq_forward(self):
         S = len(self.T)
         st = _stream()
@@ -287,11 +305,11 @@ class TrainEngine:
         li = 0
         for s in range(S):
             for _ in range(3):
-                _lib.call("fcn_train_forward", C.byref(self.layers[li]), _ptr(self.workspace), self.workspace.numel(), st)
+                self._layer_forward(li, st)
                 li += 1
             _lib.call("fcn_train_pool", C.byref(self.pools[s]), 0, st)
         while li < len(self.layers):
-            _lib.call("fcn_train_forward", C.byref(self.layers[li]), _ptr(self.workspace), self.workspace.numel(), st)
+            self._layer_forward(li, st)
             li += 1
 
     def _seq_backward(self, stage, update_running):
@@ -301,7 +319,7 @@ class TrainEngine:
             # FCN + heads in reverse creation order (a topological order of the backward graph: every consumer of
             # a tensor was created after it)
             for li in range(len(self.layers) - 1, self.n_pn_layers - 1, -1):
-                _lib.call("fcn_train_backward", C.byref(self.layers[li]), self.dx_mask[li], st)
+                self._layer_backward(li, st)
             # BN bookkeeping of the FCN layers: their dgamma / dbeta belong to the first gradient bucket
             nf = len(self.layers) - self.n_pn_layers
             _lib.call("fcn_train_finalize", _ptr(self.table_dev) + self.n_pn_layers * C.sizeof(_lib.TrainLayer), nf,
@@ -311,7 +329,7 @@ class TrainEngine:
                 _lib.call("fcn_train_pool", C.byref(self.pools[s]), 1, st)
                 for j in (2, 1, 0):
                     li = 3 * s + j
-                    _lib.call("fcn_train_backward", C.byref(self.layers[li]), self.dx_mask[li], st)
+                    self._layer_backward(li, st)
             _lib.call("fcn_train_finalize", _ptr(self.table_dev), self.n_pn_layers, 1 if update_running else 0, st)
             if update_running and self._bn_counters:
                 torch._foreach_add_(self._bn_counters, 1)
@@ -369,6 +387,8 @@ class TrainEngine:
             self._seq_backward(stage, update_running)
 
     def kernel_launches_per_step(self):
+        """Launches of one step in the DEFAULT mode (the layer GEMMs, pools, grouping, finalize and the optimizer).
+        The deterministic mode adds its ordered-sum launches (slots, dW and dX slices), which this does not count."""
         n_fwd = len(self.layers) + len(self.pools) + 2
         n_bwd = sum(1 + L.n_seg + bin(m).count("1") for L, m in zip(self.layers, self.dx_mask)) + len(self.pools) + 1
         return n_fwd + n_bwd + 1      # + fused Adam or SGD
@@ -594,10 +614,12 @@ class TrainStep:
     TrainingStates update).  ``optimizer`` ("adam" or "sgd", the values of cfg.TRAIN.OPTIMIZER,
     train_net_det.py:321-328) selects a torch.optim.Adam (FlatAdam) or torch.optim.SGD (FlatSGD, with ``momentum``)
     for lr schedulers and checkpoints; ``states`` (validate.TrainStates) collects every step's losses and metrics on
-    the device."""
+    the device.  ``deterministic`` (settable): True runs the step bit-reproducibly (deterministic layer kernels and
+    fused loss; one GPU, one build, same inputs and hyper-parameters), False the default kernels, None follows
+    ``torch.use_deterministic_algorithms`` at every step.  True requires ``loss_impl == "kernel"``."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, comm_stream=None,
-                 states_capacity=None, optimizer="adam", momentum=0.0):
+                 states_capacity=None, optimizer="adam", momentum=0.0, deterministic=None):
         from .validate import TrainStates
         if optimizer not in ("adam", "sgd"):
             raise ValueError("TrainStep: optimizer %r is not supported; the fused steps are 'adam' and 'sgd'"
@@ -618,6 +640,7 @@ class TrainStep:
         # losses + d/dlogits: "kernel" = fused hand-written kernels (csrc/loss.cu), "graph" = the PyTorch ops as one
         # CUDA graph (train_path.LossGraph), "eager" = the reference-shaped PyTorch ops
         self.loss_impl = "kernel"
+        self.deterministic = deterministic
 
     @property
     def lr(self):
@@ -656,22 +679,40 @@ class TrainStep:
     def step_count(self):
         return self.optimizer.step_count
 
-    def engine(self, B, N, T) -> TrainEngine:
-        key = (int(B), int(N), tuple(int(t) for t in T))
+    def _mode(self) -> bool:
+        """This step's mode: ``deterministic``, or torch's flag when it is None."""
+        from .train_path import deterministic_mode
+        if self.deterministic is True and self.loss_impl != "kernel":
+            raise ValueError("TrainStep: deterministic=True needs loss_impl='kernel' (the fused loss); loss_impl=%r "
+                             "runs PyTorch ops, which follow torch.use_deterministic_algorithms" % (self.loss_impl,))
+        return deterministic_mode(self.deterministic)
+
+    def engine(self, B, N, T, deterministic=False) -> TrainEngine:
+        key = (int(B), int(N), tuple(int(t) for t in T), bool(deterministic))
         e = self.engines.get(key)
         if e is None:
-            e = self.engines[key] = TrainEngine(self.model, *key)
+            e = self.engines[key] = TrainEngine(self.model, *key[:3], deterministic=key[3])
         return e
+
+    @staticmethod
+    def _fused_loss_key(eng):
+        return ("kernel-deterministic" if eng.deterministic else "kernel", eng.B, eng.T2)
 
     def _losses(self, eng, cls, reg, center_ref2, data):
         """-> (losses, metrics, dcls, dreg)."""
         from .train_path import FusedLoss, LossGraph, losses_from_logits
-        if self.loss_impl in ("kernel", "graph"):
-            key = (self.loss_impl, eng.B, eng.T2)
+        if self.loss_impl == "kernel":
+            key = self._fused_loss_key(eng)
             lg = self._loss_graphs.get(key)
             if lg is None:
-                cls_ = FusedLoss if self.loss_impl == "kernel" else LossGraph
-                lg = self._loss_graphs[key] = cls_(self.model, eng.B, eng.T2, reg.shape[1], cls.device)
+                lg = self._loss_graphs[key] = FusedLoss(self.model, eng.B, eng.T2, reg.shape[1], cls.device,
+                                                        eng.deterministic)
+            return lg.run(cls, reg, center_ref2, data)
+        if self.loss_impl == "graph":
+            key = ("graph", eng.B, eng.T2)
+            lg = self._loss_graphs.get(key)
+            if lg is None:
+                lg = self._loss_graphs[key] = LossGraph(self.model, eng.B, eng.T2, reg.shape[1], cls.device)
             return lg.run(cls, reg, center_ref2, data)
         cls_l = cls.detach().clone().requires_grad_(True)
         reg_l = reg.detach().clone().requires_grad_(True)
@@ -686,7 +727,7 @@ class TrainStep:
         S = model.ARCH.num_scales
         pc = data["point_cloud"][:, :3, :].contiguous()
         centers = [data["center_ref%d" % (i + 1)].contiguous() for i in range(S)]
-        eng = self.engine(pc.shape[0], pc.shape[2], [c.shape[2] for c in centers])
+        eng = self.engine(pc.shape[0], pc.shape[2], [c.shape[2] for c in centers], self._mode())
         self.flat.grad.zero_()
         cls, reg = eng.forward(pc, centers, data.get("one_hot"))
         losses, metrics, dcls, dreg = self._losses(eng, cls, reg, centers[1], data)
@@ -705,7 +746,7 @@ class TrainStep:
         S = model.ARCH.num_scales
         pc = data["point_cloud"][:, :3, :].contiguous()
         centers = [data["center_ref%d" % (i + 1)].contiguous() for i in range(S)]
-        eng = self.engine(pc.shape[0], pc.shape[2], [c.shape[2] for c in centers])
+        eng = self.engine(pc.shape[0], pc.shape[2], [c.shape[2] for c in centers], self._mode())
         self.flat.grad.zero_()
         cls, reg = eng.forward(pc, centers, data.get("one_hot"))
         losses, metrics, dcls, dreg = self._losses(eng, cls, reg, centers[1], data)
@@ -739,7 +780,7 @@ class TrainStep:
         """The step's 16-float block for ``states``: fcn_det_loss's result as it stands, or the same layout stacked
         on the device from the PyTorch losses (loss_impl "graph" / "eager")."""
         if self.loss_impl == "kernel":
-            return self._loss_graphs[("kernel", eng.B, eng.T2)].out
+            return self._loss_graphs[self._fused_loss_key(eng)].out
         vals = {**losses, **metrics}
         lab = data["cls_label"]
         return torch.stack([vals[k].detach().reshape(()).float() for k in self.states.keys] +

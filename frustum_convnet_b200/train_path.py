@@ -152,6 +152,12 @@ def pointnet_det_torch(model, data):
     return losses_from_logits(model, cls_scores, outputs, centers[1], data)
 
 
+def deterministic_mode(setting):
+    """The training kernels' mode for a ``deterministic`` setting: True / False as given, None follows
+    ``torch.are_deterministic_algorithms_enabled()`` (read at every step)."""
+    return torch.are_deterministic_algorithms_enabled() if setting is None else bool(setting)
+
+
 def pointnet_det_kernels(model, data):
     """Train branch on the hand-written kernels (csrc/train.cu): everything up to the head logits runs through
     ``TrainEngine`` behind an autograd.Function, the losses are the PyTorch ops below."""
@@ -159,11 +165,12 @@ def pointnet_det_kernels(model, data):
     S = model.ARCH.num_scales
     pc = data["point_cloud"][:, :3, :].contiguous()
     centers = [data["center_ref%d" % (i + 1)].contiguous() for i in range(S)]
-    key = (pc.shape[0], pc.shape[2], tuple(c.shape[2] for c in centers))
+    det = deterministic_mode(getattr(model, "deterministic", None))
+    key = (pc.shape[0], pc.shape[2], tuple(c.shape[2] for c in centers), det)
     cache = model.__dict__.setdefault("_train_engines", {})
     eng = cache.get(key)
     if eng is None:
-        eng = cache[key] = TrainEngine(model, *key)
+        eng = cache[key] = TrainEngine(model, *key[:3], deterministic=det)
     params = tuple(model.parameters())
     cls, reg = LogitsFn.apply(eng, pc, data.get("one_hot"), S, *centers, *params)
     return losses_from_logits(model, cls, reg, centers[1], data)
@@ -408,12 +415,13 @@ class LossGraph:
 
 class FusedLoss:
     """Losses, metrics and d(total_loss)/d(logits) by the fused kernels of csrc/loss.cu (``fcn_det_loss``): three
-    tiny launches instead of ~300 PyTorch ops + their autograd backward (or their 1.07 ms CUDA-graph replay)."""
+    tiny launches instead of ~300 PyTorch ops + their autograd backward (or their 1.07 ms CUDA-graph replay).
+    ``deterministic``: ``fcn_det_loss_deterministic``, whose 16 outputs are bit-reproducible."""
 
     LOSS_KEYS = ("total_loss", "cls_loss", "center_loss", "head_cls_loss", "head_res_loss", "size_cls_loss",
                  "size_res_loss", "corners_loss")
 
-    def __init__(self, model, B, T2, out_size, device):
+    def __init__(self, model, B, T2, out_size, device, deterministic=False):
         import ctypes as C
 
         from . import _lib
@@ -424,7 +432,11 @@ class FusedLoss:
         self.dcls = torch.zeros((N, 2), dtype=f32, device=device)
         self.dreg = torch.zeros((N, out_size), dtype=f32, device=device)
         self.out = torch.zeros(16, dtype=f32, device=device)
-        self.scratch = torch.zeros(16, dtype=f32, device=device)
+        self.deterministic = bool(deterministic)
+        n_scratch = int(_lib.load().fcn_det_loss_deterministic_scratch_floats(N)) if self.deterministic else 16
+        if n_scratch <= 0:
+            raise ValueError("FusedLoss: %d rows are outside the deterministic loss's range [1, 2^24]" % N)
+        self.scratch = torch.zeros(n_scratch, dtype=f32, device=device)
         self.mean_size = torch.from_numpy(np.asarray(model.mean_size_array)).to(device=device, dtype=f32).contiguous()
         a = _lib.LossArgs()
         a.B, a.T2, a.NH, a.NS = B, T2, model.num_bins, model.num_size_cluster
@@ -449,7 +461,8 @@ class FusedLoss:
         (a.cls, a.reg, a.center_ref2, a.cls_label, a.size_class, a.box3d_center, a.box3d_heading,
          a.box3d_size) = [t.data_ptr() for t in keep]
         self._keep = keep
-        self._lib.call("fcn_det_loss", self._C.byref(a), torch.cuda.current_stream().cuda_stream)
+        self._lib.call("fcn_det_loss_deterministic" if self.deterministic else "fcn_det_loss", self._C.byref(a),
+                       torch.cuda.current_stream().cuda_stream)
         o = self.out
         losses = {k: o[i] for i, k in enumerate(self.LOSS_KEYS)}
         metrics = {"cls_acc": o[8], "head_acc": o[9], "size_acc": o[10], "IoU_2D": o[11], "IoU_3D": o[12],

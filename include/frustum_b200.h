@@ -313,6 +313,24 @@ FCN_API int fcn_train_forward(const fcn_train_layer *layer, float *workspace, lo
  * source read by several segments or layers receives the sum of their gradients), dW, dbias, dgamma / dbeta,
  * `sums` and `dsums`.  The forward OVERWRITES Y. */
 FCN_API int fcn_train_backward(const fcn_train_layer *layer, int need_dx_mask, fcn_stream_t stream);
+/* Deterministic mode: the same layer forward / backward with bit-reproducible results.  No float atomics: partial
+ * results go to `workspace` with plain stores and are added in a fixed order (BN statistics and Sum(dz), Sum(dz*xh)
+ * as fp32 per-row-block column sums added in fp64; dW and dX as fp32 slices added in slice order, then added once to
+ * the accumulating buffer).  Every split depends on the layer's shape only, never on the workspace offered or on the
+ * device, so one build gives the same bits for the same inputs on every run, stream and graph replay, whatever the
+ * workspace held before.  The accumulation contract of fcn_train_forward / fcn_train_backward holds.  The bits
+ * differ from the default path's (another summation order).
+ * fcn_train_deterministic_workspace_floats(layer): the floats both entries need, from the layer's shape and its
+ * structure only: its sizes, taps and strides, the layout strides and offsets that decide between the plain and
+ * the generic kernels, and whether `bias` is NULL (a BN layer with a bias cannot take the plain kernels, whose
+ * split differs).  No pointer is dereferenced and no device is needed;
+ * 0 for a NULL layer or a bad shape.  A NULL workspace or one with
+ * fewer floats returns FCN_ERR_INVALID before anything is launched.  Calls on one stream may share one workspace. */
+FCN_API long long fcn_train_deterministic_workspace_floats(const fcn_train_layer *layer);
+FCN_API int fcn_train_forward_deterministic(const fcn_train_layer *layer, float *workspace, long long workspace_floats,
+                                            fcn_stream_t stream);
+FCN_API int fcn_train_backward_deterministic(const fcn_train_layer *layer, int need_dx_mask, float *workspace,
+                                             long long workspace_floats, fcn_stream_t stream);
 /* PointNet pooling: feat[(b,t), c] = (cnt > 0) * max_k relu(bn(Y[(b,t,k), c])), one-hot columns appended
  * (det_base.py:100-101,134-157); backward scatters dfeat to the arg-max rows of a zero-filled dA. */
 typedef struct {
@@ -366,6 +384,12 @@ typedef struct {
     float *dcls, *dreg, *out /* 16 floats */, *scratch /* 16 floats */;
 } fcn_loss_args;
 FCN_API int fcn_det_loss(const fcn_loss_args *args, fcn_stream_t stream);
+/* Deterministic variant: the same outputs, with the 16 floats of `out` bit-reproducible (per-CTA sums added in CTA
+ * order instead of float atomics); dcls / dreg are bit-identical to fcn_det_loss's.  `scratch` holds
+ * fcn_det_loss_deterministic_scratch_floats(B*T2) floats (0 when rows is outside [1, 2^24]: beyond 2^24 rows the
+ * float row counts would no longer be exact). */
+FCN_API long long fcn_det_loss_deterministic_scratch_floats(long long rows);
+FCN_API int fcn_det_loss_deterministic(const fcn_loss_args *args, fcn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * (8) Inference post-processing ("next" row 8(f)-4): batched rotated 3-D NMS on the device.  Replaces
