@@ -12,16 +12,24 @@
 //     order this is deadlock-free under ANY co-residency: the smallest unfinished job is always owned by a running
 //     CTA whose dependencies are complete - no grid-wide barrier, no co-residency requirement, late CTAs
 //     (several forwards are in flight on other streams) simply pick up what is left;
-//   * layer-to-layer dependencies are per row tile: the epilogue of a tile publishes a counter
-//     (release, gpu scope); the scheduler warp acquires the counters of the (<= 4) source tiles a job reads
-//     (taps +-1, stride 2, pixel-shuffled transposed convs) one job ahead, the TMA producer then crosses to the
-//     async proxy;
+//   * layer-to-layer dependencies are per row tile: a finished tile publishes a counter (release, gpu scope); the
+//     scheduler warp acquires the counters of the (<= 4) source tiles a job reads (taps +-1, stride 2,
+//     pixel-shuffled transposed convs) one job ahead, the TMA producer then crosses to the async proxy;
 //   * inside a CTA the same warp-specialised pipeline as conv_gemm_tma.cu, made continuous across jobs: warp 9 =
 //     scheduler (job fetch, descriptor, dependency polling), warp 8 = TMA producer (A boxes by cp.async.bulk.tensor
-//     with the conv taps / stride in the coordinates, weight atoms by bulk copies), warps 0-7 = two consumer
-//     warpgroups (wgmma, 64 rows each, N = NT = 256 | 128 | 64) that also run the epilogue; the smem stage ring of
-//     32-wide K atoms runs across job boundaries (the next job's operands stream while the current one is still
-//     multiplied or stored);
+//     with the conv taps / stride in the coordinates, weight atoms and the job's bias slice by bulk copies),
+//     warps 0-7 = two consumer warpgroups (wgmma, 64 rows each, N = NT = 256 | 128 | 64), warp 10 = store warp;
+//     the smem stage ring of 32-wide K atoms runs across job boundaries (the next job's operands stream while the
+//     current one is still multiplied or stored);
+//   * epilogue off the tensor-core path: a consumer warpgroup adds the bias (from shared memory), applies ReLU and
+//     TF32 rounding, writes zeros at pad positions and stages the result in its own [64 rows x 128 columns] buffer
+//     (128-byte swizzled [32 x 32] boxes of the layer's store map, conflict-free fragment writes), arrives on
+//     `staged` and goes straight into the next job's K loop.  The store warp stores the boxes by
+//     cp.async.bulk.tensor (the transposed convs' pixel shuffle and the concat offset are in the map coordinates,
+//     rows past the map are clipped), hands the buffer back (`staging_free`) once the bulk reads are done, waits
+//     for the writes, crosses from the async proxy (fence.proxy.async.global) and publishes ONE count per tile
+//     (red.release.gpu).  NT = 256 passes through the buffer in two 128-column halves.  The store warp waits only
+//     on its own CTA's job queue and consumers and on its own bulk groups, so the argument above still holds;
 //   * the heads tile (NT = 64: all 2 + 39 logits of a position) stores the logits row and decodes it
 //     (decode.cuh - the same function the stand-alone decode kernel uses), writing the 6-tuple to the local
 //     result block AND to the peers' gather buffers over NVLink (multi-GPU: no NCCL all-gather, no extra
@@ -37,28 +45,39 @@ namespace fcn {
 using namespace gmma;
 
 constexpr int MG_ROWS = 128;
-constexpr int MG_MMA_WARPS = 8;      // warps 0-7: two consumer warpgroups (MMA + epilogue)
-constexpr int MG_TMA_WARP = MG_MMA_WARPS, MG_SCHED_WARP = MG_MMA_WARPS + 1;
-constexpr int MG_THREADS = (MG_MMA_WARPS + 2) * 32;
-// Stage ring: every stage carries ONE 32-wide K atom, a slot = [128 x 32] A box + [NT x 32] W image of the table's
-// widest tile, and the ring holds as many slots as fit in MG_RING_BYTES (NT <= 128: 6 x 32 KB, NT = 256: 4 x 48 KB).
-// Fine-grained slots keep more K ahead of the MMAs: the consumers hold two slots (the stage being multiplied and
-// the one whose wgmma group has not retired yet), the producer fills the rest.
+constexpr int MG_MMA_WARPS = 8;      // warps 0-7: two consumer warpgroups (MMA + staging of the epilogue)
+constexpr int MG_TMA_WARP = MG_MMA_WARPS, MG_SCHED_WARP = MG_MMA_WARPS + 1, MG_STORE_WARP = MG_MMA_WARPS + 2;
+constexpr int MG_THREADS = (MG_MMA_WARPS + 3) * 32;
+constexpr int MG_SMEM_LIMIT = 232448;                         // 227 KB of dynamic shared memory per CTA
+// Epilogue staging: per consumer warpgroup 64 rows x 128 fp32 columns as eight 128-byte-swizzled [32 x 32] boxes of
+// the store map, box (column block cb, row block rb) at (2 cb + rb) * 4 KB.
+constexpr int MG_STG_COLS = 128, MG_BOX_BYTES = 32 * 128, MG_STG_BYTES = 64 * MG_STG_COLS * 4;
 constexpr int MG_A_ATOM = MG_ROWS * 128;
-constexpr int MG_RING_BYTES = 192 * 1024, MG_MAX_SLOTS = 8;
+constexpr int MG_MAX_SLOTS = 8;
+constexpr int MG_JOBQ = 4;                                    // job descriptors in flight inside a CTA
+// full/empty, job_full/job_empty, taken, staged[2], staging_free[2]
+constexpr int MG_NBAR = 2 * MG_MAX_SLOTS + 2 * MG_JOBQ + 1 + 4;
+constexpr int MG_OFF_BAR = 2 * MG_STG_BYTES;
+// barriers and the last-CTA flag, then fcn_mega_job[MG_JOBQ] (64 B each)
+constexpr int MG_OFF_JOBQ = MG_OFF_BAR + ((MG_NBAR * 8 + 4 + 63) & ~63);
+constexpr int MG_BIAS_FLOATS = 256;                          // bias slice of one queued job (NT <= 256 columns)
+constexpr int MG_OFF_BIAS = MG_OFF_JOBQ + MG_JOBQ * 64;
+constexpr int MG_OFF_RING = (MG_OFF_BIAS + MG_JOBQ * MG_BIAS_FLOATS * 4 + 1023) & ~1023;
+// Stage ring: every stage carries ONE 32-wide K atom, a slot = [128 x 32] A box + [NT x 32] W image of the table's
+// widest tile, and the ring takes what the staging buffers, barriers, job queue and bias slices leave of the 227 KB
+// (less 1 KB for aligning the dynamic shared memory): NT <= 128: 4 x 32 KB, NT = 256: 3 x 48 KB.  The consumers
+// hold two slots (the stage being multiplied and the one whose wgmma group has not retired yet), the producer
+// fills the rest.
+constexpr int MG_RING_BYTES = MG_SMEM_LIMIT - 1024 - MG_OFF_RING;
 __host__ __device__ constexpr int mg_slot_bytes(int nt_max) { return MG_A_ATOM + nt_max * 128; }
 __host__ __device__ constexpr int mg_slots(int nt_max) {
     return MG_RING_BYTES / mg_slot_bytes(nt_max) < MG_MAX_SLOTS ? MG_RING_BYTES / mg_slot_bytes(nt_max) : MG_MAX_SLOTS;
 }
 static_assert(mg_slots(256) >= 3, "the widest tile needs a ring of at least three slots");
 __host__ __device__ constexpr int mg_k_atoms(int NT) { return NT == 256 ? 1 : 2; }   // per stage of the weight image
-constexpr int MG_OFF_BAR = MG_RING_BYTES;
-constexpr int MG_JOBQ = 4;                                    // job descriptors in flight inside a CTA
-constexpr int MG_NBAR = 2 * MG_MAX_SLOTS + 2 * MG_JOBQ + 1;   // full/empty, job_full/job_empty, taken
-constexpr int MG_OFF_JOBQ = MG_OFF_BAR + ((MG_NBAR * 8 + 63) & ~63);   // fcn_mega_job[MG_JOBQ] (64 B each)
 constexpr int MG_MAX_LAYERS = 24, MG_MAX_MAPS = 48;
-constexpr int MG_BYTES = MG_OFF_JOBQ + MG_JOBQ * (int)sizeof(fcn_mega_job) + 1024;
-static_assert(MG_BYTES <= 232448, "exceeds the 227 KB shared-memory limit per CTA");
+constexpr int MG_BYTES = MG_OFF_RING + MG_RING_BYTES + 1024;
+static_assert(MG_BYTES <= MG_SMEM_LIMIT, "exceeds the 227 KB shared-memory limit per CTA");
 static_assert(sizeof(fcn_mega_job) == 64 && sizeof(fcn_mega_layer) % 8 == 0, "table record layout");
 
 // Tensor maps and the layer table travel in the kernel parameters (constant bank; CUDA >= 12.1 allows 32 KB).
@@ -78,6 +97,16 @@ __device__ __forceinline__ void mg_tma_load_3d(uint32_t dst, const void *map, in
         "l"((uint64_t)map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
         : "memory");
 }
+// one staged [32 rows x 32 fp32] box -> the output map (rows past the map are clipped by the TMA unit)
+__device__ __forceinline__ void mg_tma_store_3d(const void *map, uint32_t src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(
+                     (uint64_t)map),
+                 "r"(src), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
 
 __device__ __forceinline__ int ld_acquire_gpu(const int *p) {
     int v;
@@ -87,20 +116,25 @@ __device__ __forceinline__ int ld_acquire_gpu(const int *p) {
 __device__ __forceinline__ void red_release_gpu_add(int *p, int v) {
     asm volatile("red.release.gpu.global.add.s32 [%0], %1;\n" ::"l"(p), "r"(v) : "memory");
 }
-// generic-proxy writes of other SMs (observed through the acquire above) -> subsequent async-proxy (TMA) reads
+// Between the generic and the async proxy on global memory: on the consumer side, generic-proxy writes of other SMs
+// (observed through the acquire above) -> subsequent TMA reads; on the store side, this thread's completed TMA
+// stores -> its release of the tile counter.
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;\n" ::: "memory"); }
 
-// Phase timeline (off unless fcn_mega_args.dbg_clocks is set): one row of 16 clock64 values per job, for the first
-// MG_DBG_JOBS jobs of every CTA, at dbg_clocks[(blockIdx.x * MG_DBG_JOBS + q) * 16]:
+// Phase timeline (off unless fcn_mega_args.dbg_clocks is set): one row of MG_DBG_ROW clock64 values per job, for
+// the first MG_DBG_JOBS jobs of every CTA, at dbg_clocks[(blockIdx.x * MG_DBG_JOBS + q) * MG_DBG_ROW]:
 //   [0] TMA lane took the job  [1] job index  [2] scheduler fetched it  [3] its dependencies were met
 //   [4] TMA lane issued its last box  [5] TMA clocks spent in `empty` waits
 //   [6 + 4 wg] first `full` satisfied  [7 + 4 wg] clocks in `full` waits  [8 + 4 wg] last MMA retired
-//   [9 + 4 wg] epilogue done (warp 0 of consumer warpgroup wg)  [14] layer  [15] SM id
+//   [9 + 4 wg] epilogue done: tile staged, or heads rows decoded (warp 0 of consumer warpgroup wg)
+//   [14] layer  [15] SM id
+//   store warp: [20] first staged half received  [21] last box store issued  [22] tile counter published
 // Clocks are per SM: compare them within a row or a CTA only.
-constexpr int MG_DBG_JOBS = 64;
+constexpr int MG_DBG_JOBS = 64, MG_DBG_ROW = 32;
 __device__ __forceinline__ long long *mg_dbg_row(const fcn_mega_args &p, uint32_t q) {
-    return (p.dbg_clocks != nullptr && q < MG_DBG_JOBS) ? p.dbg_clocks + 16 * ((size_t)blockIdx.x * MG_DBG_JOBS + q)
-                                                        : nullptr;
+    return (p.dbg_clocks != nullptr && q < MG_DBG_JOBS)
+               ? p.dbg_clocks + MG_DBG_ROW * ((size_t)blockIdx.x * MG_DBG_JOBS + q)
+               : nullptr;
 }
 __device__ __forceinline__ int smid() {
     int v;
@@ -108,16 +142,15 @@ __device__ __forceinline__ int smid() {
     return v;
 }
 
-// column groups whose bias pairs the epilogue loads together (NT = 256: the accumulator leaves room for two)
-__host__ __device__ constexpr int mg_epi_batch(int NT) { return NT == 256 ? 2 : 8; }
-
 // One job of a consumer warpgroup: the K loop of its 64 rows x NT columns over the stage ring (ring position
 // `st`, phase `ph` run on across jobs), then the epilogue.  A stage is handed back when the wgmma group that read
-// it has retired.
+// it has retired.  `stg` is this warpgroup's staging buffer, `nstg` the number of halves it has staged so far
+// (the parity of `staged` / `staging_free`), `bias` the job's NT-column bias slice in shared memory.
 template <int NT>
 __device__ __forceinline__ void mg_job(const MegaParams &P, const fcn_mega_layer &L, int m_tile, int n_tile,
                                        uint32_t &st, uint32_t &ph, uint8_t *ring, uint64_t *full, uint64_t *empty,
-                                       int *flags, long long *dbg) {
+                                       uint32_t stg, uint64_t *staged, uint64_t *staging_free, uint32_t &nstg,
+                                       const float *bias, int *flags, long long *dbg) {
     const fcn_mega_args &p = P.a;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3, t = tid & 127;
     const int NS = L.n_stage * L.k_atoms;                              // 32-wide K stages of this tile
@@ -157,49 +190,52 @@ __device__ __forceinline__ void mg_job(const MegaParams &P, const fcn_mega_layer
 
     const int rbase = m_tile * MG_ROWS + 64 * wg;                     // first flattened GEMM row of this warpgroup
     if (!L.is_heads) {
-        // +bias (+ReLU, TF32 rounding) -> the output map.  One GEMM row holds `up` consecutive output positions
-        // (pixel shuffle of the transposed convs): row r, column n = jj*Cout + co -> out[r][jj][c_off + co].
-        // Pad positions (past T_out / T_store) are written as zeros: the next layer's taps read them.
-        // The bias pairs of mg_epi_batch(NT) column groups are loaded together, unconditionally (clamped to a valid
-        // column), ahead of their stores: a load behind each store's conditions serialised the epilogue on the
-        // load latency.
-        constexpr int EB = mg_epi_batch(NT);
-        const float *bias = L.bias;
-        const int ncols = L.up * L.Cout;
+        // +bias (+ReLU, TF32 rounding) -> the staging buffer; the store warp writes it through the output map.
+        // One GEMM row holds `up` consecutive output positions (pixel shuffle of the transposed convs): column
+        // n = jj*Cout + co -> output position rt*up + jj.  Cout % 32 == 0, so a 32-column box has one jj.  Pad
+        // positions (past T_out / T_store) are staged as zeros: the next layer's taps read them.
+        // Fragment (row y, columns 2c, 2c+1 of group j) -> box (j / 4, y / 32), row y % 32, 16-byte chunk
+        // (2 (j % 4) + c / 2) ^ (y % 8): the eight rows of a warp store land in eight different chunks.
+        constexpr int CW = NT < MG_STG_COLS ? NT : MG_STG_COLS;        // columns per staged half
+        int rt[2];
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int r = rbase + 16 * wq + (lane >> 2) + 8 * half;
-            if (r >= L.n_rows) continue;
-            const int rt = r % L.P_m;
-            float *orow = L.out + (size_t)r * L.up * L.ld_out + L.c_off;
+        for (int half = 0; half < 2; ++half) rt[half] = (rbase + 16 * wq + (lane >> 2) + 8 * half) % L.P_m;
+        const uint32_t row_off = (uint32_t)(wq >> 1) * MG_BOX_BYTES + (uint32_t)(16 * (wq & 1) + (lane >> 2)) * 128u;
+        const uint32_t sub = (uint32_t)(lane & 1) * 8u;
 #pragma unroll
-            for (int j0 = 0; j0 < NT / 8; j0 += EB) {
-                float2 bb[EB];
+        for (int h = 0; h < NT / CW; ++h) {
+            mbar_wait(staging_free, (nstg & 1) ^ 1);                   // the store warp has read the previous half
 #pragma unroll
-                for (int u = 0; u < EB; ++u) {
-                    const int n = n_tile * NT + 8 * (j0 + u) + 2 * (lane & 3);
-                    bb[u] = __ldg((const float2 *)(bias + min(n, ncols - 2)));
-                }
+            for (int cb = 0; cb < CW / 32; ++cb) {
+                const int jj = (n_tile * NT + h * CW + 32 * cb) / L.Cout;
+                bool keep[2];
 #pragma unroll
-                for (int u = 0; u < EB; ++u) {
-                    const int j = j0 + u;
-                    const int n = n_tile * NT + 8 * j + 2 * (lane & 3);   // even; a pair never crosses a Cout boundary
-                    if (n >= ncols) continue;
-                    const int jj = n / L.Cout, co = n - jj * L.Cout;
-                    float2 o = make_float2(0.f, 0.f);
-                    if (rt < L.T_out && rt * L.up + jj < L.T_store) {
-                        o = make_float2(acc[4 * j + 2 * half] + bb[u].x, acc[4 * j + 2 * half + 1] + bb[u].y);
-                        if (L.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
-                        if (L.round_out) { o.x = to_tf32(o.x); o.y = to_tf32(o.y); }
+                for (int half = 0; half < 2; ++half)
+                    keep[half] = rt[half] < L.T_out && rt[half] * L.up + jj < L.T_store;
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const int j = h * (CW / 8) + cb * 4 + u;           // accumulator column group
+                    const float2 bb = *(const float2 *)(bias + 8 * j + 2 * (lane & 3));
+                    const uint32_t chunk = (uint32_t)((2 * u + ((lane & 3) >> 1)) ^ ((lane >> 2) & 7));
+#pragma unroll
+                    for (int half = 0; half < 2; ++half) {
+                        float2 o = make_float2(0.f, 0.f);
+                        if (keep[half]) {
+                            o = make_float2(acc[4 * j + 2 * half] + bb.x, acc[4 * j + 2 * half + 1] + bb.y);
+                            if (L.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                            if (L.round_out) { o.x = to_tf32(o.x); o.y = to_tf32(o.y); }
+                        }
+                        const uint32_t a = stg + (uint32_t)(2 * cb) * MG_BOX_BYTES + row_off + (uint32_t)half * 1024u +
+                                           (chunk << 4) + sub;
+                        asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(a), "f"(o.x), "f"(o.y) : "memory");
                     }
-                    *(float2 *)(orow + jj * L.ld_out + co) = o;
                 }
             }
+            fence_proxy_async();                                       // generic smem writes -> the TMA unit
+            __syncwarp();
+            if (lane == 0) mbar_arrive(staged);
+            ++nstg;
         }
-        // publish: one count per consumer warp once its stores are visible at gpu scope
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) red_release_gpu_add(flags + L.flag_base + m_tile, 1);
         if (dbg && lane == 0) dbg[3] = clock64();
         return;
     }
@@ -279,19 +315,24 @@ fcn_mega_kernel(const __grid_constant__ MegaParams P) {
     const fcn_mega_args &p = P.a;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t *smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-    uint8_t *ring = smem;
+    uint8_t *ring = smem + MG_OFF_RING;
+    const uint32_t stg0 = smem_u32(smem);           // staging buffer of warpgroup wg at stg0 + wg * MG_STG_BYTES
     uint64_t *bars = (uint64_t *)(smem + MG_OFF_BAR);
     uint64_t *full = bars, *empty = bars + MG_MAX_SLOTS;
     uint64_t *job_full = bars + 2 * MG_MAX_SLOTS, *job_empty = job_full + MG_JOBQ, *taken = job_empty + MG_JOBQ;
+    uint64_t *staged = taken + 1, *staging_free = staged + 2;
     fcn_mega_job *jobq = (fcn_mega_job *)(smem + MG_OFF_JOBQ);
+    float *bias_q = (float *)(smem + MG_OFF_BIAS);  // bias slice of queue entry i at bias_q + MG_BIAS_FLOATS i
     const fcn_mega_layer *s_layers = P.layers;      // kernel parameters (constant bank)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
         for (int i = 0; i < MG_MAX_SLOTS; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], MG_MMA_WARPS); }
-        // a queue entry is read by the 8 consumer warps and the TMA lane
-        for (int i = 0; i < MG_JOBQ; ++i) { mbar_init(&job_full[i], 1); mbar_init(&job_empty[i], MG_MMA_WARPS + 1); }
+        // a queue entry is read by the 8 consumer warps, the TMA lane and the store warp; the consumers release it
+        // after their epilogue, which reads the entry's bias slice
+        for (int i = 0; i < MG_JOBQ; ++i) { mbar_init(&job_full[i], 1); mbar_init(&job_empty[i], MG_MMA_WARPS + 2); }
         mbar_init(taken, 1);
+        for (int i = 0; i < 2; ++i) { mbar_init(&staged[i], 4); mbar_init(&staging_free[i], 1); }
         fence_barrier_init();
     }
     __syncthreads();
@@ -369,7 +410,10 @@ fcn_mega_kernel(const __grid_constant__ MegaParams P) {
                     mbar_wait(&empty[st], ph ^ 1);
                     if (dbg) t_empty += clock64() - t0;
                     uint8_t *sl = ring + st * slot_bytes;
-                    mbar_arrive_expect_tx(&full[st], MG_A_ATOM + w_bytes);
+                    // the job's bias slice rides on its first stage (the consumers read it in the epilogue)
+                    const bool with_bias = s == 0 && !L.is_heads;
+                    mbar_arrive_expect_tx(&full[st], MG_A_ATOM + w_bytes + (with_bias ? L.NT * 4 : 0));
+                    if (with_bias) bulk_g2s(bias_q + MG_BIAS_FLOATS * slot, L.bias + n_tile * L.NT, L.NT * 4, &full[st]);
                     bulk_g2s(sl + MG_A_ATOM, wsrc + (size_t)s * w_bytes, w_bytes, &full[st]);
                     if (seg < L.n_seg) {
                         const fcn_mega_seg &sgm = L.seg[seg];
@@ -383,29 +427,83 @@ fcn_mega_kernel(const __grid_constant__ MegaParams P) {
                 if (dbg) { dbg[4] = clock64(); dbg[5] = t_empty; }
             }
         }
+    } else if (warp == MG_STORE_WARP) {
+        // ================= store warp (one lane): staged tiles -> TMA stores -> tile counter =================
+        // Waits only on the job queue (an entry is full before the consumers start that job), on this CTA's
+        // consumers (`staged`) and on its own bulk groups.
+        if (lane == 0) {
+            uint32_t nstg[2] = {0, 0};               // halves received per warpgroup (parity of `staged`)
+            for (uint32_t q = 0;; ++q) {
+                const uint32_t slot = q % MG_JOBQ;
+                mbar_wait(&job_full[slot], (q / MG_JOBQ) & 1);
+                const int layer = jobq[slot].layer, m_tile = jobq[slot].m_tile, n_tile = jobq[slot].n_tile;
+                mbar_arrive(&job_empty[slot]);
+                if (layer < 0) break;
+                const fcn_mega_layer &L = s_layers[layer];
+                if (L.is_heads) continue;            // the heads epilogue stores and publishes by itself
+                long long *dbg = mg_dbg_row(p, q);
+                const void *map = &P.maps[L.out_map];
+                const int cw = L.NT < MG_STG_COLS ? L.NT : MG_STG_COLS, ncols = L.up * L.Cout;
+                for (int h = 0; h < L.NT / cw; ++h) {
+                    for (int wg = 0; wg < 2; ++wg) {
+                        mbar_wait(&staged[wg], nstg[wg]++ & 1);
+                        if (dbg && h == 0 && wg == 0) dbg[20] = clock64();
+                        const int row0 = m_tile * MG_ROWS + 64 * wg;
+                        const uint32_t src = stg0 + (uint32_t)wg * MG_STG_BYTES;
+                        for (int cb = 0; cb < cw / 32; ++cb) {
+                            const int n0 = n_tile * L.NT + h * cw + 32 * cb;   // columns past up*Cout: padding
+                            if (n0 >= ncols) break;
+                            const int jj = n0 / L.Cout, c = jj * L.ld_out + L.c_off + (n0 - jj * L.Cout);
+                            for (int rb = 0; rb < 2; ++rb)
+                                if (row0 + 32 * rb < L.n_rows)
+                                    mg_tma_store_3d(map, src + (uint32_t)(2 * cb + rb) * MG_BOX_BYTES, c, row0 + 32 * rb, 0);
+                        }
+                        bulk_commit();
+                        bulk_wait_read_all();        // the TMA unit has read the buffer: the warpgroup may refill it
+                        mbar_arrive(&staging_free[wg]);
+                    }
+                }
+                if (dbg) dbg[21] = clock64();
+                // the tile's stores are complete; async-proxy writes -> generic release -> the dependent tiles'
+                // acquire + fence.proxy.async.global before their TMA loads
+                bulk_wait_all();
+                fence_proxy_async_global();
+                red_release_gpu_add(flags + L.flag_base + m_tile, 1);
+                if (dbg) dbg[22] = clock64();
+            }
+        }
     } else {
-        // ================= consumer warpgroups: MMA + epilogue of every job, 64 rows each =================
-        uint32_t st = 0, ph = 0;
+        // ================= consumer warpgroups: MMA + epilogue staging of every job, 64 rows each ===========
+        const int wg = warp >> 2;
+        uint32_t st = 0, ph = 0, nstg = 0;
+        const uint32_t stg = stg0 + (uint32_t)wg * MG_STG_BYTES;
         for (uint32_t q = 0;; ++q) {
             const uint32_t slot = q % MG_JOBQ;
             mbar_wait(&job_full[slot], (q / MG_JOBQ) & 1);
             const int layer = jobq[slot].layer, m_tile = jobq[slot].m_tile, n_tile = jobq[slot].n_tile;
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&job_empty[slot]);
             if (layer < 0) break;
             const fcn_mega_layer &L = s_layers[layer];
             long long *dbg = (warp & 3) == 0 ? mg_dbg_row(p, q) : nullptr;   // warp 0 of each warpgroup
-            if (dbg) dbg += 6 + 4 * (warp >> 2);
-            if (L.NT == 256) mg_job<256>(P, L, m_tile, n_tile, st, ph, ring, full, empty, flags, dbg);
-            else if (L.NT == 128) mg_job<128>(P, L, m_tile, n_tile, st, ph, ring, full, empty, flags, dbg);
-            else mg_job<64>(P, L, m_tile, n_tile, st, ph, ring, full, empty, flags, dbg);
+            if (dbg) dbg += 6 + 4 * wg;
+            const float *bias = bias_q + MG_BIAS_FLOATS * slot;
+            if (L.NT == 256)
+                mg_job<256>(P, L, m_tile, n_tile, st, ph, ring, full, empty, stg, &staged[wg], &staging_free[wg], nstg,
+                            bias, flags, dbg);
+            else if (L.NT == 128)
+                mg_job<128>(P, L, m_tile, n_tile, st, ph, ring, full, empty, stg, &staged[wg], &staging_free[wg], nstg,
+                            bias, flags, dbg);
+            else
+                mg_job<64>(P, L, m_tile, n_tile, st, ph, ring, full, empty, stg, &staged[wg], &staging_free[wg], nstg,
+                           bias, flags, dbg);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&job_empty[slot]);   // descriptor and bias slice no longer needed
         }
     }
     if (p.n_out > 1) __threadfence_system();      // this thread's remote (NVLink) result stores, if any
     __syncthreads();
     // self-cleaning: the last CTA out resets the scheduler state for the next forward and, on the multi-GPU
     // path, raises this rank's epoch flag in every peer (all result rows were fenced at system scope above)
-    __shared__ int s_last;
+    int &s_last = *(int *)(bars + MG_NBAR);         // behind the barriers: no static shared memory
     if (tid == 0) {
         __threadfence();
         s_last = atomicAdd(done_ctas, 1) == (int)gridDim.x - 1;
@@ -446,6 +544,8 @@ extern "C" int fcn_mega_forward(const fcn_mega_args *args, fcn_stream_t stream) 
         const fcn_mega_layer &L = a.layers[i];
         FCN_REQUIRE((L.NT == 64 || L.NT == 128 || L.NT == 256) && L.k_atoms == mg_k_atoms(L.NT),
                     "layer tile width must be 64, 128 or 256, with k_atoms = 1 for 256 and 2 otherwise");
+        FCN_REQUIRE(L.is_heads || ((uintptr_t)L.bias & 15) == 0,
+                    "layer bias must be 16-byte aligned (its NT-column slices are bulk-copied)");
         nt_max = L.NT > nt_max ? L.NT : nt_max;
     }
     if (a.n_jobs == 0) return FCN_OK;

@@ -19,7 +19,7 @@ from typing import Dict, List, Sequence
 from . import _lib
 
 ROWS = 128
-EPI_WARPS = 8          # completion counts per finished tile (one per consumer warp)
+EPI_WARPS = 1          # completion counts per finished tile (the store warp publishes each tile once)
 
 
 class LayerDesc:

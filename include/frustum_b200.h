@@ -192,7 +192,10 @@ FCN_API int fcn_decode_eval(int B, int T, int pitch, int ld, int num_heading_bin
  *                 kernel parameters at launch, like the HOST layer table;
  *        sync   : DEVICE int32[4 + n_flags], zero-initialised ONCE by the caller; [0] job counter, [1] finished
  *                 CTAs, [2] epoch (forwards completed), [4..] per-(layer,row-tile) completion counters.  The
- *                 kernel resets [0],[1],[4..] itself at the end of every forward.
+ *                 kernel resets [0],[1],[4..] itself at the end of every forward.  A finished tile of a
+ *                 non-heads layer adds 1 to its row tile's counter, so a row tile of a layer with n_tiles_n column
+ *                 tiles is complete at n_tiles_n.
+ *      The bias of a non-heads layer is bulk-copied in NT-column slices and must be 16-byte aligned.
  *      Persistent CTAs fetch jobs with an atomic counter (deadlock-free under any co-residency, see fcn_mega.cu).
  *      The heads layer (is_heads) stores the logits row and decodes it in place into `n_out` output sets:
  *      outs[0] is the local 6-tuple block, outs[1..] are peer buffers (mapped NVLink peer memory) - the
@@ -216,7 +219,7 @@ typedef struct {
     int P_m, T_out, n_rows;      /* GEMM row space: row r = b*P_m + t, valid iff t < T_out; n_rows = B*P_m */
     int ld_out, P_store, T_store, c_off;
     int is_heads, flag_base;
-    int out_map;                 /* tensor map of the epilogue's TMA store (fcn_encode_store_map); unused for heads */
+    int out_map;                 /* tensor map of the epilogue's TMA stores (fcn_encode_store_map); unused for heads */
     int k_atoms;                 /* 32-wide K atoms per weight-image stage: 2 (NT <= 128) or 1 (NT = 256); the kernel
                                     streams n_stage * k_atoms stages of one atom each */
     const void *w_tc;            /* packed stage images, N-tile major */
@@ -239,8 +242,8 @@ typedef struct {
     int n_out, n_flag_out;
     fcn_decode_out outs[FCN_MAX_PEERS];
     int32_t *flag_out[FCN_MAX_PEERS];
-    long long *dbg_clocks;                 /* optional (NULL): phase timeline, 16 clocks per job for the first 64
-                                              jobs of every CTA (grid x 64 x 16 values; fcn_mega.cu) */
+    long long *dbg_clocks;                 /* optional (NULL): phase timeline, 32 clocks per job for the first 64
+                                              jobs of every CTA (grid x 64 x 32 values; fcn_mega.cu) */
 } fcn_mega_args;
 FCN_API int fcn_mega_forward(const fcn_mega_args *args, fcn_stream_t stream);
 

@@ -1,10 +1,14 @@
 """Phase timeline of the persistent FCN kernel (csrc/fcn_mega.cu) for one B = 32 forward in isolation.
 
 Runs one forward of each workload to fill the feature maps, then launches fcn_mega with `dbg_clocks` set (every
-CTA records 16 clocks per job for its first 64 jobs) and splits each consumer warpgroup's time per job into
+CTA records 32 clocks per job for its first 64 jobs) and splits each consumer warpgroup's time per job into
   full_wait   clocks waiting for operand stages (`full` barriers), the first stage of the job included,
   mma         the rest of the K loop up to the last retired MMA (MMA issue and execution),
-  epilogue    last MMA retired -> counter published,
+  epilogue    last MMA retired -> tile staged for the store warp (heads: rows decoded and counter published),
+and the store warp's time per tile:
+  store_issue first staged half received -> last box store issued (the rest of the staging included),
+  publish     last box store issued -> stores complete and the counter published,
+  store_lag   both warpgroups staged the tile -> counter published,
 and reports per layer the scheduler's dependency wait (fetched -> dependencies met), the TMA lane's wait for the
 next job descriptor (last box of the previous job -> job taken) and its `empty` waits.  All values are SM clocks,
 averaged over the recorded jobs of the layer (a CTA's first job is skipped: it has no previous epilogue).
@@ -22,6 +26,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 ROWS_PER_JOB = 64           # recorded jobs per CTA (MG_DBG_JOBS)
+ROW = 32                    # clocks per recorded job (MG_DBG_ROW)
 
 
 def timeline(workload, B, reps):
@@ -45,7 +50,7 @@ def timeline(workload, B, reps):
     assert m is not None, "the persistent FCN kernel is not selected for this workload"
     descs = plan.mega_descs()
     grid = plan.mega_grid
-    buf = torch.zeros(grid * ROWS_PER_JOB * 16, dtype=torch.int64, device="cuda")
+    buf = torch.zeros(grid * ROWS_PER_JOB * ROW, dtype=torch.int64, device="cuda")
     m.dbg_clocks = buf.data_ptr()
     try:
         for _ in range(reps):                      # the last launch is the one read back
@@ -54,7 +59,7 @@ def timeline(workload, B, reps):
         torch.cuda.synchronize()
     finally:
         m.dbg_clocks = None
-    rows = buf.cpu().numpy().reshape(grid, ROWS_PER_JOB, 16)
+    rows = buf.cpu().numpy().reshape(grid, ROWS_PER_JOB, ROW)
 
     per = {}
     for c in range(grid):
@@ -63,7 +68,8 @@ def timeline(workload, B, reps):
             if r[0] == 0 or pr[0] == 0:
                 continue
             d = per.setdefault(int(r[14]), dict(jobs=0, full_wait=0.0, mma=0.0, epilogue=0.0, dep_wait=0.0,
-                                                desc_wait=0.0, tma_empty_wait=0.0, job=0.0))
+                                                desc_wait=0.0, tma_empty_wait=0.0, job=0.0, stored=0,
+                                                store_issue=0.0, publish=0.0, store_lag=0.0))
             d["jobs"] += 1
             for wg in range(2):
                 o = 6 + 4 * wg
@@ -76,10 +82,18 @@ def timeline(workload, B, reps):
             d["dep_wait"] += r[3] - r[2]
             d["desc_wait"] += max(0, r[0] - pr[4])
             d["tma_empty_wait"] += r[5]
+            if r[22] != 0:                           # store warp (tiles of non-heads layers)
+                d["stored"] += 1
+                d["store_issue"] += r[21] - r[20]
+                d["publish"] += r[22] - r[21]
+                d["store_lag"] += r[22] - max(r[9], r[13])
     layers = []
     for li in sorted(per):
         d = per[li]
         n = d.pop("jobs")
+        ns = max(1, d.pop("stored"))
+        for k in ("store_issue", "publish", "store_lag"):
+            d[k] *= n / ns                           # averaged over the stored tiles below
         L = descs[li]
         stages = L.K_pad // 32
         out = {k: round(v / n) for k, v in d.items()}
@@ -109,8 +123,10 @@ def main():
         print(r["workload"], "grid", r["grid"], r["share_of_consumer_time"])
         for l in r["layers"]:
             print("  %-16s NT %3d stages %3d jobs %3d | mma/stage %5d full_wait %6d mma %6d epi %5d dep %6d desc %6d"
+                  " | store issue %5d publish %5d lag %5d"
                   % (l["layer"], l["NT"], l["k_stages"], l["jobs_recorded"], l["mma_clocks_per_stage"], l["full_wait"],
-                     l["mma"], l["epilogue"], l["dep_wait"], l["desc_wait"]))
+                     l["mma"], l["epilogue"], l["dep_wait"], l["desc_wait"], l["store_issue"], l["publish"],
+                     l["store_lag"]))
 
 
 if __name__ == "__main__":
