@@ -7,8 +7,9 @@ tensors, executed by csrc/train.cu:
     grouping (fcn_group_rows, all T*K rows incl. the reference's back-fill duplicates - they weight the batch
     statistics)  ->  per scale conv1..3 (+BN batch stats) -> mask + max over K -> FCN -> deconvs -> heads
 
-The losses stay PyTorch ops on the (B*T2, 2+39) logits (SURVEY.md 8-a6; ~320 rows); their autograd gives dlogits,
-from which ``backward`` runs the hand-written backward kernels.  Parameters live in ONE flat fp32 buffer (every
+``TrainStep`` takes the losses and dlogits of the (B*T2, 2+39) logits from the fused loss kernels (csrc/loss.cu), the
+drop-in ``model(data)`` path from PyTorch ops and their autograd (train_path.losses_from_logits); from dlogits
+``backward`` runs the hand-written backward kernels.  Parameters live in ONE flat fp32 buffer (every
 ``nn.Parameter`` is a view), gradients in ONE flat bucket written in the parameter layout by the kernels:
 one ``all_reduce`` per step (SURVEY.md 8(e)) and one fused optimizer launch (``fcn_adam_step`` or ``fcn_sgd_step``).
 BatchNorm statistics are per rank (the reference's DataParallel semantics: per-replica BN, no SyncBN).
@@ -52,6 +53,15 @@ class FlatParams:
             self.offsets[id(p)] = off
             off += k
         self.numel = n
+
+    @staticmethod
+    def of(model) -> "FlatParams":
+        """The model's bucket: created on first use and cached on the model, so every TrainStep and TrainEngine of
+        one model shares it."""
+        flat = getattr(model, "_flat_params", None)
+        if flat is None:
+            flat = model._flat_params = FlatParams(model)
+        return flat
 
     def gptr(self, p) -> int:
         return self.grad.data_ptr() + 4 * self.offsets[id(p)]
@@ -100,9 +110,7 @@ class TrainEngine:
         self.B, self.N, self.T = int(B), int(N), tuple(int(t) for t in T)
         self.dev = next(model.parameters()).device
         self.V = model.num_vec
-        self.flat = getattr(model, "_flat_params", None)
-        if self.flat is None:
-            self.flat = model._flat_params = FlatParams(model)
+        self.flat = FlatParams.of(model)
         dev, f32 = self.dev, torch.float32
         K = arch.nsample
         self.K = K
@@ -394,21 +402,59 @@ class TrainEngine:
         return n_fwd + n_bwd + 1      # + fused Adam or SGD
 
 
-def _one_group(opt, state_dict):
-    """-> (group, parameter ids, opt's parameters) of a loaded optimizer state that has the one parameter group over
-    all of the model's parameters that a fused step over the flat bucket takes; ValueError otherwise."""
-    groups = state_dict["param_groups"]
-    if len(groups) != 1:
-        raise ValueError("TrainStep.optimizer: the loaded state has %d parameter groups; the fused step takes "
-                         "exactly one (all parameters of the model)" % len(groups))
-    ids, params = groups[0]["params"], opt.param_groups[0]["params"]
-    if len(ids) != len(params):
-        raise ValueError("TrainStep.optimizer: the loaded state has %d parameters, the model has %d"
-                         % (len(ids), len(params)))
-    return groups[0], ids, params
+class _FlatOptimizer:
+    """What FlatAdam and FlatSGD share, mixed in before their torch optimizer class: one parameter group over all of
+    a model's parameters (FlatParams order) whose state lives in flat buffers of the bucket's layout, a
+    `load_state_dict` that checks the loaded state before the subclass adopts it into those buffers, and a `step`
+    that is ONE fused launch over the whole bucket.  A subclass supplies its flat buffers (`_flat_state`), the checks
+    of the group settings (`_check_group`) and of the loaded per-parameter state (`_check_states`), `_adopt_loaded`
+    and the launch (`_launch`)."""
+
+    def __init__(self, model, flat, **hyper):
+        super().__init__(list(model.parameters()), **hyper)
+        self.model, self.flat = model, flat
+        self.step_count = 0
+        self.grad_scale = 1.0          # multiplies the gradient first: 1/world after a summing all-reduce
+        self.register_load_state_dict_pre_hook(type(self)._check_loaded)
+        self.register_load_state_dict_post_hook(type(self)._adopt_loaded)
+
+    def _views(self):
+        """-> (parameter, its view of each flat state buffer) for every parameter."""
+        bufs = self._flat_state()
+        for p in self.param_groups[0]["params"]:
+            off, n = self.flat.offsets[id(p)], p.numel()
+            yield (p,) + tuple(b[off: off + n].view(p.shape) for b in bufs)
+
+    def _check_loaded(self, state_dict):
+        """ValueError unless the loaded state has the one parameter group over all of the model's parameters that a
+        fused step over the flat bucket takes, with settings and per-parameter state that step can continue."""
+        groups = state_dict["param_groups"]
+        if len(groups) != 1:
+            raise ValueError("TrainStep.optimizer: the loaded state has %d parameter groups; the fused step takes "
+                             "exactly one (all parameters of the model)" % len(groups))
+        ids, params = groups[0]["params"], self.param_groups[0]["params"]
+        if len(ids) != len(params):
+            raise ValueError("TrainStep.optimizer: the loaded state has %d parameters, the model has %d"
+                             % (len(ids), len(params)))
+        self._check_group(groups[0])
+        self._check_states(state_dict["state"], ids, params)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        """One step of every parameter from the gradient in the flat bucket (``TrainStep.forward_backward`` leaves it
+        there)."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        g = self.param_groups[0]
+        self._check_group(g)
+        self.model.refresh()       # parameters change behind autograd's version counters: eval pack must rebuild
+        self._launch(g)
+        return loss
 
 
-class FlatAdam(torch.optim.Adam):
+class FlatAdam(_FlatOptimizer, torch.optim.Adam):
     """``torch.optim.Adam`` over a model's parameters (one param group, FlatParams order) whose state is the flat
     bucket: each parameter's ``exp_avg`` / ``exp_avg_sq`` are views of two flat buffers and the step count is shared,
     so `state_dict` / `load_state_dict` speak torch's own format (the reference's checkpoints,
@@ -418,21 +464,14 @@ class FlatAdam(torch.optim.Adam):
     `state_dict`; ``step_count`` is the live value."""
 
     def __init__(self, model, flat, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
-        super().__init__(list(model.parameters()), lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
-        self.model, self.flat = model, flat
+        super().__init__(model, flat, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
         self.exp_avg = torch.zeros_like(flat.param)
         self.exp_avg_sq = torch.zeros_like(flat.param)
-        self.step_count = 0
-        self.grad_scale = 1.0          # multiplies the gradient first: 1/world after a summing all-reduce
         self._bind()
         self.register_state_dict_pre_hook(FlatAdam._sync_steps)
-        self.register_load_state_dict_pre_hook(FlatAdam._check_loaded)
-        self.register_load_state_dict_post_hook(FlatAdam._adopt_loaded)
 
-    def _views(self):
-        for p in self.param_groups[0]["params"]:
-            off, n = self.flat.offsets[id(p)], p.numel()
-            yield p, self.exp_avg[off: off + n].view(p.shape), self.exp_avg_sq[off: off + n].view(p.shape)
+    def _flat_state(self):
+        return self.exp_avg, self.exp_avg_sq
 
     def _bind(self):
         for p, m, v in self._views():
@@ -450,13 +489,10 @@ class FlatAdam(torch.optim.Adam):
         for p in opt.param_groups[0]["params"]:
             opt.state[p]["step"] = torch.tensor(float(opt.step_count))
 
-    @staticmethod
-    def _check_loaded(opt, state_dict):
-        group, ids, params = _one_group(opt, state_dict)
-        FlatAdam._check_group(group)
+    def _check_states(self, states, ids, params):
         steps = set()
         for i, (k, p) in enumerate(zip(ids, params)):
-            st = state_dict["state"].get(k)
+            st = states.get(k)
             if not st:
                 steps.add(0.0)
                 continue
@@ -472,12 +508,11 @@ class FlatAdam(torch.optim.Adam):
             raise ValueError("TrainStep.optimizer: the loaded per-parameter step counts differ (%s); the fused step "
                              "keeps one count for all parameters" % sorted(steps))
 
-    @staticmethod
     @torch.no_grad()
-    def _adopt_loaded(opt):
+    def _adopt_loaded(self):
         step = 0
-        for p, m, v in opt._views():
-            st = opt.state.get(p)
+        for p, m, v in self._views():
+            st = self.state.get(p)
             if st:
                 m.copy_(st["exp_avg"])
                 v.copy_(st["exp_avg_sq"])
@@ -485,30 +520,19 @@ class FlatAdam(torch.optim.Adam):
             else:
                 m.zero_()
                 v.zero_()
-        opt.step_count = step
-        opt._bind()
+        self.step_count = step
+        self._bind()
 
-    @torch.no_grad()
-    def step(self, closure=None):
-        """One Adam step of every parameter from the gradient in the flat bucket (``TrainStep.forward_backward``
-        leaves it there)."""
-        loss = None
-        if closure is not None:
-            with torch.enable_grad():
-                loss = closure()
-        g = self.param_groups[0]
-        FlatAdam._check_group(g)
+    def _launch(self, g):
         b1, b2 = g["betas"]
         self.step_count += 1
-        self.model.refresh()       # parameters change behind autograd's version counters: eval pack must rebuild
         f = self.flat
         _lib.call("fcn_adam_step", _ptr(f.param), _ptr(f.grad), _ptr(self.exp_avg), _ptr(self.exp_avg_sq), f.numel,
                   float(g["lr"]), float(b1), float(b2), float(g["eps"]), float(g["weight_decay"]), self.step_count,
                   float(self.grad_scale), _stream())
-        return loss
 
 
-class FlatSGD(torch.optim.SGD):
+class FlatSGD(_FlatOptimizer, torch.optim.SGD):
     """``torch.optim.SGD`` over a model's parameters (one param group, FlatParams order) whose state is the flat
     bucket: each parameter's ``momentum_buffer`` is a view of one flat buffer, so `state_dict` / `load_state_dict`
     speak torch's own format while `step` is ONE ``fcn_sgd_step`` launch over the whole bucket.  `step` reads lr,
@@ -519,19 +543,12 @@ class FlatSGD(torch.optim.SGD):
     has no step count to restore it from."""
 
     def __init__(self, model, flat, lr=1e-3, momentum=0.0, weight_decay=0.0):
-        super().__init__(list(model.parameters()), lr=lr, momentum=momentum, weight_decay=weight_decay)
-        self.model, self.flat = model, flat
+        super().__init__(model, flat, lr=lr, momentum=momentum, weight_decay=weight_decay)
         self.momentum_buffer = torch.zeros_like(flat.param)
         self.has_buffers = False
-        self.step_count = 0
-        self.grad_scale = 1.0          # multiplies the gradient first: 1/world after a summing all-reduce
-        self.register_load_state_dict_pre_hook(FlatSGD._check_loaded)
-        self.register_load_state_dict_post_hook(FlatSGD._adopt_loaded)
 
-    def _views(self):
-        for p in self.param_groups[0]["params"]:
-            off, n = self.flat.offsets[id(p)], p.numel()
-            yield p, self.momentum_buffer[off: off + n].view(p.shape)
+    def _flat_state(self):
+        return (self.momentum_buffer,)
 
     def _bind(self):
         self.state.clear()
@@ -548,13 +565,10 @@ class FlatSGD(torch.optim.SGD):
             raise ValueError("TrainStep.optimizer: %s is set; the fused step (fcn_sgd_step) is plain SGD with momentum "
                              "and L2 weight decay" % " / ".join(bad))
 
-    @staticmethod
-    def _check_loaded(opt, state_dict):
-        group, ids, params = _one_group(opt, state_dict)
-        FlatSGD._check_group(group)
+    def _check_states(self, states, ids, params):
         with_buffer = 0
         for i, (k, p) in enumerate(zip(ids, params)):
-            st = state_dict["state"].get(k) or {}
+            st = states.get(k) or {}
             other = sorted(set(st) - {"momentum_buffer"})
             if other:
                 raise ValueError("TrainStep.optimizer: parameter %d: the loaded state has %s (not an SGD state)"
@@ -570,33 +584,22 @@ class FlatSGD(torch.optim.SGD):
             raise ValueError("TrainStep.optimizer: the loaded state has momentum buffers on %d of %d parameters; the "
                              "fused step keeps buffers for all parameters or none" % (with_buffer, len(params)))
 
-    @staticmethod
     @torch.no_grad()
-    def _adopt_loaded(opt):
-        loaded = [opt.state.get(p, {}).get("momentum_buffer") for p in opt.param_groups[0]["params"]]
-        opt.has_buffers = loaded[0] is not None        # _check_loaded admits buffers on all parameters or on none
-        if opt.has_buffers:
+    def _adopt_loaded(self):
+        loaded = [self.state.get(p, {}).get("momentum_buffer") for p in self.param_groups[0]["params"]]
+        self.has_buffers = loaded[0] is not None       # _check_loaded admits buffers on all parameters or on none
+        if self.has_buffers:
             # each source onto its own view: a source may BE that view (torch keeps a loaded tensor that already has
             # the parameter's dtype and device, as in opt.load_state_dict(opt.state_dict())), so nothing is zeroed first
-            for (p, b), src in zip(opt._views(), loaded):
+            for (p, b), src in zip(self._views(), loaded):
                 b.copy_(src)
         else:
-            opt.momentum_buffer.zero_()
-        opt._bind()
+            self.momentum_buffer.zero_()
+        self._bind()
 
-    @torch.no_grad()
-    def step(self, closure=None):
-        """One SGD step of every parameter from the gradient in the flat bucket (``TrainStep.forward_backward``
-        leaves it there)."""
-        loss = None
-        if closure is not None:
-            with torch.enable_grad():
-                loss = closure()
-        g = self.param_groups[0]
-        FlatSGD._check_group(g)
+    def _launch(self, g):
         momentum = float(g["momentum"])
         first = not self.has_buffers
-        self.model.refresh()       # parameters change behind autograd's version counters: eval pack must rebuild
         f = self.flat
         _lib.call("fcn_sgd_step", _ptr(f.param), _ptr(f.grad), _ptr(self.momentum_buffer), f.numel, float(g["lr"]),
                   momentum, float(g["weight_decay"]), int(first), float(self.grad_scale), _stream())
@@ -604,19 +607,18 @@ class FlatSGD(torch.optim.SGD):
         if momentum != 0 and first:
             self.has_buffers = True
             self._bind()
-        return loss
 
 
 class TrainStep:
-    """One optimizer step of PointNetDet on the hand-written kernels: forward -> losses (PyTorch ops on the logits)
-    -> backward kernels -> ONE all-reduce of the flat gradient bucket (when torch.distributed is initialised and
-    world > 1) -> fused Adam or SGD.  Mirrors train/train_net_det.py:121-134 (zero_grad / backward / step and the
-    TrainingStates update).  ``optimizer`` ("adam" or "sgd", the values of cfg.TRAIN.OPTIMIZER,
+    """One optimizer step of PointNetDet on the hand-written kernels: forward -> fused losses and d/dlogits
+    (``fcn_det_loss``) -> backward kernels -> ONE all-reduce of the flat gradient bucket (when torch.distributed is
+    initialised and world > 1) -> fused Adam or SGD.  Mirrors train/train_net_det.py:121-134 (zero_grad / backward /
+    step and the TrainingStates update).  ``optimizer`` ("adam" or "sgd", the values of cfg.TRAIN.OPTIMIZER,
     train_net_det.py:321-328) selects a torch.optim.Adam (FlatAdam) or torch.optim.SGD (FlatSGD, with ``momentum``)
     for lr schedulers and checkpoints; ``states`` (validate.TrainStates) collects every step's losses and metrics on
     the device.  ``deterministic`` (settable): True runs the step bit-reproducibly (deterministic layer kernels and
     fused loss; one GPU, one build, same inputs and hyper-parameters), False the default kernels, None follows
-    ``torch.use_deterministic_algorithms`` at every step.  True requires ``loss_impl == "kernel"``."""
+    ``torch.use_deterministic_algorithms`` at every step."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, comm_stream=None,
                  states_capacity=None, optimizer="adam", momentum=0.0, deterministic=None):
@@ -626,9 +628,7 @@ class TrainStep:
                              % (optimizer,))
         self.model = model
         self.engines: Dict[tuple, TrainEngine] = {}
-        self.flat = getattr(model, "_flat_params", None)
-        if self.flat is None:
-            self.flat = model._flat_params = FlatParams(model)
+        self.flat = FlatParams.of(model)
         if optimizer == "adam":
             self.optimizer = FlatAdam(model, self.flat, lr, betas, eps, weight_decay)
         else:
@@ -636,11 +636,13 @@ class TrainStep:
         self.states = TrainStates(self.flat.param.device, states_capacity)
         self._comm = None
         self._split = 0
-        self._loss_graphs = {}
-        # losses + d/dlogits: "kernel" = fused hand-written kernels (csrc/loss.cu), "graph" = the PyTorch ops as one
-        # CUDA graph (train_path.LossGraph), "eager" = the reference-shaped PyTorch ops
-        self.loss_impl = "kernel"
+        self._fused_losses = {}        # train_path.FusedLoss per (deterministic, B, T2)
         self.deterministic = deterministic
+
+    @property
+    def loss_impl(self):
+        """How the losses and d/dlogits are computed: "kernel", the fused kernels of csrc/loss.cu."""
+        return "kernel"
 
     @property
     def lr(self):
@@ -679,14 +681,6 @@ class TrainStep:
     def step_count(self):
         return self.optimizer.step_count
 
-    def _mode(self) -> bool:
-        """This step's mode: ``deterministic``, or torch's flag when it is None."""
-        from .train_path import deterministic_mode
-        if self.deterministic is True and self.loss_impl != "kernel":
-            raise ValueError("TrainStep: deterministic=True needs loss_impl='kernel' (the fused loss); loss_impl=%r "
-                             "runs PyTorch ops, which follow torch.use_deterministic_algorithms" % (self.loss_impl,))
-        return deterministic_mode(self.deterministic)
-
     def engine(self, B, N, T, deterministic=False) -> TrainEngine:
         key = (int(B), int(N), tuple(int(t) for t in T), bool(deterministic))
         e = self.engines.get(key)
@@ -694,45 +688,37 @@ class TrainStep:
             e = self.engines[key] = TrainEngine(self.model, *key[:3], deterministic=key[3])
         return e
 
-    @staticmethod
-    def _fused_loss_key(eng):
-        return ("kernel-deterministic" if eng.deterministic else "kernel", eng.B, eng.T2)
+    def _fused_loss(self, eng):
+        from .train_path import FusedLoss
+        key = (eng.deterministic, eng.B, eng.T2)
+        fl = self._fused_losses.get(key)
+        if fl is None:
+            fl = self._fused_losses[key] = FusedLoss(self.model, eng.B, eng.T2, eng.act["reg_out"]["cols"], eng.dev,
+                                                     eng.deterministic)
+        return fl
 
     def _losses(self, eng, cls, reg, center_ref2, data):
         """-> (losses, metrics, dcls, dreg)."""
-        from .train_path import FusedLoss, LossGraph, losses_from_logits
-        if self.loss_impl == "kernel":
-            key = self._fused_loss_key(eng)
-            lg = self._loss_graphs.get(key)
-            if lg is None:
-                lg = self._loss_graphs[key] = FusedLoss(self.model, eng.B, eng.T2, reg.shape[1], cls.device,
-                                                        eng.deterministic)
-            return lg.run(cls, reg, center_ref2, data)
-        if self.loss_impl == "graph":
-            key = ("graph", eng.B, eng.T2)
-            lg = self._loss_graphs.get(key)
-            if lg is None:
-                lg = self._loss_graphs[key] = LossGraph(self.model, eng.B, eng.T2, reg.shape[1], cls.device)
-            return lg.run(cls, reg, center_ref2, data)
-        cls_l = cls.detach().clone().requires_grad_(True)
-        reg_l = reg.detach().clone().requires_grad_(True)
-        losses, metrics = losses_from_logits(self.model, cls_l, reg_l, center_ref2, data)
-        losses["total_loss"].backward()
-        return losses, metrics, cls_l.grad, reg_l.grad
+        return self._fused_loss(eng).run(cls, reg, center_ref2, data)
+
+    def _forward_losses(self, data):
+        """This step's engine (shape and mode), a zeroed gradient bucket, the forward and the losses -> (engine,
+        losses, metrics, dcls, dreg)."""
+        from .train_path import deterministic_mode
+        S = self.model.ARCH.num_scales
+        pc = data["point_cloud"][:, :3, :].contiguous()
+        centers = [data["center_ref%d" % (i + 1)].contiguous() for i in range(S)]
+        eng = self.engine(pc.shape[0], pc.shape[2], [c.shape[2] for c in centers],
+                          deterministic_mode(self.deterministic))
+        self.flat.grad.zero_()
+        cls, reg = eng.forward(pc, centers, data.get("one_hot"))
+        return (eng,) + self._losses(eng, cls, reg, centers[1], data)
 
     def forward_backward(self, data, update_running=True):
         """-> (losses, metrics); gradients (this rank's) are left in the flat bucket."""
-        from .train_path import losses_from_logits
-        model = self.model
-        S = model.ARCH.num_scales
-        pc = data["point_cloud"][:, :3, :].contiguous()
-        centers = [data["center_ref%d" % (i + 1)].contiguous() for i in range(S)]
-        eng = self.engine(pc.shape[0], pc.shape[2], [c.shape[2] for c in centers], self._mode())
-        self.flat.grad.zero_()
-        cls, reg = eng.forward(pc, centers, data.get("one_hot"))
-        losses, metrics, dcls, dreg = self._losses(eng, cls, reg, centers[1], data)
+        eng, losses, metrics, dcls, dreg = self._forward_losses(data)
         eng.backward(dcls, dreg, update_running=update_running)
-        self.flat.expose_grads(model)
+        self.flat.expose_grads(self.model)
         return losses, metrics
 
     def step(self, data):
@@ -740,21 +726,13 @@ class TrainStep:
         TWO pieces on a communication stream: the FCN + heads part (92 % of the parameters, complete after the
         first ~15 % of the backward) overlaps the PointNet backward; the PointNet part follows."""
         import torch.distributed as dist
-        from .train_path import losses_from_logits
         world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-        model = self.model
-        S = model.ARCH.num_scales
-        pc = data["point_cloud"][:, :3, :].contiguous()
-        centers = [data["center_ref%d" % (i + 1)].contiguous() for i in range(S)]
-        eng = self.engine(pc.shape[0], pc.shape[2], [c.shape[2] for c in centers], self._mode())
-        self.flat.grad.zero_()
-        cls, reg = eng.forward(pc, centers, data.get("one_hot"))
-        losses, metrics, dcls, dreg = self._losses(eng, cls, reg, centers[1], data)
-        self.states.append(self._state_block(eng, losses, metrics, data), eng.B)
+        eng, losses, metrics, dcls, dreg = self._forward_losses(data)
+        self.states.append(self._fused_loss(eng).out, eng.B)     # fcn_det_loss's 16-float result block as it stands
         if world > 1:
             if self._comm is None:
                 self._comm = torch.cuda.Stream(device=self.flat.grad.device)
-                first = next(model.conv_net.parameters())
+                first = next(self.model.conv_net.parameters())
                 self._split = self.flat.offsets[id(first)]        # [0, split): feat_net, [split, n): conv_net + heads
             cur = torch.cuda.current_stream()
             eng.backward(dcls, dreg, stage="fcn")
@@ -775,13 +753,3 @@ class TrainStep:
         self.optimizer.grad_scale = 1.0 / world
         self.optimizer.step()
         return losses, metrics
-
-    def _state_block(self, eng, losses, metrics, data):
-        """The step's 16-float block for ``states``: fcn_det_loss's result as it stands, or the same layout stacked
-        on the device from the PyTorch losses (loss_impl "graph" / "eager")."""
-        if self.loss_impl == "kernel":
-            return self._loss_graphs[self._fused_loss_key(eng)].out
-        vals = {**losses, **metrics}
-        lab = data["cls_label"]
-        return torch.stack([vals[k].detach().reshape(()).float() for k in self.states.keys] +
-                           [(lab == 1).sum().float(), (lab != -1).sum().float()])

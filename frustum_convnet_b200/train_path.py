@@ -260,162 +260,9 @@ def losses_from_logits(model, cls_scores, outputs, center_ref2, data):
     return losses, metrics
 
 
-# ------------------------------------------------------------------ static-shape losses (CUDA-graph capturable)
-def losses_masked(model, cls_scores, outputs, ref2, lab, center_label, heading_label, size_label, size_class,
-                  mean_size, bidx, iou_fn=None):
-    """Same value as ``losses_from_logits`` (det_base.py:414-525) with foreground WEIGHTS instead of the
-    reference's ``nonzero()`` row selection: every tensor keeps the static shape (B*T2, ...), there is no host
-    sync, so losses + their autograd backward can be captured in one CUDA graph.  Means over the foreground rows
-    become  sum(w * term) / sum(w)."""
-    cfg = get_cfg()
-    nb, ns = model.num_bins, model.num_size_cluster
-    fg = lab == 1
-    w = fg.float()
-    nfg = w.sum().clamp(min=1.0)
-    zero = torch.zeros((), dtype=cls_scores.dtype, device=cls_scores.device)
-
-    def fg_mean(v):
-        return torch.where(fg, v, zero).sum() / nfg
-
-    cls_probs = F.softmax(cls_scores, -1)
-    keep = lab != -1
-    alpha_t = 0.75 * (lab == 0).float() + 0.25 * (lab >= 1).float()
-    p_t = torch.gather(cls_probs, 1, lab.clamp(min=0).unsqueeze(1)).squeeze(1)
-    focal = -alpha_t * (1 - p_t) ** 2 * torch.log(p_t + 1e-14)
-    cls_loss = torch.where(keep, focal, zero).sum() / ((lab > 0).sum() + 1e-14)
-
-    ctr, h_sc, h_res, s_sc, s_res = slice_output(outputs, nb, ns)
-    h_pr, s_pr = F.softmax(h_sc, -1), F.softmax(s_sc, -1)
-    center_l, heading_l = center_label[bidx], heading_label.view(-1)[bidx]
-    size_l, size_c = size_label[bidx], size_class.view(-1)[bidx]
-    center_gt = center_l - ref2
-    h_cls, h_res_lab = angle_encode(heading_l, nb)
-    ex = mean_size[size_c]
-    s_res_lab = (size_l - ex) / ex
-
-    def huber_rows(err, delta):
-        a = err.abs()
-        q = torch.clamp(a, max=delta)
-        return 0.5 * q * q + delta * (a - q)
-
-    center_loss = fg_mean(huber_rows(torch.norm(center_gt - ctr, 2, dim=-1), 3.0))
-    head_cls_loss = fg_mean(F.cross_entropy(h_sc, h_cls, reduction="none"))
-    head_res_loss = fg_mean(huber_rows(torch.gather(h_res, 1, h_cls.view(-1, 1)).squeeze(1) - h_res_lab, 1.0))
-    size_cls_loss = fg_mean(F.cross_entropy(s_sc, size_c, reduction="none"))
-    s_sel = torch.gather(s_res, 1, size_c.view(-1, 1, 1).expand(-1, 1, 3)).squeeze(1)
-    size_res_loss = fg_mean(huber_rows(torch.norm(s_res_lab - s_sel, 2, dim=-1), 1.0))
-
-    center_preds = ref2 + ctr
-    heading = angle_decode(h_res, h_cls, nb)
-    size = size_decode(s_res, mean_size, size_c)
-    c_gt = box_corners(center_l, heading_l, size_l)
-    c_flip = box_corners(center_l, heading_l + np.pi, size_l)
-    c_pred = box_corners(center_preds, heading, size)
-    corner_dist = torch.min(torch.norm(c_pred - c_gt, 2, dim=-1).mean(-1),
-                            torch.norm(c_pred - c_flip, 2, dim=-1).mean(-1))
-    corners_loss = fg_mean(huber_rows(corner_dist, 1.0))
-
-    L = cfg.LOSS
-    loss = cls_loss + L.BOX_LOSS_WEIGHT * (center_loss + head_cls_loss + size_cls_loss +
-                                           L.HEAD_REG_WEIGHT * head_res_loss +
-                                           L.SIZE_REG_WEIGHT * size_res_loss +
-                                           L.CORNER_LOSS_WEIGHT * corners_loss)
-    with torch.no_grad():
-        nkeep = keep.float().sum().clamp(min=1.0)
-        cls_prec = (torch.where(keep, (torch.argmax(cls_probs, -1) == lab), torch.zeros_like(keep))).float().sum() / nkeep
-        head_prec = fg_mean((torch.argmax(h_pr, -1) == h_cls).float())
-        size_prec = fg_mean((torch.argmax(s_pr, -1) == size_c).float())
-        if iou_fn is not None:
-            h_lab, s_lab = torch.argmax(h_pr, -1), torch.argmax(s_pr, -1)
-            c_metric = box_corners(center_preds, angle_decode(h_res, h_lab, nb), size_decode(s_res, mean_size, s_lab))
-            iou = iou_fn(c_metric, c_gt)                                   # (N, 2) per row, no host sync
-            iou2d, iou3d = fg_mean(iou[:, 0]), fg_mean(iou[:, 1])
-            iou3d_gt = fg_mean((iou[:, 1] >= cfg.IOU_THRESH).float())
-        else:
-            iou2d = iou3d = iou3d_gt = torch.full((), float("nan"), device=loss.device)
-    losses = {"total_loss": loss, "cls_loss": cls_loss, "center_loss": center_loss,
-              "head_cls_loss": head_cls_loss, "head_res_loss": head_res_loss,
-              "size_cls_loss": size_cls_loss, "size_res_loss": size_res_loss, "corners_loss": corners_loss}
-    metrics = {"cls_acc": cls_prec, "head_acc": head_prec, "size_acc": size_prec,
-               "IoU_2D": iou2d, "IoU_3D": iou3d, "IoU_" + str(cfg.IOU_THRESH): iou3d_gt}
-    return losses, metrics
-
-
-class LossGraph:
-    """Losses + their backward w.r.t. the head logits as ONE CUDA graph (static shapes via ``losses_masked``):
-    ~100 tiny PyTorch ops cost milliseconds of host time per step when issued eagerly,
-    a replay costs one launch.  Falls back to eager execution of the same function if capture is not possible."""
-
-    def __init__(self, model, B, T2, out_size, device):
-        from .box_iou import rbbox_iou_3d_pair
-        N, f32 = B * T2, torch.float32
-        self.model, self.N = model, N
-        self.cls = torch.zeros((N, 2), dtype=f32, device=device, requires_grad=True)
-        self.reg = torch.zeros((N, out_size), dtype=f32, device=device, requires_grad=True)
-        self.ref2 = torch.zeros((N, 3), dtype=f32, device=device)
-        self.lab = torch.zeros(N, dtype=torch.int64, device=device)
-        self.center = torch.zeros((B, 3), dtype=f32, device=device)
-        self.heading = torch.zeros((B, 1), dtype=f32, device=device)
-        self.size = torch.zeros((B, 3), dtype=f32, device=device)
-        self.size_class = torch.zeros((B, 1), dtype=torch.int64, device=device)
-        self.mean_size = torch.from_numpy(np.asarray(model.mean_size_array)).to(device=device, dtype=f32)
-        self.bidx = torch.arange(N, device=device) // T2
-        self.iou_fn = (lambda a, b: rbbox_iou_3d_pair(a, b)) if getattr(model, "gpu_iou_metrics", True) else None
-        self.graph = None
-        self.losses = self.metrics = None
-        self._tried = False
-
-    def _compute(self):
-        losses, metrics = losses_masked(self.model, self.cls, self.reg, self.ref2, self.lab, self.center, self.heading,
-                                        self.size, self.size_class, self.mean_size, self.bidx, self.iou_fn)
-        losses["total_loss"].backward()
-        return losses, metrics
-
-    def _capture(self):
-        self._tried = True
-        try:
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(3):
-                    self.cls.grad = self.reg.grad = None
-                    self._compute()
-            torch.cuda.current_stream().wait_stream(side)
-            self.cls.grad = self.reg.grad = None
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.losses, self.metrics = self._compute()
-            self.graph = g
-        except Exception as e:   # keep training possible: eager evaluation of the same static-shape function
-            import sys
-            sys.stderr.write("LossGraph: CUDA-graph capture failed (%r); running the loss ops eagerly\n" % (e,))
-            self.graph = None
-            torch.cuda.synchronize()
-
-    def run(self, cls, reg, center_ref2, data):
-        """-> (losses, metrics, dcls, dreg); the returned tensors are overwritten by the next call."""
-        with torch.no_grad():
-            self.cls.copy_(cls)
-            self.reg.copy_(reg)
-            self.ref2.copy_(center_ref2.permute(0, 2, 1).reshape(-1, 3))
-            self.lab.copy_(data["cls_label"].reshape(-1))
-            self.center.copy_(data["box3d_center"])
-            self.heading.copy_(data["box3d_heading"])
-            self.size.copy_(data["box3d_size"])
-            self.size_class.copy_(data["size_class"])
-        if self.graph is None and not self._tried:
-            self._capture()
-        if self.graph is not None:
-            self.graph.replay()
-        else:
-            self.cls.grad = self.reg.grad = None
-            self.losses, self.metrics = self._compute()
-        return self.losses, self.metrics, self.cls.grad, self.reg.grad
-
-
 class FusedLoss:
     """Losses, metrics and d(total_loss)/d(logits) by the fused kernels of csrc/loss.cu (``fcn_det_loss``): three
-    tiny launches instead of ~300 PyTorch ops + their autograd backward (or their 1.07 ms CUDA-graph replay).
+    tiny launches instead of ~300 PyTorch ops + their autograd backward.
     ``deterministic``: ``fcn_det_loss_deterministic``, whose 16 outputs are bit-reproducible."""
 
     LOSS_KEYS = ("total_loss", "cls_loss", "center_loss", "head_cls_loss", "head_res_loss", "size_cls_loss",

@@ -295,11 +295,3 @@ def test_trainstep_follows_the_torch_flag_both_ways(torch_deterministic):
     torch.use_deterministic_algorithms(True, warn_only=True)
     ts.step(data)
     assert len(ts.engines) == 2
-
-
-def test_deterministic_with_a_pytorch_loss_path_raises():
-    from frustum_convnet_b200.train_engine import TrainStep
-    ts = TrainStep(tr.make_model("refine_car", seed=4), deterministic=True)
-    ts.loss_impl = "graph"
-    with pytest.raises(ValueError, match="loss_impl"):
-        ts.step(_data("refine_car", 2, 8))

@@ -131,9 +131,9 @@ def test_fused_adam_matches_torch_adam():
 
 
 @pytest.mark.parametrize("wl,B,seed", [("refine_car", 32, 1), ("refine_car", 4, 2), ("car", 6, 3)])
-def test_fused_loss_kernel_matches_pytorch_losses(wl, B, seed):
-    """csrc/loss.cu (fcn_det_loss) vs the PyTorch formulation (train_path.losses_masked, itself proven equal to the
-    reference-shaped losses on the CPU): all eight losses, six metrics and d(total)/d(logits) - hand-derived
+def test_fused_loss_kernel_matches_reference_shaped_losses(wl, B, seed):
+    """csrc/loss.cu (fcn_det_loss) vs the reference-shaped PyTorch formulation (train_path.losses_from_logits,
+    nonzero() row selection, and its autograd): all eight losses, six metrics and d(total)/d(logits) - hand-derived
     gradients of the focal / Huber / cross-entropy / corner terms.  Tolerances: losses 1e-5 relative, gradients
     1e-5 * max|g| (+ 1e-8), accuracies exact, IoU means 1e-5."""
     from frustum_convnet_b200 import config, synth, train_path as tp
@@ -146,12 +146,12 @@ def test_fused_loss_kernel_matches_pytorch_losses(wl, B, seed):
     g = torch.Generator(device="cuda").manual_seed(seed)
     cls = torch.randn(B * T2, 2, generator=g, device="cuda")
     reg = torch.randn(B * T2, 39, generator=g, device="cuda") * 0.7
-    lg = tp.LossGraph(m, B, T2, 39, cls.device)
-    lg.graph, lg._tried = None, True                      # eager evaluation of the same static-shape function
-    la, ma, dca, dra = lg.run(cls, reg, data["center_ref2"], data)
+    cls_l, reg_l = cls.clone().requires_grad_(True), reg.clone().requires_grad_(True)
+    la, ma = tp.losses_from_logits(m, cls_l, reg_l, data["center_ref2"], data)
+    la["total_loss"].backward()
     la = {k: float(v) for k, v in la.items()}
     ma = {k: float(v) for k, v in ma.items()}
-    dca, dra = dca.clone(), dra.clone()
+    dca, dra = cls_l.grad, reg_l.grad
     fl = tp.FusedLoss(m, B, T2, 39, cls.device)
     lb, mb, dcb, drb = fl.run(cls, reg, data["center_ref2"], data)
     torch.cuda.synchronize()

@@ -56,7 +56,7 @@ def _same(a, b):
 
 
 @pytest.mark.parametrize("wl,B", CASES)
-def test_every_step_appends_the_fused_loss_block_and_finalize_replays_average_meter(wl, B):
+def test_every_step_appends_its_cached_fused_loss_block_and_finalize_replays_average_meter(wl, B):
     from frustum_convnet_b200.train_engine import TrainStep
     m, cfg = _model(wl)
     ts = TrainStep(m, lr=1e-3, weight_decay=1e-4)
@@ -66,7 +66,7 @@ def test_every_step_appends_the_fused_loss_block_and_finalize_replays_average_me
         d = _data(wl, b, 500 + i)
         ts.step(d)
         torch.cuda.synchronize()
-        want.append(ts._loss_graphs[("kernel", b, d["center_ref2"].shape[2])].out.cpu().numpy())
+        want.append(ts._fused_losses[(False, b, d["center_ref2"].shape[2])].out.cpu().numpy())
     rows = ts.states.per_step(full=True)
     assert rows.shape == (7, 18)
     for i, (r, o, b) in enumerate(zip(rows, want, sizes)):
@@ -83,21 +83,6 @@ def test_every_step_appends_the_fused_loss_block_and_finalize_replays_average_me
     ts.states.reset()                                          # a new epoch starts from row 0
     ts.step(_data(wl, B, 600))
     assert ts.states.per_step().shape == (1, 14)
-
-
-def test_pytorch_loss_paths_append_through_the_same_entry():
-    from frustum_convnet_b200.train_engine import TrainStep
-    m, _ = _model("refine_car")
-    ts = TrainStep(m)
-    ts.loss_impl = "graph"
-    data = _data("refine_car", 4, 41)
-    losses, metrics = ts.step(data)
-    torch.cuda.synchronize()
-    row = ts.states.per_step(full=True)[0]
-    vals = {**losses, **metrics}
-    assert _same(row[:14], [float(vals[k].detach()) for k in ts.states.keys])
-    lab = data["cls_label"].cpu().numpy()
-    assert (row[14], row[15], row[16]) == (4, (lab == 1).sum(), (lab != -1).sum())
 
 
 def test_steps_run_without_a_host_sync():

@@ -1,8 +1,6 @@
-"""Host logic of the training path on the CPU (no CUDA): the static-shape loss formulation used for CUDA-graph capture
-equals the reference-shaped one (values AND gradients w.r.t. the head logits), and the flat parameter bucket keeps
-nn.Module / optimizer semantics."""
+"""Host logic of the training path on the CPU (no CUDA): TrainStep's one loss path is the fused kernel, and the flat
+parameter bucket keeps nn.Module / optimizer semantics."""
 import numpy as np
-import pytest
 import torch
 
 from frustum_convnet_b200 import config, synth
@@ -17,35 +15,11 @@ def _model():
     return m, cfg
 
 
-@pytest.mark.parametrize("seed", [1, 2, 3])
-def test_masked_losses_equal_reference_shaped_losses(seed):
-    """losses_masked (foreground WEIGHTS, static shapes) == losses_from_logits (nonzero() row selection, the
-    reference's formulation, det_base.py:414-476): every loss term, the accuracies and d(total)/d(logits)."""
-    from frustum_convnet_b200 import train_path as tp
-    m, cfg = _model()
-    m.gpu_iou_metrics = False                       # the IoU metric is a CUDA kernel; everything else is torch
-    B = 5
-    data = {k: torch.from_numpy(v) for k, v in synth.make_frustums("refine_car", B, seed=40 + seed, with_labels=True).items()}
-    T2 = data["center_ref2"].shape[2]
-    g = torch.Generator().manual_seed(seed)
-    cls = torch.randn(B * T2, 2, generator=g).requires_grad_(True)
-    reg = (torch.randn(B * T2, 39, generator=g) * 0.5).requires_grad_(True)
-    la, ma = tp.losses_from_logits(m, cls, reg, data["center_ref2"], data)
-    la["total_loss"].backward()
-    ga = (cls.grad.clone(), reg.grad.clone())
-    cls.grad = reg.grad = None
-    ref2 = data["center_ref2"].permute(0, 2, 1).reshape(-1, 3)
-    mean_size = torch.from_numpy(np.asarray(m.mean_size_array)).float()
-    bidx = torch.arange(B * T2) // T2
-    lb, mb = tp.losses_masked(m, cls, reg, ref2, data["cls_label"].reshape(-1), data["box3d_center"],
-                              data["box3d_heading"], data["box3d_size"], data["size_class"], mean_size, bidx, None)
-    lb["total_loss"].backward()
-    for k in la:
-        assert abs(float(la[k]) - float(lb[k])) <= 2e-6 * max(1.0, abs(float(la[k]))), (k, float(la[k]), float(lb[k]))
-    for k in ("cls_acc", "head_acc", "size_acc"):
-        assert abs(float(ma[k]) - float(mb[k])) < 1e-6, k
-    for a, b in zip(ga, (cls.grad, reg.grad)):
-        assert float((a - b).abs().max()) <= 1e-6 * max(1.0, float(a.abs().max()))
+def test_loss_impl_is_the_fused_kernel_and_read_only():
+    from frustum_convnet_b200.train_engine import TrainStep
+    prop = TrainStep.__dict__["loss_impl"]
+    assert isinstance(prop, property) and prop.fset is None
+    assert prop.fget(None) == "kernel"
 
 
 def test_flat_parameter_bucket_semantics():
