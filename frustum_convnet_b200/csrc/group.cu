@@ -487,6 +487,8 @@ extern "C" int fcn_group_rows(const fcn_group_args *args, fcn_stream_t stream) {
     for (int s = 0; s < a.num_scales; ++s) {
         FCN_REQUIRE(a.T[s] >= 1 && a.K[s] >= 1, "bad T/K");
         FCN_REQUIRE(a.centers[s] && a.rows[s] && a.cnt[s] && a.tiles[s], "NULL per-scale pointer");
+        // checked on both paths: only the section-scan pair uses it, but which pair runs depends on the shape
+        FCN_REQUIRE(a.idx_scratch[s] != nullptr, "NULL idx_scratch");
         FCN_REQUIRE(a.row_cap[s] >= a.T[s] * a.K[s], "row_cap too small");
         FCN_REQUIRE(a.feat[s] == nullptr || a.ld_feat[s] % 4 == 0, "ld_feat must be a multiple of 4");
         FCN_REQUIRE(a.feat[s] == nullptr || a.ld_feat[s] >= a.c3[s] + a.num_vec, "ld_feat too small");
@@ -511,7 +513,6 @@ extern "C" int fcn_group_rows(const fcn_group_args *args, fcn_stream_t stream) {
                             (cudaStream_t)stream, P));
         return FCN_OK;
     }
-    for (int s = 0; s < a.num_scales; ++s) FCN_REQUIRE(a.idx_scratch[s] != nullptr, "NULL idx_scratch");
     const size_t smem_e = sizeof(int) * 5 * (size_t)maxT;
     FCN_REQUIRE(smem_e <= 200 * 1024, "T too large for the shared-memory staging");
     if (smem_e > 48 * 1024)

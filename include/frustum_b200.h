@@ -67,12 +67,17 @@ FCN_API int fcn_query_depth_point_b3n(int b, int n, int m, float dis_z, int nsam
  *     cnt = min(hits, K_s) rows (unique_rows=1) or exactly K_s rows with the reference's
  *     back-fill duplicates (unique_rows=0).  A row record is float4 {x-cx, y-cy, z-cz, bits(t)}
  *     (bits(t) = section index as int; sign bit set when the section is empty/masked).
- *     Rows of (b,s) are stored contiguously at rows[s] + b*row_cap[s]; tiles of `tile_rows`
- *     rows are appended to tiles[s] (int4 {b, row0, nrows, 0}) and counted in ntiles[s].
- *     Side outputs: cnt[s] (B,T_s) int32; feat[s] (B,T_s,ld_feat[s]) fp32 position-major is
- *     zero-filled and its one-hot channels [c3[s], c3[s]+num_vec) are written (det_base.py:145-157).
- *     idx_scratch[s] receives the selected point indices (the valid prefix of the reference idx).
- *     `ntiles` (int32[FCN_MAX_SCALES]) is reset by the call itself.
+ *     Rows of (b,s) are stored contiguously at rows[s] + b*row_cap[s]; record slots past them
+ *     are not written.  Tiles of `tile_rows` rows are appended to tiles[s] (int4 {b, row0,
+ *     nrows, 0}), the tiles of one frustum in consecutive slots; ntiles[s] counts all of them
+ *     but only the first tile_cap[s] are stored.
+ *     Side outputs: cnt[s] (B,T_s) int32; rows [0,T_s) of each frustum's block of feat[s]
+ *     (B,feat_pitch[s],ld_feat[s]) fp32 position-major are zero-filled and their one-hot
+ *     channels [c3[s], c3[s]+num_vec) written (det_base.py:145-157); rows [T_s, feat_pitch[s])
+ *     are not written.
+ *     idx_scratch[s] is caller-provided scratch of (B,T_s,K_s) int32, required on every path;
+ *     its contents after the call are unspecified.
+ *     `ntiles` (int32[FCN_MAX_SCALES]) is reset by the call itself, every entry of it.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
     int num_scales, B, N, num_vec, tile_rows, unique_rows;
@@ -88,7 +93,7 @@ typedef struct {
     int32_t *cnt[FCN_MAX_SCALES];           /* (B,T_s) */
     float *feat[FCN_MAX_SCALES];            /* (B,T_s,ld_feat) or NULL */
     void *tiles[FCN_MAX_SCALES];            /* int4[tile_cap] */
-    int32_t *idx_scratch[FCN_MAX_SCALES];   /* (B,T_s,K_s) int32: first min(hits,K) point indices */
+    int32_t *idx_scratch[FCN_MAX_SCALES];   /* (B,T_s,K_s) int32 scratch, contents unspecified after the call */
     int feat_pitch[FCN_MAX_SCALES];         /* rows per frustum of feat[s] (>= T_s; 0 means T_s) */
     int32_t *ntiles;                        /* int32[FCN_MAX_SCALES] */
     int force_scan;                         /* 1: section-scan kernel pair instead of the bit-matrix kernel (A/B) */

@@ -14,6 +14,7 @@ Every generator checks its own bound (sum |a|*|w| + |b| per output, over every i
 
 References restate two C-ABI contracts of include/frustum_b200.h:
   ``pointnet_pooled_ref``  fcn_pointnet_tiles, pooled output;
+  ``pointnet_unpooled_ref`` fcn_pointnet_tiles, un-pooled output of the fp32 path;
   ``conv_ref``             fcn_conv_gemm (segments, taps, strides, pitches, channel pad, pixel shuffle, crop,
                            output slice, relu, round_out).
 ``pointnet_args`` and ``ConvLaunch`` turn the same descriptions into kernel arguments (ctypes structs, tensor maps).
@@ -300,6 +301,26 @@ def pointnet_pooled_ref(case: PointnetCase, round_tf32: bool = True) -> torch.Te
     cur = out[:, :C3].double()
     out[:, :C3] = torch.where(pooled > cur, pooled, cur).float()
     return out.view_as(case.feat_init)
+
+
+def pointnet_unpooled_ref(case: PointnetCase, K: int, out_init: torch.Tensor) -> torch.Tensor:
+    """Expected output of fcn_pointnet_tiles, un-pooled (fp32 path): out (B, C3, T*K) channel-first.  Every record
+    row r < nrows of the first `ntiles` tiles, at flat position p = row0 + r of frustum b, writes
+    relu(layer3 + b3) to out[b, :, p], or 0 when its tag has the sign bit set (a masked section, whose coordinates
+    are never evaluated); positions no tile covers keep out_init."""
+    C3 = case.W.dims[2]
+    rows_i = case.rows.view(torch.int32)
+    out = out_init.clone().view(case.B, C3, case.T * K)
+    for b, row0, n, _ in case.tiles[:case.ntiles].tolist():
+        p = torch.arange(row0, row0 + n)
+        tag = rows_i[b, p, 3]
+        live = tag >= 0
+        assert (tag[live] < case.T).all() and (p < case.T * K).all()
+        vals = torch.zeros(n, C3, dtype=torch.float64)
+        if live.any():
+            vals[live] = torch.relu(pointnet_row_values(case.rows[b, p[live], :3].double(), case.W, round_tf32=False))
+        out[b][:, p] = vals.t().float()
+    return out.view_as(out_init)
 
 
 def pointnet_pooled_loop_ref(case: PointnetCase, round_tf32: bool = True) -> torch.Tensor:
