@@ -262,18 +262,16 @@ def losses_from_logits(model, cls_scores, outputs, center_ref2, data):
 
 class FusedLoss:
     """Losses, metrics and d(total_loss)/d(logits) by the fused kernels of csrc/loss.cu (``fcn_det_loss``): three
-    tiny launches instead of ~300 PyTorch ops + their autograd backward.
+    tiny launches instead of ~300 PyTorch ops + their autograd backward.  Its settings (``validate.set_loss_settings``)
+    and the names of its 14 values (``keys``, ``validate.state_keys``) are read once, at construction.
     ``deterministic``: ``fcn_det_loss_deterministic``, whose 16 outputs are bit-reproducible."""
-
-    LOSS_KEYS = ("total_loss", "cls_loss", "center_loss", "head_cls_loss", "head_res_loss", "size_cls_loss",
-                 "size_res_loss", "corners_loss")
 
     def __init__(self, model, B, T2, out_size, device, deterministic=False):
         import ctypes as C
 
         from . import _lib
+        from .validate import loss_weights, set_loss_settings, state_keys
         self._C, self._lib = C, _lib
-        cfg = get_cfg()
         f32 = torch.float32
         N = B * T2
         self.dcls = torch.zeros((N, 2), dtype=f32, device=device)
@@ -286,17 +284,13 @@ class FusedLoss:
         self.scratch = torch.zeros(n_scratch, dtype=f32, device=device)
         self.mean_size = torch.from_numpy(np.asarray(model.mean_size_array)).to(device=device, dtype=f32).contiguous()
         a = _lib.LossArgs()
-        a.B, a.T2, a.NH, a.NS = B, T2, model.num_bins, model.num_size_cluster
+        a.B, a.T2 = B, T2
+        set_loss_settings(a, model, loss_weights())
         assert out_size == 3 + 2 * a.NH + 4 * a.NS
-        a.with_iou = 1 if getattr(model, "gpu_iou_metrics", True) else 0
-        L = cfg.LOSS
-        a.w_box, a.w_head_reg, a.w_size_reg, a.w_corner = (float(L.BOX_LOSS_WEIGHT), float(L.HEAD_REG_WEIGHT),
-                                                           float(L.SIZE_REG_WEIGHT), float(L.CORNER_LOSS_WEIGHT))
-        a.iou_thresh = float(cfg.IOU_THRESH)
         a.mean_size, a.dcls, a.dreg = self.mean_size.data_ptr(), self.dcls.data_ptr(), self.dreg.data_ptr()
         a.out, a.scratch = self.out.data_ptr(), self.scratch.data_ptr()
         self.args = a
-        self.iou_key = "IoU_" + str(cfg.IOU_THRESH)
+        self.keys = state_keys()
 
     def run(self, cls, reg, center_ref2, data):
         """-> (losses, metrics, dcls, dreg); 0-dim views of one result block, overwritten by the next call."""
@@ -310,8 +304,7 @@ class FusedLoss:
         self._keep = keep
         self._lib.call("fcn_det_loss_deterministic" if self.deterministic else "fcn_det_loss", self._C.byref(a),
                        torch.cuda.current_stream().cuda_stream)
-        o = self.out
-        losses = {k: o[i] for i, k in enumerate(self.LOSS_KEYS)}
-        metrics = {"cls_acc": o[8], "head_acc": o[9], "size_acc": o[10], "IoU_2D": o[11], "IoU_3D": o[12],
-                   self.iou_key: o[13]}
+        o = self.out                                   # the eight losses, then the six metrics
+        losses = {k: o[i] for i, k in enumerate(self.keys[:8])}
+        metrics = {k: o[i] for i, k in enumerate(self.keys[8:], 8)}
         return losses, metrics, self.dcls, self.dreg

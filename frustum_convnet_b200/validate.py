@@ -25,19 +25,26 @@ import torch
 from . import _lib
 from .config import get_cfg
 
-LOSS_KEYS = ("total_loss", "cls_loss", "center_loss", "head_cls_loss", "head_res_loss", "size_cls_loss",
-             "size_res_loss", "corners_loss")
-
 
 def state_keys():
     """The 14 names of the reference's TrainingStates in its order (det_base.py:505-523), IoU_<cfg.IOU_THRESH> last."""
-    return LOSS_KEYS + ("cls_acc", "head_acc", "size_acc", "IoU_2D", "IoU_3D", "IoU_" + str(get_cfg().IOU_THRESH))
+    return ("total_loss", "cls_loss", "center_loss", "head_cls_loss", "head_res_loss", "size_cls_loss", "size_res_loss",
+            "corners_loss", "cls_acc", "head_acc", "size_acc", "IoU_2D", "IoU_3D", "IoU_" + str(get_cfg().IOU_THRESH))
 
 
-def _replay_meters(table, capacity, state, result, stream):
-    """fcn_val_finalize over a (capacity, VAL_ROW) table on `stream`, then one host read -> ValResult."""
-    _lib.call("fcn_val_finalize", table.data_ptr(), capacity, state.data_ptr(), result.data_ptr(), stream.cuda_stream)
-    return _lib.ValResult.from_buffer_copy(result.cpu().numpy().tobytes())
+def loss_weights():
+    """The cfg's (w_box, w_head_reg, w_size_reg, w_corner, iou_thresh), read now."""
+    cfg = get_cfg()
+    L = cfg.LOSS
+    return (float(L.BOX_LOSS_WEIGHT), float(L.HEAD_REG_WEIGHT), float(L.SIZE_REG_WEIGHT),
+            float(L.CORNER_LOSS_WEIGHT), float(cfg.IOU_THRESH))
+
+
+def set_loss_settings(a, model, weights):
+    """NH, NS, with_iou of `model` (read now) and `weights` (`loss_weights()`) into a LossArgs or a ValBatchArgs."""
+    a.NH, a.NS = model.num_bins, model.num_size_cluster
+    a.with_iou = 1 if getattr(model, "gpu_iou_metrics", True) else 0
+    a.w_box, a.w_head_reg, a.w_size_reg, a.w_corner, a.iou_thresh = weights
 
 
 class _PlanLabels:
@@ -56,7 +63,7 @@ class _PlanLabels:
         self.partials = torch.zeros(max(n, 1), dtype=f32, device=dev)
         logits, pitch, ld, ref2 = plan.head_logits()
         a = _lib.ValBatchArgs()
-        a.B, a.T2, a.NH, a.NS = B, T2, eng.num_bins, eng.num_size
+        a.B, a.T2 = B, T2
         a.logit_pitch, a.ld_logit = pitch, ld
         a.logits, a.center_ref2, a.mean_size = logits.data_ptr(), ref2.data_ptr(), eng.mean_size.data_ptr()
         a.cls_label, a.size_class = self.cls_label.data_ptr(), self.size_class.data_ptr()
@@ -73,33 +80,67 @@ class _PlanLabels:
         self.size.copy_(data["box3d_size"].reshape(B, 3), non_blocking=True)
 
 
-class Validator:
+class _MeterTable:
+    """A device table of `capacity` ``FCN_VAL_ROW`` rows, its 4-int state and their float64 AverageMeter replay; a
+    subclass appends the rows and names them by ``_NAMES`` = (class, row, rows, reference loop, capacity call)."""
+
+    def __init__(self, device, capacity=None):
+        self.device = torch.device(device)
+        self.capacity = int(capacity) if capacity is not None else 4096
+        if self.capacity < 1:
+            raise ValueError("capacity must be >= 1")
+        self.keys = state_keys()
+        self.table = torch.zeros((self.capacity, _lib.VAL_ROW), dtype=torch.float32, device=self.device)
+        self.state = torch.zeros(4, dtype=torch.int32, device=self.device)
+        self._result = torch.zeros(C.sizeof(_lib.ValResult), dtype=torch.uint8, device=self.device)
+        self.last_result = None
+
+    def _join(self):
+        """-> the stream the reads are ordered on, after every append so far."""
+        return torch.cuda.current_stream(self.device)
+
+    def _check(self, status, first_no_fg, added):
+        name, row, rows, loop, call = self._NAMES
+        if status & _lib.VAL_NO_FG:
+            raise RuntimeError("%s: %s %d of the epoch has no foreground row (cls_label == 1); the reference %s "
+                               "rejects it (assert fg_idx.numel() != 0)" % (name, row, first_no_fg, loop))
+        if status & _lib.VAL_OVERFLOW:
+            raise RuntimeError("%s: %d %s were added but the capacity is %d; construct %s or more"
+                               % (name, added, rows, self.capacity, call % added))
+
+    def _rows(self, full):
+        with torch.cuda.device(self.device):
+            self._join()
+            n = min(int(self.state[0].item()), self.capacity)
+            t = self.table[:n].cpu().numpy()
+        return np.ascontiguousarray(t if full else t[:, :_lib.VAL_VALUES])
+
+    def _replay(self, table, state):
+        """fcn_val_finalize over `table` and `state`, one host read and the status check -> the 14 averages."""
+        with torch.cuda.device(self.device):
+            _lib.call("fcn_val_finalize", table.data_ptr(), self.capacity, state.data_ptr(), self._result.data_ptr(),
+                      self._join().cuda_stream)
+            r = _lib.ValResult.from_buffer_copy(self._result.cpu().numpy().tobytes())
+        self.last_result = r
+        self._check(r.status, r.first_no_fg, r.added)
+        return OrderedDict((k, float(r.avg[i])) for i, k in enumerate(self.keys))
+
+
+class Validator(_MeterTable):
     """Eval-mode losses and metrics of one epoch on the device (see the module docstring).  One process, one
     device; `capacity` = batches one epoch may add (default 4096)."""
 
     LABEL_KEYS = ("cls_label", "size_class", "box3d_center", "box3d_heading", "box3d_size")
+    _NAMES = ("Validator", "batch", "batches", "validate()", "Validator(model, capacity=%d)")
 
     def __init__(self, model, capacity=None):
         self.model = model
         p = next(model.parameters(), None)
         if p is None or p.device.type != "cuda":
             raise RuntimeError("Validator: the model must live on a CUDA device (there is no CPU fallback)")
-        self.device = p.device
-        self.capacity = int(capacity) if capacity is not None else 4096
-        if self.capacity < 1:
-            raise ValueError("capacity must be >= 1")
-        cfg = get_cfg()
-        self.keys = state_keys()
-        self.iou_key = self.keys[-1]
-        L = cfg.LOSS
-        self._weights = (float(L.BOX_LOSS_WEIGHT), float(L.HEAD_REG_WEIGHT), float(L.SIZE_REG_WEIGHT),
-                         float(L.CORNER_LOSS_WEIGHT), float(cfg.IOU_THRESH))
-        dev = self.device
-        self.table = torch.zeros((self.capacity, _lib.VAL_ROW), dtype=torch.float32, device=dev)
-        self.state = torch.zeros(4, dtype=torch.int32, device=dev)
-        self._result = torch.zeros(C.sizeof(_lib.ValResult), dtype=torch.uint8, device=dev)
+        super().__init__(p.device, capacity)
+        self._weights = loss_weights()
         self._streams = {}
-        self.last_result = None
         self._reset_event, self._reset_waited = None, set()
         self._engine, self._pinned = None, {}
 
@@ -156,8 +197,7 @@ class Validator:
             lab.stage(data, B, plan.T[1])
             plan.forward_staged(pc, centers, one_hot)
             a = lab.args
-            a.with_iou = 1 if getattr(m, "gpu_iou_metrics", True) else 0
-            a.w_box, a.w_head_reg, a.w_size_reg, a.w_corner, a.iou_thresh = self._weights
+            set_loss_settings(a, m, self._weights)
             a.capacity, a.state, a.table = self.capacity, self.state.data_ptr(), self.table.data_ptr()
             _lib.call("fcn_val_batch", C.byref(a), stream.cuda_stream)
         self._streams[stream.cuda_stream] = stream
@@ -173,16 +213,7 @@ class Validator:
         """-> OrderedDict of the 14 epoch averages in the order of the reference's
         ``TrainingStates.get_states(avg=True)``; one host read.  Raises if a batch had no foreground row or the
         table overflowed."""
-        with torch.cuda.device(self.device):
-            r = _replay_meters(self.table, self.capacity, self.state, self._result, self._join())
-        self.last_result = r
-        if r.status & _lib.VAL_NO_FG:
-            raise RuntimeError("Validator: batch %d of the epoch has no foreground row (cls_label == 1); the reference "
-                               "validate() rejects it (assert fg_idx.numel() != 0)" % r.first_no_fg)
-        if r.status & _lib.VAL_OVERFLOW:
-            raise RuntimeError("Validator: %d batches were added but the capacity is %d; construct "
-                               "Validator(model, capacity=%d) or more" % (r.added, self.capacity, r.added))
-        return OrderedDict((k, float(r.avg[i])) for i, k in enumerate(self.keys))
+        return self._replay(self.table, self.state)
 
     def meters(self):
         """(sum, count) of each AverageMeter after the last `finalize`, keyed like its result."""
@@ -194,14 +225,10 @@ class Validator:
     def per_batch(self, full=False):
         """(n, 14) float32 values of the batches added so far (the `val` of each meter, for logging); full=True
         returns the whole rows (n, 18) with B, nfg and nkeep in columns 14-16."""
-        with torch.cuda.device(self.device):
-            self._join()
-            n = min(int(self.state[0].item()), self.capacity)
-            t = self.table[:n].cpu().numpy()
-        return np.ascontiguousarray(t if full else t[:, :_lib.VAL_VALUES])
+        return self._rows(full)
 
 
-class TrainStates:
+class TrainStates(_MeterTable):
     """The training loop's TrainingStates (train/train_net_det.py:131-134) on the device: every optimizer step of
     ``TrainStep.step`` appends its 14 losses and metrics and its batch size to a device table
     (``fcn_train_states_append``, no host sync), and the epoch's averages are the same float64 AverageMeter replay as
@@ -216,16 +243,7 @@ class TrainStates:
 
     `capacity` = steps one epoch may add (default 4096)."""
 
-    def __init__(self, device, capacity=None):
-        self.device = torch.device(device)
-        self.capacity = int(capacity) if capacity is not None else 4096
-        if self.capacity < 1:
-            raise ValueError("capacity must be >= 1")
-        self.keys = state_keys()
-        self.table = torch.zeros((self.capacity, _lib.VAL_ROW), dtype=torch.float32, device=self.device)
-        self.state = torch.zeros(4, dtype=torch.int32, device=self.device)
-        self._result = torch.zeros(C.sizeof(_lib.ValResult), dtype=torch.uint8, device=self.device)
-        self.last_result = None
+    _NAMES = ("TrainStates", "step", "steps", "train()", "TrainStep(..., states_capacity=%d)")
 
     def reset(self):
         """Start a new epoch (stream-ordered: the counter is zeroed on the current stream)."""
@@ -239,14 +257,6 @@ class TrainStates:
             raise ValueError("TrainStates.append: block must be 16 contiguous float32 values on the device")
         _lib.call("fcn_train_states_append", block.data_ptr(), int(B), self.table.data_ptr(), self.capacity,
                   self.state.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
-
-    def _check(self, status, first_no_fg, added):
-        if status & _lib.VAL_NO_FG:
-            raise RuntimeError("TrainStates: step %d of the epoch has no foreground row (cls_label == 1); the reference "
-                               "train() rejects it (assert fg_idx.numel() != 0)" % first_no_fg)
-        if status & _lib.VAL_OVERFLOW:
-            raise RuntimeError("TrainStates: %d steps were added but the capacity is %d; construct "
-                               "TrainStep(..., states_capacity=%d) or more" % (added, self.capacity, added))
 
     def last(self):
         """-> OrderedDict of the last step's 14 values (``get_states(avg=False)``); one host read, meant for every
@@ -263,10 +273,7 @@ class TrainStates:
     def per_step(self, full=False):
         """(n, 14) float32 values of the steps added so far; full=True returns the whole rows (n, 18) with B, nfg and
         nkeep in columns 14-16."""
-        with torch.cuda.device(self.device):
-            n = min(int(self.state[0].item()), self.capacity)
-            t = self.table[:n].cpu().numpy()
-        return np.ascontiguousarray(t if full else t[:, :_lib.VAL_VALUES])
+        return self._rows(full)
 
     def _over_ranks(self, world):
         """The table as the reference's DataParallel loop logs it: each step's values averaged over the replicas,
@@ -292,7 +299,4 @@ class TrainStates:
         world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         with torch.cuda.device(self.device):
             table, state = self._over_ranks(world) if world > 1 else (self.table, self.state)
-            r = _replay_meters(table, self.capacity, state, self._result, torch.cuda.current_stream(self.device))
-        self.last_result = r
-        self._check(r.status, r.first_no_fg, r.added)
-        return OrderedDict((k, float(r.avg[i])) for i, k in enumerate(self.keys))
+        return self._replay(table, state)
