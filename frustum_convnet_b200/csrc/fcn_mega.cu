@@ -546,6 +546,8 @@ extern "C" int fcn_mega_forward(const fcn_mega_args *args, fcn_stream_t stream) 
                     "layer tile width must be 64, 128 or 256, with k_atoms = 1 for 256 and 2 otherwise");
         FCN_REQUIRE(L.is_heads || ((uintptr_t)L.bias & 15) == 0,
                     "layer bias must be 16-byte aligned (its NT-column slices are bulk-copied)");
+        // every heads job decodes whole logit rows right after storing its own NT columns
+        FCN_REQUIRE(!L.is_heads || L.n_tiles_n == 1, "the heads layer must be a single N tile (ld_logit <= 128)");
         nt_max = L.NT > nt_max ? L.NT : nt_max;
     }
     if (a.n_jobs == 0) return FCN_OK;

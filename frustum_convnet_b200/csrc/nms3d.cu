@@ -3,10 +3,11 @@
 // `rotate_non_max_suppression_3d_cpu`, which today costs a device->host copy of every prediction, a Python loop
 // per image / class and a CPU Boost polygon clip per box pair.
 //
-// One CTA per segment (= one image x class list of detections, <= NMS_MAX_DETS boxes):
+// One CTA per segment (= one image x class list of detections, <= NMS_MAX_DETS boxes; nms.py refuses longer lists,
+// the kernel would consider only their first NMS_MAX_DETS rows):
 //   1. corners of every box (boxes3d2corners, rbbox_iou.py:121-148) and its axis-aligned bounding cube;
 //   2. rank by descending score (the reference: scores.argsort()[::-1]; ties: larger index first, i.e. the
-//      reverse of a stable ascending sort);
+//      reverse of a stable ascending sort, where NaN sorts above every number and -0.0 equals +0.0);
 //   3. suppression bit matrix in RANK order: bit (i, j) for j > i is set iff the bounding cubes overlap
 //      (standup IoU > 0, nms_cpu.h:192) and the rotated 3-D IoU (box_iou.cuh, the same function as the train
 //      metric, incl. its degenerate-ring rule) is >= thresh (nms_cpu.h:226-227);
@@ -22,6 +23,15 @@ constexpr int NMS_MAX_DETS = 512;
 constexpr int NMS_WORDS = NMS_MAX_DETS / 32;
 constexpr int NMS_THREADS = 256;
 
+// Row j ranks before row i.  A strict total order, so the ranks are a permutation whatever the scores: NaN above
+// every number (numpy sorts NaN last, the reversed order puts it first), equal scores (NaN with NaN, -0.0 with
+// +0.0) by the larger index first.
+__device__ __forceinline__ bool nms_ranks_before(float sj, int j, float si, int i) {
+    const bool nj = sj != sj, ni = si != si;
+    if (nj || ni) return nj && (!ni || j > i);
+    return sj > si || (sj == si && j > i);
+}
+
 __global__ void __launch_bounds__(NMS_THREADS)
 nms3d_kernel(const float *__restrict__ dets, const int *__restrict__ seg_offsets, float thresh, int top_k,
              int *__restrict__ keep, int *__restrict__ keep_count, int keep_stride) {
@@ -34,13 +44,13 @@ nms3d_kernel(const float *__restrict__ dets, const int *__restrict__ seg_offsets
     const int base = seg_offsets[seg], n = min(seg_offsets[seg + 1] - base, NMS_MAX_DETS);
     const int tid = threadIdx.x;
     const float *d = dets + (size_t)base * 8;
-    // ---- rank by descending score (ties: larger index first)
+    // ---- rank by descending score (ties: larger index first; NaN first)
     for (int i = tid; i < n; i += NMS_THREADS) {
         const float si = d[i * 8 + 7];
         int rank = 0;
         for (int j = 0; j < n; ++j) {
             const float sj = d[j * 8 + 7];
-            rank += (sj > si || (sj == si && j > i)) ? 1 : 0;
+            rank += nms_ranks_before(sj, j, si, i) ? 1 : 0;
         }
         order[rank] = i;
     }

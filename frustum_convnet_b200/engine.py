@@ -409,8 +409,15 @@ class _Plan:
 
         self.mega_args = None
         self.mega_grid = 0
-        if eng.use_mega and eng.has_heads and all(a.precision in (3, 4) for a in self.conv_args):
+        if (eng.use_mega and eng.has_heads and self.heads_one_tile()
+                and all(a.precision in (3, 4) for a in self.conv_args)):
             self._build_mega()
+
+    def heads_one_tile(self):
+        """The persistent kernel's heads epilogue decodes whole logit rows, so the heads layer must be ONE N tile
+        (ld_logit <= 128).  Wider heads (e.g. 48 heading bins on SUN-RGBD, 64 on KITTI: ld_logit = 192, three
+        64-column tiles) run the per-layer path: the GEMM per layer, then fcn_decode_eval."""
+        return all(nt == L.n_cols for L, (_, _, nt) in zip(self.eng.layers, self.geom) if L.kind == "heads")
 
     def mega_descs(self):
         """Shape-level layer descriptions for the persistent FCN kernel (pure host arithmetic, testable on the CPU)."""

@@ -13,11 +13,18 @@ from . import _lib
 
 
 def rotate_nms_3d_batched(dets: torch.Tensor, seg_offsets: torch.Tensor, thresh: float, top_k: int = 300):
-    """-> (keep (S, top_k) int32 global row indices in descending-score order, counts (S,) int32)."""
+    """-> (keep (S, top_k) int32 global row indices in descending-score order, counts (S,) int32).  Every list
+    holds at most ``fcn_rotate_nms_3d_max_dets()`` (512) rows; a longer one raises RuntimeError."""
     if not dets.is_cuda:
         raise RuntimeError("rotate_nms_3d: CUDA tensors required (there is no CPU fallback)")
     assert dets.dim() == 2 and dets.shape[1] == 8, "dets must be (n, 8): cx, cy, cz, l, w, h, ry, score"
     d = dets.detach().to(torch.float32).contiguous()
+    lens = torch.diff(seg_offsets.detach().to("cpu", torch.int64))
+    cap = int(_lib.load().fcn_rotate_nms_3d_max_dets())
+    if lens.numel() and int(lens.max()) > cap:
+        # the kernel ranks and suppresses one list in shared memory; a longer list would be cut to its first rows
+        raise RuntimeError("rotate_nms_3d: a list of %d detections exceeds the %d one launch handles per list"
+                           % (int(lens.max()), cap))
     off = seg_offsets.to(device=d.device, dtype=torch.int32).contiguous()
     S = off.numel() - 1
     keep = torch.full((max(S, 0), top_k), -1, dtype=torch.int32, device=d.device)

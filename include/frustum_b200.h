@@ -404,10 +404,11 @@ FCN_API int fcn_det_loss_deterministic(const fcn_loss_args *args, fcn_stream_t s
  *     `cube_nms` = rotate_nms_3d_cc (ops/pybind11/rbbox_iou.py:294-311) -> rotate_non_max_suppression_3d_cpu
  *     (ops/pybind11/nms_cpu.h:148-240), called per image and class from train/test_net_det.py:126-152.
  *     dets: (total, 8) fp32 rows [cx, cy, cz, l, w, h, ry, score]; segment s = rows
- *     [seg_offsets[s], seg_offsets[s+1]) (one image x class list, at most fcn_rotate_nms_3d_max_dets() rows are
- *     considered); keep: (num_segments, keep_stride) int32 GLOBAL row indices in descending-score order,
- *     keep_count[s] <= top_k of them are valid.  A box is suppressed by a kept, higher-scored box when their
- *     axis-aligned bounding cubes overlap and the rotated 3-D IoU is >= thresh.
+ *     [seg_offsets[s], seg_offsets[s+1]) (one image x class list of at most fcn_rotate_nms_3d_max_dets() rows: only
+ *     that many are considered, so callers split or refuse longer lists; nms.py refuses them); keep:
+ *     (num_segments, keep_stride) int32 GLOBAL row indices in descending-score order (NaN scores first, equal
+ *     scores by the larger index first), keep_count[s] <= top_k of them are valid.  A box is suppressed by a kept,
+ *     higher-scored box when their axis-aligned bounding cubes overlap and the rotated 3-D IoU is >= thresh.
  * ------------------------------------------------------------------------------------------ */
 FCN_API int fcn_rotate_nms_3d(int num_segments, const float *dets, const int32_t *seg_offsets, float thresh, int top_k,
                               int32_t *keep, int32_t *keep_count, int keep_stride, fcn_stream_t stream);

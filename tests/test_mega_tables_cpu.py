@@ -149,3 +149,28 @@ def test_wide_tile_rule_is_by_tile_count():
     assert max(d.NT for d in small) == 128 and max(d.NT for d in big) == 256
     for d in big:
         assert d.k_atoms == (1 if d.NT == 256 else 2) and d.K_pad % (32 * d.k_atoms) == 0
+
+
+@pytest.mark.parametrize("wl,NH,one_tile", [("car", 12, True), ("car", 24, True), ("car", 1, True), ("car", 64, False),
+                                           ("people", 64, False), ("sunrgbd", 24, True), ("sunrgbd", 48, False)])
+def test_planner_runs_wide_heads_on_the_per_layer_path(wl, NH, one_tile, monkeypatch):
+    """The persistent kernel's heads epilogue decodes whole rows, so it takes the heads layer as ONE N tile: a logit
+    row of 192 columns (KITTI with 64 heading bins, SUN-RGBD with 48) makes three 64-column tiles, and the planner
+    must build no persistent-kernel tables for it (the per-layer GEMMs and fcn_decode_eval run instead)."""
+    from frustum_convnet_b200 import _lib, config, synth
+    calls = []
+    monkeypatch.setattr(_lib, "call", lambda name, *a: calls.append(name))   # tensor-map encodes need a driver
+    monkeypatch.setenv("FCN_MEGA", "1")
+    cfg, w = config.load_workload(wl)
+    sd = synth.make_state_dict(w["arch"], w["num_vec"], cfg.DATA.DATASET_NAME, seed=7, num_bins=NH)
+    eng = FrustumEngine(w["arch"], w["num_vec"], cfg.DATA.DATASET_NAME, cfg.DATA.HEIGHT_HALF, NH,
+                        {k: torch.from_numpy(np.asarray(v)) for k, v in sd.items()}, "cpu", precision=1)
+    assert eng.use_mega and eng.use_tma
+    T = (280, 140, 70, 35) if w["arch"].num_scales == 4 else (280, 140, 70, 35, 18)
+    plan = _Plan(eng, 32, 1024, T)
+    heads = [d for d in plan.mega_descs() if d.kind == "heads"]
+    assert len(heads) == 1 and (eng.ld_logit == 192) == (not one_tile)
+    assert heads[0].n_tiles == (1 if one_tile else 3)
+    assert plan.heads_one_tile() == one_tile
+    assert (plan.mega_args is not None) == one_tile
+    assert ("fcn_encode_store_map" in calls) == one_tile        # only the persistent kernel's tables encode stores
