@@ -309,6 +309,16 @@ class GtExtractArgs(C.Structure):
                [(n, C.c_void_p) for n in ("info", "job_points", "points", "labels", "offsets")]
 
 
+DET_FEED_NONFINITE = 1
+
+
+class DetEvalFeedArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("num_segments", "num_rows", "num_out", "reserved0")] + \
+               [(n, C.c_void_p) for n in ("rows", "seg_offsets", "keep_count", "seg_dst", "seg_value",
+                                          "host_seg_offsets", "host_keep_count", "host_seg_dst", "records", "corners",
+                                          "scores", "segments", "status")]
+
+
 SUNRGBD_MAX_POINTS = 2048
 
 
@@ -394,6 +404,8 @@ SIGNATURES = {
     "fcn_sunrgbd_extract_count": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
     "fcn_sunrgbd_extract_select": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
     "fcn_sunrgbd_extract_write": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
+    "fcn_det_kitti_records": (_I, [C.POINTER(DetEvalFeedArgs), _P]),
+    "fcn_det_sunrgbd_feed": (_I, [C.POINTER(DetEvalFeedArgs), _P]),
 }
 
 _lib = None

@@ -110,8 +110,9 @@ class DetectionCollector:
         self._streams[stream.cuda_stream] = stream
         self.added[first:first + B] = True
 
-    def finalize(self):
-        """-> {data_idx: {class_type: float32 (n, 12)}}; one host sync to size the NMS bit matrix, one copy back."""
+    def finalize_device(self):
+        """-> CollectedDetections: the kept rows stay on the device; one host sync to size the NMS bit matrix and one
+        read of the per-segment offsets and keep counts (O(segments), no row crosses to the host)."""
         dev = self.device
         cur = torch.cuda.current_stream(dev)
         for st in self._streams.values():
@@ -137,16 +138,76 @@ class DetectionCollector:
             mask = torch.empty(max(mask_words, 1), dtype=torch.int32, device=dev)
             a.mask, a.mask_words = mask.data_ptr(), mask_words
             _lib.call("fcn_det_select", C.byref(a), cur.cuda_stream)
-            n = n_counted
-            rows_h = rows[:n].cpu().numpy()
-            off_h, kc_h = off.cpu().numpy(), kc[:S].cpu().numpy()
-        self.last_counts = {"rows": n, "kept": int(kc_h.sum()) if S else 0}
+            offkc = torch.cat([off, kc[:S]]).cpu().numpy()                      # O(S) metadata, one copy
+        off_h, kc_h = offkc[:S + 1].copy(), offkc[S + 1:].copy()
+        self.last_counts = {"rows": n_counted, "kept": int(kc_h.sum()) if S else 0}
         # dict order of the frustums that were added, in dataset order
         segs = self._seg_host[self.added]
         _, first_pos = np.unique(segs, return_index=True)
         order = segs[np.sort(first_pos)]
+        return CollectedDetections(self.dataset, rows, off, kc, off_h, kc_h, list(self.segments), order, cur)
+
+    def finalize(self):
+        """-> {data_idx: {class_type: float32 (n, 12)}}; one host sync to size the NMS bit matrix, one copy back."""
+        return self.finalize_device().to_dict()
+
+
+class CollectedDetections:
+    """The result of DetectionCollector.finalize_device(), left on the device for the evaluators'
+    ``evaluate_collected``.
+
+    rows (n_rows, 12) float32 (device): kept row k of segment s at seg_offsets[s] + k, k < keep_count[s], in the
+    reference's list order; seg_offsets / keep_count: the same offsets and counts on the device; host_seg_offsets
+    (S + 1) / host_keep_count (S): their host copies; segments: the (data_idx, class_type) key of each segment;
+    order: the segments of the added frustums in the reference's dict order (images by first appearance, classes by
+    first appearance within the image).  `stream`: the stream the rows were written on."""
+
+    def __init__(self, dataset, rows, seg_offsets, keep_count, host_seg_offsets, host_keep_count, segments, order,
+                 stream):
+        self.dataset = dataset
+        self.num_rows = int(host_seg_offsets[-1])
+        self.rows = rows
+        self.seg_offsets, self.keep_count = seg_offsets, keep_count
+        self.host_seg_offsets = np.ascontiguousarray(host_seg_offsets, dtype=np.int32)
+        self.host_keep_count = np.ascontiguousarray(host_keep_count, dtype=np.int32)
+        self.segments, self.order, self.stream = segments, np.asarray(order, dtype=np.int64), stream
+        self.device = rows.device
+
+    @property
+    def num_segments(self):
+        return len(self.segments)
+
+    def image_order(self):
+        """The images of the dict in its order, and for each segment of `order` the rank of its image there."""
+        images, rank, seg_rank = [], {}, np.empty(len(self.order), dtype=np.int64)
+        for j, s in enumerate(self.order.tolist()):
+            idx = self.segments[s][0]
+            r = rank.get(idx)
+            if r is None:
+                r = rank[idx] = len(images)
+                images.append(idx)
+            seg_rank[j] = r
+        return images, seg_rank
+
+    def to_dict(self):
+        """-> {data_idx: {class_type: float32 (n, 12)}}, what DetectionCollector.finalize() returns (one copy of the
+        rows to the host)."""
+        rows_h = self.rows[:self.num_rows].cpu().numpy()
+        off_h, kc_h = self.host_seg_offsets, self.host_keep_count
         res = {}
-        for s in order:
+        for s in self.order:
             idx, ct = self.segments[s]
             res.setdefault(idx, {})[ct] = rows_h[off_h[s]: off_h[s] + kc_h[s]].copy()
         return res
+
+    def feed_args(self, seg_dst, seg_value, num_out, plan_ptrs):
+        """fcn_det_eval_feed_args for a gather plan: seg_dst / seg_value (S) int32 host arrays (kept alive by the
+        caller), plan_ptrs = their device addresses."""
+        a = _lib.DetEvalFeedArgs()
+        a.num_segments, a.num_rows, a.num_out = self.num_segments, self.num_rows, int(num_out)
+        a.rows, a.seg_offsets, a.keep_count = self.rows.data_ptr(), self.seg_offsets.data_ptr(), \
+            self.keep_count.data_ptr()
+        a.seg_dst, a.seg_value = plan_ptrs
+        a.host_seg_offsets, a.host_keep_count = self.host_seg_offsets.ctypes.data, self.host_keep_count.ctypes.data
+        a.host_seg_dst = seg_dst.ctypes.data
+        return a

@@ -24,7 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._host import csr_offsets, cuda_device, workspace
+from ._host import csr_offsets, cuda_device, upload, workspace
 
 CLASS_NAMES = ("car", "pedestrian", "cyclist")
 METRICS = ("image", "ground", "3d")
@@ -168,8 +168,9 @@ class KittiEvaluator:
         self.gt = gt
         self.device = gt.device
 
-    def evaluate(self, det_results):
-        """{idx: {class_type: (n, 12)}} -> KittiEvalResult over every image of the ground truth."""
+    def evaluate(self, det_results, stream=None, timer=None):
+        """{idx: {class_type: (n, 12)}} -> KittiEvalResult over every image of the ground truth (`stream`, `timer`:
+        as for ``evaluate_records``)."""
         per_image = [[] for _ in self.gt.image_ids]
         for idx, by_class in det_results.items():
             i = self.gt.index.get(int(idx))
@@ -178,7 +179,8 @@ class KittiEvaluator:
             for class_type, dets in by_class.items():
                 if len(dets):
                     per_image[i].append(detection_records(dets, class_type))
-        return self.evaluate_records([np.concatenate(p) if p else np.zeros((0, DET_COLS)) for p in per_image])
+        return self.evaluate_records([np.concatenate(p) if p else np.zeros((0, DET_COLS)) for p in per_image], stream,
+                                     timer)
 
     def evaluate_dir(self, result_dir):
         """Result files result_dir/data/<index>.txt (the evaluator's layout) -> KittiEvalResult over the images that
@@ -196,6 +198,55 @@ class KittiEvaluator:
         sub = KittiGroundTruth(ids, [self.gt.records[self.gt.index[i]] for i in ids], self.device)
         return KittiEvaluator(sub).evaluate_records([recs[i] for i in ids])
 
+    def gather_plan(self, collected):
+        """The host half of ``evaluate_collected``, from segment metadata only -> (seg_dst, seg_code, det_offsets):
+        per segment of the collector the first record it owns in the per-image CSR of ``evaluate`` (-1: not written)
+        and its type code, and the (num_images + 1) offsets of that CSR.  Within an image its classes keep the dict
+        order, then the row order.  An image of the dict that is not in the ground truth raises KeyError."""
+        S = collected.num_segments
+        order = collected.order
+        gt_index = np.empty(len(order), dtype=np.int64)
+        seen = {}
+        for j, s in enumerate(order.tolist()):
+            idx = collected.segments[s][0]
+            i = seen.get(idx)
+            if i is None:
+                i = self.gt.index.get(int(idx))
+                if i is None:
+                    raise KeyError("detections for image %s, which is not in the ground truth's image_ids" % idx)
+                seen[idx] = i
+            gt_index[j] = i
+        kept = collected.host_keep_count[order].astype(np.int64)
+        by_image = order[np.argsort(gt_index, kind="stable")]        # images in ground-truth order, dict order within
+        seg_dst = np.full(S, -1, dtype=np.int32)
+        counts = collected.host_keep_count[by_image].astype(np.int64)
+        seg_dst[by_image] = (np.cumsum(counts) - counts).astype(np.int32)
+        seg_code = np.array([type_code(ct) for _, ct in collected.segments], dtype=np.int32)
+        det_off = csr_offsets(np.bincount(gt_index, weights=kept, minlength=len(self.gt.image_ids)).astype(np.int64))
+        return seg_dst, seg_code, det_off
+
+    def evaluate_collected(self, collected, stream=None, timer=None):
+        """DetectionCollector.finalize_device()'s CollectedDetections -> the KittiEvalResult ``evaluate`` gives for
+        its dict, without the rows crossing to the host: the records are written on the device
+        (``fcn_det_kitti_records``) into the per-image order ``evaluate`` builds, the gather plan coming from the
+        segment keys alone.  Alpha uses the correctly rounded float32 atan2 (numpy's float32 arctan2 can differ from it
+        in the last bit, by at most one '%.4f' step after the rounding); every other field is identical."""
+        dev = self.device
+        seg_dst, seg_code, det_off = self.gather_plan(collected)
+        num_det = int(det_off[-1])
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.device(dev), torch.cuda.stream(stream):
+            if collected.stream.cuda_stream != stream.cuda_stream:
+                stream.wait_stream(collected.stream)
+            buf, (p_dst, p_code, p_off) = upload([seg_dst, seg_code, det_off], dev)
+            det = torch.empty((max(num_det, 1), DET_COLS), dtype=torch.float64, device=dev)
+            if timer is not None:
+                timer("feed_start")
+            a = collected.feed_args(seg_dst, seg_code, num_det, (p_dst, p_code))
+            a.records = det.data_ptr()
+            _lib.call("fcn_det_kitti_records", C.byref(a), stream.cuda_stream)
+            return self._launch(det.data_ptr(), p_off, det_off, stream, timer)
+
     def evaluate_records(self, det_records, stream=None, timer=None):
         """One (nd_i, 14) float64 record array per image of the ground truth, in its order -> KittiEvalResult.
         `timer(name)` (optional) is called before the first device call ("start") and after each of the three is
@@ -210,20 +261,26 @@ class KittiEvaluator:
         with torch.cuda.device(dev), torch.cuda.stream(stream):
             det = torch.from_numpy(np.ascontiguousarray(flat)).to(dev, non_blocking=False)
             det_off = torch.from_numpy(host_det_off).to(dev)
-            a = _lib.KittiEvalArgs()
-            a.num_images, a.num_gt, a.num_det = len(self.gt.image_ids), self.gt.num_gt, int(host_det_off[-1])
-            a.gt, a.det = self.gt.gt.data_ptr(), det.data_ptr()
-            a.gt_offsets, a.det_offsets = self.gt.offsets.data_ptr(), det_off.data_ptr()
-            a.host_gt_offsets = self.gt.host_offsets.ctypes.data
-            a.host_det_offsets = host_det_off.ctypes.data
-            ws, nbytes = workspace("fcn_kitti_eval_workspace_bytes", dev, C.byref(a))
-            res = torch.zeros(C.sizeof(_lib.KittiEvalResult), dtype=torch.uint8, device=dev)   # + tail padding
-            a.workspace, a.workspace_bytes, a.result = ws.data_ptr(), nbytes, res.data_ptr()
+            return self._launch(det.data_ptr(), det_off.data_ptr(), host_det_off, stream, timer)
+
+    def _launch(self, det, det_off, host_det_off, stream, timer):
+        """The three evaluator entries on `stream` (current, on the evaluator's device) over device records `det` with
+        device offsets `det_off` and their host copy -> KittiEvalResult after the one read back."""
+        dev = self.device
+        a = _lib.KittiEvalArgs()
+        a.num_images, a.num_gt, a.num_det = len(self.gt.image_ids), self.gt.num_gt, int(host_det_off[-1])
+        a.gt, a.det = self.gt.gt.data_ptr(), det
+        a.gt_offsets, a.det_offsets = self.gt.offsets.data_ptr(), det_off
+        a.host_gt_offsets = self.gt.host_offsets.ctypes.data
+        a.host_det_offsets = host_det_off.ctypes.data
+        ws, nbytes = workspace("fcn_kitti_eval_workspace_bytes", dev, C.byref(a))
+        res = torch.zeros(C.sizeof(_lib.KittiEvalResult), dtype=torch.uint8, device=dev)   # + tail padding
+        a.workspace, a.workspace_bytes, a.result = ws.data_ptr(), nbytes, res.data_ptr()
+        if timer is not None:
+            timer("start")
+        for name in ("fcn_kitti_eval_overlaps", "fcn_kitti_eval_thresholds", "fcn_kitti_eval_statistics"):
+            _lib.call(name, C.byref(a), stream.cuda_stream)
             if timer is not None:
-                timer("start")
-            for name in ("fcn_kitti_eval_overlaps", "fcn_kitti_eval_thresholds", "fcn_kitti_eval_statistics"):
-                _lib.call(name, C.byref(a), stream.cuda_stream)
-                if timer is not None:
-                    timer(name)
-            raw = _lib.KittiEvalResult.from_buffer_copy(res.cpu().numpy().tobytes())   # the one read back
+                timer(name)
+        raw = _lib.KittiEvalResult.from_buffer_copy(res.cpu().numpy().tobytes())   # the one read back
         return KittiEvalResult(raw)

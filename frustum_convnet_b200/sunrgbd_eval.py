@@ -226,6 +226,62 @@ class SunrgbdEvaluator:
         seg = np.concatenate(segs) if segs else np.zeros(0, np.int32)
         return self._run(cor, np.asarray(scores, dtype=np.float64), seg, counts, ovthresh, stream, timer)
 
+    def gather_plan(self, collected):
+        """The host half of ``evaluate_collected``, from segment metadata only -> (seg_dst, seg_gt, det_class_offsets):
+        per segment of the collector the first detection it owns in the gather order of ``evaluate`` (class after
+        class, images in dict order, then rows; -1: not written, as for a class without ground truth), its ground-truth
+        segment (or -1), and the (num_classes + 1) offsets of that order.  Every image of the dict is checked as
+        ``evaluate`` checks it."""
+        gt = self.gt
+        S, order = collected.num_segments, collected.order
+        _, img_rank = collected.image_order()
+        seg_ci = np.full(len(order), -1, dtype=np.int64)
+        seg_gt = np.full(S, -1, dtype=np.int32)
+        checked = {}
+        for j, s in enumerate(order.tolist()):
+            idx, name = collected.segments[s]
+            key = checked.get(idx)
+            if key is None:
+                key = checked[idx] = self._check_image(idx)
+            ci = gt.class_index.get(name)
+            if ci is not None:
+                seg_ci[j] = ci
+                seg_gt[s] = gt.segment_of.get((ci, key), -1)
+        sel = seg_ci >= 0
+        rank = np.lexsort((img_rank[sel], seg_ci[sel]))                  # class, then the image's dict position
+        gathered = order[sel][rank]
+        counts = collected.host_keep_count[gathered].astype(np.int64)
+        seg_dst = np.full(S, -1, dtype=np.int32)
+        seg_dst[gathered] = (np.cumsum(counts) - counts).astype(np.int32)
+        per_class = np.bincount(seg_ci[sel], weights=collected.host_keep_count[order[sel]].astype(np.int64),
+                                minlength=len(gt.classes)).astype(np.int64)
+        return seg_dst, seg_gt, csr_offsets(per_class)
+
+    def evaluate_collected(self, collected, ovthresh=0.25, stream=None, timer=None):
+        """DetectionCollector.finalize_device()'s CollectedDetections -> the SunrgbdEvalResult ``evaluate`` gives for
+        its dict, without the rows crossing to the host: corners, scores and ground-truth segments are written on the
+        device (``fcn_det_sunrgbd_feed``) in ``evaluate``'s gather order, the plan coming from the segment keys alone.
+        cos and sin are the correctly rounded float32 values (numpy's float32 loops can differ in the last bit, so a
+        corner can move by an ulp or two of its magnitude)."""
+        dev = self.device
+        seg_dst, seg_gt, det_off = self.gather_plan(collected)
+        D = int(det_off[-1])
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.device(dev), torch.cuda.stream(stream):
+            if collected.stream.cuda_stream != stream.cuda_stream:
+                stream.wait_stream(collected.stream)
+            buf, (p_dst, p_gt, p_off) = upload([seg_dst, seg_gt, det_off], dev)
+            det = torch.empty(max(D, 1) * 26 + 1, dtype=torch.float64, device=dev)    # corners | scores | segments
+            dp = det.data_ptr()
+            status = torch.zeros(1, dtype=torch.int32, device=dev)
+            if timer is not None:
+                timer("feed_start")
+            a = collected.feed_args(seg_dst, seg_gt, D, (p_dst, p_gt))
+            a.corners, a.scores, a.segments = dp, dp + 8 * 24 * max(D, 1), dp + 8 * 25 * max(D, 1)
+            a.status = status.data_ptr()
+            _lib.call("fcn_det_sunrgbd_feed", C.byref(a), stream.cuda_stream)
+            return self._launch(a.corners, a.scores, a.segments, p_off, det_off, D, ovthresh, stream, timer, status)
+
     def _run(self, corners, scores, seg, counts, ovthresh, stream, timer):
         """(D, 8, 3) corners, (D,) scores and ground-truth segments, gathered class after class -> result.  One upload
         of the detections, one read-back of the result.  `timer(name)` (optional) is called before the first device
@@ -234,35 +290,48 @@ class SunrgbdEvaluator:
             raise ValueError("detection scores must be finite")
         if not np.isfinite(corners).all():
             raise ValueError("detection corners must be finite")
-        gt, dev = self.gt, self.device
-        D, Cn = len(scores), len(gt.classes)
+        D = len(scores)
         det_off = csr_offsets(counts)
+        dev = self.device
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
             buf, ptrs = upload([np.asarray(corners, np.float64), np.asarray(scores, np.float64),
                                 np.asarray(seg, np.int32), det_off], dev)
-            a = _lib.SunrgbdEvalArgs()
-            a.num_classes, a.num_gt, a.num_gt_segments, a.num_det = Cn, gt.num_gt, gt.num_segments, D
-            a.ovthresh = float(ovthresh)
-            a.gt_corners, a.gt_segment_offsets, a.gt_class_offsets = (gt.corners.data_ptr(),
-                                                                      gt.segment_offsets.data_ptr(),
-                                                                      gt.class_offsets.data_ptr())
-            a.det_corners, a.det_scores, a.det_segments, a.det_class_offsets = ptrs
-            a.host_gt_segment_offsets = gt.host_segment_offsets.ctypes.data
-            a.host_gt_class_offsets = gt.host_class_offsets.ctypes.data
-            a.host_det_class_offsets = det_off.ctypes.data
-            ws, nbytes = workspace("fcn_sunrgbd_eval_workspace_bytes", dev, C.byref(a))
-            out = torch.zeros(Cn * _RES + 16 * D, dtype=torch.uint8, device=dev)     # results | rec | prec
-            ob = out.data_ptr()
-            a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
-            a.result, a.rec, a.prec = ob, ob + Cn * _RES, ob + Cn * _RES + 8 * D
+            return self._launch(*ptrs, det_off, D, ovthresh, stream, timer)
+
+    def _launch(self, corners, scores, seg, det_off_dev, det_off, D, ovthresh, stream, timer, status=None):
+        """The two evaluator entries on `stream` (current, on the evaluator's device) over device detections -> result
+        after the one read back.  `status` (optional, device int32): the feed's flags, read back with the result; a
+        non-finite corner or score raises ValueError as ``evaluate`` does."""
+        gt, dev = self.gt, self.device
+        Cn = len(gt.classes)
+        a = _lib.SunrgbdEvalArgs()
+        a.num_classes, a.num_gt, a.num_gt_segments, a.num_det = Cn, gt.num_gt, gt.num_segments, D
+        a.ovthresh = float(ovthresh)
+        a.gt_corners, a.gt_segment_offsets, a.gt_class_offsets = (gt.corners.data_ptr(),
+                                                                  gt.segment_offsets.data_ptr(),
+                                                                  gt.class_offsets.data_ptr())
+        a.det_corners, a.det_scores, a.det_segments, a.det_class_offsets = corners, scores, seg, det_off_dev
+        a.host_gt_segment_offsets = gt.host_segment_offsets.ctypes.data
+        a.host_gt_class_offsets = gt.host_class_offsets.ctypes.data
+        a.host_det_class_offsets = det_off.ctypes.data
+        ws, nbytes = workspace("fcn_sunrgbd_eval_workspace_bytes", dev, C.byref(a))
+        out = torch.zeros(Cn * _RES + 16 * D + 16, dtype=torch.uint8, device=dev)     # results | rec | prec | status
+        ob = out.data_ptr()
+        a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
+        a.result, a.rec, a.prec = ob, ob + Cn * _RES, ob + Cn * _RES + 8 * D
+        if timer is not None:
+            timer("start")
+        for name in ("fcn_sunrgbd_eval_match", "fcn_sunrgbd_eval_curves"):
+            _lib.call(name, C.byref(a), stream.cuda_stream)
             if timer is not None:
-                timer("start")
-            for name in ("fcn_sunrgbd_eval_match", "fcn_sunrgbd_eval_curves"):
-                _lib.call(name, C.byref(a), stream.cuda_stream)
-                if timer is not None:
-                    timer(name)
-            back = out.cpu().numpy()                                         # the one read back
+                timer(name)
+        if status is not None:
+            out[Cn * _RES + 16 * D:Cn * _RES + 16 * D + 4].copy_(status.view(torch.uint8))
+        back = out.cpu().numpy()                                             # the one read back
+        flags = int(back[Cn * _RES + 16 * D:Cn * _RES + 16 * D + 4].view(np.int32)[0])
+        if flags & _lib.DET_FEED_NONFINITE:
+            raise ValueError("detection scores and corners must be finite")
         raw = (_lib.SunrgbdEvalResult * Cn).from_buffer_copy(back[:Cn * _RES].tobytes()) if Cn else []
         bad = [gt.classes[i] for i in range(Cn) if raw[i].status]
         if bad:

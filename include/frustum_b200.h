@@ -1037,6 +1037,43 @@ FCN_API int fcn_sunrgbd_extract_count(const fcn_sunrgbd_extract_args *args, fcn_
 FCN_API int fcn_sunrgbd_extract_select(const fcn_sunrgbd_extract_args *args, fcn_stream_t stream);
 FCN_API int fcn_sunrgbd_extract_write(const fcn_sunrgbd_extract_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (19) The evaluators' inputs from the detection collector's device rows: sections (13) and (14) fed from the rows of
+ *      section (10) with no host pass over the rows.
+ *
+ *      rows / seg_offsets / keep_count are fcn_det_select's and fcn_det_prepare's outputs: kept row k of segment s is
+ *      rows[seg_offsets[s] + k], k < keep_count[s].  The gather plan is per segment: seg_dst[s] is the output record of
+ *      the segment's first kept row (its rows follow in row order), or -1 when the segment is not written;
+ *      seg_value[s] is the KITTI type code (FCN_KITTI_*) or the SUN-RGBD ground-truth segment (or -1) of its rows.
+ *      host_* are HOST copies, validated before anything is launched: seg_offsets start at 0, never decrease and end
+ *      at num_rows, keep_count[s] fits its segment, every written segment stays inside [0, num_out) and their kept
+ *      rows add up to num_out.  One launch (one thread per counted row), no host sync, no allocation, no workspace.
+ *        fcn_det_kitti_records : records (num_out, FCN_KITTI_DET_COLS) of section (13): the type code, alpha =
+ *                                compute_alpha(tx, tz, ry), box2d, h, w, l, tx, ty, tz, ry, each as '%.4f' then strtod
+ *                                would give it, and the score as '%f' (exact: rint(x * 10^d) / 10^d in float64).
+ *        fcn_det_sunrgbd_feed  : corners (num_out, 8, 3), scores (num_out) and segments (num_out) of section (14):
+ *                                compute_box_3d's corners (float32 cos, sin and half sizes, float64 rotation and
+ *                                translation, each operation rounded on its own), the float64 score and seg_value[s];
+ *                                *status |= FCN_DET_FEED_NONFINITE (status may be NULL) when a score or corner is not
+ *                                finite.
+ *      atan2, cos and sin are computed in float64 and rounded once to float32 (the correctly rounded float32 value;
+ *      numpy's float32 loops differ from it in the last bit on some inputs, depending on the CPU).
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_DET_FEED_NONFINITE 1
+typedef struct {
+    int num_segments, num_rows, num_out, reserved0;
+    const float *rows;                              /* DEVICE (num_rows, 12) */
+    const int32_t *seg_offsets, *keep_count;        /* DEVICE (num_segments + 1), (num_segments) */
+    const int32_t *seg_dst, *seg_value;             /* DEVICE (num_segments) each */
+    const int32_t *host_seg_offsets, *host_keep_count, *host_seg_dst;   /* HOST copies */
+    double *records;                                /* fcn_det_kitti_records: DEVICE (num_out, FCN_KITTI_DET_COLS) */
+    double *corners, *scores;                       /* fcn_det_sunrgbd_feed: DEVICE (num_out, 8, 3), (num_out) */
+    int32_t *segments;                              /* fcn_det_sunrgbd_feed: DEVICE (num_out) */
+    int32_t *status;                                /* fcn_det_sunrgbd_feed: DEVICE int32, optional */
+} fcn_det_eval_feed_args;
+FCN_API int fcn_det_kitti_records(const fcn_det_eval_feed_args *args, fcn_stream_t stream);
+FCN_API int fcn_det_sunrgbd_feed(const fcn_det_eval_feed_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
