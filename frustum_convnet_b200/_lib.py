@@ -319,6 +319,32 @@ class DetEvalFeedArgs(C.Structure):
                                           "scores", "segments", "status")]
 
 
+REFINE_ROW_NONFINITE, REFINE_ROW_EXTENTS, REFINE_ROW_DROPPED = 1, 2, 4
+REFINE_LIST_COLS = 34
+
+
+class RefineJobData(C.Structure):
+    _fields_ = [("cut", C.c_double * 7), ("box2d", C.c_double * 4), ("prob", C.c_double), ("image", C.c_int32),
+                ("cls_index", C.c_int32)]
+
+
+class RefineGtTerms(C.Structure):
+    _fields_ = [("center", C.c_double * 3), ("heading", C.c_double), ("size", C.c_double * 3), ("dist", C.c_double)]
+
+
+class RefineJobsArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("mode", "num_pieces", "num_jobs", "num_rows")] + \
+               [(n, C.c_void_p) for n in ("rows", "piece_offsets", "piece_row", "piece_frame", "piece_image",
+                                          "piece_class", "host_piece_offsets", "host_piece_row", "jobs", "job_frame",
+                                          "job_ref", "status", "det_corners", "job_data")]
+
+
+class RefineFrustumTableArgs(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("mode", "labels", "num_kept", "num_jobs", "num_gt", "num_scales")] + \
+               [("stride", C.c_double * MAX_SCALES)] + \
+               [(n, C.c_void_p) for n in ("kept", "job_gt", "job_data", "gt_terms", "lists", "records", "words")]
+
+
 SUNRGBD_MAX_POINTS = 2048
 
 
@@ -406,6 +432,8 @@ SIGNATURES = {
     "fcn_sunrgbd_extract_write": (_I, [C.POINTER(SunrgbdExtractArgs), _P]),
     "fcn_det_kitti_records": (_I, [C.POINTER(DetEvalFeedArgs), _P]),
     "fcn_det_sunrgbd_feed": (_I, [C.POINTER(DetEvalFeedArgs), _P]),
+    "fcn_refine_jobs_from_rows": (_I, [C.POINTER(RefineJobsArgs), _P]),
+    "fcn_refine_frustum_table": (_I, [C.POINTER(RefineFrustumTableArgs), _P]),
 }
 
 _lib = None

@@ -17,6 +17,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "det_quantize.cuh"
 
 namespace fcn {
 
@@ -40,9 +41,6 @@ __device__ __forceinline__ int df_destination(const fcn_det_eval_feed_args &a, i
     const int dst = a.seg_dst[s];
     return (dst < 0 || k >= a.keep_count[s]) ? -1 : dst + k;
 }
-
-// '%.<d>f' then strtod of a float32 value, s = 10^d
-__device__ __forceinline__ double df_quantize(float v, double s) { return __ddiv_rn(rint(__dmul_rn((double)v, s)), s); }
 
 // compute_alpha (datasets/provider_sample.py:389-394) in numpy's float32 order: (-sign(b) * pi) / 2 + b + ry
 __device__ __forceinline__ float df_alpha(float x, float z, float ry) {

@@ -130,24 +130,28 @@ def read_counts(summary, n, who, bad_what):
     return K, M, words, kept
 
 
-def run_extract(family, a, sc, so, n, word_fields, outputs, dev, stream, timer, bad_what):
+def run_extract(family, a, sc, so, n, word_fields, outputs, dev, stream, timer, bad_what, extra_words=0, before=None):
     """The two device calls of an extractor family ('frustum_extract', 'refine_extract', 'gt_extract') on the current
     stream `stream`.  a: the family's args struct with its counts and inputs filled; sc, so: scan_table's scans and
     host scan offsets.  Uploads the scans, queries the workspace, runs fcn_<family>_count into one summary (info, then
     the per-job int32 words: n of them for each args field of word_fields), reads it back once (read_counts, naming
     bad_what), then runs fcn_<family>_write into new points, offsets and the tensors of outputs(K, M, words), a dict
     {args field: tensor or None}.  `timer(name)` (optional) marks "start", "count", "write_start" and "write".
+    extra_words int32 words follow the fields' words in the summary; before(their device address) (optional) runs just
+    before the count call, so a job-building launch can leave per-job words in the same read.
     -> (the int32 words, the kept jobs, {args field: output tensor}, points and offsets included)."""
     scan_dev = upload_scans(sc, dev)            # like so and the caller's upload, alive until the write is enqueued
     a.scans = scan_dev.data_ptr() if int(so[-1]) > 0 else None
     a.host_scan_offsets = so.ctypes.data
     ws, nbytes = workspace("fcn_%s_workspace_bytes" % family, dev, C.byref(a))
-    summary = torch.empty(4 + (len(word_fields) * n + 1) // 2, dtype=torch.int64, device=dev)
+    summary = torch.empty(4 + (len(word_fields) * n + extra_words + 1) // 2, dtype=torch.int64, device=dev)
     a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), nbytes, summary.data_ptr()
     for k, field in enumerate(word_fields):
         setattr(a, field, summary.data_ptr() + 32 + 4 * n * k)
     if timer is not None:
         timer("start")
+    if before is not None:
+        before(summary.data_ptr() + 32 + 4 * n * len(word_fields))
     _lib.call("fcn_%s_count" % family, C.byref(a), stream.cuda_stream)
     if timer is not None:
         timer("count")

@@ -33,9 +33,15 @@ not pinned.
 Detections are the collector's {idx: {class: (n, 12)}} taken as the values the reference reads back from the text
 write_detection_results writes (kitti_eval.detection_records), lines in class then row order; or the result files
 themselves (read_result_dir).  Ground truth is a label_2 directory (or a {idx: [KittiObject]} dict).  One host sync
-per call, to learn the kept frustums and their points.  No CPU fallback: CPU tensors and devices raise."""
+per call, to learn the kept frustums and their points.  No CPU fallback: CPU tensors and devices raise.
+
+from_collected / from_matched_collected take DetectionCollector.finalize_device()'s CollectedDetections instead of the
+dict: the rows stay on the device (csrc/refine_jobs.cu).  The host plans the jobs from segment metadata alone, the
+device reads each row back as its text, builds and checks its box and writes the job; after the count pass it writes
+the kept frustums' lists and their TrainBatchBuilder records (CollectedRefineFrustums).  Same one host read."""
 from __future__ import annotations
 
+import ctypes as C
 import os
 
 import numpy as np
@@ -45,9 +51,11 @@ from . import _lib
 from ._host import csr_offsets, cuda_device, upload
 from .frustum_extract import LabelledFrustums, frame_order, run_extract, scan_table
 from .kitti_eval import detection_records
+from .train_inputs import KITTI_CLASSES
 
 RATIO = 1.2                # the enlargement of every box that cuts points (prepare_data_refine.py:319, :489, :724)
 PERTURB_RATIO = 0.05       # random_shift_rotate_box3d(., 0.05) of the training set (:328-329)
+REFINE_STRIDES = (0.1, 0.2, 0.4, 0.8)   # cfg.DATA.STRIDE of cfgs/refine_car.yaml: the strides of the records
 
 
 class KittiObject:
@@ -303,6 +311,19 @@ class RefineFrustumExtractor:
         jobs, _ = job_table(_lib.REFINE_DET, image_ids, dets, None, self.type_whitelist)
         return self._run(_lib.REFINE_DET, scans, calibs, image_hw, jobs, {}, stream, timer)
 
+    def from_collected(self, scans, calibs, image_hw, image_ids, collected, strides=REFINE_STRIDES, stream=None,
+                       timer=None):
+        """from_detections(.., collected.to_dict()) without the rows leaving the device -> CollectedRefineFrustums.
+        collected: DetectionCollector.finalize_device()'s CollectedDetections; strides: those of the records."""
+        return self._run_collected(_lib.REFINE_DET, scans, calibs, image_hw, image_ids, collected, None, False,
+                                   strides, stream, timer)
+
+    def from_matched_collected(self, scans, calibs, image_hw, image_ids, collected, gt, remove_diff=False,
+                               strides=REFINE_STRIDES, stream=None, timer=None):
+        """from_matched_detections(.., collected.to_dict(), gt, remove_diff) without the rows leaving the device."""
+        return self._run_collected(_lib.REFINE_MATCHED, scans, calibs, image_hw, image_ids, collected, gt,
+                                   remove_diff, strides, stream, timer)
+
     @property
     def iou_thresh(self):
         return iou_thresh(self.type_whitelist)
@@ -372,6 +393,104 @@ class RefineFrustumExtractor:
         return self._result(mode, out["points"], out["offsets"], out["labels"], job_points[kept].astype(np.int64),
                             kept.astype(np.int64), job_gt[kept].astype(np.int64), jobs, gt_flat, calibs, stream)
 
+    def _run_collected(self, mode, scans, calibs, image_hw, image_ids, collected, gt, remove_diff, strides, stream,
+                       timer):
+        dev = self.device
+        strides = [float(s) for s in strides]
+        if not 1 <= len(strides) <= _lib.MAX_SCALES:
+            raise ValueError("need 1..%d strides" % _lib.MAX_SCALES)
+        gts = None
+        if mode == _lib.REFINE_MATCHED:
+            gt = objects_of(gt, image_ids)
+            gts = {int(i): ground_truth_boxes(gt[int(i)], self.type_whitelist, remove_diff) for i in image_ids}
+        plan = collected_plan(image_ids, collected, self.type_whitelist, gts)
+        frame_ids, J = plan["frame_ids"], int(plan["offsets"][-1])
+        gt_flat, gt_off = [], [0]
+        for k in frame_ids:
+            gt_flat += gts[k] if gts is not None else []
+            gt_off.append(len(gt_flat))
+        G = len(gt_flat)
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.device(dev), torch.cuda.stream(stream):
+            if collected.stream.cuda_stream != stream.cuda_stream:
+                stream.wait_stream(collected.stream)
+            if J == 0:
+                return CollectedRefineFrustums.empty(mode, dev, strides, stream)
+            sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "RefineFrustumExtractor")
+            gt_arr = [obj_array(o) for o in gt_flat]
+            parts = [bytes(frames), so, plan["offsets"], plan["row"], plan["frame"], plan["image"], plan["class"],
+                     np.array([box_record(a) for a in gt_arr], dtype=np.dtype(_lib.RefineBox))]
+            if mode == _lib.REFINE_MATCHED:
+                job_frame = np.repeat(plan["frame"], np.diff(plan["offsets"]))
+                po = csr_offsets(np.diff(np.asarray(gt_off, np.int64))[job_frame])
+                parts += [iou_corners(np.stack(gt_arr)) if G else np.zeros(0), np.asarray(gt_off, np.int32), po,
+                          gt_terms(gt_flat, gt_arr)]
+            inp, ptrs = upload(parts, dev)
+            f64 = lambda *shape: torch.empty(shape, dtype=torch.float64, device=dev)
+            i32 = lambda n: torch.empty(n, dtype=torch.int32, device=dev)
+            jobs = f64(J, 8)                                       # fcn_refine_box
+            job_frame_d, job_ref = i32(J), i32(J)
+            job_data = torch.empty((J, C.sizeof(_lib.RefineJobData)), dtype=torch.uint8, device=dev)
+            det_c = f64(J, 24) if mode == _lib.REFINE_MATCHED else None
+            ja = _lib.RefineJobsArgs()
+            ja.mode, ja.num_pieces, ja.num_jobs, ja.num_rows = mode, len(plan["row"]), J, collected.num_rows
+            ja.rows = collected.rows.data_ptr()
+            ja.piece_offsets, ja.piece_row, ja.piece_frame, ja.piece_image, ja.piece_class = ptrs[2:7]
+            ja.host_piece_offsets, ja.host_piece_row = plan["offsets"].ctypes.data, plan["row"].ctypes.data
+            ja.jobs, ja.job_frame, ja.job_ref = jobs.data_ptr(), job_frame_d.data_ptr(), job_ref.data_ptr()
+            ja.job_data = job_data.data_ptr()
+            ja.det_corners = None if det_c is None else det_c.data_ptr()
+
+            def build_jobs(status_ptr):
+                ja.status = status_ptr
+                _lib.call("fcn_refine_jobs_from_rows", C.byref(ja), stream.cuda_stream)
+
+            a = _lib.RefineExtractArgs()
+            a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, len(frame_ids), int(so[-1]), J, G
+            a.iou_thresh = self.iou_thresh
+            a.frames, a.scan_offsets = ptrs[0], ptrs[1]
+            a.jobs, a.job_frame, a.job_ref = jobs.data_ptr(), job_frame_d.data_ptr(), job_ref.data_ptr()
+            a.gt_boxes = ptrs[7] if G > 0 else None
+            if mode == _lib.REFINE_MATCHED:
+                a.num_dets, a.num_pairs = J, int(po[-1])
+                a.det_frame, a.det_corners = a.job_frame, det_c.data_ptr()
+                a.gt_corners, a.gt_offsets, a.pair_offsets = ptrs[8:11]
+
+            def outputs(K, M, words):
+                check_collected(mode, plan, collected, words[J:2 * J], words[2 * J:3 * J], gt_flat, gt_arr)
+                return {"labels": None if mode == _lib.REFINE_DET else torch.empty(M, dtype=torch.uint8, device=dev)}
+
+            words, kept, out = run_extract("refine_extract", a, sc, so, J, ("job_points", "job_gt"), outputs, dev,
+                                           stream, timer, "jobs or pairs reference no frame or box", J, build_jobs)
+            K, S = len(kept), len(strides)
+            labels = mode == _lib.REFINE_MATCHED
+            kept_d = torch.from_numpy(kept.astype(np.int32)).to(dev, non_blocking=False)
+            lists = f64(K, _lib.REFINE_LIST_COLS)
+            records = torch.zeros((K, C.sizeof(_lib.TrainFrustum)), dtype=torch.uint8, device=dev)
+            rwords = torch.empty((K, S + 1), dtype=torch.int32, device=dev)
+            ta = _lib.RefineFrustumTableArgs()
+            ta.mode, ta.labels, ta.num_kept, ta.num_jobs, ta.num_gt, ta.num_scales = mode, int(labels), K, J, G, S
+            for q, st in enumerate(strides):
+                ta.stride[q] = st
+            ta.kept, ta.job_data = kept_d.data_ptr(), job_data.data_ptr()
+            job_gt_d = None
+            if labels:
+                job_gt_d = torch.from_numpy(np.ascontiguousarray(words[J:2 * J])).to(dev)
+                ta.job_gt, ta.gt_terms = job_gt_d.data_ptr(), ptrs[11]
+            ta.lists, ta.records, ta.words = lists.data_ptr(), records.data_ptr(), rwords.data_ptr()
+            if timer is not None:
+                timer("table_start")
+            _lib.call("fcn_refine_frustum_table", C.byref(ta), stream.cuda_stream)
+            if timer is not None:
+                timer("table")
+        pk = np.searchsorted(plan["offsets"], kept, side="right") - 1
+        kept_gt = words[J:2 * J][kept].astype(np.int64)
+        return CollectedRefineFrustums(mode, out["points"], out["offsets"], out["labels"],
+                                       words[kept].astype(np.int64), kept.astype(np.int64),
+                                       plan["image"][pk].tolist(), [plan["types"][p] for p in pk.tolist()],
+                                       bool((plan["class"][pk] >= 0).all()), lists, records, rwords, strides,
+                                       kept_gt, gt_flat, calibs, stream)
+
     @staticmethod
     def _result(mode, points, offsets, label, counts, kept, kept_gt, jobs, gt_flat, calibs, stream):
         L = {n: [] for n in ("id_list", "box2d_list", "type_list", "frustum_angle_list", "prob_list", "calib_list",
@@ -402,3 +521,139 @@ class RefineFrustumExtractor:
             for n in ("box3d_list", "heading_list", "size_list"):
                 L[n] = None
         return RefineFrustums(mode, points, offsets, label, counts, kept, L, stream)
+
+
+# ------------------------------------------------------------------------------ from the collector's device rows
+def collected_plan(image_ids, collected, type_whitelist, gts=None):
+    """The gather plan of fcn_refine_jobs_from_rows from the collector's segment metadata alone, in the dict path's job
+    order: the images of image_ids (in matched mode, gts given, only those with ground truth), the whitelisted classes
+    of each in the collector's dict order, their kept rows.  -> dict of the pieces (one per segment with kept rows):
+    offsets (P + 1) int32 (the first job of each), row / frame / image / class (P) int32 (the first row, the frame's
+    position in frame_ids, the image, the KITTI_CLASSES index or -1), types (P) class names, and frame_ids (the images
+    with jobs, in first-appearance order)."""
+    by_image = {}
+    for s in collected.order.tolist():
+        idx, ct = collected.segments[s]
+        if ct in type_whitelist and collected.host_keep_count[s] > 0:
+            by_image.setdefault(int(idx), []).append(s)
+    segs, frame, pos = [], [], {}
+    for idx in image_ids:
+        idx = int(idx)
+        if gts is not None and not gts[idx]:
+            continue                                                     # :458-459
+        for s in by_image.get(idx, ()):
+            segs.append(s)
+            frame.append(pos.setdefault(idx, len(pos)))
+    segs = np.asarray(segs, dtype=np.int64)
+    types = [collected.segments[s][1] for s in segs.tolist()]
+    return {"offsets": csr_offsets(collected.host_keep_count[segs]),
+            "row": np.ascontiguousarray(collected.host_seg_offsets[segs], dtype=np.int32),
+            "frame": np.asarray(frame, dtype=np.int32),
+            "image": np.array([int(collected.segments[s][0]) for s in segs.tolist()], dtype=np.int32),
+            "class": np.array([KITTI_CLASSES.index(t) if t in KITTI_CLASSES else -1 for t in types], dtype=np.int32),
+            "types": types, "segs": segs, "frame_ids": list(pos)}
+
+
+def gt_terms(gt_flat, gt_arr):
+    """The ground-truth terms of the refine records, per ground truth, with frustum_table's expressions."""
+    t = np.zeros(len(gt_flat), dtype=np.dtype(_lib.RefineGtTerms))
+    for r, o, a in zip(t, gt_flat, gt_arr):
+        b3 = compute_box_3d_obj_array(a)
+        size = np.array([o.l, o.w, o.h])
+        l, w, h = size
+        r["center"], r["heading"], r["size"] = (b3[0, :] + b3[6, :]) / 2, o.ry, size
+        r["dist"] = np.sqrt(np.sum(l ** 2 + w ** 2))
+    return t
+
+
+def collected_object(plan, collected, j):
+    """Job j's row as from_detections sees it: the KittiObject objects_from_detections makes (one row read)."""
+    p = int(np.searchsorted(plan["offsets"], j, side="right") - 1)
+    n = int(j - plan["offsets"][p])
+    row = collected.rows[int(plan["row"][p]) + n].cpu().numpy()
+    idx, ct = int(plan["image"][p]), plan["types"][p]
+    r = detection_records(row.reshape(1, 12), ct)[0]
+    return KittiObject(ct, -1.0, -1, float(r[1]), [float(v) for v in r[2:6]], float(r[6]), float(r[7]), float(r[8]),
+                       [float(v) for v in r[9:12]], float(r[12]), float(r[13]), "detections[%d][%r] row %d" % (idx, ct, n))
+
+
+def check_collected(mode, plan, collected, job_gt, status, gt_flat, gt_arr):
+    """The ValueError the dict path raises for the same rows, from the jobs' status words (read back with the count):
+    a non-finite box, or (in matched mode only for a matched pair, check_matched_extents) a non-positive extent."""
+    bad = status & (_lib.REFINE_ROW_NONFINITE | (_lib.REFINE_ROW_EXTENTS if mode == _lib.REFINE_DET else 0))
+    if bad.any():
+        j = int(np.argmax(bad != 0))
+        obj = collected_object(plan, collected, j)
+        _check_box(obj_array(obj), obj, mode == _lib.REFINE_DET)
+    if mode != _lib.REFINE_MATCHED:
+        return
+    m = np.flatnonzero(job_gt >= 0)
+    gt_bad = np.array([not (np.isfinite(a).all() and a[3] > 0 and a[4] > 0 and a[5] > 0) for a in gt_arr], bool)
+    bad = ((status[m] & _lib.REFINE_ROW_EXTENTS) != 0) | gt_bad[job_gt[m]] if len(m) else np.zeros(0, bool)
+    if bad.any():
+        j = int(m[np.argmax(bad)])
+        obj = collected_object(plan, collected, j)
+        _check_box(obj_array(obj), obj)
+        g = gt_flat[job_gt[j]]
+        _check_box(obj_array(g), g)
+
+
+class CollectedRefineFrustums(RefineFrustums):
+    """RefineFrustums from the collector's device rows.  Device: points, offsets, label as RefineFrustums; lists (K,
+    FCN_REFINE_LIST_COLS) float64 and its views frustum_angle (K), pred_box3d (K, 8, 3), pred_box3d_size (K, 3),
+    pred_box3d_angle (K), box2d (K, 4), prob (K); frustum_records (K fcn_train_frustum records for record_strides,
+    which TrainBatchBuilder.from_frustums installs as they are) and record_words (K, S + 1) int32 (T per scale, the
+    degenerate flag).  Host, at once: counts, job_index, id_list, type_list.  The provider's other lists are built on
+    first use from one copy of `lists`."""
+
+    _LAZY = ("box2d_list", "frustum_angle_list", "prob_list", "calib_list", "box3d_list", "heading_list", "size_list",
+             "pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list")
+
+    def __init__(self, mode, points, offsets, label, counts, job_index, id_list, type_list, classes_ok, lists,
+                 records, record_words, strides, kept_gt, gt_flat, calibs, stream):
+        LabelledFrustums.__init__(self, points, offsets, label, counts, job_index, stream)
+        self.mode = mode
+        self.has_labels = mode != _lib.REFINE_DET
+        self.pickle_names = _GT_NAMES if self.has_labels else _DET_NAMES
+        self.id_list, self.type_list = id_list, type_list
+        K = len(id_list)
+        self.lists = lists
+        self.frustum_angle, self.pred_box3d = lists[:, 0], lists[:, 1:25].view(K, 8, 3)
+        self.pred_box3d_size, self.pred_box3d_angle = lists[:, 25:28], lists[:, 28]
+        self.box2d, self.prob = lists[:, 29:33], lists[:, 33]
+        self.frustum_records, self.record_words = records, record_words
+        self.record_strides, self.record_labels = list(strides), self.has_labels
+        self.record_classes = KITTI_CLASSES if classes_ok else None
+        self._kept_gt, self._gt_flat, self._calibs = kept_gt, gt_flat, calibs
+
+    @classmethod
+    def empty(cls, mode, dev, strides, stream):
+        z = lambda *shape, dt=torch.float64: torch.zeros(shape, dtype=dt, device=dev)
+        return cls(mode, z(0, 4, dt=torch.float32), z(1, dt=torch.int32),
+                   None if mode == _lib.REFINE_DET else z(0, dt=torch.uint8), np.zeros(0, np.int64),
+                   np.zeros(0, np.int64), [], [], True, z(0, _lib.REFINE_LIST_COLS),
+                   z(0, C.sizeof(_lib.TrainFrustum), dt=torch.uint8), z(0, len(strides) + 1, dt=torch.int32), strides,
+                   np.zeros(0, np.int64), [], {}, stream)
+
+    def __getattr__(self, name):
+        if name in CollectedRefineFrustums._LAZY:
+            self._host_lists()
+            return self.__dict__[name]
+        raise AttributeError(name)
+
+    def _host_lists(self):
+        self.wait()
+        L = self.lists.cpu().numpy()
+        K = len(L)
+        d = {"frustum_angle_list": list(L[:, 0]), "pred_box3d_list": list(L[:, 1:25].reshape(K, 8, 3)),
+             "pred_box3d_size_list": list(L[:, 25:28]), "pred_box3d_angle_list": list(L[:, 28]),
+             "calib_list": [self._calibs[k] for k in self.id_list]}
+        if self.mode == _lib.REFINE_DET:
+            d.update(box2d_list=list(L[:, 29:33]), prob_list=L[:, 33].tolist(), box3d_list=None, heading_list=None,
+                     size_list=None)
+        else:
+            gts = [self._gt_flat[g] for g in self._kept_gt.tolist()]
+            d.update(box2d_list=[g.box2d for g in gts], prob_list=None,
+                     box3d_list=[compute_box_3d_obj_array(obj_array(g)) for g in gts],
+                     heading_list=[g.ry for g in gts], size_list=[np.array([g.l, g.w, g.h]) for g in gts])
+        self.__dict__.update(d)

@@ -280,14 +280,26 @@ class TrainBatchBuilder:
             raise RuntimeError("the frustums live on %s, the builder on %s" % (fr.points.device, tb.device))
         counts = np.asarray(fr.counts, dtype=np.int64)
         fr.wait()                          # the points and labels were written on the extraction's stream
+        tb.points_f64 = False
+        d_seg = fr.label.to(torch.int32) if gt else None
+        rec = getattr(fr, "frustum_records", None)
+        if rec is not None and fr.record_strides == tb.strides and fr.record_labels == tb.labels and \
+                fr.record_classes is not None and (classes is None or tuple(classes) == fr.record_classes):
+            # the extractor's device records (refine_extract.CollectedRefineFrustums): one read for T and the flags
+            S = len(tb.strides)
+            words = fr.record_words.cpu().numpy()
+            if words[:, S].any():
+                i = int(np.argmax(words[:, S]))
+                raise ValueError("frustum %d: degenerate predicted box (size %s)" % (i, fr.pred_box3d_size_list[i]))
+            tb._install_device(words[:, :S].astype(np.int64), rec, counts, fr.points[:, :3].contiguous(), None, d_seg)
+            return tb
         names = ("box3d_list", "heading_list", "size_list") + (
             ("frustum_angle_list", "box2d_list", "calib_list") if gt else
             ("prob_list", "pred_box3d_list", "pred_box3d_size_list", "pred_box3d_angle_list"))
         table = frustum_table(kind, tb.strides, tb.max_depth, tb.labels,
                               KITTI_CLASSES if classes is None else classes, fr.type_list,
                               **{n: getattr(fr, n) for n in names})
-        tb.points_f64 = False
-        tb._install(table, counts, fr.points[:, :3].contiguous(), None, fr.label.to(torch.int32) if gt else None)
+        tb._install(table, counts, fr.points[:, :3].contiguous(), None, d_seg)
         return tb
 
     @classmethod
@@ -312,13 +324,17 @@ class TrainBatchBuilder:
         return tb
 
     def _install(self, fr, counts, d_points, label_list, d_seg=None):
-        S = len(self.strides)
-        self.T_of = fr["T"][:, :S].astype(np.int64)
+        self._install_device(fr["T"][:, :len(self.strides)].astype(np.int64),
+                             torch.from_numpy(fr.view(np.uint8)).to(self.device), counts, d_points, label_list, d_seg)
+
+    def _install_device(self, T_of, d_frustums, counts, d_points, label_list, d_seg=None):
+        """T_of (F, S) host sections per scale, d_frustums the fcn_train_frustum records already on the device."""
+        self.T_of = T_of
         self.counts = counts
         dev = self.device
         self.d_points = d_points
         self.d_offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)).to(dev)
-        self.d_frustums = torch.from_numpy(fr.view(np.uint8)).to(dev)
+        self.d_frustums = d_frustums
         self.d_seg = d_seg
         if self._has_seg and d_seg is None:
             seg = np.concatenate([np.asarray(s).astype(np.int64) for s in label_list])  # provider_sample.py:206

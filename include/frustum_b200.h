@@ -1074,6 +1074,83 @@ typedef struct {
 FCN_API int fcn_det_kitti_records(const fcn_det_eval_feed_args *args, fcn_stream_t stream);
 FCN_API int fcn_det_sunrgbd_feed(const fcn_det_eval_feed_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (20) The refinement stage's inputs from the detection collector's device rows: the jobs of section (16) in
+ *      FCN_REFINE_DET or FCN_REFINE_MATCHED mode and the kept frustums' lists and fcn_train_frustum records of section
+ *      (11), with no host pass over the rows (kitti/prepare_data_refine.py --gen_val_det / --gen_from_folder fed from
+ *      the collector instead of result files).
+ *
+ *      The gather plan is per piece: piece p is the kept rows [piece_row[p], piece_row[p] + n_p) of one collector
+ *      segment (section (19)'s rows), n_p = piece_offsets[p + 1] - piece_offsets[p]; job piece_offsets[p] + i is row
+ *      piece_row[p] + i, in frame piece_frame[p] (an index into section (16)'s frames), image piece_image[p], class
+ *      index piece_class[p] (the fcn_train_frustum cls_index).  The host builds the plan from segment metadata alone,
+ *      in the job order of the dict path: the images of image_ids, then the collector's classes of each image in its
+ *      dict order (whitelisted ones only), then the rows.  host_piece_offsets / host_piece_row are HOST copies,
+ *      validated before anything is launched.  One launch each, no host sync, no allocation, no workspace.
+ *        fcn_refine_jobs_from_rows    one thread per job.  The row read back as its '%.4f' / '%f' text (section (19)'s
+ *                                     quantization), the box array a = [tx, ty - h/2, tz, l, w, h, ry] in float64,
+ *                                     every operation rounded on its own; status[j] |= FCN_REFINE_ROW_NONFINITE when a
+ *                                     is not finite, FCN_REFINE_ROW_EXTENTS when l, w or h is not positive, and in
+ *                                     FCN_REFINE_DET mode FCN_REFINE_ROW_DROPPED when ymax - ymin < 5 or xmax - xmin < 1
+ *                                     (the quantized 2-D box).  jobs[j]: the box enlarged x1.2 (centre, half extents,
+ *                                     cos / sin of ry); a bad or dropped job of FCN_REFINE_DET mode gets half extents
+ *                                     -1, so section (16)'s count pass keeps none of its points and drops it.
+ *                                     job_frame[j] = piece_frame, job_ref[j] = j; FCN_REFINE_MATCHED: det_corners[j]
+ *                                     (8, 3), rbbox_iou_3d's corners of a (not enlarged).  job_data[j]: the enlarged
+ *                                     box array, the quantized 2-D box and score, image and class index.
+ *        fcn_refine_frustum_table     after section (16)'s count pass, one thread per kept job kept[k]: lists (num_kept,
+ *                                     FCN_REFINE_LIST_COLS) float64: frustum_angle -atan2(cz, cx), the 24 corners of
+ *                                     compute_box_3d_obj_array (np.dot's dgemm order: the first product rounded, then
+ *                                     one FMA per term), the 3 sizes, the angle, the 2-D box, the score; records
+ *                                     (num_kept, zeroed by the caller): the refine fields of section (11) - rot, cs,
+ *                                     sn, ref_center, line0, line_delta, z_start, z_step and T for stride[0 ..
+ *                                     num_scales), cls_index and, when labels, the matched ground truth's terms
+ *                                     gt_terms[job_gt[j]] in the predicted box's frame, else rgb_prob = the score;
+ *                                     words (num_kept, num_scales + 1) int32: T per scale, then 1 when the predicted
+ *                                     box is degenerate (a T below 1 or a zero line), else 0.
+ *      cos, sin and atan2 are CUDA's float64 functions (within 2 ulp); everything else follows numpy's expressions.
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_REFINE_ROW_NONFINITE 1
+#define FCN_REFINE_ROW_EXTENTS 2
+#define FCN_REFINE_ROW_DROPPED 4
+#define FCN_REFINE_LIST_COLS 34   /* frustum_angle, pred_box3d (24), pred_box3d_size (3), pred_box3d_angle, box2d (4), prob */
+typedef struct {
+    double cut[7];      /* enlarged box array [tx, ty - h/2, tz, 1.2 l, 1.2 w, 1.2 h, ry] */
+    double box2d[4];    /* quantized x1, y1, x2, y2 */
+    double prob;        /* quantized score */
+    int32_t image, cls_index;
+} fcn_refine_job_data;
+typedef struct {
+    double center[3];   /* (box3d[0] + box3d[6]) / 2 of the ground truth's compute_box_3d_obj_array corners */
+    double heading;     /* ry */
+    double size[3];     /* l, w, h */
+    double dist;        /* sqrt(l^2 + w^2) */
+} fcn_refine_gt_terms;
+typedef struct {
+    int mode, num_pieces, num_jobs, num_rows;
+    const float *rows;                              /* DEVICE (num_rows, 12), the collector's rows */
+    const int32_t *piece_offsets;                   /* DEVICE (num_pieces + 1) */
+    const int32_t *piece_row, *piece_frame, *piece_image, *piece_class;   /* DEVICE (num_pieces) each */
+    const int32_t *host_piece_offsets, *host_piece_row;                    /* HOST copies */
+    fcn_refine_box *jobs;                           /* DEVICE (num_jobs) outputs */
+    int32_t *job_frame, *job_ref, *status;
+    double *det_corners;                            /* DEVICE (num_jobs, 8, 3), FCN_REFINE_MATCHED only */
+    fcn_refine_job_data *job_data;
+} fcn_refine_jobs_args;
+typedef struct {
+    int mode, labels, num_kept, num_jobs, num_gt, num_scales;
+    double stride[FCN_MAX_SCALES];
+    const int32_t *kept;                            /* DEVICE (num_kept): the job of each kept frustum */
+    const int32_t *job_gt;                          /* DEVICE (num_jobs): section (16)'s job_gt, labels only */
+    const fcn_refine_job_data *job_data;            /* DEVICE (num_jobs) */
+    const fcn_refine_gt_terms *gt_terms;            /* DEVICE (num_gt), labels only */
+    double *lists;                                  /* DEVICE (num_kept, FCN_REFINE_LIST_COLS) */
+    fcn_train_frustum *records;                     /* DEVICE (num_kept) */
+    int32_t *words;                                 /* DEVICE (num_kept, num_scales + 1) */
+} fcn_refine_frustum_table_args;
+FCN_API int fcn_refine_jobs_from_rows(const fcn_refine_jobs_args *args, fcn_stream_t stream);
+FCN_API int fcn_refine_frustum_table(const fcn_refine_frustum_table_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
