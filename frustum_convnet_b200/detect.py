@@ -11,10 +11,15 @@ train/test_net_det.py:243-305 (test_net_det_sunrgbd.py:197-266), with no per-bat
 `add` appends the foreground rows of a batch to device records (csrc/detect.cu, ``fcn_det_candidates``);
 `finalize` orders them as the reference's lists, runs rotated 3-D NMS on every image x class list of any length and
 returns {data_idx: {class_type: float32 (n, 12)}} in the reference's dict order, zero-row lists included (as
-(0, 12) arrays).  The collector belongs to one process and one device.  No CPU fallback: CPU tensors raise."""
+(0, 12) arrays).  The collector belongs to one device.  No CPU fallback: CPU tensors raise.
+
+With one process per GPU, ``DetectionCollector(..., group=pg)`` collects a sharded pass: every rank adds the frustums
+of its own chunk of each batch (``first`` stays the dataset index), and ``finalize_device()`` / ``finalize()`` on every
+rank of the group return what one collector that received every rank's adds would return."""
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 
 import numpy as np
 import torch
@@ -24,11 +29,60 @@ from ._host import cuda_device, workspace
 
 _DATASETS = {"KITTI": 0, "SUNRGBD": 1}
 _METHODS = {"nms": 0}          # every other cfg.TEST.METHOD behaves as 'top' (test_net_det.py:256-263)
+_SETUP_FIELDS = ("id_list", "type_list", "box2d_list", "dataset", "method", "thresh", "top_k", "num_frustums")
+
+
+def setup_digests(id_list, type_list, box2d_list, dataset, method, thresh, top_k):
+    """One digest per argument that defines the segment table and the finalize, in _SETUP_FIELDS order."""
+    h = lambda b: hashlib.sha256(b).hexdigest()
+    text = lambda xs: h("\x1f".join(str(x) for x in xs).encode())
+    return (text(id_list), text(type_list), h(np.ascontiguousarray(box2d_list, dtype=np.float32).tobytes()),
+            str(dataset), "nms" if method == "nms" else "top", repr(float(thresh)), repr(int(top_k)),
+            repr(len(id_list)))
+
+
+def check_same_setup(group, digests):
+    """Collective over `group`: raises the same ValueError on every rank unless every rank passed the same
+    setup_digests."""
+    import torch.distributed as dist
+    everyone = [None] * dist.get_world_size(group)
+    dist.all_gather_object(everyone, tuple(digests), group=group)
+    for r, theirs in enumerate(everyone):
+        differ = [name for name, a, b in zip(_SETUP_FIELDS, everyone[0], theirs) if a != b]
+        if differ:
+            raise ValueError("DetectionCollector: rank %d of the group was constructed with a different %s than rank "
+                             "0; every rank must describe the same dataset and finalize" % (r, ", ".join(differ)))
+
+
+def shard_merge_plan(counts, capacities, added):
+    """The host decisions of a sharded finalize, made alike on every rank from the gathered block: counts and
+    capacities (world,) of every rank's records, added (world, num_frustums) bool.  -> the frustums added on any rank
+    (num_frustums,) bool.  Raises ValueError naming the first frustum added on two ranks, and RuntimeError naming the
+    first rank whose rows overflowed its capacity."""
+    added = np.asarray(added, dtype=bool)
+    twice = np.flatnonzero(added.sum(axis=0) > 1)
+    if len(twice):
+        f = int(twice[0])
+        ranks = np.flatnonzero(added[:, f])
+        raise ValueError("DetectionCollector: frustum %d was added on ranks %d and %d; the shards of a pass must not "
+                         "overlap" % (f, ranks[0], ranks[1]))
+    for r, (n, cap) in enumerate(zip(np.asarray(counts).tolist(), np.asarray(capacities).tolist())):
+        if n > cap:
+            raise RuntimeError("DetectionCollector: record capacity exceeded on rank %d: %d rows were produced, the "
+                               "capacity is %d (needs capacity >= %d)" % (r, n, cap, n))
+    return added.any(axis=0)
 
 
 class DetectionCollector:
     def __init__(self, id_list, type_list, box2d_list, dataset="KITTI", method="nms", thresh=0.1, top_k=300,
-                 capacity=None, device=None):
+                 capacity=None, device=None, group=None):
+        """group: a torch.distributed process group for a sharded pass (None: this process's adds alone).  With a
+        group, construction is collective and raises the same ValueError on every rank if the ranks' id_list,
+        type_list, box2d_list, dataset, method, thresh or top_k differ."""
+        self.group = group
+        if group is not None:
+            with torch.cuda.device(cuda_device(device, "DetectionCollector")):
+                check_same_setup(group, setup_digests(id_list, type_list, box2d_list, dataset, method, thresh, top_k))
         if dataset not in _DATASETS:
             raise ValueError("dataset must be one of %s" % sorted(_DATASETS))
         n = len(id_list)
@@ -112,24 +166,33 @@ class DetectionCollector:
 
     def finalize_device(self):
         """-> CollectedDetections: the kept rows stay on the device; one host sync to size the NMS bit matrix and one
-        read of the per-segment offsets and keep counts (O(segments), no row crosses to the host)."""
+        read of the per-segment offsets and keep counts (O(segments), no row crosses to the host).
+
+        With a group this is collective (every rank of the group must call it) and every rank gets the same result:
+        the union of every rank's records, finalized as one collector's.  Raises the same error on every rank if a
+        frustum was added on two ranks or a rank overflowed its capacity."""
         dev = self.device
         cur = torch.cuda.current_stream(dev)
         for st in self._streams.values():
             if st.cuda_stream != cur.cuda_stream:
                 cur.wait_stream(st)
+        if self.group is None:
+            counter, records, capacity, added = self.counter, self.records, self.capacity, self.added
+        else:
+            with torch.cuda.device(dev):
+                counter, records, capacity, added = self._merge_ranks()
         S = len(self.segments)
         with torch.cuda.device(dev):
-            ws, nbytes = workspace("fcn_det_workspace_bytes", dev, self.capacity, S)
+            ws, nbytes = workspace("fcn_det_workspace_bytes", dev, capacity, S)
             info = torch.zeros(4, dtype=torch.int64, device=dev)
             off = torch.zeros(S + 1, dtype=torch.int32, device=dev)
             kc = torch.zeros(max(S, 1), dtype=torch.int32, device=dev)
-            rows = torch.empty((max(self.capacity, 1), 12), dtype=torch.float32, device=dev)
+            rows = torch.empty((max(capacity, 1), 12), dtype=torch.float32, device=dev)
             a = _lib.DetFinalizeArgs()
-            a.num_segments, a.num_frustums, a.capacity = S, self.num_frustums, self.capacity
+            a.num_segments, a.num_frustums, a.capacity = S, self.num_frustums, capacity
             a.method, a.dataset = _METHODS.get(self.method, 1), _DATASETS[self.dataset]
             a.top_k, a.thresh = self.top_k, self.thresh
-            a.counter, a.records, a.box2d = self.counter.data_ptr(), self.records.data_ptr(), self.box2d.data_ptr()
+            a.counter, a.records, a.box2d = counter.data_ptr(), records.data_ptr(), self.box2d.data_ptr()
             a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), nbytes, info.data_ptr()
             a.seg_offsets, a.keep_count, a.rows = off.data_ptr(), kc.data_ptr(), rows.data_ptr()
             _lib.call("fcn_det_prepare", C.byref(a), cur.cuda_stream)
@@ -142,10 +205,42 @@ class DetectionCollector:
         off_h, kc_h = offkc[:S + 1].copy(), offkc[S + 1:].copy()
         self.last_counts = {"rows": n_counted, "kept": int(kc_h.sum()) if S else 0}
         # dict order of the frustums that were added, in dataset order
-        segs = self._seg_host[self.added]
+        segs = self._seg_host[added]
         _, first_pos = np.unique(segs, return_index=True)
         order = segs[np.sort(first_pos)]
         return CollectedDetections(self.dataset, rows, off, kc, off_h, kc_h, list(self.segments), order, cur)
+
+    def _merge_ranks(self):
+        """-> (counter, records, capacity, added) of the union of every rank's records, on the current stream.  One
+        all_gather of each rank's counter, capacity and added flags, one host read of that block, then one all_gather
+        of the records.  Every decision is taken from the gathered block, so every rank takes it alike and none raises
+        while another waits in a collective.  The union is in rank order; fcn_det_prepare orders records by
+        (segment, frustum, t) whoever appended them, so it finalizes as one collector's records would."""
+        import torch.distributed as dist
+        dev, group, n = self.device, self.group, self.num_frustums
+        world = dist.get_world_size(group)
+        head = np.array([0, self.capacity], dtype=np.int32).view(np.uint8)
+        meta = torch.from_numpy(np.concatenate([head, self.added.view(np.uint8)])).pin_memory().to(
+            dev, non_blocking=True)
+        meta[:4].view(torch.int32).copy_(self.counter)
+        block = torch.empty((world, 8 + n), dtype=torch.uint8, device=dev)
+        dist.all_gather(list(block.unbind(0)), meta, group=group)
+        block = block.cpu().numpy()                                                # the one extra host sync
+        head = block[:, :8].copy().view(np.int32)
+        counts = head[:, 0].astype(np.int64)
+        added = shard_merge_plan(counts, head[:, 1], block[:, 8:].astype(bool))
+        total, most = int(counts.sum()), int(counts.max())
+        if most == 0:
+            records = torch.empty((1, 12), dtype=torch.int32, device=dev)
+        else:
+            send = self.records[:most]
+            if len(send) < most:                           # another rank produced more rows than this one's capacity
+                send = torch.cat([send, send.new_zeros((most - len(send), 12))])
+            recv = torch.empty((world, most, 12), dtype=torch.int32, device=dev)
+            dist.all_gather(list(recv.unbind(0)), send, group=group)
+            records = torch.cat([recv[r, :c] for r, c in enumerate(counts.tolist())])
+        counter = torch.full((1,), total, dtype=torch.int32, device=dev)
+        return counter, records, total, added
 
     def finalize(self):
         """-> {data_idx: {class_type: float32 (n, 12)}}; one host sync to size the NMS bit matrix, one copy back."""
