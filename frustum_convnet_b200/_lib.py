@@ -390,6 +390,7 @@ SIGNATURES = {
     "fcn_train_finalize": (_I, [_P, _I, _I, _P]),
     "fcn_adam_step": (_I, [_P, _P, _P, _P, C.c_longlong, _F, _F, _F, _F, _F, _I, _F, _P]),
     "fcn_sgd_step": (_I, [_P, _P, _P, C.c_longlong, _F, _F, _F, _I, _F, _P]),
+    "fcn_rank_fold": (_I, [_P, C.c_longlong, _I, C.c_longlong, _P, _P]),
     "fcn_rotate_nms_3d": (_I, [_I, _P, _P, _F, _I, _P, _P, _I, _P]),
     "fcn_rotate_nms_3d_max_dets": (_I, []),
     "fcn_det_loss": (_I, [C.POINTER(LossArgs), _P]),

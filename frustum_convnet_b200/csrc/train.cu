@@ -1436,3 +1436,63 @@ extern "C" int fcn_sgd_step(float *param, const float *grad, float *momentum_buf
     FCN_LAUNCH_CHECK();
     return FCN_OK;
 }
+
+// ------------------------------------------------------------------ rank-ordered fold of G gradient shards
+// dst[i] = ((src[i] + src[ld+i]) + src[2ld+i]) + ... + src[(G-1)ld+i], every add __fadd_rn (no FMA contraction can
+// touch it), so the sum has one order whatever the transport that gathered the G rows.  One thread per float4 of the
+// body when src, ld and dst allow 16-byte access; the threads past the body take the n % 4 tail elements one each.
+namespace fcn {
+
+template <bool V4>
+__global__ void __launch_bounds__(256) rank_fold_kernel(const float *__restrict__ src, long long ld, int G,
+                                                        long long n, float *__restrict__ dst) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    long long j = i;
+    if (V4) {
+        const long long n4 = n >> 2;
+        if (i < n4) {
+            const float4 *s = reinterpret_cast<const float4 *>(src) + i;
+            const long long ld4 = ld >> 2;
+            float4 a = __ldg(s);
+#pragma unroll 4
+            for (int r = 1; r < G; ++r) {
+                const float4 b = __ldg(s + r * ld4);
+                a.x = __fadd_rn(a.x, b.x);
+                a.y = __fadd_rn(a.y, b.y);
+                a.z = __fadd_rn(a.z, b.z);
+                a.w = __fadd_rn(a.w, b.w);
+            }
+            reinterpret_cast<float4 *>(dst)[i] = a;
+            return;
+        }
+        j = 4 * n4 + (i - n4);
+    }
+    if (j >= n) return;
+    float a = __ldg(src + j);
+#pragma unroll 4
+    for (int r = 1; r < G; ++r) a = __fadd_rn(a, __ldg(src + r * ld + j));
+    dst[j] = a;
+}
+
+}  // namespace fcn
+
+extern "C" int fcn_rank_fold(const float *src, long long ld, int G, long long n, float *dst, fcn_stream_t stream) {
+    FCN_REQUIRE(src != nullptr && dst != nullptr, "NULL src / dst");
+    FCN_REQUIRE(G >= 1, "G < 1");
+    FCN_REQUIRE(n >= 0, "n < 0");
+    FCN_REQUIRE(ld >= n, "ld < n");
+    FCN_REQUIRE(G == 1 || ld <= (INT64_MAX / 4 - n) / (G - 1), "(G - 1) * ld + n overflows the address range");
+    const uintptr_t s0 = (uintptr_t)src, s1 = s0 + 4 * (uintptr_t)((long long)(G - 1) * ld + n);
+    const uintptr_t d0 = (uintptr_t)dst, d1 = d0 + 4 * (uintptr_t)n;
+    FCN_REQUIRE(n == 0 || d1 <= s0 || s1 <= d0, "dst overlaps src");
+    if (n == 0) return FCN_OK;
+    const bool v4 = ((s0 | d0) & 15) == 0 && (ld & 3) == 0;
+    const long long threads = v4 ? (n >> 2) + (n & 3) : n;
+    const unsigned blocks = (unsigned)((threads + 255) / 256);
+    if (v4)
+        rank_fold_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(src, ld, G, n, dst);
+    else
+        rank_fold_kernel<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(src, ld, G, n, dst);
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
+}

@@ -12,7 +12,9 @@ drop-in ``model(data)`` path from PyTorch ops and their autograd (train_path.los
 ``backward`` runs the hand-written backward kernels.  Parameters live in ONE flat fp32 buffer (every
 ``nn.Parameter`` is a view), gradients in ONE flat bucket written in the parameter layout by the kernels:
 one ``all_reduce`` per step (SURVEY.md 8(e)) and one fused optimizer launch (``fcn_adam_step`` or ``fcn_sgd_step``).
-BatchNorm statistics are per rank (the reference's DataParallel semantics: per-replica BN, no SyncBN).
+BatchNorm statistics are per rank (the reference's DataParallel semantics: per-replica BN, no SyncBN).  In
+deterministic mode the gradient is summed over the ranks in rank order (all-to-all, ``fcn_rank_fold``, all-gather)
+and every rank adopts rank 0's BN running statistics after each step, DataParallel's replica-0 buffers.
 """
 from __future__ import annotations
 
@@ -402,6 +404,81 @@ class TrainEngine:
         return n_fwd + n_bwd + 1      # + fused Adam or SGD
 
 
+def piece_split(model) -> int:
+    """Where the flat bucket is cut in two for the reduction over ranks: [0, split) is the PointNet (feat_net) piece,
+    [split, n) the ConvFeatNet + heads piece, whose gradient is complete first."""
+    first = next(model.conv_net.parameters())
+    off = 0
+    for p in model.parameters():
+        if p is first:
+            return off
+        off += p.numel()
+    raise ValueError("the model's conv_net parameters are not among its parameters")
+
+
+def shard_plan(n: int, world: int):
+    """The cut of a gradient piece of `n` floats for the rank-ordered reduction over `world` ranks -> (shard,
+    padded): rank r reduces floats [r*shard, (r+1)*shard) of the piece padded to padded = world*shard floats (the
+    padding's sums are never copied back).
+    `shard` is a multiple of 4, so every shard starts 16 bytes apart in the staging buffers and the fold takes its
+    float4 path.  Depends on (n, world) only, so every rank cuts alike."""
+    if n < 1 or world < 1:
+        raise ValueError("shard_plan: n = %d and world = %d must be >= 1" % (n, world))
+    shard = ((n + world - 1) // world + 3) // 4 * 4
+    return shard, world * shard
+
+
+class _RankOrderedReduce:
+    """The deterministic mode's sum of the gradient over the ranks.  Each piece is cut by `shard_plan`; one
+    ``all_to_all_single`` hands every rank its shard of every rank's piece as [world][shard], ``fcn_rank_fold`` sums
+    them in rank order and one ``all_gather_into_tensor`` writes the summed shards back.  The collectives only copy,
+    so the bits do not depend on the transport's algorithm.  Per rank the two copies move 2 (world-1)/world of the
+    piece, as a ring all-reduce does.  The staging buffers are allocated once, for the larger piece."""
+
+    def __init__(self, pieces, world, device):
+        self.world = world
+        plans = [shard_plan(n, world) for n in pieces]
+        padded = max(p for _, p in plans)
+        self.send = torch.zeros(padded, dtype=torch.float32, device=device)
+        self.recv = torch.zeros(padded, dtype=torch.float32, device=device)
+        self.out = torch.zeros(max(s for s, _ in plans), dtype=torch.float32, device=device)
+
+    def __call__(self, piece):
+        """Sum `piece` (contiguous float32) over the ranks in place, on the current stream."""
+        import torch.distributed as dist
+        n = piece.numel()
+        shard, padded = shard_plan(n, self.world)
+        send, recv, out = self.send[:padded], self.recv[:padded], self.out[:shard]
+        send[:n].copy_(piece)
+        dist.all_to_all_single(recv, send)
+        _lib.call("fcn_rank_fold", _ptr(recv), shard, self.world, shard, _ptr(out), _stream())
+        dist.all_gather_into_tensor(send, out)
+        piece.copy_(send[:n])
+
+
+class _BufferBroadcast:
+    """Rank 0's BatchNorm buffers (running_mean, running_var, num_batches_tracked of every BN) to every rank in one
+    broadcast of one packed byte buffer, on the current stream."""
+
+    def __init__(self, model, device):
+        bns = [m for m in model.modules()
+               if isinstance(m, torch.nn.modules.batchnorm._BatchNorm) and m.track_running_stats]
+        counters = [m.num_batches_tracked.view(-1) for m in bns]
+        stats = [b for m in bns for b in (m.running_mean, m.running_var)]
+        assert all(b.dtype == torch.float32 for b in stats) and all(c.dtype == torch.int64 for c in counters)
+        nc, nf = 8 * len(counters), 4 * sum(b.numel() for b in stats)
+        self.packed = torch.zeros(nc + nf, dtype=torch.uint8, device=device)
+        views = list(self.packed[:nc].view(torch.int64).split([1] * len(counters))) + \
+            list(self.packed[nc:].view(torch.float32).split([b.numel() for b in stats]))
+        self.bufs, self.views = counters + stats, views
+
+    def __call__(self):
+        import torch.distributed as dist
+        torch._foreach_copy_(self.views, self.bufs)
+        dist.broadcast(self.packed, src=0)
+        torch._foreach_copy_(self.bufs, self.views)
+
+
 class _FlatOptimizer:
     """What FlatAdam and FlatSGD share, mixed in before their torch optimizer class: one parameter group over all of
     a model's parameters (FlatParams order) whose state lives in flat buffers of the bucket's layout, a
@@ -617,7 +694,8 @@ class TrainStep:
     train_net_det.py:321-328) selects a torch.optim.Adam (FlatAdam) or torch.optim.SGD (FlatSGD, with ``momentum``)
     for lr schedulers and checkpoints; ``states`` (validate.TrainStates) collects every step's losses and metrics on
     the device.  ``deterministic`` (settable): True runs the step bit-reproducibly (deterministic layer kernels and
-    fused loss; one GPU, one build, same inputs and hyper-parameters), False the default kernels, None follows
+    fused loss; one build, same inputs and hyper-parameters; with world > 1 a rank-ordered gradient sum and rank 0's
+    BN buffers on every rank, so every rank holds the same model), False the default kernels, None follows
     ``torch.use_deterministic_algorithms`` at every step."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, comm_stream=None,
@@ -633,9 +711,11 @@ class TrainStep:
             self.optimizer = FlatAdam(model, self.flat, lr, betas, eps, weight_decay)
         else:
             self.optimizer = FlatSGD(model, self.flat, lr, momentum, weight_decay)
-        self.states = TrainStates(self.flat.param.device, states_capacity)
+        self.states = TrainStates(self.flat.param.device, states_capacity, deterministic=self._deterministic_now)
         self._comm = None
         self._split = 0
+        self._ordered = None           # _RankOrderedReduce and _BufferBroadcast, built on the first such step
+        self._bn_bcast = None
         self._fused_losses = {}        # train_path.FusedLoss per (deterministic, B, T2)
         self.deterministic = deterministic
 
@@ -681,6 +761,10 @@ class TrainStep:
     def step_count(self):
         return self.optimizer.step_count
 
+    def _deterministic_now(self) -> bool:
+        from .train_path import deterministic_mode
+        return deterministic_mode(self.deterministic)
+
     def engine(self, B, N, T, deterministic=False) -> TrainEngine:
         key = (int(B), int(N), tuple(int(t) for t in T), bool(deterministic))
         e = self.engines.get(key)
@@ -724,7 +808,9 @@ class TrainStep:
     def step(self, data):
         """forward + losses + backward + gradient all-reduce + Adam or SGD.  With world > 1 the flat bucket is reduced in
         TWO pieces on a communication stream: the FCN + heads part (92 % of the parameters, complete after the
-        first ~15 % of the backward) overlaps the PointNet backward; the PointNet part follows."""
+        first ~15 % of the backward) overlaps the PointNet backward; the PointNet part follows.  In deterministic mode
+        each piece is summed in rank order (`_RankOrderedReduce`) and rank 0's BN buffers are then broadcast on the
+        same stream, so every rank ends the step with the same parameters, optimizer state and buffers."""
         import torch.distributed as dist
         world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         eng, losses, metrics, dcls, dreg = self._forward_losses(data)
@@ -732,21 +818,27 @@ class TrainStep:
         if world > 1:
             if self._comm is None:
                 self._comm = torch.cuda.Stream(device=self.flat.grad.device)
-                first = next(self.model.conv_net.parameters())
-                self._split = self.flat.offsets[id(first)]        # [0, split): feat_net, [split, n): conv_net + heads
+                self._split = piece_split(self.model)       # [0, split): feat_net, [split, n): conv_net + heads
+            if eng.deterministic and (self._ordered is None or self._ordered.world != world):
+                dev = self.flat.grad.device
+                self._ordered = _RankOrderedReduce((self._split, self.flat.numel - self._split), world, dev)
+                self._bn_bcast = _BufferBroadcast(self.model, dev)
+            reduce = self._ordered if eng.deterministic else dist.all_reduce
             cur = torch.cuda.current_stream()
             eng.backward(dcls, dreg, stage="fcn")
             ev = torch.cuda.Event()
             ev.record(cur)
             self._comm.wait_event(ev)
             with torch.cuda.stream(self._comm):
-                dist.all_reduce(self.flat.grad[self._split:])
+                reduce(self.flat.grad[self._split:])
             eng.backward(None, None, stage="pointnet")
             ev2 = torch.cuda.Event()
             ev2.record(cur)
             self._comm.wait_event(ev2)
             with torch.cuda.stream(self._comm):
-                dist.all_reduce(self.flat.grad[: self._split])
+                reduce(self.flat.grad[: self._split])
+                if eng.deterministic:
+                    self._bn_bcast()
             cur.wait_stream(self._comm)
         else:
             eng.backward(dcls, dreg)

@@ -9,6 +9,10 @@ of every batch from the fused forward's head logits, averaged over the epoch wit
 
 `TrainStates` keeps the reference train() loop's per-step TrainingStates the same way (``TrainStep.states``).
 
+A sharded pass (one process per GPU, each rank adding its chunk of every batch) constructs
+``Validator(model, group=dist.group.WORLD)``: `finalize` is then collective and every rank returns the same averages,
+those of each batch's values averaged over the ranks, as the reference logs them under DataParallel.
+
 `add` stages the batch into the forward plan of its (B, N, T) shape, replays the plan's forward graph and runs
 ``fcn_val_batch`` (csrc/validate.cu) on the plan's pitched head logits; the batch's 14 values are appended to a
 device table.  `finalize` replays the reference's float64 AverageMeter over that table (``fcn_val_finalize``) and
@@ -115,6 +119,33 @@ class _MeterTable:
             t = self.table[:n].cpu().numpy()
         return np.ascontiguousarray(t if full else t[:, :_lib.VAL_VALUES])
 
+    def _over_ranks(self, group, ordered):
+        """(table, state) as the reference's DataParallel loop logs them: each row's values averaged over the
+        ranks of `group`, B / nfg / nkeep summed (the full batch), the status bits of every rank and the earliest
+        row without a foreground row on any rank.  ordered=True sums the rows in rank order (one all_gather of the
+        table and ``fcn_rank_fold``), so the bits do not depend on the transport; False takes one all_reduce.  The
+        flags are reduced by one integer MAX all_reduce, which is exact.  Collective; runs on the current stream."""
+        import torch.distributed as dist
+        world = dist.get_world_size(group)
+        if ordered:
+            n = self.table.numel()
+            rows = torch.empty(world * n, dtype=self.table.dtype, device=self.device)
+            dist.all_gather_into_tensor(rows, self.table.view(-1), group=group)
+            table = torch.empty_like(self.table)
+            _lib.call("fcn_rank_fold", rows.data_ptr(), n, world, n, table.data_ptr(),
+                      torch.cuda.current_stream(self.device).cuda_stream)
+        else:
+            table = self.table.clone()
+            dist.all_reduce(table, group=group)
+        table[:, :_lib.VAL_VALUES] /= world
+        s = self.state
+        no_fg = (s[1] & _lib.VAL_NO_FG) != 0
+        flags = torch.stack([s[1] & _lib.VAL_NO_FG, s[1] & _lib.VAL_OVERFLOW,
+                             torch.where(no_fg, -s[2], torch.full_like(s[2], -(2 ** 31 - 1)))])
+        dist.all_reduce(flags, op=dist.ReduceOp.MAX, group=group)   # OR of the bits, earliest row without foreground
+        state = torch.stack([s[0], flags[0] | flags[1], -flags[2], s[3]])
+        return table, state
+
     def _replay(self, table, state):
         """fcn_val_finalize over `table` and `state`, one host read and the status check -> the 14 averages."""
         with torch.cuda.device(self.device):
@@ -127,14 +158,17 @@ class _MeterTable:
 
 
 class Validator(_MeterTable):
-    """Eval-mode losses and metrics of one epoch on the device (see the module docstring).  One process, one
-    device; `capacity` = batches one epoch may add (default 4096)."""
+    """Eval-mode losses and metrics of one epoch on the device (see the module docstring); `capacity` = batches one
+    epoch may add (default 4096).  Without `group`: one process, one device.  With `group` (a torch.distributed
+    process group, NCCL or gloo; every rank adds its chunk of every batch): `add` is unchanged and `finalize` is
+    collective, returning on every rank the same averages of the rank-ordered mean of each batch's values."""
 
     LABEL_KEYS = ("cls_label", "size_class", "box3d_center", "box3d_heading", "box3d_size")
     _NAMES = ("Validator", "batch", "batches", "validate()", "Validator(model, capacity=%d)")
 
-    def __init__(self, model, capacity=None):
+    def __init__(self, model, capacity=None, group=None):
         self.model = model
+        self.group = group
         p = next(model.parameters(), None)
         if p is None or p.device.type != "cuda":
             raise RuntimeError("Validator: the model must live on a CUDA device (there is no CPU fallback)")
@@ -212,8 +246,26 @@ class Validator(_MeterTable):
     def finalize(self):
         """-> OrderedDict of the 14 epoch averages in the order of the reference's
         ``TrainingStates.get_states(avg=True)``; one host read.  Raises if a batch had no foreground row or the
-        table overflowed."""
-        return self._replay(self.table, self.state)
+        table overflowed.  With `group` every rank of it must call it: the batch counters of all ranks are gathered
+        and read once, each batch's row is summed over the ranks in rank order, its 14 values divided by the number
+        of ranks, and B / nfg / nkeep kept summed.  Every verdict is taken from the gathered values, so every rank
+        raises the same error: ValueError if the ranks added different numbers of batches, RuntimeError if a batch
+        had no foreground row on some rank or a rank's table overflowed."""
+        if self.group is None:
+            return self._replay(self.table, self.state)
+        import torch.distributed as dist
+        world = dist.get_world_size(self.group)
+        with torch.cuda.device(self.device):
+            self._join()
+            states = torch.empty(world * 4, dtype=torch.int32, device=self.device)
+            dist.all_gather_into_tensor(states, self.state, group=self.group)
+            added = states.view(world, 4)[:, 0].cpu().tolist()
+            if len(set(added)) > 1:
+                raise ValueError("Validator: the ranks of the group added different numbers of batches (%s); every "
+                                 "rank must add its chunk of every batch"
+                                 % ", ".join("rank %d: %d" % (r, a) for r, a in enumerate(added)))
+            table, state = self._over_ranks(self.group, ordered=True)
+        return self._replay(table, state)
 
     def meters(self):
         """(sum, count) of each AverageMeter after the last `finalize`, keyed like its result."""
@@ -241,9 +293,14 @@ class TrainStates(_MeterTable):
                 print(ts.states.last())            # training_states.get_states(avg=False); one sync
         epoch = ts.states.finalize()               # training_states.get_states(avg=True)
 
-    `capacity` = steps one epoch may add (default 4096)."""
+    `capacity` = steps one epoch may add (default 4096); `deterministic`: a callable read at `finalize`, True when
+    the owning TrainStep runs in deterministic mode (then the mean over ranks is summed in rank order)."""
 
     _NAMES = ("TrainStates", "step", "steps", "train()", "TrainStep(..., states_capacity=%d)")
+
+    def __init__(self, device, capacity=None, deterministic=None):
+        super().__init__(device, capacity)
+        self._deterministic = deterministic
 
     def reset(self):
         """Start a new epoch (stream-ordered: the counter is zeroed on the current stream)."""
@@ -275,28 +332,18 @@ class TrainStates(_MeterTable):
         nkeep in columns 14-16."""
         return self._rows(full)
 
-    def _over_ranks(self, world):
-        """The table as the reference's DataParallel loop logs it: each step's values averaged over the replicas,
-        B / nfg / nkeep summed (the full batch), and the status bits of every rank; one all_reduce of the table."""
-        import torch.distributed as dist
-        table = self.table.clone()
-        dist.all_reduce(table)
-        table[:, :_lib.VAL_VALUES] /= world
-        s = self.state
-        no_fg = (s[1] & _lib.VAL_NO_FG) != 0
-        flags = torch.stack([s[1] & _lib.VAL_NO_FG, s[1] & _lib.VAL_OVERFLOW,
-                             torch.where(no_fg, -s[2], torch.full_like(s[2], -(2 ** 31 - 1)))])
-        dist.all_reduce(flags, op=dist.ReduceOp.MAX)        # OR of the bits, earliest step without a foreground row
-        state = torch.stack([s[0], flags[0] | flags[1], -flags[2], s[3]])
-        return table, state
-
     def finalize(self):
         """-> OrderedDict of the 14 epoch averages (``get_states(avg=True)``); one host read.  With torch.distributed
         initialised and world > 1 every rank must call it (ranks step in lockstep, so row i is the same step on every
-        rank).  Raises, naming the step, if a step had no foreground row, and if more steps were added than
+        rank); in deterministic mode the rows are summed over the ranks in rank order, so every rank returns the same
+        bits.  Raises, naming the step, if a step had no foreground row, and if more steps were added than
         `capacity`, naming the capacity needed."""
         import torch.distributed as dist
         world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         with torch.cuda.device(self.device):
-            table, state = self._over_ranks(world) if world > 1 else (self.table, self.state)
+            if world > 1:
+                ordered = bool(self._deterministic()) if self._deterministic is not None else False
+                table, state = self._over_ranks(None, ordered)
+            else:
+                table, state = self.table, self.state
         return self._replay(table, state)

@@ -371,6 +371,13 @@ FCN_API int fcn_adam_step(float *param, const float *grad, float *exp_avg, float
  * momentum == 0 (then it is neither read nor written). */
 FCN_API int fcn_sgd_step(float *param, const float *grad, float *momentum_buffer, long long n, float lr,
                          float momentum, float weight_decay, int first, float grad_scale, fcn_stream_t stream);
+/* rank-ordered fold of G rows of n floats, row r at src + r*ld (the G ranks' shards of a gradient piece, as an
+ * all-to-all leaves them): dst[i] = ((src[i] + src[ld+i]) + src[2ld+i]) + ... + src[(G-1)ld+i], a left fold in rank
+ * order with every add rounded on its own (no FMA), so the sum does not depend on how the rows were gathered.
+ * G == 1 is a copy.  One thread per float4 where src, dst and ld allow 16-byte access, per float otherwise; no
+ * atomics.  NULL pointers, G < 1, n < 0, ld < n, or dst overlapping [src, src + (G-1)*ld + n) return
+ * FCN_ERR_INVALID before anything is launched; n == 0 is a no-op. */
+FCN_API int fcn_rank_fold(const float *src, long long ld, int G, long long n, float *dst, fcn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * (7b) Fused detection losses + gradient w.r.t. the head logits (row 8(f)-2, train half): everything of
