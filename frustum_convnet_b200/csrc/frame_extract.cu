@@ -73,12 +73,13 @@ frame_slots_kernel(const fcn_frame_extract_args a, const int32_t *__restrict__ d
     __shared__ typename Scan::TempStorage tmp;
     const int F = a.num_frames, D = a.det_capacity, B = F * D, Pout = a.out_capacity;
     int bits = 0;
-    // class ranks by first appearance among each frame's kept detections
+    // class ranks by first appearance among each frame's kept detections that fit its budget (the test of the loop
+    // below), so a class whose frustums were all dropped for the budget gets no segment
     for (int f = threadIdx.x; f < F; f += FRAME_THREADS) {
         int r[3] = {-1, -1, -1}, n = 0;
         for (int j = 0; j < D; ++j) {
             const int d = f * D + j;
-            if (det_points[d] < 0) continue;
+            if (det_points[d] < 0 || cnt_pos[d] - cnt_pos[(size_t)f * D] + det_points[d] > Pout) continue;
             const int c = a.det_class[d];
             if (r[c] < 0) {
                 a.seg_class[3 * f + n] = c;

@@ -1174,6 +1174,7 @@ FCN_API int fcn_refine_frustum_table(const fcn_refine_frustum_table_args *args, 
  *          det_index (B): the slot, -1 for a dummy      valid (B): 1 for a kept frustum
  *          cls_index (B): det_class of the slot         rgb_prob (B): det_prob of the slot (float32)
  *          seg (B): f * 3 + r, r the rank of the frustum's class among its frame's kept classes by first appearance
+ *            (the classes of the frustums in the batch: one dropped for P_out gives its class no rank)
  *          seg_class (F * 3): the class of segment f * 3 + r, -1 when the frame has fewer kept classes
  *        *status gets FCN_FRAME_* bits OR-ed in (the caller clears it).
  *      fcn_resample_choice : the (B, N) int32 `choice` of section (9), one CTA per entry b with n = offsets[b+1] -
