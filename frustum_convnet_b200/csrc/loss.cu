@@ -89,24 +89,11 @@ __global__ void det_loss_slots_kernel(int nblk, const float *__restrict__ slots,
     acc[threadIdx.x] = (float)t;
 }
 
-// out[0..7]  = total, cls, center, head_cls, head_res, size_cls, size_res, corners   (det_base.py:505-514)
-// out[8..13] = cls_acc, head_acc, size_acc, IoU_2D, IoU_3D, IoU_>=thresh            (:516-523)
+// out[0..13] = the 14 values of loss_final_values (loss_terms.cuh); out[14..15] = #foreground, #non-ignored rows
 __global__ void det_loss_final_kernel(const __grid_constant__ fcn_loss_args a, const float *__restrict__ counts,
                                       const float *__restrict__ acc, float *__restrict__ out) {
     if (threadIdx.x != 0) return;
-    const float nfg = fmaxf(counts[0], 1.f), nkeep = fmaxf(counts[1], 1.f);
-    const float cls = acc[A_CLS] / (counts[0] + 1e-14f);
-    const float center = acc[A_CENTER] / nfg, hcls = acc[A_HCLS] / nfg, hres = acc[A_HRES] / nfg;
-    const float scls = acc[A_SCLS] / nfg, sres = acc[A_SRES] / nfg, corner = acc[A_CORNER] / nfg;
-    out[0] = cls + a.w_box * (center + hcls + scls + a.w_head_reg * hres + a.w_size_reg * sres + a.w_corner * corner);
-    out[1] = cls; out[2] = center; out[3] = hcls; out[4] = hres; out[5] = scls; out[6] = sres; out[7] = corner;
-    out[8] = acc[A_CLSACC] / nkeep;
-    out[9] = acc[A_HACC] / nfg;
-    out[10] = acc[A_SACC] / nfg;
-    const float nan = __int_as_float(0x7fc00000);
-    out[11] = a.with_iou ? acc[A_IOU2] / nfg : nan;
-    out[12] = a.with_iou ? acc[A_IOU3] / nfg : nan;
-    out[13] = a.with_iou ? acc[A_IOUGT] / nfg : nan;
+    loss_final_values(a, acc, counts[0], counts[1], out);
     out[14] = counts[0];
     out[15] = counts[1];
 }

@@ -81,4 +81,35 @@ __device__ __forceinline__ float softmax_denom(const float *s, int n, float &mx)
     return sum;
 }
 
+// The 14 values of a batch (det_base.py:505-523) from its summed row terms acc[A_*] and its foreground and
+// non-ignored row counts; `a` is the caller's settings record (fcn_loss_args or fcn_val_batch_args).
+//   out[0..7]  = total, cls, center, head_cls, head_res, size_cls, size_res, corners
+//   out[8..13] = cls_acc, head_acc, size_acc, IoU_2D, IoU_3D, IoU_>=thresh   (NaN IoU values when with_iou == 0)
+// Every product, sum and quotient is rounded on its own, as the reference's float32 tensor operations round them:
+// the total in Python's evaluation order of det_base.py:468-474, and each accuracy as get_accuracy
+// (utils/utils.py:28-48) forms it, correct.sum() * float32(1.0 / n).  The explicit _rn intrinsics keep nvcc from
+// contracting the total into FFMAs.
+template <class Args>
+__device__ __forceinline__ void loss_final_values(const Args &a, const float *acc, float nfg_raw, float nkeep_raw,
+                                                  float *out) {
+    const float nfg = fmaxf(nfg_raw, 1.f), nkeep = fmaxf(nkeep_raw, 1.f);
+    const float cls = __fdiv_rn(acc[A_CLS], __fadd_rn(nfg_raw, 1e-14f));   // loss.sum() / (num_fg + 1e-14)
+    const float center = __fdiv_rn(acc[A_CENTER], nfg), hcls = __fdiv_rn(acc[A_HCLS], nfg);
+    const float hres = __fdiv_rn(acc[A_HRES], nfg), scls = __fdiv_rn(acc[A_SCLS], nfg);
+    const float sres = __fdiv_rn(acc[A_SRES], nfg), corner = __fdiv_rn(acc[A_CORNER], nfg);
+    float box = __fadd_rn(__fadd_rn(center, hcls), scls);
+    box = __fadd_rn(box, __fmul_rn(a.w_head_reg, hres));
+    box = __fadd_rn(box, __fmul_rn(a.w_size_reg, sres));
+    box = __fadd_rn(box, __fmul_rn(a.w_corner, corner));
+    out[0] = __fadd_rn(cls, __fmul_rn(a.w_box, box));
+    out[1] = cls; out[2] = center; out[3] = hcls; out[4] = hres; out[5] = scls; out[6] = sres; out[7] = corner;
+    out[8] = __fmul_rn(acc[A_CLSACC], __double2float_rn(1.0 / (double)nkeep));
+    out[9] = __fmul_rn(acc[A_HACC], __double2float_rn(1.0 / (double)nfg));
+    out[10] = __fmul_rn(acc[A_SACC], __double2float_rn(1.0 / (double)nfg));
+    const float nan = __int_as_float(0x7fc00000);
+    out[11] = a.with_iou ? __fdiv_rn(acc[A_IOU2], nfg) : nan;
+    out[12] = a.with_iou ? __fdiv_rn(acc[A_IOU3], nfg) : nan;
+    out[13] = a.with_iou ? __fdiv_rn(acc[A_IOUGT], nfg) : nan;
+}
+
 }  // namespace fcn

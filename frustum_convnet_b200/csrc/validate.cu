@@ -3,8 +3,8 @@
 // float64 AverageMeter replay of utils/utils.py:51-67 at the end of the epoch.
 //   val_rows_kernel   : one thread per (frustum, position) row, the forward terms of loss_terms.cuh; each CTA
 //                       writes its 15 sums (13 terms, nfg, nkeep) to its own slot of `partials`
-//   val_final_kernel  : one warp sums the slots in CTA order, forms the 14 values with the reference's denominators
-//                       and appends one table row at the index taken from the device counter
+//   val_final_kernel  : one warp sums the slots in CTA order, forms the 14 values as fcn_det_loss does
+//                       (loss_final_values) and appends one table row at the index taken from the device counter
 //   val_finalize_kernel: one thread per meter replays sum += val * n, count += n (count from 1e-14) in row order
 //   train_states_append_kernel: appends a training step's fcn_det_loss result block as one row of the same table
 // No float atomics anywhere, so a batch gives the same bits on every run, stream and graph replay.
@@ -172,27 +172,8 @@ __global__ void val_final_kernel(const __grid_constant__ fcn_val_batch_args a, i
     __syncthreads();
     if (threadIdx.x != 0) return;
     const float nfg_raw = acc[VAL_NFG], nkeep_raw = acc[VAL_NKEEP];
-    const float nfg = fmaxf(nfg_raw, 1.f), nkeep = fmaxf(nkeep_raw, 1.f);
     float out[FCN_VAL_VALUES];
-    const float cls = __fdiv_rn(acc[A_CLS], __fadd_rn(nfg_raw, 1e-14f));   // loss.sum() / (num_fg + 1e-14)
-    const float center = __fdiv_rn(acc[A_CENTER], nfg), hcls = __fdiv_rn(acc[A_HCLS], nfg);
-    const float hres = __fdiv_rn(acc[A_HRES], nfg), scls = __fdiv_rn(acc[A_SCLS], nfg);
-    const float sres = __fdiv_rn(acc[A_SRES], nfg), corner = __fdiv_rn(acc[A_CORNER], nfg);
-    // det_base.py:468-474 in Python's evaluation order, every product and sum rounded on its own
-    float box = __fadd_rn(__fadd_rn(center, hcls), scls);
-    box = __fadd_rn(box, __fmul_rn(a.w_head_reg, hres));
-    box = __fadd_rn(box, __fmul_rn(a.w_size_reg, sres));
-    box = __fadd_rn(box, __fmul_rn(a.w_corner, corner));
-    out[0] = __fadd_rn(cls, __fmul_rn(a.w_box, box));
-    out[1] = cls; out[2] = center; out[3] = hcls; out[4] = hres; out[5] = scls; out[6] = sres; out[7] = corner;
-    // get_accuracy (utils/utils.py:28-48): correct.sum() * float32(1.0 / n)
-    out[8] = __fmul_rn(acc[A_CLSACC], __double2float_rn(1.0 / (double)nkeep));
-    out[9] = __fmul_rn(acc[A_HACC], __double2float_rn(1.0 / (double)nfg));
-    out[10] = __fmul_rn(acc[A_SACC], __double2float_rn(1.0 / (double)nfg));
-    const float nan = __int_as_float(0x7fc00000);
-    out[11] = a.with_iou ? __fdiv_rn(acc[A_IOU2], nfg) : nan;
-    out[12] = a.with_iou ? __fdiv_rn(acc[A_IOU3], nfg) : nan;
-    out[13] = a.with_iou ? __fdiv_rn(acc[A_IOUGT], nfg) : nan;
+    loss_final_values(a, acc, nfg_raw, nkeep_raw, out);
     append_row(out, a.B, nfg_raw, nkeep_raw, a.table, a.capacity, a.state);
 }
 

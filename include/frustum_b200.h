@@ -388,6 +388,9 @@ FCN_API int fcn_rank_fold(const float *src, long long ld, int G, long long n, fl
  *      data dict holds them (cls_label int64 (B,T2) in {-1,0,1}, size_class int64 (B), box3d_* fp32).
  *      out[0..7] = total, cls, center, head_cls, head_res, size_cls, size_res, corners; out[8..13] = cls_acc,
  *      head_acc, size_acc, IoU_2D, IoU_3D, IoU_>=thresh; out[14..15] = #foreground, #non-ignored rows.
+ *      out[0] and out[8..10] follow the reference's float32 roundings: the total is det_base.py:468-474 in Python's
+ *      evaluation order with every product and sum rounded on its own, and each accuracy is the float32 count times
+ *      float32(1.0 / n), as get_accuracy (utils/utils.py:28-48) forms it.  fcn_val_batch forms its values the same way.
  *      scratch: 16 floats.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {

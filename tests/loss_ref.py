@@ -66,6 +66,27 @@ def half_bin(NH):
     return float(np.float32(2 * np.pi / float(NH) / 2))
 
 
+def total_f32(means, weights):
+    """The total loss of det_base.py:468-474 as float32 tensors compute it from the seven float32 means
+    [cls, center, head_cls, head_res, size_cls, size_res, corners] and the four loss weights (w_box, w_head_reg,
+    w_size_reg, w_corner): Python's evaluation order, each Python-float weight entering as float32, every product and
+    sum rounded on its own.  Returns a numpy float32."""
+    f = np.float32
+    cls, center, hcls, hres, scls, sres, corner = (f(m) for m in means)
+    w_box, w_hr, w_sr, w_c = (f(w) for w in weights)
+    box = f(f(center + hcls) + scls)
+    box = f(box + f(w_hr * hres))
+    box = f(box + f(w_sr * sres))
+    box = f(box + f(w_c * corner))
+    return f(cls + f(w_box * box))
+
+
+def accuracy_f32(correct, n):
+    """get_accuracy (utils/utils.py:28-48) of `correct` hits over n >= 1 rows: the float32 count times the Python
+    double 1.0 / n, which enters the float32 multiply rounded to float32.  Returns a numpy float32."""
+    return np.float32(np.float32(correct) * np.float32(1.0 / n))
+
+
 def corners(ctr, heading, size):
     """(n, 8, 3) float64 corners of model_util.py:48-72 (x: +-l/2, y: +-h/2, z: +-w/2; rotation about y)."""
     x = SX * size[:, :1] * 0.5

@@ -95,6 +95,51 @@ def test_corner_tie_sends_the_gradient_to_the_gt_box():
     assert abs(corner - (-4 * w[0] * w[3] / 8 / math.sqrt(1.0625) * 1.5)) <= 1e-12
 
 
+def test_float32_composition_matches_the_reference_expressions():
+    """loss_ref.total_f32 and loss_ref.accuracy_f32, which the GPU tests hold the kernels' total and accuracies to bit
+    for bit, against the reference's own expressions evaluated by torch on float32 tensors: the total of
+    det_base.py:468-474 on 0-dim tensors with Python-float weights, and get_accuracy's
+    correct.float().sum(0, keepdim=True).mul_(1.0 / n), for random means, weights and counts with n up to 4096."""
+    rng = np.random.default_rng(17)
+    f32 = np.float32
+    once = 0
+    for i in range(3000):
+        means = (10.0 ** rng.uniform(-4, 4, 7)).astype(f32)
+        means[rng.random(7) < 0.1] = 0
+        weights = [float(w) for w in rng.uniform(0, 30, 4)]
+        if i % 5 < 4:
+            weights[i % 5] = (0.0, 1.0, 2.0, 20.0)[i // 5 % 4]     # zero, integral and power-of-two weights too
+        cls_loss, center_loss, heading_class_loss, heading_res_norm_loss, size_class_loss, size_res_norm_loss, \
+            corners_loss = (torch.tensor(m) for m in means)
+        BOX_LOSS_WEIGHT, HEAD_REG_WEIGHT, SIZE_REG_WEIGHT, CORNER_LOSS_WEIGHT = weights
+        loss = cls_loss + \
+            BOX_LOSS_WEIGHT * (center_loss +
+                               heading_class_loss + size_class_loss +
+                               HEAD_REG_WEIGHT * heading_res_norm_loss +
+                               SIZE_REG_WEIGHT * size_res_norm_loss +
+                               CORNER_LOSS_WEIGHT * corners_loss)
+        assert loss.dtype == torch.float32
+        got = lr.total_f32(means, weights)
+        assert loss.numpy().view(np.int32) == got.view(np.int32), (i, means, weights, float(loss), got)
+        m, (w_box, w_hr, w_sr, w_c) = means.astype(np.float64), weights
+        exact = m[0] + w_box * (m[1] + m[2] + m[4] + w_hr * m[3] + w_sr * m[5] + w_c * m[6])
+        once += f32(exact) != got
+    assert once > 300, once          # a total rounded once (or through FMAs) is not the reference's
+    div = 0
+    for i in range(3000):
+        n = int(rng.integers(1, 4097)) if i >= 3 else (6, 7, 10)[i]
+        c = int(rng.integers(0, n + 1)) if i >= 3 else (5, 3, 9)[i]
+        correct = torch.zeros(1, n, dtype=torch.bool)
+        correct[0, :c] = True
+        ref = correct[:1].view(-1).float().sum(0, keepdim=True).mul_(1.0 / n)
+        got = lr.accuracy_f32(c, n)
+        assert ref.numpy()[0].view(np.int32) == got.view(np.int32), (c, n, float(ref[0]), got)
+        div += f32(f32(c) / f32(n)) != got
+        if i < 3:
+            assert f32(f32(c) / f32(n)) != got, (c, n)      # 5/6, 3/7, 9/10: c / n is not the reference's value
+    assert div > 300, div
+
+
 def test_no_foreground_reference_is_defined():
     c = lr.make_case(3, 20, 12, 3, seed=2)
     c["cls_label"][c["cls_label"] == 1] = 0

@@ -15,8 +15,11 @@ terms the kernel rounds, each built so that the kernel's error is at most a few 
   * losses: each term is a sum over rows of non-negative values reduced by warp shuffles, shared and global fp32
     atomics in any order (<= 5 + 4 + ceil(N/128) additions on a path): |L - L64| <= u ((ceil(N/128) + 16) L64
     + 4 mag_rows) / n  + 4 ulp(L), n = nfg (num_fg + 1e-14 for the focal term); the total adds its terms with the
-    weights and 8u |total|;
-  * accuracies exact (first maximum on exact ties); IoU means 1e-4 against oracle/box_iou.py on the same boxes.
+    weights and 8u |total|, and is bit-equal to the reference's float32 composition of the kernel's own seven means
+    (loss_ref.total_f32: Python's evaluation order, every product and sum rounded on its own);
+  * accuracies: the count c = rint(acc * n) exact (first maximum on exact ties), and the value bit-equal to the
+    reference's float32 c * float32(1 / n) (loss_ref.accuracy_f32); IoU means 1e-4 against oracle/box_iou.py on the
+    same boxes.
 A row whose flip choice |dg - df| is within rounding may take either box and must match one of the two float64
 gradients; a row whose arg-max has two scores within rounding (not equal) may take either class.  The number of such
 rows is printed; the crafted cases keep them rare.
@@ -115,28 +118,43 @@ def _grad_within(got, g64, mag, what, rows=None):
     return ratio
 
 
-def check(call, out, dcls, dreg, ref=None):
-    """Kernel output of one call vs loss_ref; returns the reference."""
-    ref = ref if ref is not None else call.ref()
-    out = out.double().cpu().numpy()
+def check_values(out, ref, N, weights, with_iou, iou_thresh):
+    """A kernel's 14 values of one batch (float32 out[0..13]) against the reference of the same inputs."""
+    out = np.asarray(out, np.float32)
+    o64 = out.astype(np.float64)
     L = ref.losses.numpy()
-    tol = _loss_tol(ref, call.N, call.weights)
-    bad = np.abs(out[:8] - L) > tol
-    assert not bad.any(), ("losses", out[:8], L, tol)
-    assert out[14] == ref.nfg and out[15] == ref.nkeep
-    # accuracies: exact, up to rows whose arg-max is within rounding
+    tol = _loss_tol(ref, N, weights)
+    bad = np.abs(o64[:8] - L) > tol
+    assert not bad.any(), ("losses", o64[:8], L, tol)
+    # the total: the reference's float32 composition of the kernel's own means, bit for bit
+    total = lr.total_f32(out[1:8], weights)
+    assert out[0].view(np.int32) == total.view(np.int32), ("total", out[0], total)
+    # accuracies: the reference's float32 correct * (1 / n) of an exact count, and the count exact up to rows whose
+    # arg-max is within rounding
     n_amb = [int(ref.amb_cls.sum()), int(ref.amb_h.sum()), int(ref.amb_s.sum())]
     den = [max(ref.nkeep, 1), max(ref.nfg, 1), max(ref.nfg, 1)]
     M = ref.metrics.numpy()
     for k in range(3):
-        assert abs(out[8 + k] - M[k]) <= n_amb[k] / den[k] + 2 * _ulp(M[k]), ("accuracy", k, out[8 + k], M[k])
-    if call.args.with_iou:
+        c, c_ref = np.rint(o64[8 + k] * den[k]), np.rint(M[k] * den[k])
+        acc = lr.accuracy_f32(c, den[k])
+        assert out[8 + k].view(np.int32) == acc.view(np.int32), ("accuracy", k, out[8 + k], acc)
+        assert abs(c - c_ref) <= n_amb[k], ("accuracy", k, c, c_ref, n_amb[k])
+    if with_iou:
         amb_iou = int(ref.amb_h.sum() + ref.amb_s.sum())
-        assert np.all(np.abs(out[11:13] - M[3:5]) <= 1e-4 + amb_iou / den[1]), ("IoU", out[11:14], M[3:])
-        near = int((np.abs(ref.iou[:, 1] - call.args.iou_thresh) <= 1e-4).sum()) + amb_iou
-        assert abs(out[13] - M[5]) <= near / den[1] + 1e-6, ("IoU >= thresh", out[13], M[5])
+        assert np.all(np.abs(o64[11:13] - M[3:5]) <= 1e-4 + amb_iou / den[1]), ("IoU", o64[11:14], M[3:])
+        near = int((np.abs(ref.iou[:, 1] - iou_thresh) <= 1e-4).sum()) + amb_iou
+        assert abs(o64[13] - M[5]) <= near / den[1] + 1e-6, ("IoU >= thresh", o64[13], M[5])
     else:
-        assert np.isnan(out[11:14]).all()
+        assert np.isnan(o64[11:14]).all()
+    return n_amb
+
+
+def check(call, out, dcls, dreg, ref=None):
+    """Kernel output of one call vs loss_ref; returns the reference."""
+    ref = ref if ref is not None else call.ref()
+    out = out.cpu().numpy()
+    n_amb = check_values(out[:14], ref, call.N, call.weights, call.args.with_iou, call.args.iou_thresh)
+    assert out[14] == ref.nfg and out[15] == ref.nkeep
     # gradients: every row written, each element within its bound
     assert bool(torch.isfinite(dcls).all()) and bool(torch.isfinite(dreg).all()), "a row was not written"
     r1 = _grad_within(dcls, ref.dcls, ref.mag_dcls, "dcls")
@@ -227,10 +245,9 @@ def test_batch_without_foreground(labels):
 
 
 # ============================================================================ branch points
-def test_corner_tie_goes_to_gt_box():
-    """dg == df exactly (a zero-size predicted box at the centre of a GT box of zero width, heading 0): the
-    whole corner gradient goes to the GT side, so the length residual gets -4 gD / |corner| where torch.min's
-    half split would give 0."""
+def corner_tie_case():
+    """One foreground row with dg == df exactly: a zero-size predicted box at the centre of a GT box of zero width,
+    heading 0 (NH = 12, NS = 1)."""
     case = {"cls": np.array([[0.0, 1.0]], np.float32), "cls_label": np.array([[1]], np.int64),
             "center_ref2": np.zeros((1, 3, 1), np.float32), "box3d_center": np.zeros((1, 3), np.float32),
             "box3d_heading": np.zeros(1, np.float32), "box3d_size": np.array([[2.0, 0.0, 0.5]], np.float32),
@@ -239,6 +256,14 @@ def test_corner_tie_goes_to_gt_box():
     reg = np.zeros((1, 3 + 2 * NH + 4 * NS), np.float32)
     reg[0, 3 + 2 * NH + NS:] = -1.0                            # predicted size 0
     case["reg"] = reg
+    return case, NH, NS
+
+
+def test_corner_tie_goes_to_gt_box():
+    """dg == df exactly (a zero-size predicted box at the centre of a GT box of zero width, heading 0): the
+    whole corner gradient goes to the GT side, so the length residual gets -4 gD / |corner| where torch.min's
+    half split would give 0."""
+    case, NH, NS = corner_tie_case()
     call = Call(case, NH, NS)
     out, dcls, dreg = call.run()
     ref = check(call, out, dcls, dreg)
@@ -306,15 +331,9 @@ def test_heading_bin_boundaries(NH):
 
 
 # ============================================================================ metrics
-def test_without_iou_gives_nan():
-    call = Call(lr.make_case(3, 33, 12, 3, seed=4), 12, 3, with_iou=0)
-    out, dcls, dreg = call.run()
-    check(call, out, dcls, dreg)
-
-
-def test_iou_against_oracle_near_gt():
-    """Predicted boxes near their GT box (non-trivial IoU) with predicted classes that differ from the labels on
-    part of the rows: the IoU metrics use the PREDICTED heading and size classes."""
+def near_gt_case():
+    """6 x 40 rows (NH = 12, NS = 3) whose foreground rows predict boxes near their GT box, with predicted heading
+    and size classes that differ from the labels on part of the rows."""
     case = lr.make_case(6, 40, 12, 3, seed=31)
     NH, NS = 12, 3
     rng = np.random.default_rng(1)
@@ -331,6 +350,19 @@ def test_iou_against_oracle_near_gt():
         ss[int(case["size_class"][b]) if r % 4 else (int(case["size_class"][b]) + 1) % NS] = ss.max() + 2
         ms = case["mean_size"]
         reg[r, 3 + 2 * NH + NS:] = ((case["box3d_size"][b] - ms) / ms).reshape(-1) + rng.normal(0, 0.05, 3 * NS)
+    return case, NH, NS
+
+
+def test_without_iou_gives_nan():
+    call = Call(lr.make_case(3, 33, 12, 3, seed=4), 12, 3, with_iou=0)
+    out, dcls, dreg = call.run()
+    check(call, out, dcls, dreg)
+
+
+def test_iou_against_oracle_near_gt():
+    """Predicted boxes near their GT box (non-trivial IoU) with predicted classes that differ from the labels on
+    part of the rows: the IoU metrics use the PREDICTED heading and size classes."""
+    case, NH, NS = near_gt_case()
     call = Call(case, NH, NS, iou_thresh=0.5)
     out, dcls, dreg = call.run()
     ref = check(call, out, dcls, dreg)
