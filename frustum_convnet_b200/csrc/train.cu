@@ -21,6 +21,7 @@
 //     Conv2d (Co,Ci,1,1)) through strides, so gradients land directly in one flat bucket (one all-reduce);
 //   * fp32 FMA arithmetic (parity with the fp32 reference fixture: losses 2e-4, gradients 2e-3).
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -141,109 +142,8 @@ __device__ __forceinline__ size_t w_index(const fcn_train_layer &L, const fcn_tr
 // are therefore linearised and split over gridDim.z; slices write partial sums to a workspace and
 // train_fwd_finish_kernel adds them in a fixed order (deterministic), adds the bias, stores Y and accumulates
 // the batch statistics.  gridDim.z == 1 stores Y / statistics directly.
-__global__ void __launch_bounds__(TG_THREADS)
-train_fwd_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ partial, int tiles_per_slice) {
-    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];
-    __shared__ float s_scale[TG_BK], s_shift[TG_BK];
-    __shared__ float s_sum[TG_BN], s_sq[TG_BN];
-    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int r0 = blockIdx.x * TG_BM, n0 = blockIdx.y * TG_BN;
-    const int M = L.B * L.T_out;
-    const int q_lo = blockIdx.z * tiles_per_slice, q_hi = q_lo + tiles_per_slice;
-    float acc[4][4] = {};
-    // this K loop and the partial-sum store below are repeated in fwd_k_tiles / fwd_store_partial (deterministic
-    // forward): change them together
-    int q0 = 0;                                              // first linear K tile of the current segment
-    for (int sg = 0; sg < L.n_seg; ++sg) {
-        const fcn_train_seg &g = L.seg[sg];
-        const fcn_train_src &s = g.src;
-        const double inv = s.sums != nullptr ? 1.0 / s.count : 0.0;
-        const int nt = (g.C + TG_BK - 1) / TG_BK;
-        const int t_lo = max(q_lo - q0, 0), t_hi = min(q_hi - q0, nt);
-        q0 += nt;
-        for (int t = t_lo; t < t_hi; ++t) {
-            const int k0 = t * TG_BK;
-            __syncthreads();
-            if (tid < TG_BK) {          // src_coef, with the inverse count hoisted out of the tile loop
-                const int c = k0 + tid;
-                float sc = 1.f, sh = 0.f;
-                if (s.sums != nullptr && c < g.C) {
-                    const BnCoef b = bn_coef(s.sums, s.gamma, s.beta, s.Cstat, (s.coff + c) % s.Cstat, inv);
-                    sc = b.scale; sh = b.shift;
-                }
-                s_scale[tid] = sc; s_shift[tid] = sh;
-            }
-            __syncthreads();
-            // A tile: 64 rows x 16 channels (consecutive threads -> consecutive channels)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int rr = ty + 16 * i, r = r0 + rr, c = k0 + tx;
-                float v = 0.f;
-                if (r < M && c < g.C) {
-                    const int b = r / L.T_out, tt = r - b * L.T_out;
-                    v = src_act(s, b, tt * g.stride + g.tap, c, s_scale[tx], s_shift[tx]);
-                }
-                As[tx][rr] = v;
-            }
-            // B tile: 16 channels x 64 columns
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int kk = tid / 64 + 4 * i, nn = tid % 64, c = k0 + kk, n = n0 + nn;
-                Bs[kk][nn] = (c < g.C && n < L.N) ? L.W[w_index(L, g, c, n)] : 0.f;
-            }
-            __syncthreads();
-            tile_fma_4x4(acc, As, Bs, tx, ty);
-        }
-    }
-    if (gridDim.z > 1) {                                     // partial sums of this K slice
-        float *dst = partial + (size_t)blockIdx.z * M * L.N;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int r = r0 + ty * 4 + i;
-            if (r >= M) continue;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int n = n0 + tx * 4 + j;
-                if (n < L.N) dst[(size_t)r * L.N + n] = acc[i][j];
-            }
-        }
-        return;
-    }
-    // epilogue: store raw output (+bias), per-channel Sum(y), Sum(y^2)
-    if (tid < TG_BN) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int n = n0 + tx * 4 + j;
-        float ps = 0.f, pq = 0.f;
-        if (n < L.N) {
-            const float bias = L.bias != nullptr ? L.bias[n] : 0.f;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = r0 + ty * 4 + i;
-                if (r < M) {
-                    const float y = acc[i][j] + bias;
-                    L.Y[(size_t)r * L.N + n] = y;
-                    ps += y; pq += y * y;
-                }
-            }
-            if (L.has_bn) { atomicAdd(&s_sum[tx * 4 + j], ps); atomicAdd(&s_sq[tx * 4 + j], pq); }
-        }
-    }
-    if (L.has_bn) {
-        __syncthreads();
-        if (tid < TG_BN && n0 + tid < L.N) {
-            const int co = (n0 + tid) % L.Cout;
-            atomicAdd(&L.sums[co], (double)s_sum[tid]);
-            atomicAdd(&L.sums[L.Cout + co], (double)s_sq[tid]);
-        }
-    }
-}
 
-// Deterministic forward, generic layers: the CTA's 64 x 64 output tile over the linear K tiles [q_lo, q_hi) of all
-// segments.  This is train_fwd_kernel's K loop and partial-sum store, and the two copies must stay in step:
-// train_fwd_kernel keeps its own, because calling these helpers there changes its register allocation (the default
-// path's code stays as it was).
+// the CTA's 64 x 64 output tile over the linear K tiles [q_lo, q_hi) of all segments
 __device__ __forceinline__ void fwd_k_tiles(const fcn_train_layer &L, int tid, int tx, int ty, int M, int r0, int n0,
                                             int q_lo, int q_hi, float (&acc)[4][4], float (&As)[TG_BK][TG_BM + 4],
                                             float (&Bs)[TG_BK][TG_BN + 4], float (&s_scale)[TG_BK],
@@ -309,15 +209,15 @@ __device__ __forceinline__ void fwd_store_partial(const fcn_train_layer &L, int 
     }
 }
 
-// Deterministic forward (fcn_train_forward_deterministic): gridDim.z > 1 stores the K slices' partial sums as
-// train_fwd_kernel does; gridDim.z == 1 stores Y (+bias) and, for a BN layer, this CTA's column sums Sum(y), Sum(y^2)
-// over its 64 rows (16 row groups added in group order) to slot blockIdx.x of `slots` [row block][2N], plain stores.
+// Generic forward.  gridDim.z > 1 stores the K slices' partial sums; gridDim.z == 1 stores Y (+bias) and, for a BN
+// layer, this CTA's column sums Sum(y), Sum(y^2) over its 64 rows: ORDERED adds its 16 row groups in group order and
+// stores them to slot blockIdx.x of `slots` [row block][2N] (plain stores), else they go to `sums` by atomics.
+template <bool ORDERED>
 __global__ void __launch_bounds__(TG_THREADS)
-train_fwd_det_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ partial, int tiles_per_slice,
-                     float *__restrict__ slots) {
+train_fwd_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ partial, int tiles_per_slice,
+                 float *__restrict__ slots) {
     __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];
     __shared__ float s_scale[TG_BK], s_shift[TG_BK];
-    __shared__ float s_ps[16][TG_BN + 1], s_pq[16][TG_BN + 1];
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
     const int r0 = blockIdx.x * TG_BM, n0 = blockIdx.y * TG_BN;
     const int M = L.B * L.T_out;
@@ -328,33 +228,66 @@ train_fwd_det_kernel(const __grid_constant__ fcn_train_layer L, float *__restric
         fwd_store_partial(L, M, r0, n0, partial, acc);
         return;
     }
+    if constexpr (ORDERED) {
+        __shared__ float s_ps[16][TG_BN + 1], s_pq[16][TG_BN + 1];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int n = n0 + tx * 4 + j;
-        float ps = 0.f, pq = 0.f;
-        if (n < L.N) {
-            const float bias = L.bias != nullptr ? L.bias[n] : 0.f;
+        for (int j = 0; j < 4; ++j) {
+            const int n = n0 + tx * 4 + j;
+            float ps = 0.f, pq = 0.f;
+            if (n < L.N) {
+                const float bias = L.bias != nullptr ? L.bias[n] : 0.f;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = r0 + ty * 4 + i;
-                if (r < M) {
-                    const float y = acc[i][j] + bias;
-                    L.Y[(size_t)r * L.N + n] = y;
-                    ps += y; pq += y * y;
+                for (int i = 0; i < 4; ++i) {
+                    const int r = r0 + ty * 4 + i;
+                    if (r < M) {
+                        const float y = acc[i][j] + bias;
+                        L.Y[(size_t)r * L.N + n] = y;
+                        ps += y; pq += y * y;
+                    }
                 }
             }
+            s_ps[ty][tx * 4 + j] = ps; s_pq[ty][tx * 4 + j] = pq;
         }
-        s_ps[ty][tx * 4 + j] = ps; s_pq[ty][tx * 4 + j] = pq;
-    }
-    if (!L.has_bn) return;
-    __syncthreads();
-    if (tid < TG_BN && n0 + tid < L.N) {
-        float a1 = 0.f, a2 = 0.f;
+        if (!L.has_bn) return;
+        __syncthreads();
+        if (tid < TG_BN && n0 + tid < L.N) {
+            float a1 = 0.f, a2 = 0.f;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) { a1 += s_ps[i][tid]; a2 += s_pq[i][tid]; }
-        float *slot = slots + (size_t)blockIdx.x * 2 * L.N;
-        slot[n0 + tid] = a1;
-        slot[L.N + n0 + tid] = a2;
+            for (int i = 0; i < 16; ++i) { a1 += s_ps[i][tid]; a2 += s_pq[i][tid]; }
+            float *slot = slots + (size_t)blockIdx.x * 2 * L.N;
+            slot[n0 + tid] = a1;
+            slot[L.N + n0 + tid] = a2;
+        }
+    } else {
+        __shared__ float s_sum[TG_BN], s_sq[TG_BN];
+        if (tid < TG_BN) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int n = n0 + tx * 4 + j;
+            float ps = 0.f, pq = 0.f;
+            if (n < L.N) {
+                const float bias = L.bias != nullptr ? L.bias[n] : 0.f;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int r = r0 + ty * 4 + i;
+                    if (r < M) {
+                        const float y = acc[i][j] + bias;
+                        L.Y[(size_t)r * L.N + n] = y;
+                        ps += y; pq += y * y;
+                    }
+                }
+                if (L.has_bn) { atomicAdd(&s_sum[tx * 4 + j], ps); atomicAdd(&s_sq[tx * 4 + j], pq); }
+            }
+        }
+        if (L.has_bn) {
+            __syncthreads();
+            if (tid < TG_BN && n0 + tid < L.N) {
+                const int co = (n0 + tid) % L.Cout;
+                atomicAdd(&L.sums[co], (double)s_sum[tid]);
+                atomicAdd(&L.sums[L.Cout + co], (double)s_sq[tid]);
+            }
+        }
     }
 }
 
@@ -373,10 +306,12 @@ __device__ __forceinline__ void fwd_finish_rows(const fcn_train_layer &L, int M,
     }
 }
 
-// Y = sum over K slices (fixed order) + bias; batch statistics.  Block = 32 columns x 8 row lanes.
+// Y = sum over K slices (fixed order) + bias; batch statistics of row block blockIdx.y: to its slot [row block][2N]
+// with plain stores (ORDERED), else to `sums` by atomics.  Block = 32 columns x 8 row lanes.
+template <bool ORDERED>
 __global__ void __launch_bounds__(256)
 train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *__restrict__ partial, int nslice,
-                        int rows_per_block) {
+                        int rows_per_block, float *__restrict__ slots) {
     const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
     const int n = blockIdx.x * 32 + nl;
     const int M = L.B * L.T_out;
@@ -385,28 +320,15 @@ train_fwd_finish_kernel(const __grid_constant__ fcn_train_layer L, const float *
     fwd_finish_rows(L, M, partial, nslice, n, rl, rb, re, a1, a2);
     if (!L.has_bn) return;
     if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
-        const int co = n % L.Cout;
-        atomicAdd(&L.sums[co], (double)a1);
-        atomicAdd(&L.sums[L.Cout + co], (double)a2);
-    }
-}
-
-// train_fwd_finish_kernel of the deterministic forward: the statistics of row block blockIdx.y go to its slot
-// [row block][2N] (plain stores)
-__global__ void __launch_bounds__(256)
-train_fwd_finish_det_kernel(const __grid_constant__ fcn_train_layer L, const float *__restrict__ partial, int nslice,
-                            int rows_per_block, float *__restrict__ slots) {
-    const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
-    const int n = blockIdx.x * 32 + nl;
-    const int M = L.B * L.T_out;
-    const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
-    float a1 = 0.f, a2 = 0.f;
-    fwd_finish_rows(L, M, partial, nslice, n, rl, rb, re, a1, a2);
-    if (!L.has_bn) return;
-    if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
-        float *slot = slots + (size_t)blockIdx.y * 2 * L.N;
-        slot[n] = a1;
-        slot[L.N + n] = a2;
+        if constexpr (ORDERED) {
+            float *slot = slots + (size_t)blockIdx.y * 2 * L.N;
+            slot[n] = a1;
+            slot[L.N + n] = a2;
+        } else {
+            const int co = n % L.Cout;
+            atomicAdd(&L.sums[co], (double)a1);
+            atomicAdd(&L.sums[L.Cout + co], (double)a2);
+        }
     }
 }
 
@@ -456,9 +378,11 @@ __device__ __forceinline__ void reduce_rows(const fcn_train_layer &L, int M, int
     }
 }
 
+// Sum(dz), Sum(dz*xh) of row block blockIdx.y (Sum(dA) without BN): to its slot [row block][h*N] (h = 2 with BN, 1
+// without) with plain stores (ORDERED), else to `dsums` by atomics.  Block = 32 columns x 8 row lanes.
+template <bool ORDERED>
 __global__ void __launch_bounds__(256)
-train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block) {
-    // block = 32 columns x 8 row lanes
+train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block, float *__restrict__ slots) {
     const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
     const int n = blockIdx.x * 32 + nl;
     const int M = L.B * L.T_out;
@@ -466,27 +390,16 @@ train_reduce_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_bloc
     float a1 = 0.f, a2 = 0.f;
     reduce_rows(L, M, n, rl, rb, re, a1, a2);
     if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
-        const int co = L.has_bn ? n % L.Cout : n;
-        const int C = L.has_bn ? L.Cout : L.N;
-        atomicAdd(&L.dsums[co], (double)a1);
-        if (L.has_bn) atomicAdd(&L.dsums[C + co], (double)a2);
-    }
-}
-
-// train_reduce_kernel of the deterministic backward: row block blockIdx.y's sums go to its slot [row block][h*N]
-// (h = 2 with BN: Sum(dz), Sum(dz*xh); h = 1 without: Sum(dA)), plain stores
-__global__ void __launch_bounds__(256)
-train_reduce_det_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block, float *__restrict__ slots) {
-    const int nl = threadIdx.x % 32, rl = threadIdx.x / 32;
-    const int n = blockIdx.x * 32 + nl;
-    const int M = L.B * L.T_out;
-    const int rb = blockIdx.y * rows_per_block, re = min(M, rb + rows_per_block);
-    float a1 = 0.f, a2 = 0.f;
-    reduce_rows(L, M, n, rl, rb, re, a1, a2);
-    if (column_pair_sum(a1, a2, nl, rl, rl == 0 && n < L.N)) {
-        float *slot = slots + (size_t)blockIdx.y * (L.has_bn ? 2 : 1) * L.N;
-        slot[n] = a1;
-        if (L.has_bn) slot[L.N + n] = a2;
+        if constexpr (ORDERED) {
+            float *slot = slots + (size_t)blockIdx.y * (L.has_bn ? 2 : 1) * L.N;
+            slot[n] = a1;
+            if (L.has_bn) slot[L.N + n] = a2;
+        } else {
+            const int co = L.has_bn ? n % L.Cout : n;
+            const int C = L.has_bn ? L.Cout : L.N;
+            atomicAdd(&L.dsums[co], (double)a1);
+            if (L.has_bn) atomicAdd(&L.dsums[C + co], (double)a2);
+        }
     }
 }
 
@@ -528,36 +441,12 @@ __device__ __forceinline__ void dw_tile(const fcn_train_layer &L, const fcn_trai
     }
 }
 
+// dW tile of row slice blockIdx.z: to part[z][C][N] with plain stores (ORDERED; train_dw_sum_kernel adds the
+// slices), else added to dW by atomics
+template <bool ORDERED>
 __global__ void __launch_bounds__(TG_THREADS)
-train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows_per_block) {
+train_dw_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows_per_block, float *__restrict__ part) {
     __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[row][k-channel], Bs[row][n]
-    __shared__ float s_scale[TG_BM], s_shift[TG_BM];
-    __shared__ DyCoef s_dy[TG_BN];
-    const fcn_train_seg &g = L.seg[seg_idx];
-    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int c0 = blockIdx.x * TG_BM, n0 = blockIdx.y * TG_BN;
-    const int M = L.B * L.T_out;
-    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
-    float acc[4][4] = {};
-    dw_tile(L, g, rb, re, acc, As, Bs, s_scale, s_shift, s_dy);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int c = c0 + ty * 4 + i;
-        if (c >= g.C) continue;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int n = n0 + tx * 4 + j;
-            if (n < L.N) atomicAdd(&L.dW[w_index(L, g, c, n)], acc[i][j]);
-        }
-    }
-}
-
-// train_dw_kernel of the deterministic backward: row slice blockIdx.z's tile goes to part[z][C][N] (plain stores);
-// train_dw_sum_kernel adds the slices
-__global__ void __launch_bounds__(TG_THREADS)
-train_dw_det_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int rows_per_block,
-                    float *__restrict__ part) {
-    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];
     __shared__ float s_scale[TG_BM], s_shift[TG_BM];
     __shared__ DyCoef s_dy[TG_BN];
     const fcn_train_seg &g = L.seg[seg_idx];
@@ -575,7 +464,10 @@ train_dw_det_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int 
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int n = n0 + tx * 4 + j;
-            if (n < L.N) dst[(size_t)c * L.N + n] = acc[i][j];
+            if (n < L.N) {
+                if constexpr (ORDERED) dst[(size_t)c * L.N + n] = acc[i][j];
+                else atomicAdd(&L.dW[w_index(L, g, c, n)], acc[i][j]);
+            }
         }
     }
 }
@@ -631,55 +523,45 @@ __device__ __forceinline__ bool dx_target(const fcn_train_layer &L, const fcn_tr
     return true;
 }
 
+// dX tile of column slice blockIdx.z: to part[z][M][C] with plain stores (ORDERED; train_dx_sum_kernel adds the
+// slices), else added to src.grad through the operand's index map by atomics
+template <bool ORDERED>
 __global__ void __launch_bounds__(TG_THREADS)
-train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_per_slice) {
+train_dx_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_per_slice, float *__restrict__ part) {
     __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];   // As[n][row], Bs[n][channel]
     __shared__ DyCoef s_dy[TG_BK];
     const fcn_train_seg &g = L.seg[seg_idx];
-    const fcn_train_src &s = g.src;
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
     const int r0 = blockIdx.x * TG_BM, c0 = blockIdx.y * TG_BN;
     const int M = L.B * L.T_out;
     float acc[4][4] = {};
     const int n_lo = blockIdx.z * n_per_slice, n_hi = min(L.N, n_lo + n_per_slice);
     dx_tile(L, g, M, r0, c0, n_lo, n_hi, acc, As, Bs, s_dy);
+    if constexpr (ORDERED) {
+        float *dst = part + (size_t)blockIdx.z * M * g.C;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int r = r0 + ty * 4 + i;
-        if (r >= M) continue;
-        int row, colb;
-        if (!dx_target(L, g, r, row, colb)) continue;
+        for (int i = 0; i < 4; ++i) {
+            const int r = r0 + ty * 4 + i;
+            if (r >= M) continue;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int c = c0 + tx * 4 + j;
-            if (c < g.C) atomicAdd(&s.grad[(size_t)row * s.ld + colb + c], acc[i][j]);
+            for (int j = 0; j < 4; ++j) {
+                const int c = c0 + tx * 4 + j;
+                if (c < g.C) dst[(size_t)r * g.C + c] = acc[i][j];
+            }
         }
-    }
-}
-
-// train_dx_kernel of the deterministic backward: column slice blockIdx.z's tile goes to part[z][M][C] (plain
-// stores); train_dx_sum_kernel adds the slices
-__global__ void __launch_bounds__(TG_THREADS)
-train_dx_det_kernel(const __grid_constant__ fcn_train_layer L, int seg_idx, int n_per_slice,
-                    float *__restrict__ part) {
-    __shared__ float As[TG_BK][TG_BM + 4], Bs[TG_BK][TG_BN + 4];
-    __shared__ DyCoef s_dy[TG_BK];
-    const fcn_train_seg &g = L.seg[seg_idx];
-    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int r0 = blockIdx.x * TG_BM, c0 = blockIdx.y * TG_BN;
-    const int M = L.B * L.T_out;
-    float acc[4][4] = {};
-    const int n_lo = blockIdx.z * n_per_slice, n_hi = min(L.N, n_lo + n_per_slice);
-    dx_tile(L, g, M, r0, c0, n_lo, n_hi, acc, As, Bs, s_dy);
-    float *dst = part + (size_t)blockIdx.z * M * g.C;
+    } else {
+        const fcn_train_src &s = g.src;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int r = r0 + ty * 4 + i;
-        if (r >= M) continue;
+        for (int i = 0; i < 4; ++i) {
+            const int r = r0 + ty * 4 + i;
+            if (r >= M) continue;
+            int row, colb;
+            if (!dx_target(L, g, r, row, colb)) continue;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int c = c0 + tx * 4 + j;
-            if (c < g.C) dst[(size_t)r * g.C + c] = acc[i][j];
+            for (int j = 0; j < 4; ++j) {
+                const int c = c0 + tx * 4 + j;
+                if (c < g.C) atomicAdd(&s.grad[(size_t)row * s.ld + colb + c], acc[i][j]);
+            }
         }
     }
 }
@@ -853,55 +735,16 @@ __device__ __forceinline__ void fwd_plain_tiles(const fcn_train_layer &L, const 
     }
 }
 
-// Y[M,N] = act(X[M,K]) * W^T   (W in parameter layout (N,K): both operands contiguous along K)
+// Y[M,N] = act(X[M,K]) * W^T   (W in parameter layout (N,K): both operands contiguous along K).  This CTA's column
+// sums over its 128 rows: ORDERED adds its 16 row groups in group order and stores them to slot blockIdx.x of `slots`
+// [row block][2N] (plain stores), else they go to `sums` by atomics.
+template <bool ORDERED>
 __global__ void __launch_bounds__(FP_THREADS)
-train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L) {
+train_fwd_plain_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ slots) {
     __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
     __shared__ float s_scale[512], s_shift[512];
-    __shared__ float s_sum[FP_BN], s_sq[FP_BN];
-    const fcn_train_seg &g = L.seg[0];
-    const fcn_train_src &s = g.src;
-    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int r0 = blockIdx.x * FP_BM, n0 = blockIdx.y * FP_BN;
-    const int M = L.B * L.T_out, K = g.C;
-    for (int c = tid; c < K; c += FP_THREADS) {
-        const float2 k = src_coef(s, c, true);
-        s_scale[c] = k.x; s_shift[c] = k.y;
-    }
-    if (tid < FP_BN) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
-    __syncthreads();
-    float acc[8][4] = {};
-    fwd_plain_tiles(L, g, tid, tx, ty, r0, n0, M, K, acc, As, Bs, s_scale, s_shift);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int n = n0 + tx * 4 + j;
-        float ps = 0.f, pq = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const int r = r0 + ty * 8 + i;
-            if (r < M) {
-                const float y = acc[i][j];
-                L.Y[(size_t)r * L.N + n] = y;
-                ps += y; pq += y * y;
-            }
-        }
-        atomicAdd(&s_sum[tx * 4 + j], ps);
-        atomicAdd(&s_sq[tx * 4 + j], pq);
-    }
-    __syncthreads();
-    if (tid < FP_BN) {
-        atomicAdd(&L.sums[n0 + tid], (double)s_sum[tid]);
-        atomicAdd(&L.sums[L.Cout + n0 + tid], (double)s_sq[tid]);
-    }
-}
-
-// train_fwd_plain_kernel of the deterministic forward: this CTA's column sums over its 128 rows (16 row groups added
-// in group order) go to slot blockIdx.x of `slots` [row block][2N], plain stores
-__global__ void __launch_bounds__(FP_THREADS)
-train_fwd_plain_det_kernel(const __grid_constant__ fcn_train_layer L, float *__restrict__ slots) {
-    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
-    __shared__ float s_scale[512], s_shift[512];
-    __shared__ float s_ps[16][FP_BN + 1], s_pq[16][FP_BN + 1];
+    // column sums Sum(y), Sum(y^2): per row group (ORDERED), else one per column, zeroed before the main loop
+    __shared__ std::conditional_t<ORDERED, float[16][FP_BN + 1], float[FP_BN]> s_ps, s_pq;
     const fcn_train_seg &g = L.seg[0];
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
     const int r0 = blockIdx.x * FP_BM, n0 = blockIdx.y * FP_BN;
@@ -910,6 +753,8 @@ train_fwd_plain_det_kernel(const __grid_constant__ fcn_train_layer L, float *__r
         const float2 k = src_coef(g.src, c, true);
         s_scale[c] = k.x; s_shift[c] = k.y;
     }
+    if constexpr (!ORDERED)
+        if (tid < FP_BN) { s_ps[tid] = 0.f; s_pq[tid] = 0.f; }
     __syncthreads();
     float acc[8][4] = {};
     fwd_plain_tiles(L, g, tid, tx, ty, r0, n0, M, K, acc, As, Bs, s_scale, s_shift);
@@ -926,16 +771,26 @@ train_fwd_plain_det_kernel(const __grid_constant__ fcn_train_layer L, float *__r
                 ps += y; pq += y * y;
             }
         }
-        s_ps[ty][tx * 4 + j] = ps; s_pq[ty][tx * 4 + j] = pq;
+        if constexpr (ORDERED) {
+            s_ps[ty][tx * 4 + j] = ps; s_pq[ty][tx * 4 + j] = pq;
+        } else {
+            atomicAdd(&s_ps[tx * 4 + j], ps);
+            atomicAdd(&s_pq[tx * 4 + j], pq);
+        }
     }
     __syncthreads();
     if (tid < FP_BN) {
-        float a1 = 0.f, a2 = 0.f;
+        if constexpr (ORDERED) {
+            float a1 = 0.f, a2 = 0.f;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) { a1 += s_ps[i][tid]; a2 += s_pq[i][tid]; }
-        float *slot = slots + (size_t)blockIdx.x * 2 * L.N;
-        slot[n0 + tid] = a1;
-        slot[L.N + n0 + tid] = a2;
+            for (int i = 0; i < 16; ++i) { a1 += s_ps[i][tid]; a2 += s_pq[i][tid]; }
+            float *slot = slots + (size_t)blockIdx.x * 2 * L.N;
+            slot[n0 + tid] = a1;
+            slot[L.N + n0 + tid] = a2;
+        } else {
+            atomicAdd(&L.sums[n0 + tid], (double)s_ps[tid]);
+            atomicAdd(&L.sums[L.Cout + n0 + tid], (double)s_pq[tid]);
+        }
     }
 }
 
@@ -1064,34 +919,12 @@ __device__ __forceinline__ void dw_plain_tiles(const fcn_train_layer &L, const f
     }
 }
 
-// dW[N,K] += dY[M,N]^T * act(X[M,K])   over the row slice [z*rows_per_block, ...): atomicAdd into the bucket
+// dW[N,K] += dY[M,N]^T * act(X[M,K])   over the row slice [z*rows_per_block, ...): to part[z][N][C] with plain
+// float4 stores (ORDERED; train_dw_sum_kernel adds the slices), else atomicAdd into the bucket
+template <bool ORDERED>
 __global__ void __launch_bounds__(FP_THREADS)
-train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block) {
+train_dw_plain_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block, float *__restrict__ part) {
     __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];   // As[row][n], Bs[row][k]
-    __shared__ DyCoef s_c[FP_BM];
-    __shared__ float s_scale[FP_BN], s_shift[FP_BN];
-    const fcn_train_seg &g = L.seg[0];
-    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int n0 = blockIdx.x * FP_BM, c0 = blockIdx.y * FP_BN;
-    const int M = L.B * L.T_out, N = L.N;
-    const int rb = blockIdx.z * rows_per_block, re = min(M, rb + rows_per_block);
-    float acc[8][4] = {};
-    dw_plain_tiles(L, g, tid, n0, c0, N, rb, re, acc, As, Bs, s_c, s_scale, s_shift);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int n = n0 + ty * 8 + i;
-        if (n >= N) continue;
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-            atomicAdd(&L.dW[g.w_off + (size_t)n * L.s_co + c0 + tx * 4 + j], acc[i][j]);
-    }
-}
-
-// train_dw_plain_kernel of the deterministic backward: row slice blockIdx.z's tile goes to part[z][N][C] (plain
-// float4 stores); train_dw_sum_kernel adds the slices
-__global__ void __launch_bounds__(FP_THREADS)
-train_dw_plain_det_kernel(const __grid_constant__ fcn_train_layer L, int rows_per_block, float *__restrict__ part) {
-    __shared__ __align__(16) float As[FP_BK][FP_BM + 4], Bs[FP_BK][FP_BN + 4];
     __shared__ DyCoef s_c[FP_BM];
     __shared__ float s_scale[FP_BN], s_shift[FP_BN];
     const fcn_train_seg &g = L.seg[0];
@@ -1105,8 +938,14 @@ train_dw_plain_det_kernel(const __grid_constant__ fcn_train_layer L, int rows_pe
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int n = n0 + ty * 8 + i;
-        if (n < N)
+        if (n >= N) continue;
+        if constexpr (ORDERED) {
             *(float4 *)(dst + (size_t)n * C + c0 + tx * 4) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                atomicAdd(&L.dW[g.w_off + (size_t)n * L.s_co + c0 + tx * 4 + j], acc[i][j]);
+        }
     }
 }
 
@@ -1164,121 +1003,36 @@ static int split_len(int len, int ctas) {
     return per < 2 * TG_BK ? 2 * TG_BK : per;
 }
 
-extern "C" long long fcn_train_workspace_floats(const fcn_train_layer *L) {
-    // enough for the split the launcher would like to use: SPLIT_CTAS CTAs' worth of partial tiles, at most K/32 slices
-    if (L == nullptr) return 0;
-    int tps = 0;
-    const int n = fwd_slices(*L, (long long)1 << 40, &tps);
-    return n > 1 ? (long long)n * L->B * L->T_out * L->N : 0;
-}
+// How a layer's GEMMs are split.  Both modes launch these splits.  The forward's K split is the largest that
+// `fwd_workspace_floats` holds: the default forward passes its workspace, the deterministic mode and the workspace
+// queries pass FWD_UNBOUNDED, so every split the deterministic mode uses depends on the layer's shape only.
+constexpr long long FWD_UNBOUNDED = (long long)1 << 40;
 
-extern "C" int fcn_train_forward(const fcn_train_layer *L, float *workspace, long long workspace_floats,
-                                 fcn_stream_t stream) {
-    FCN_REQUIRE(L != nullptr, "NULL layer");
-    if (int rc = check_layer(*L)) return rc;
-    const int M = L->B * L->T_out;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (host_plain(*L)) {
-        dim3 grid(ceil_div(M, FP_BM), L->N / FP_BN);
-        train_fwd_plain_kernel<<<grid, FP_THREADS, 0, st>>>(*L);
-        FCN_LAUNCH_CHECK();
-        return FCN_OK;
-    }
-    int tps = 0;
-    const int nslice = workspace != nullptr ? fwd_slices(*L, workspace_floats, &tps) : (fwd_slices(*L, 0, &tps), 1);
-    dim3 grid(ceil_div(M, TG_BM), ceil_div(L->N, TG_BN), nslice);
-    train_fwd_kernel<<<grid, TG_THREADS, 0, st>>>(*L, workspace, tps);
-    FCN_LAUNCH_CHECK();
-    if (nslice > 1) {
-        const int rpb = 32;
-        dim3 gf(ceil_div(L->N, 32), ceil_div(M, rpb));
-        train_fwd_finish_kernel<<<gf, 256, 0, st>>>(*L, workspace, nslice, rpb);
-        FCN_LAUNCH_CHECK();
-    }
-    return FCN_OK;
-}
-
-extern "C" int fcn_train_backward(const fcn_train_layer *L, int need_dx_mask, fcn_stream_t stream) {
-    FCN_REQUIRE(L != nullptr, "NULL layer");
-    if (int rc = check_layer(*L)) return rc;
-    FCN_REQUIRE(L->dA && L->dW && L->dsums, "NULL gradient buffers");
-    const int M = L->B * L->T_out;
-    cudaStream_t st = (cudaStream_t)stream;
-    {   // Sum(dz), Sum(dz * xh) per channel
-        const int rpb = M >= 4096 ? 256 : 32;
-        dim3 grid(ceil_div(L->N, 32), ceil_div(M, rpb));
-        train_reduce_kernel<<<grid, 256, 0, st>>>(*L, rpb);
-        FCN_LAUNCH_CHECK();
-    }
-    if (host_plain(*L)) {
-        const int rpb = 1024;
-        dim3 grid(ceil_div(L->N, FP_BM), L->seg[0].C / FP_BN, ceil_div(M, rpb));
-        train_dw_plain_kernel<<<grid, FP_THREADS, 0, st>>>(*L, rpb);
-        FCN_LAUNCH_CHECK();
-        if ((need_dx_mask & 1) && L->seg[0].src.grad != nullptr) {
-            dim3 gx(ceil_div(M, FP_BM), L->seg[0].C / FP_BN);
-            train_dx_plain_kernel<<<gx, FP_THREADS, 0, st>>>(*L);
-            FCN_LAUNCH_CHECK();
-        }
-        return FCN_OK;
-    }
-    for (int sg = 0; sg < L->n_seg; ++sg) {
-        const int rpb = split_len(M, ceil_div(L->seg[sg].C, TG_BM) * ceil_div(L->N, TG_BN));
-        dim3 grid(ceil_div(L->seg[sg].C, TG_BM), ceil_div(L->N, TG_BN), ceil_div(M, rpb));
-        train_dw_kernel<<<grid, TG_THREADS, 0, st>>>(*L, sg, rpb);
-        FCN_LAUNCH_CHECK();
-        if (((need_dx_mask >> sg) & 1) && L->seg[sg].src.grad != nullptr) {
-            const int nps = split_len(L->N, ceil_div(M, TG_BM) * ceil_div(L->seg[sg].C, TG_BN));
-            dim3 gx(ceil_div(M, TG_BM), ceil_div(L->seg[sg].C, TG_BN), ceil_div(L->N, nps));
-            train_dx_kernel<<<gx, TG_THREADS, 0, st>>>(*L, sg, nps);
-            FCN_LAUNCH_CHECK();
-        }
-    }
-    return FCN_OK;
-}
-
-// ------------------------------------------------------------------ deterministic mode
-// The same GEMMs with every float atomic replaced by plain stores of partial results into the workspace and ordered
-// sums of those partials: per-row-block column sums (slots) for Sum(y), Sum(y^2), Sum(dz), Sum(dz*xh), row-slice
-// tiles for dW and column-slice tiles for dX.  Every split depends on the layer's shape only: the forward's K split
-// is the one fwd_slices picks for an unbounded workspace, the backward's splits are fcn_train_backward's.
-constexpr int DET_FINISH_RPB = 32;     // rows per block of train_fwd_finish_det_kernel
-constexpr int PLAIN_DW_RPB = 1024;     // rows per row slice of the plain dW kernels
-
-static int reduce_rpb(int M) { return M >= 4096 ? 256 : 32; }
-
-// sizes, in floats, of what the deterministic forward keeps in the workspace: K-split partials, then the slots
-struct DetFwdPlan {
-    int nslice, tiles_per_slice, nrb;
-    long long partial, slots;
+struct TrainPlan {
+    bool plain;                  // host_plain: the 128 x 64 kernels, which split neither K nor the dX columns
+    int nslice, tiles_per_slice; // K slices of the generic forward and linear K tiles per slice
+    long long partial;           // floats of the generic forward's K-slice partial sums (0 without a split)
+    int stats_rpb;               // rows per block of the forward statistics: the plain or generic CTA's rows, or the
+                                 // finish kernel's when K is split
+    int reduce_rpb;              // rows per block of the backward's column reduction
+    int dw_rpb[FCN_MAX_SEGS];    // per segment: rows per slice of dW
+    int dx_nps[FCN_MAX_SEGS];    // per segment: columns per slice of the generic dX
 };
-static DetFwdPlan det_fwd_plan(const fcn_train_layer &L) {
-    const int M = L.B * L.T_out;
-    DetFwdPlan p{1, 0, 0, 0, 0};
-    if (host_plain(L)) {
-        p.nrb = ceil_div(M, FP_BM);
-    } else {
-        p.nslice = fwd_slices(L, (long long)1 << 40, &p.tiles_per_slice);
-        p.partial = p.nslice > 1 ? (long long)p.nslice * M * L.N : 0;
-        p.nrb = ceil_div(M, p.nslice > 1 ? DET_FINISH_RPB : TG_BM);
-    }
-    p.slots = L.has_bn ? (long long)p.nrb * 2 * L.N : 0;
-    return p;
-}
 
-// the largest piece the deterministic backward keeps in the workspace (its launches use it one after another)
-static long long det_bwd_floats(const fcn_train_layer &L) {
+static TrainPlan train_plan(const fcn_train_layer &L, long long fwd_workspace_floats) {
     const int M = L.B * L.T_out;
-    long long need = (long long)ceil_div(M, reduce_rpb(M)) * (L.has_bn ? 2 : 1) * L.N;
-    if (host_plain(L)) return std::max(need, (long long)ceil_div(M, PLAIN_DW_RPB) * L.N * L.seg[0].C);
+    TrainPlan p{};
+    p.plain = host_plain(L);
+    p.nslice = fwd_slices(L, fwd_workspace_floats, &p.tiles_per_slice);
+    p.partial = p.nslice > 1 ? (long long)p.nslice * M * L.N : 0;
+    p.stats_rpb = p.plain ? FP_BM : p.nslice > 1 ? 32 : TG_BM;
+    p.reduce_rpb = M >= 4096 ? 256 : 32;
     for (int sg = 0; sg < L.n_seg; ++sg) {
         const int C = L.seg[sg].C;
-        const int rpb = split_len(M, ceil_div(C, TG_BM) * ceil_div(L.N, TG_BN));
-        const int nps = split_len(L.N, ceil_div(M, TG_BM) * ceil_div(C, TG_BN));
-        need = std::max(need, (long long)ceil_div(M, rpb) * C * L.N);
-        need = std::max(need, (long long)ceil_div(L.N, nps) * M * C);
+        p.dw_rpb[sg] = p.plain ? 1024 : split_len(M, ceil_div(C, TG_BM) * ceil_div(L.N, TG_BN));
+        p.dx_nps[sg] = p.plain ? 0 : split_len(L.N, ceil_div(M, TG_BM) * ceil_div(C, TG_BN));
     }
-    return need;
+    return p;
 }
 
 static bool shape_ok(const fcn_train_layer &L) {
@@ -1289,9 +1043,22 @@ static bool shape_ok(const fcn_train_layer &L) {
     return true;
 }
 
+// ------------------------------------------------------------------ deterministic mode
+// The same GEMMs with every float atomic replaced by plain stores of partial results into the workspace and ordered
+// sums of those partials: per-row-block column sums (slots) for Sum(y), Sum(y^2), Sum(dz), Sum(dz*xh), row-slice
+// tiles for dW and column-slice tiles for dX.  The forward keeps its K-split partials, then the slots; the backward's
+// launches use the workspace one after another.
 static long long det_floats(const fcn_train_layer &L) {
-    const DetFwdPlan f = det_fwd_plan(L);
-    return std::max(f.partial + f.slots, det_bwd_floats(L));
+    const TrainPlan p = train_plan(L, FWD_UNBOUNDED);
+    const int M = L.B * L.T_out;
+    const long long fwd = (p.plain ? 0 : p.partial) + (L.has_bn ? (long long)ceil_div(M, p.stats_rpb) * 2 * L.N : 0);
+    long long bwd = (long long)ceil_div(M, p.reduce_rpb) * (L.has_bn ? 2 : 1) * L.N;
+    for (int sg = 0; sg < L.n_seg; ++sg) {
+        const int C = L.seg[sg].C;
+        bwd = std::max(bwd, (long long)ceil_div(M, p.dw_rpb[sg]) * C * L.N);
+        if (!p.plain) bwd = std::max(bwd, (long long)ceil_div(L.N, p.dx_nps[sg]) * M * C);
+    }
+    return std::max(fwd, bwd);
 }
 
 static int det_workspace_check(const fcn_train_layer &L, const float *ws, long long ws_floats) {
@@ -1306,85 +1073,125 @@ static int launch_slots_sum(double *dst, const float *slots, int nrb, int N, int
     return FCN_OK;
 }
 
+// cudaGetLastError after a launch, reported as an error of the entry `fn`
+static int launch_error(const char *fn) {
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? FCN_OK : cuda_fail(fn, e);
+}
+
+// Forward of one layer for the entry `fn`; `ordered` is the deterministic mode, whose statistics go to slots after
+// the K-split partials.
+static int train_forward(const char *fn, const fcn_train_layer *L, float *ws, long long ws_floats, bool ordered,
+                         cudaStream_t st) {
+    if (L == nullptr) return invalid(fn, "NULL layer");
+    if (int rc = check_layer(*L)) return rc;
+    if (ordered)
+        if (int rc = det_workspace_check(*L, ws, ws_floats)) return rc;
+    const TrainPlan p = train_plan(*L, ordered ? FWD_UNBOUNDED : ws != nullptr ? ws_floats : 0);
+    const int M = L->B * L->T_out, nrb = ceil_div(M, p.stats_rpb);
+    float *slots = ordered ? ws + (p.plain ? 0 : p.partial) : nullptr;
+    if (p.plain) {
+        dim3 grid(nrb, L->N / FP_BN);
+        (ordered ? train_fwd_plain_kernel<true> : train_fwd_plain_kernel<false>)<<<grid, FP_THREADS, 0, st>>>(*L, slots);
+        if (int rc = launch_error(fn)) return rc;
+    } else {
+        dim3 grid(ceil_div(M, TG_BM), ceil_div(L->N, TG_BN), p.nslice);
+        (ordered ? train_fwd_kernel<true> : train_fwd_kernel<false>)<<<grid, TG_THREADS, 0, st>>>(
+            *L, ws, p.tiles_per_slice, slots);
+        if (int rc = launch_error(fn)) return rc;
+        if (p.nslice > 1) {
+            dim3 gf(ceil_div(L->N, 32), nrb);
+            (ordered ? train_fwd_finish_kernel<true> : train_fwd_finish_kernel<false>)<<<gf, 256, 0, st>>>(
+                *L, ws, p.nslice, p.stats_rpb, slots);
+            if (int rc = launch_error(fn)) return rc;
+        }
+    }
+    if (ordered && L->has_bn) return launch_slots_sum(L->sums, slots, nrb, L->N, L->Cout, 2, st);
+    return FCN_OK;
+}
+
+// Backward of one layer for the entry `fn`; `ordered` is the deterministic mode, which adds every set of partials it
+// stores in the workspace before its next launch.
+static int train_backward(const char *fn, const fcn_train_layer *L, int need_dx_mask, float *ws, long long ws_floats,
+                          bool ordered, cudaStream_t st) {
+    if (L == nullptr) return invalid(fn, "NULL layer");
+    if (int rc = check_layer(*L)) return rc;
+    if (!(L->dA && L->dW && L->dsums)) return invalid(fn, "NULL gradient buffers");
+    if (ordered)
+        if (int rc = det_workspace_check(*L, ws, ws_floats)) return rc;
+    const TrainPlan p = train_plan(*L, FWD_UNBOUNDED);
+    const int M = L->B * L->T_out, N = L->N;
+    {   // Sum(dz), Sum(dz * xh) per channel
+        const int nrb = ceil_div(M, p.reduce_rpb);
+        (ordered ? train_reduce_kernel<true> : train_reduce_kernel<false>)<<<dim3(ceil_div(N, 32), nrb), 256, 0, st>>>(
+            *L, p.reduce_rpb, ws);
+        if (int rc = launch_error(fn)) return rc;
+        if (ordered)
+            if (int rc = launch_slots_sum(L->dsums, ws, nrb, N, L->has_bn ? L->Cout : N, L->has_bn ? 2 : 1, st))
+                return rc;
+    }
+    for (int sg = 0; sg < L->n_seg; ++sg) {
+        const int C = L->seg[sg].C, nz = ceil_div(M, p.dw_rpb[sg]);
+        if (p.plain) {
+            dim3 grid(ceil_div(N, FP_BM), C / FP_BN, nz);
+            (ordered ? train_dw_plain_kernel<true> : train_dw_plain_kernel<false>)<<<grid, FP_THREADS, 0, st>>>(
+                *L, p.dw_rpb[sg], ws);
+        } else {
+            dim3 grid(ceil_div(C, TG_BM), ceil_div(N, TG_BN), nz);
+            (ordered ? train_dw_kernel<true> : train_dw_kernel<false>)<<<grid, TG_THREADS, 0, st>>>(
+                *L, sg, p.dw_rpb[sg], ws);
+        }
+        if (int rc = launch_error(fn)) return rc;
+        if (ordered) {
+            train_dw_sum_kernel<<<ceil_div(C * N, 256), 256, 0, st>>>(*L, sg, ws, nz, !p.plain);
+            if (int rc = launch_error(fn)) return rc;
+        }
+        if (!((need_dx_mask >> sg) & 1) || L->seg[sg].src.grad == nullptr) continue;
+        if (p.plain) {      // one CTA per element, no split: order-free in both modes
+            train_dx_plain_kernel<<<dim3(ceil_div(M, FP_BM), C / FP_BN), FP_THREADS, 0, st>>>(*L);
+            if (int rc = launch_error(fn)) return rc;
+            continue;
+        }
+        const int nzx = ceil_div(N, p.dx_nps[sg]);
+        (ordered ? train_dx_kernel<true> : train_dx_kernel<false>)<<<dim3(ceil_div(M, TG_BM), ceil_div(C, TG_BN), nzx),
+                                                                      TG_THREADS, 0, st>>>(*L, sg, p.dx_nps[sg], ws);
+        if (int rc = launch_error(fn)) return rc;
+        if (ordered) {
+            train_dx_sum_kernel<<<(unsigned)(((long long)M * C + 255) / 256), 256, 0, st>>>(*L, sg, ws, nzx);
+            if (int rc = launch_error(fn)) return rc;
+        }
+    }
+    return FCN_OK;
+}
+
+extern "C" long long fcn_train_workspace_floats(const fcn_train_layer *L) {
+    // enough for the split the launcher would like to use: SPLIT_CTAS CTAs' worth of partial tiles, at most K/32 slices
+    if (L == nullptr || !shape_ok(*L)) return 0;
+    return train_plan(*L, FWD_UNBOUNDED).partial;
+}
+
 extern "C" long long fcn_train_deterministic_workspace_floats(const fcn_train_layer *L) {
     if (L == nullptr || !shape_ok(*L)) return 0;
     return det_floats(*L);
 }
 
+extern "C" int fcn_train_forward(const fcn_train_layer *L, float *workspace, long long workspace_floats,
+                                 fcn_stream_t stream) {
+    return train_forward(__func__, L, workspace, workspace_floats, false, (cudaStream_t)stream);
+}
+
 extern "C" int fcn_train_forward_deterministic(const fcn_train_layer *L, float *workspace, long long workspace_floats,
                                                fcn_stream_t stream) {
-    FCN_REQUIRE(L != nullptr, "NULL layer");
-    if (int rc = check_layer(*L)) return rc;
-    if (int rc = det_workspace_check(*L, workspace, workspace_floats)) return rc;
-    const int M = L->B * L->T_out;
-    cudaStream_t st = (cudaStream_t)stream;
-    const DetFwdPlan p = det_fwd_plan(*L);
-    float *slots = workspace + p.partial;
-    if (host_plain(*L)) {
-        dim3 grid(p.nrb, L->N / FP_BN);
-        train_fwd_plain_det_kernel<<<grid, FP_THREADS, 0, st>>>(*L, slots);
-        FCN_LAUNCH_CHECK();
-    } else {
-        dim3 grid(ceil_div(M, TG_BM), ceil_div(L->N, TG_BN), p.nslice);
-        train_fwd_det_kernel<<<grid, TG_THREADS, 0, st>>>(*L, workspace, p.tiles_per_slice, slots);
-        FCN_LAUNCH_CHECK();
-        if (p.nslice > 1) {
-            dim3 gf(ceil_div(L->N, 32), p.nrb);
-            train_fwd_finish_det_kernel<<<gf, 256, 0, st>>>(*L, workspace, p.nslice, DET_FINISH_RPB, slots);
-            FCN_LAUNCH_CHECK();
-        }
-    }
-    if (L->has_bn) return launch_slots_sum(L->sums, slots, p.nrb, L->N, L->Cout, 2, st);
-    return FCN_OK;
+    return train_forward(__func__, L, workspace, workspace_floats, true, (cudaStream_t)stream);
+}
+
+extern "C" int fcn_train_backward(const fcn_train_layer *L, int need_dx_mask, fcn_stream_t stream) {
+    return train_backward(__func__, L, need_dx_mask, nullptr, 0, false, (cudaStream_t)stream);
 }
 
 extern "C" int fcn_train_backward_deterministic(const fcn_train_layer *L, int need_dx_mask, float *workspace,
                                                 long long workspace_floats, fcn_stream_t stream) {
-    FCN_REQUIRE(L != nullptr, "NULL layer");
-    if (int rc = check_layer(*L)) return rc;
-    FCN_REQUIRE(L->dA && L->dW && L->dsums, "NULL gradient buffers");
-    if (int rc = det_workspace_check(*L, workspace, workspace_floats)) return rc;
-    const int M = L->B * L->T_out;
-    cudaStream_t st = (cudaStream_t)stream;
-    {   // Sum(dz), Sum(dz * xh) per channel
-        const int rpb = reduce_rpb(M), nrb = ceil_div(M, rpb);
-        train_reduce_det_kernel<<<dim3(ceil_div(L->N, 32), nrb), 256, 0, st>>>(*L, rpb, workspace);
-        FCN_LAUNCH_CHECK();
-        if (int rc = launch_slots_sum(L->dsums, workspace, nrb, L->N, L->has_bn ? L->Cout : L->N, L->has_bn ? 2 : 1, st))
-            return rc;
-    }
-    if (host_plain(*L)) {
-        const int C = L->seg[0].C, nz = ceil_div(M, PLAIN_DW_RPB);
-        dim3 grid(ceil_div(L->N, FP_BM), C / FP_BN, nz);
-        train_dw_plain_det_kernel<<<grid, FP_THREADS, 0, st>>>(*L, PLAIN_DW_RPB, workspace);
-        FCN_LAUNCH_CHECK();
-        train_dw_sum_kernel<<<ceil_div(C * L->N, 256), 256, 0, st>>>(*L, 0, workspace, nz, 0);
-        FCN_LAUNCH_CHECK();
-        if ((need_dx_mask & 1) && L->seg[0].src.grad != nullptr) {     // one CTA per element, no split: order-free
-            dim3 gx(ceil_div(M, FP_BM), C / FP_BN);
-            train_dx_plain_kernel<<<gx, FP_THREADS, 0, st>>>(*L);
-            FCN_LAUNCH_CHECK();
-        }
-        return FCN_OK;
-    }
-    for (int sg = 0; sg < L->n_seg; ++sg) {
-        const int C = L->seg[sg].C;
-        const int rpb = split_len(M, ceil_div(C, TG_BM) * ceil_div(L->N, TG_BN)), nz = ceil_div(M, rpb);
-        dim3 grid(ceil_div(C, TG_BM), ceil_div(L->N, TG_BN), nz);
-        train_dw_det_kernel<<<grid, TG_THREADS, 0, st>>>(*L, sg, rpb, workspace);
-        FCN_LAUNCH_CHECK();
-        train_dw_sum_kernel<<<ceil_div(C * L->N, 256), 256, 0, st>>>(*L, sg, workspace, nz, 1);
-        FCN_LAUNCH_CHECK();
-        if (((need_dx_mask >> sg) & 1) && L->seg[sg].src.grad != nullptr) {
-            const int nps = split_len(L->N, ceil_div(M, TG_BM) * ceil_div(C, TG_BN)), nzx = ceil_div(L->N, nps);
-            dim3 gx(ceil_div(M, TG_BM), ceil_div(C, TG_BN), nzx);
-            train_dx_det_kernel<<<gx, TG_THREADS, 0, st>>>(*L, sg, nps, workspace);
-            FCN_LAUNCH_CHECK();
-            train_dx_sum_kernel<<<(unsigned)(((long long)M * C + 255) / 256), 256, 0, st>>>(*L, sg, workspace, nzx);
-            FCN_LAUNCH_CHECK();
-        }
-    }
-    return FCN_OK;
+    return train_backward(__func__, L, need_dx_mask, workspace, workspace_floats, true, (cudaStream_t)stream);
 }
 
 extern "C" int fcn_train_pool(const fcn_train_pool_args *P, int backward, fcn_stream_t stream) {

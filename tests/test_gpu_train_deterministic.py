@@ -114,7 +114,7 @@ def test_every_layer_is_bit_identical_across_streams_and_workspace_contents(wl, 
         ev, es = tr.scatter(nW, widx, torch.cat(dWv), torch.cat(dWs))
         off = (L.dW - eng.flat.grad.data_ptr()) // 4
         _assert_within(eng.flat.grad[off:off + nW], ev, es, "%s %s dW" % (wl, nm))
-        # dX (train_dx_det_kernel + train_dx_sum_kernel, or train_dx_plain_kernel): summed over every consumer
+        # dX (train_dx_kernel<true> + train_dx_sum_kernel, or train_dx_plain_kernel): summed over every consumer
         for j in range(L.n_seg):
             s = L.seg[j].src
             if not ((eng.dx_mask[li] >> j) & 1) or not s.grad:

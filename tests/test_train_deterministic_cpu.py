@@ -8,11 +8,12 @@ import subprocess
 import pytest
 
 from frustum_convnet_b200 import _lib, build
+from test_train_kernels_compile_cpu import kernel_key
 
 TRAIN_KERNELS = [
-    "train_fwd_det_kernel", "train_fwd_finish_det_kernel", "train_slots_sum_kernel", "train_reduce_det_kernel",
-    "train_dw_det_kernel", "train_dw_sum_kernel", "train_dx_det_kernel", "train_dx_sum_kernel",
-    "train_fwd_plain_det_kernel", "train_dw_plain_det_kernel",
+    "train_fwd_kernel<true>", "train_fwd_finish_kernel<true>", "train_slots_sum_kernel", "train_reduce_kernel<true>",
+    "train_dw_kernel<true>", "train_dw_sum_kernel", "train_dx_kernel<true>", "train_dx_sum_kernel",
+    "train_fwd_plain_kernel<true>", "train_dw_plain_kernel<true>",
 ]
 ENTRIES = ["fcn_train_deterministic_workspace_floats", "fcn_train_forward_deterministic",
            "fcn_train_backward_deterministic", "fcn_det_loss_deterministic_scratch_floats", "fcn_det_loss_deterministic"]
@@ -28,9 +29,9 @@ def _ptxas(src, tmp_path):
     assert r.returncode == 0, r.stdout + r.stderr
     res, cur = {}, None
     for ln in (r.stdout + r.stderr).splitlines():
-        m = re.search(r"Compiling entry function '_ZN3fcn(\d+)(\S+)'", ln)
+        m = re.search(r"Compiling entry function '(\S+)'", ln)
         if m:
-            cur = m.group(2)[:int(m.group(1))]
+            cur = kernel_key(m.group(1))
         m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", ln)
         if m and cur is not None:
             res[cur] = tuple(int(v) for v in m.groups())
@@ -44,11 +45,11 @@ def test_deterministic_train_kernels_no_stack_no_spills(tmp_path):
 
 
 def test_deterministic_loss_kernels_compile_like_the_default(tmp_path):
-    """The row kernel shares its body with det_loss_rows_kernel, whose corner arrays live in a local frame: the same
-    frame, and no spills."""
+    """The ordered row kernel is the default one's template instantiation, whose corner arrays live in a local frame:
+    the same frame, and no spills."""
     res = _ptxas("loss.cu", tmp_path)
-    assert res["det_loss_rows_det_kernel"] == res["det_loss_rows_kernel"]
-    assert res["det_loss_rows_det_kernel"][1:] == (0, 0)
+    assert res["det_loss_rows_kernel<true>"] == res["det_loss_rows_kernel<false>"]
+    assert res["det_loss_rows_kernel<true>"][1:] == (0, 0)
     assert res["det_loss_slots_kernel"] == (0, 0, 0)
 
 

@@ -15,9 +15,9 @@ import pytest
 from frustum_convnet_b200 import build
 
 KERNELS = [
-    "train_fwd_kernel", "train_fwd_finish_kernel", "train_reduce_kernel", "train_dw_kernel", "train_dx_kernel",
-    "train_pool_fwd_kernel", "train_pool_bwd_kernel", "train_finalize_kernel", "train_adam_kernel",
-    "train_fwd_plain_kernel", "train_dx_plain_kernel", "train_dw_plain_kernel",
+    "train_fwd_kernel<false>", "train_fwd_finish_kernel<false>", "train_reduce_kernel<false>", "train_dw_kernel<false>",
+    "train_dx_kernel<false>", "train_pool_fwd_kernel", "train_pool_bwd_kernel", "train_finalize_kernel",
+    "train_adam_kernel", "train_fwd_plain_kernel<false>", "train_dx_plain_kernel", "train_dw_plain_kernel<false>",
 ]
 
 
@@ -26,6 +26,17 @@ def _nvcc():
         return build._nvcc()
     except RuntimeError:
         pytest.skip("nvcc is not installed")
+
+
+def kernel_key(mangled):
+    """_ZN3fcn<length><name>E... -> name, and _ZN3fcn<length><name>ILb0EE... -> name<false> (ILb1E: name<true>):
+    the two instantiations of a `template <bool>` kernel are told apart."""
+    m = re.match(r"_ZN3fcn(\d+)", mangled)
+    if not m:
+        return None
+    end = m.end() + int(m.group(1))
+    t = re.match(r"ILb([01])E", mangled[end:])
+    return mangled[m.end():end] + ("<%s>" % ("true" if t.group(1) == "1" else "false") if t else "")
 
 
 def _resources(log):
@@ -49,10 +60,10 @@ def test_train_kernels_no_stack_no_spills(tmp_path):
     assert r.returncode == 0, r.stdout + r.stderr
     res = _resources(r.stdout + r.stderr)
     by_name = {}
-    for mangled, usage in res.items():                    # _ZN3fcn<length><name>E...
-        m = re.match(r"_ZN3fcn(\d+)", mangled)
-        if m:
-            by_name[mangled[m.end():m.end() + int(m.group(1))]] = usage
+    for mangled, usage in res.items():
+        k = kernel_key(mangled)
+        if k:
+            by_name[k] = usage
     missing = [k for k in KERNELS if k not in by_name]
     assert not missing, "kernels not compiled: %s (found %s)" % (missing, sorted(by_name))
     for k in KERNELS:
