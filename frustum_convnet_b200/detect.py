@@ -28,7 +28,7 @@ from . import _lib
 from ._host import cuda_device, workspace
 
 _DATASETS = {"KITTI": 0, "SUNRGBD": 1}
-_METHODS = {"nms": 0}          # every other cfg.TEST.METHOD behaves as 'top' (test_net_det.py:256-263)
+_METHODS = {"nms": _lib.DET_NMS}   # every other cfg.TEST.METHOD behaves as 'top' (test_net_det.py:256-263)
 _SETUP_FIELDS = ("id_list", "type_list", "box2d_list", "dataset", "method", "thresh", "top_k", "num_frustums")
 
 
@@ -150,7 +150,7 @@ class DetectionCollector:
         cp, ce, he, sz, sp, ra = keep_alive[:6]
         a = _lib.DetCandidateArgs()
         a.B, a.T2, a.NS = B, T2, int(sp.shape[-1])
-        a.dataset, a.method = _DATASETS[self.dataset], _METHODS.get(self.method, 1)
+        a.dataset, a.method = _DATASETS[self.dataset], _METHODS.get(self.method, _lib.DET_TOP)
         a.first, a.num_frustums, a.capacity = first, self.num_frustums, self.capacity
         a.cls_probs, a.center, a.heading, a.size, a.size_probs = (t.data_ptr() for t in (cp, ce, he, sz, sp))
         a.rot_angle = ra.data_ptr()
@@ -190,7 +190,7 @@ class DetectionCollector:
             rows = torch.empty((max(capacity, 1), 12), dtype=torch.float32, device=dev)
             a = _lib.DetFinalizeArgs()
             a.num_segments, a.num_frustums, a.capacity = S, self.num_frustums, capacity
-            a.method, a.dataset = _METHODS.get(self.method, 1), _DATASETS[self.dataset]
+            a.method, a.dataset = _METHODS.get(self.method, _lib.DET_TOP), _DATASETS[self.dataset]
             a.top_k, a.thresh = self.top_k, self.thresh
             a.counter, a.records, a.box2d = counter.data_ptr(), records.data_ptr(), self.box2d.data_ptr()
             a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), nbytes, info.data_ptr()

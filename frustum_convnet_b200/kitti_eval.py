@@ -28,8 +28,9 @@ from ._host import csr_offsets, cuda_device, upload, workspace
 
 CLASS_NAMES = ("car", "pedestrian", "cyclist")
 METRICS = ("image", "ground", "3d")
-TYPE_CODES = {"car": 0, "pedestrian": 1, "cyclist": 2, "van": 3, "person_sitting": 4, "dontcare": 5}
-OTHER = 6
+TYPE_CODES = {"car": _lib.KITTI_CAR, "pedestrian": _lib.KITTI_PEDESTRIAN, "cyclist": _lib.KITTI_CYCLIST,
+              "van": _lib.KITTI_VAN, "person_sitting": _lib.KITTI_PERSON_SITTING, "dontcare": _lib.KITTI_DONTCARE}
+OTHER = _lib.KITTI_OTHER
 GT_COLS, DET_COLS, PTS = _lib.KITTI_GT_COLS, _lib.KITTI_DET_COLS, _lib.KITTI_PTS
 
 

@@ -232,8 +232,11 @@ typedef struct {
     float *out;
 } fcn_mega_layer;
 typedef struct {
+    int first, count, target;
+} fcn_mega_dep;
+typedef struct {
     int layer, m_tile, n_tile, n_dep;
-    struct { int first, count, target; } dep[FCN_MEGA_MAX_DEPS];
+    fcn_mega_dep dep[FCN_MEGA_MAX_DEPS];
 } fcn_mega_job;
 typedef struct {
     int n_layers, n_jobs, n_flags, grid;   /* grid: persistent CTAs (0 = one per SM) */

@@ -107,23 +107,89 @@ def test_public_header_is_plain_c(tmp_path):
     assert includes and all(i in ("stdint.h", "stddef.h") for i in includes), includes   # no torch / CUDA headers
 
 
-def test_ctypes_mirrors_have_the_size_of_the_c_structs(tmp_path):
-    """frustum_convnet_b200/_lib.py restates every argument struct of include/frustum_b200.h for ctypes: a field
-    added on one side only would silently shift everything behind it.  Compare sizeof() as gcc sees the header."""
+def test_ctypes_layout_signatures_and_constants_match_the_compiler(tmp_path):
+    """_lib reads its structs, prototypes and constants from include/frustum_b200.h.  A C99 program generated from
+    what it read must see, as gcc compiles the header, the same size and alignment of every struct, the same offset
+    and size of every field and the same value of every define, and every prototype must have exactly the parameter
+    and return types the reader split out of it."""
     import ctypes
     import subprocess
     from frustum_convnet_b200 import _lib
-    pairs = [("fcn_group_args", _lib.GroupArgs), ("fcn_pointnet_args", _lib.PointnetArgs),
-             ("fcn_conv_seg", _lib.ConvSeg), ("fcn_conv_args", _lib.ConvArgs), ("fcn_decode_out", _lib.DecodeOut),
-             ("fcn_mega_seg", _lib.MegaSeg), ("fcn_mega_layer", _lib.MegaLayer), ("fcn_mega_job", _lib.MegaJob),
-             ("fcn_mega_args", _lib.MegaArgs), ("fcn_train_src", _lib.TrainSrc), ("fcn_train_seg", _lib.TrainSeg),
-             ("fcn_train_layer", _lib.TrainLayer), ("fcn_train_pool_args", _lib.TrainPool),
-             ("fcn_loss_args", _lib.LossArgs), ("fcn_input_args", _lib.InputArgs)]
-    src = tmp_path / "sizes.c"
-    src.write_text('#include <stdio.h>\n#include "frustum_b200.h"\nint main(void) {\n' +
-                   "".join('    printf("%s %%zu\\n", sizeof(%s));\n' % (n, n) for n, _ in pairs) + "    return 0;\n}\n")
-    exe = tmp_path / "sizes"
+    aliases = {cls.__name__: cls for cls in vars(_lib).values()
+               if isinstance(cls, type) and issubclass(cls, ctypes.Structure) and cls is not ctypes.Structure}
+    assert aliases == _lib.STRUCTS   # every header struct has its one Python name, and no other class is bound
+    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "frustum_b200.h"']
+    for fn, (ret, args) in _lib.PROTOTYPES.items():
+        lines.append('_Static_assert(__builtin_types_compatible_p(__typeof__(&%s), %s (*)(%s)), "%s");'
+                     % (fn, ret, ", ".join(t for t, _ in args) or "void", fn))
+    lines.append("int main(void) {")
+    for name, cls in _lib.STRUCTS.items():
+        lines.append('    printf("%s %%zu %%zu\\n", sizeof(%s), _Alignof(%s));' % (name, name, name))
+        lines += ['    printf("%s.%s %%zu %%zu\\n", offsetof(%s, %s), sizeof(((%s *)0)->%s));'
+                  % (name, f, name, f, name, f) for f, _ in cls._fields_]
+    lines += ['    printf("%s %%lld\\n", (long long)(%s));' % (d, d) for d in _lib.DEFINES]
+    src = tmp_path / "abi.c"
+    src.write_text("\n".join(lines + ["    return 0;", "}", ""]))
+    exe = tmp_path / "abi"
     subprocess.check_call(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    sizes = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    for name, cls in pairs:
-        assert int(sizes[name]) == ctypes.sizeof(cls), (name, sizes[name], ctypes.sizeof(cls))
+    out = subprocess.check_output([str(exe)], text=True)
+    seen = {k: [int(v) for v in vs] for k, *vs in (ln.split() for ln in out.splitlines())}
+    for name, cls in _lib.STRUCTS.items():
+        assert seen[name] == [ctypes.sizeof(cls), ctypes.alignment(cls)], name
+        for f, _ in cls._fields_:
+            assert seen[name + "." + f] == [getattr(cls, f).offset, getattr(cls, f).size], (name, f)
+    assert len(_lib.DEFINES) >= 40 and len(_lib.STRUCTS) >= 40 and len(_lib.PROTOTYPES) >= 70
+    for d, v in _lib.DEFINES.items():
+        assert seen[d] == [v] == [getattr(_lib, d[len("FCN_"):])], d
+
+
+def test_header_types_map_to_ctypes():
+    import ctypes as C
+    from frustum_convnet_b200 import _lib
+    _, structs, protos = _lib.read_header(
+        "#define FCN_N 4\n"
+        "typedef void *fcn_stream_t;\n"
+        "typedef struct { int first, count; } fcn_b;\n"
+        "typedef struct {\n"
+        "    const float *w1t, *b1;   /* pointers */\n"
+        "    double m[2][FCN_N];\n"
+        "    fcn_b dep[FCN_N];\n"
+        "    struct fcn_c_ *result;\n"
+        "    uint8_t flag;\n"
+        "} fcn_a;\n"
+        "FCN_API int fcn_f(const fcn_a *args, fcn_stream_t stream);\n")
+    assert structs["fcn_a"]._fields_ == [("w1t", C.c_void_p), ("b1", C.c_void_p), ("m", C.c_double * 4 * 2),
+                                         ("dep", structs["fcn_b"] * 4), ("result", C.c_void_p), ("flag", C.c_uint8)]
+    assert protos == {"fcn_f": ("int", [("const fcn_a *", "args"), ("fcn_stream_t", "stream")])}
+    S = _lib.STRUCTS
+    for text, name, want in [("int", "n", C.c_int), ("int32_t", "n", C.c_int), ("long long", "n", C.c_longlong),
+                             ("unsigned long long", "seed", C.c_ulonglong), ("float", "lr", C.c_float),
+                             ("fcn_stream_t", "stream", C.c_void_p), ("const float *", "src", C.c_void_p),
+                             ("int64_t *", "idx", C.c_void_p), ("const void *", "handle_64B", C.c_void_p),
+                             ("const fcn_group_args *", "args", C.POINTER(S["fcn_group_args"])),
+                             ("const fcn_train_layer *", "layers_dev", C.c_void_p),   # a device table
+                             ("fcn_val_result *", "result", C.c_void_p),
+                             ("long long *", "offset_bytes", C.POINTER(C.c_longlong)),
+                             ("void **", "base_out", C.POINTER(C.c_void_p))]:
+        assert _lib.param_ctype(text, name, S) is want, text
+    for text in ("fcn_group_args", "void", "size_t", "char"):
+        with pytest.raises(ValueError):
+            _lib.param_ctype(text, "x", S)
+    assert _lib.SIGNATURES["fcn_last_error"] == (C.c_char_p, [])
+
+
+@pytest.mark.parametrize("decl", [
+    "typedef struct { size_t n; } fcn_a;",                        # unknown type
+    "typedef struct { int n : 3; } fcn_a;",                       # bit-field
+    "typedef struct { union { int i; float f; } u; } fcn_a;",     # nested union
+    "typedef struct { int (*fn)(int); } fcn_a;",                  # function pointer
+    "typedef struct { fcn_b b; } fcn_a;",                         # undeclared struct
+    "typedef struct { int x[FCN_NOPE]; } fcn_a;",                 # unknown dimension
+    "typedef int fcn_int;",                                       # typedef
+    "FCN_API int fcn_f(size_t n, fcn_stream_t stream);",          # unknown parameter type
+    "#define FCN_SHIFT (1 << 3)",                                 # non-integer define
+])
+def test_header_reader_refuses_what_it_does_not_know(decl):
+    from frustum_convnet_b200 import _lib
+    with pytest.raises(ValueError):
+        _lib.read_header("#define FCN_N 4\ntypedef void *fcn_stream_t;\n" + decl + "\n")

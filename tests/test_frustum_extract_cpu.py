@@ -1,7 +1,7 @@
 """CPU: the frustum extractor's float64 restatement (oracle/frustum_extract.py) against the reference's own pickle
 (tests/golden/frustum_extract.npz, oracle/make_golden_frustum_extract.py), the detection-line reader, the fixture's
-edge cases, argument validation of the fcn_frustum_extract_* entries (on the host, before any CUDA call), the ctypes
-mirrors, the Python wrappers' input checks and the kernels' register budget."""
+edge cases, argument validation of the fcn_frustum_extract_* entries (on the host, before any CUDA call), the Python
+wrappers' input checks and the kernels' register budget."""
 import ctypes
 import os
 import re
@@ -122,21 +122,6 @@ def test_c_entries_validate_without_gpu():
     assert lib.fcn_frustum_extract_count(ctypes.byref(a), None) == -1      # NULL workspace / info
     assert b"workspace" in lib.fcn_last_error()
     assert lib.fcn_frustum_extract_write(ctypes.byref(a), None) == -1
-
-
-def test_ctypes_mirrors_have_the_size_of_the_c_structs(tmp_path):
-    from frustum_convnet_b200 import _lib
-    pairs = [("fcn_frustum_frame", _lib.FrustumFrame), ("fcn_frustum_extract_args", _lib.FrustumExtractArgs)]
-    src = tmp_path / "sizes.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "frustum_b200.h"\nint main(void) {\n' +
-                   "".join('    printf("%s %%zu\\n", sizeof(%s));\n' % (n, n) for n, _ in pairs) +
-                   '    printf("P_off %zu\\n", offsetof(fcn_frustum_extract_args, P));\n    return 0;\n}\n')
-    exe = tmp_path / "sizes"
-    subprocess.check_call(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    sizes = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    for name, cls in pairs:
-        assert int(sizes[name]) == ctypes.sizeof(cls), (name, sizes[name], ctypes.sizeof(cls))
-    assert int(sizes["P_off"]) == _lib.FrustumExtractArgs.P.offset
 
 
 def test_wrappers_reject_cpu_tensors_and_mismatched_lists():

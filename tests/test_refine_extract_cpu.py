@@ -9,7 +9,6 @@ cannot disagree."""
 import ctypes
 import os
 import pickle
-import subprocess
 
 import numpy as np
 import pytest
@@ -206,22 +205,6 @@ def test_cabi_rejects_bad_arguments():
     assert lib.fcn_refine_extract_workspace_bytes(ctypes.byref(a)) == -1
     a.num_jobs = -1
     assert lib.fcn_refine_extract_count(ctypes.byref(a), None) == -1
-
-
-def test_ctypes_structs_match_the_header(tmp_path):
-    from frustum_convnet_b200 import _lib
-    inc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include")
-    src = tmp_path / "s.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "frustum_b200.h"\nint main(void) {\n'
-                   '    printf("%zu %zu %zu\\n", sizeof(fcn_refine_box), sizeof(fcn_refine_extract_args), '
-                   'offsetof(fcn_refine_extract_args, offsets));\n    return 0;\n}\n')
-    exe = tmp_path / "s"
-    subprocess.check_call(["cc", "-I", inc, str(src), "-o", str(exe)])
-    sizes = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-    assert sizes == [ctypes.sizeof(_lib.RefineBox), ctypes.sizeof(_lib.RefineExtractArgs),
-                     _lib.RefineExtractArgs.offsets.offset]
-    for name in ("fcn_refine_extract_workspace_bytes", "fcn_refine_extract_count", "fcn_refine_extract_write"):
-        assert hasattr(_lib.load(), name) and name in _lib.SIGNATURES
 
 
 class _FakeTensor:

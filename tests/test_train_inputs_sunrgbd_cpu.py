@@ -5,12 +5,11 @@ default_collate produced (tests/golden/train_inputs_sunrgbd.npz, oracle/make_gol
 builder is checked on, and the C ABI and the host builder validate the new kind's arguments."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN_DIR, ROOT
+from conftest import GOLDEN_DIR
 
 BAND = 1e-9        # refs this close to a box face may be labelled differently by Delaunay and the half-space test
 FLOAT_KEYS = ("point_cloud", "rot_angle", "center_ref1", "center_ref2", "center_ref3", "center_ref4", "center_ref5",
@@ -166,24 +165,6 @@ def test_fixture_covers_the_cases():
         seen |= {"h-"} if (draws["height_u"] < 0.5).any() else set()
     assert seen == {"train", "val", "rgb", "+d", "-d", "0", "max", "flip", "noflip", "h+", "h-"}, seen
     assert fallback >= 1 and near >= 4
-
-
-def test_ctypes_mirrors_of_the_sunrgbd_fields(tmp_path):
-    from frustum_convnet_b200 import _lib
-    fields = [("fcn_train_frustum", _lib.TrainFrustum, f) for f in ("T", "cls_index", "cx", "cy", "K", "Rtilt")] + \
-             [("fcn_train_input_args", _lib.TrainInputArgs, f) for f in ("rgb_prob", "height_u")]
-    src = tmp_path / "offsets.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "frustum_b200.h"\nint main(void) {\n' +
-                   '    printf("%d\\n", FCN_TRAIN_SUNRGBD);\n' +
-                   "".join('    printf("%s.%s %%zu\\n", offsetof(%s, %s));\n' % (n, f, n, f) for n, _, f in fields) +
-                   "    return 0;\n}\n")
-    exe = tmp_path / "offsets"
-    subprocess.check_call(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    lines = subprocess.check_output([str(exe)], text=True).splitlines()
-    assert int(lines[0]) == _lib.TRAIN_SUNRGBD
-    offs = dict(l.split() for l in lines[1:])
-    for n, cls, f in fields:
-        assert int(offs["%s.%s" % (n, f)]) == getattr(cls, f).offset, (n, f)
 
 
 def _sun_args(labels=1):
