@@ -226,6 +226,7 @@ RefineJobsArgs = STRUCTS["fcn_refine_jobs_args"]
 RefineFrustumTableArgs = STRUCTS["fcn_refine_frustum_table_args"]
 FrameExtractArgs = STRUCTS["fcn_frame_extract_args"]
 ResampleArgs = STRUCTS["fcn_resample_args"]
+FrameRefineArgs = STRUCTS["fcn_frame_refine_args"]
 
 _lib = None
 

@@ -22,6 +22,7 @@
 #include "box_contains.cuh"
 #include "box_iou.cuh"
 #include "common.cuh"
+#include "frame_refine.cuh"
 #include "frustum_fov.cuh"
 
 namespace fcn {
@@ -209,6 +210,24 @@ rx_write_kernel(int num_kept, long long num_out, const int32_t *__restrict__ so,
 }
 
 // ------------------------------------------------------------------------------------------------ host side
+cudaError_t rx_count_det(int num_frames, int num_jobs, const int32_t *so, const fcn_refine_box *jobs,
+                         const int32_t *job_frame, const int32_t *pos, const float4 *fov_pts, int32_t *job_points,
+                         int32_t *job_gt, int32_t *keep, long long *cnt, int32_t *bad, cudaStream_t s) {
+    rx_count_kernel<<<num_jobs, FX_THREADS, 0, s>>>(FCN_REFINE_DET, num_frames, 0, 0, so, jobs, job_frame, nullptr,
+                                                    nullptr, nullptr, pos, fov_pts, job_points, job_gt, keep, cnt,
+                                                    bad);
+    return cudaGetLastError();
+}
+
+cudaError_t rx_write_det(int num_jobs, int num_kept, long long num_out, const int32_t *so, const fcn_refine_box *jobs,
+                         const int32_t *job_frame, const int32_t *job_points, const int32_t *job_gt,
+                         const int32_t *keep_pos, const long long *cnt_pos, const int32_t *pos, const float4 *fov_pts,
+                         float4 *points, int32_t *offsets, cudaStream_t s) {
+    rx_write_kernel<<<num_jobs, FX_THREADS, 0, s>>>(num_kept, num_out, so, jobs, job_frame, nullptr, job_points, job_gt,
+                                                    keep_pos, cnt_pos, pos, fov_pts, points, nullptr, offsets);
+    return cudaGetLastError();
+}
+
 struct RxWs : FovWs {
     double *iou;
     int32_t *match;

@@ -20,6 +20,7 @@
 
 #include "common.cuh"
 #include "det_quantize.cuh"
+#include "frame_refine.cuh"
 
 namespace fcn {
 
@@ -191,6 +192,16 @@ __global__ void __launch_bounds__(RJ_THREADS) rj_table_kernel(fcn_refine_frustum
 #pragma unroll
     for (int i = 0; i < 3; ++i) r->size[i] = t.size[i];
     r->dist = t.dist;
+}
+
+cudaError_t rj_jobs(const fcn_refine_jobs_args &a, cudaStream_t s) {
+    rj_jobs_kernel<<<ceil_div(a.num_jobs, RJ_THREADS), RJ_THREADS, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t rj_table(const fcn_refine_frustum_table_args &a, cudaStream_t s) {
+    rj_table_kernel<<<ceil_div(a.num_kept, RJ_THREADS), RJ_THREADS, 0, s>>>(a);
+    return cudaGetLastError();
 }
 
 // Host-side checks of the gather plan: counts, the host copies and pointers.

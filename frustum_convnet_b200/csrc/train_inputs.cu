@@ -87,10 +87,18 @@ __device__ __forceinline__ int ref_label(const fcn_train_input_args &a, const It
 
 }  // namespace
 
+// The collate widths of fcn_build_train_inputs_fixed, one per scale.
+struct Widths {
+    int32_t w[FCN_MAX_SCALES];
+};
+
 // B CTAs per launch (B = 32 in the reference cfgs) never fill the GPU, so occupancy is worth nothing here.  With
 // minBlocks = 1 ptxas keeps the whole kernel in registers (74, no spills on sm_90a); without it, it picked 64
 // registers and spilled once the SUN-RGBD projection was inlined.
-__global__ void __launch_bounds__(kThreads, 1) build_train_inputs_kernel(const __grid_constant__ fcn_train_input_args a) {
+// kFixed: each scale's collate width is widths.w[s] (fcn_build_train_inputs_fixed), not the batch's largest T.
+template <bool kFixed>
+__global__ void __launch_bounds__(kThreads, 1) build_train_inputs_kernel(const __grid_constant__ fcn_train_input_args a,
+                                                                         const Widths widths) {
     const int b = blockIdx.x, tid = threadIdx.x;
     __shared__ int s_pad[FCN_MAX_SCALES];
     __shared__ double s_wd[kThreads / 32];
@@ -125,13 +133,17 @@ __global__ void __launch_bounds__(kThreads, 1) build_train_inputs_kernel(const _
     }
     // ---- collate width of every scale: the batch's largest T (edge padding beyond an item's own T)
     if (tid < a.num_scales) {
-        int m = 1;
-        for (int i = 0; i < a.B; ++i) {
-            int g = a.index[i];
-            g = g < 0 ? 0 : (g >= a.num_frustums ? a.num_frustums - 1 : g);
-            m = max(m, a.frustums[g].T[tid]);
+        if constexpr (kFixed) {
+            s_pad[tid] = widths.w[tid];
+        } else {
+            int m = 1;
+            for (int i = 0; i < a.B; ++i) {
+                int g = a.index[i];
+                g = g < 0 ? 0 : (g >= a.num_frustums ? a.num_frustums - 1 : g);
+                m = max(m, a.frustums[g].T[tid]);
+            }
+            s_pad[tid] = m;
         }
-        s_pad[tid] = m;
     }
 
     // ---- resampled point cloud (B,3,N) and seg labels (B,N)
@@ -240,36 +252,64 @@ __global__ void __launch_bounds__(kThreads, 1) build_train_inputs_kernel(const _
 
 using namespace fcn;
 
-extern "C" int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stream_t stream) {
-    FCN_REQUIRE(args != nullptr, "args is NULL");
+// The checks both entries share; fn names the entry in the error.
+#define TI_REQUIRE(cond, msg)                                   \
+    do {                                                        \
+        if (!(cond)) return invalid(fn, msg);                   \
+    } while (0)
+static int check_train_inputs(const fcn_train_input_args *args, const char *fn) {
+    if (args == nullptr) return invalid(fn, "args is NULL");
     const fcn_train_input_args &a = *args;
-    FCN_REQUIRE(a.kind == FCN_TRAIN_DET || a.kind == FCN_TRAIN_REFINE || a.kind == FCN_TRAIN_SUNRGBD,
-                "kind must be FCN_TRAIN_DET, FCN_TRAIN_REFINE or FCN_TRAIN_SUNRGBD");
-    FCN_REQUIRE(a.labels == 0 || a.labels == 1, "labels must be 0 or 1");
-    FCN_REQUIRE(a.kind != FCN_TRAIN_DET || a.labels == 1,
-                "the detection provider's from_rgb_detection branch is fcn_build_inputs");
-    FCN_REQUIRE(a.rtc == 1, "only cfg.DATA.RTC = True is supported");
-    FCN_REQUIRE(a.extra_feat == 0, "only cfg.DATA.WITH_EXTRA_FEAT = False is supported");
-    FCN_REQUIRE(a.B >= 0 && a.N >= 1 && a.num_frustums >= 1, "bad sizes");
-    FCN_REQUIRE(a.num_scales >= 2 && a.num_scales <= FCN_MAX_SCALES, "num_scales must be in [2, FCN_MAX_SCALES]");
-    FCN_REQUIRE(a.num_classes >= 0 && a.num_classes <= 1024, "bad num_classes");
-    for (int s = 0; s < a.num_scales; ++s) FCN_REQUIRE(a.stride[s] > 0 && a.centers[s] != nullptr, "bad scale");
-    FCN_REQUIRE(a.kind != FCN_TRAIN_SUNRGBD || a.num_scales == 5, "the SUN-RGBD provider takes exactly 5 scales");
-    FCN_REQUIRE(a.kind == FCN_TRAIN_REFINE || a.max_depth > 0, "max_depth must be > 0");
+    TI_REQUIRE(a.kind == FCN_TRAIN_DET || a.kind == FCN_TRAIN_REFINE || a.kind == FCN_TRAIN_SUNRGBD,
+               "kind must be FCN_TRAIN_DET, FCN_TRAIN_REFINE or FCN_TRAIN_SUNRGBD");
+    TI_REQUIRE(a.labels == 0 || a.labels == 1, "labels must be 0 or 1");
+    TI_REQUIRE(a.kind != FCN_TRAIN_DET || a.labels == 1,
+               "the detection provider's from_rgb_detection branch is fcn_build_inputs");
+    TI_REQUIRE(a.rtc == 1, "only cfg.DATA.RTC = True is supported");
+    TI_REQUIRE(a.extra_feat == 0, "only cfg.DATA.WITH_EXTRA_FEAT = False is supported");
+    TI_REQUIRE(a.B >= 0 && a.N >= 1 && a.num_frustums >= 1, "bad sizes");
+    TI_REQUIRE(a.num_scales >= 2 && a.num_scales <= FCN_MAX_SCALES, "num_scales must be in [2, FCN_MAX_SCALES]");
+    TI_REQUIRE(a.num_classes >= 0 && a.num_classes <= 1024, "bad num_classes");
+    for (int s = 0; s < a.num_scales; ++s) TI_REQUIRE(a.stride[s] > 0 && a.centers[s] != nullptr, "bad scale");
+    TI_REQUIRE(a.kind != FCN_TRAIN_SUNRGBD || a.num_scales == 5, "the SUN-RGBD provider takes exactly 5 scales");
+    TI_REQUIRE(a.kind == FCN_TRAIN_REFINE || a.max_depth > 0, "max_depth must be > 0");
     if (a.B == 0) return FCN_OK;
-    FCN_REQUIRE(a.points && a.point_offsets && a.frustums && a.index && a.choice && a.point_cloud && a.rot_angle,
-                "NULL pointer");
+    TI_REQUIRE(a.points && a.point_offsets && a.frustums && a.index && a.choice && a.point_cloud && a.rot_angle,
+               "NULL pointer");
     if (a.labels) {
-        FCN_REQUIRE(a.cls_label && a.box3d_center && a.box3d_heading && a.box3d_size && a.size_class,
-                    "NULL label pointer");
-        FCN_REQUIRE((!a.random_flip || a.flip_u) && (!a.random_shift || a.shift_n), "NULL draw pointer");
+        TI_REQUIRE(a.cls_label && a.box3d_center && a.box3d_heading && a.box3d_size && a.size_class,
+                   "NULL label pointer");
+        TI_REQUIRE((!a.random_flip || a.flip_u) && (!a.random_shift || a.shift_n), "NULL draw pointer");
     }
-    FCN_REQUIRE(a.kind == FCN_TRAIN_REFINE || !a.labels || (a.seg && a.seg_label), "detection needs seg and seg_label");
-    FCN_REQUIRE(a.kind != FCN_TRAIN_REFINE || a.ref_center, "refinement needs ref_center");
-    FCN_REQUIRE(a.kind == FCN_TRAIN_DET || a.labels || a.rgb_prob, "from_rgb_detection needs rgb_prob");
-    FCN_REQUIRE(a.kind != FCN_TRAIN_SUNRGBD || !a.labels || !a.random_shift || a.height_u,
-                "the SUN-RGBD shift needs height_u");
-    build_train_inputs_kernel<<<a.B, kThreads, 0, (cudaStream_t)stream>>>(a);
+    TI_REQUIRE(a.kind == FCN_TRAIN_REFINE || !a.labels || (a.seg && a.seg_label), "detection needs seg and seg_label");
+    TI_REQUIRE(a.kind != FCN_TRAIN_REFINE || a.ref_center, "refinement needs ref_center");
+    TI_REQUIRE(a.kind == FCN_TRAIN_DET || a.labels || a.rgb_prob, "from_rgb_detection needs rgb_prob");
+    TI_REQUIRE(a.kind != FCN_TRAIN_SUNRGBD || !a.labels || !a.random_shift || a.height_u,
+               "the SUN-RGBD shift needs height_u");
+    return FCN_OK;
+}
+#undef TI_REQUIRE
+
+extern "C" int fcn_build_train_inputs(const fcn_train_input_args *args, fcn_stream_t stream) {
+    const int st = check_train_inputs(args, __func__);
+    if (st != FCN_OK || args->B == 0) return st;
+    build_train_inputs_kernel<false><<<args->B, kThreads, 0, (cudaStream_t)stream>>>(*args, Widths{});
+    FCN_LAUNCH_CHECK();
+    return FCN_OK;
+}
+
+extern "C" int fcn_build_train_inputs_fixed(const fcn_train_input_args *args, const int32_t *widths,
+                                            fcn_stream_t stream) {
+    const int st = check_train_inputs(args, __func__);
+    if (st != FCN_OK) return st;
+    if (widths == nullptr) return invalid(__func__, "NULL widths");
+    Widths w{};
+    for (int s = 0; s < args->num_scales; ++s) {
+        if (widths[s] < 1) return invalid(__func__, "widths must be >= 1");
+        w.w[s] = widths[s];
+    }
+    if (args->B == 0) return FCN_OK;
+    build_train_inputs_kernel<true><<<args->B, kThreads, 0, (cudaStream_t)stream>>>(*args, w);
     FCN_LAUNCH_CHECK();
     return FCN_OK;
 }

@@ -36,6 +36,7 @@ import torch
 from . import _lib
 from ._host import cuda_device, on_device, workspace
 from .input_builder import FrustumBatchBuilder
+from .refine_extract import REFINE_STRIDES
 
 CLASSES = ("Car", "Pedestrian", "Cyclist")          # det_class values 0, 1, 2 (the model's one-hot index)
 _FRAME_BYTES = C.sizeof(_lib.FrustumFrame)         # 33 float64 (P2, Tr_velo_to_cam, R0_rect), then height, width
@@ -71,12 +72,90 @@ class FrameDetections:
             res.setdefault(key, {})[CLASSES[cls[s]]] = rows[off[s]:off[s] + kc[s]].copy()
         return res
 
+    def collected(self, frame_ids=None):
+        """-> detect.CollectedDetections over the same device rows, segments (frame id, class name) in to_dict's order
+        (frame_ids names frame f, default f), so a frame call's rows go to KittiEvaluator.evaluate_collected and
+        RefineFrustumExtractor.from_collected without leaving the device.  Reads the offsets, keep counts and classes
+        back once (a host sync); a segment of no class is named ""."""
+        from .detect import CollectedDetections
+        F = self.seg_class.shape[0]
+        meta = torch.cat([self.seg_offsets, self.keep_count, self.seg_class.reshape(-1)]).cpu().numpy()
+        off, kc, cls = meta[:3 * F + 1], meta[3 * F + 1:6 * F + 1], meta[6 * F + 1:9 * F + 1]
+        ids = list(range(F)) if frame_ids is None else list(frame_ids)
+        segments = [(ids[s // 3], CLASSES[cls[s]] if cls[s] >= 0 else "") for s in range(3 * F)]
+        order = [s for s in range(3 * F) if cls[s] >= 0]
+        return CollectedDetections("KITTI", self.rows, self.seg_offsets, self.keep_count, off, kc, segments, order,
+                                   torch.cuda.current_stream(self.rows.device))
+
     def status_bits(self):
         """The status word, read back (a host sync)."""
         return int(self.status.item())
 
 
-class FrameDetector:
+class _CapacityStage:
+    """What the detection and refinement stages share: the model's eval forward on its plan for (B, N, T) and the
+    collector's candidates and capacity finalize over B entries, of which only the valid ones add rows.  A subclass
+    sets model, device, F, B, N, T (sections per scale), R, method, thresh, top_k and the entry tables seg, valid,
+    box2d32 and seg_class, then calls _init_collector."""
+
+    def _init_collector(self, per_frame):
+        """The collector's buffers; per_frame: the most entries of one frame (a segment holds rows of at most that
+        many entries)."""
+        dev, F, R, T2 = self.device, self.F, self.R, self.T[1]
+        e = lambda *shape, dtype=torch.int32: torch.empty(shape, dtype=dtype, device=dev)
+        self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.records = e(R, 12)
+        self.rows = e(R, 12, dtype=torch.float32)
+        self.seg_offsets, self.keep_count = e(3 * F + 1), e(3 * F)
+        self.info = e(4, dtype=torch.int64)
+        m = min(R, per_frame * T2)                      # the most rows one (frame, class) segment can hold
+        self.mask = e(max(R * ((m + 31) // 32), 1))
+        with torch.cuda.device(dev):
+            self._det_ws, det_bytes = workspace("fcn_det_workspace_bytes", dev, R, 3 * F)
+        fa = _lib.DetFinalizeArgs()
+        fa.num_segments, fa.num_frustums, fa.capacity, fa.method, fa.dataset = 3 * F, self.B, R, self.method, 0
+        fa.top_k, fa.thresh = self.top_k, self.thresh
+        fa.counter, fa.records, fa.box2d = self.counter.data_ptr(), self.records.data_ptr(), self.box2d32.data_ptr()
+        fa.workspace, fa.workspace_bytes, fa.info = self._det_ws.data_ptr(), det_bytes, self.info.data_ptr()
+        fa.seg_offsets, fa.keep_count, fa.rows = (self.seg_offsets.data_ptr(), self.keep_count.data_ptr(),
+                                                  self.rows.data_ptr())
+        fa.mask, fa.mask_words = self.mask.data_ptr(), self.mask.numel()
+        self._fa = fa
+        self._plan = None
+        self._keep = None
+
+    def _forward(self, data):
+        """The model's eval forward on its plan for (B, N, T), launched on the current stream (no graph of its own,
+        so an enclosing capture records the kernels)."""
+        pc = data["point_cloud"]
+        centers = [data["center_ref%d" % (s + 1)] for s in range(len(self.T))]
+        oh = data.get("one_hot") if self.model.num_vec > 0 else None
+        first = self._plan is None
+        if first:
+            self._plan = self.model.engine().plan(self.B, self.N, self.T)
+        return self._plan.run(pc, centers, oh, use_graph=False, copy_out=False, trusted=not first)
+
+    def _collect(self, out, rot_angle, rgb_prob, ref_center, st):
+        """Candidates of the valid entries, then the capacity finalize (box2d32 filled by the caller)."""
+        cls_probs, center, heading, size, _, size_probs = out
+        ts = [t.contiguous() for t in (cls_probs, center, heading, size, size_probs)]
+        a = _lib.DetCandidateArgs()
+        a.B, a.T2, a.NS, a.dataset, a.method = self.B, self.T[1], int(ts[4].shape[-1]), 0, self.method
+        a.first, a.num_frustums, a.capacity = 0, self.B, self.R
+        a.cls_probs, a.center, a.heading, a.size, a.size_probs = (t.data_ptr() for t in ts)
+        a.rot_angle, a.rgb_prob = rot_angle.data_ptr(), rgb_prob.data_ptr()
+        a.ref_center = None if ref_center is None else ref_center.data_ptr()
+        a.seg_of_frustum, a.counter, a.records = self.seg.data_ptr(), self.counter.data_ptr(), self.records.data_ptr()
+        _lib.call("fcn_det_candidates_valid", C.byref(a), self.valid.data_ptr(), st)
+        _lib.call("fcn_det_finalize_capacity", C.byref(self._fa), self.status.data_ptr(), st)
+        self._keep = ts
+
+    def _result(self):
+        return FrameDetections(self.rows, self.seg_offsets, self.keep_count, self.seg_class, self.status,
+                               self.choice, self.valid)
+
+
+class FrameDetector(_CapacityStage):
     def __init__(self, model, type_whitelist=("Car",), method="nms", thresh=0.1, top_k=300, seed=0, frames=1,
                  points=131072, dets=8, rows=None, frustum_points=None, strides=None, max_depth=None, npoints=None,
                  device=None):
@@ -99,7 +178,8 @@ class FrameDetector:
         self.fb = FrustumBatchBuilder(cfg.DATA.STRIDE if strides is None else strides,
                                       cfg.DATA.MAX_DEPTH if max_depth is None else max_depth,
                                       cfg.DATA.NUM_SAMPLES if npoints is None else npoints, device=self.device)
-        self.N, self.T2 = self.fb.N, self.fb.T[1]
+        self.N, self.T = self.fb.N, list(self.fb.T)
+        self.T2 = self.T[1]
         self.R = int(rows) if rows is not None else self.B * self.T2
         self.P_out = int(frustum_points) if frustum_points is not None else self.P
         if min(self.F, self.P, self.D, self.R, self.P_out) < 1:
@@ -118,13 +198,6 @@ class FrameDetector:
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self.call = torch.zeros(1, dtype=torch.int64, device=dev)
         self.choice = e(B, self.N)
-        self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.records = e(self.R, 12)
-        self.rows = e(self.R, 12, dtype=torch.float32)
-        self.seg_offsets, self.keep_count = e(3 * F + 1), e(3 * F)
-        self.info = e(4, dtype=torch.int64)
-        m = min(self.R, self.D * self.T2)               # the most rows one (frame, class) segment can hold
-        self.mask = e(max(self.R * ((m + 31) // 32), 1))
         self.fb.set_frustums_device(self.points3, self.offsets, self.angle, self.box2d, self.Pm, self.cls_index)
 
         a = _lib.FrameExtractArgs()
@@ -138,24 +211,13 @@ class FrameDetector:
         with torch.cuda.device(dev):
             self._ws, a.workspace_bytes = workspace("fcn_frame_extract_workspace_bytes", dev, C.byref(a))
             a.workspace = self._ws.data_ptr()
-            self._det_ws, det_bytes = workspace("fcn_det_workspace_bytes", dev, self.R, 3 * F)
         self._xa = a
         r = _lib.ResampleArgs()
         r.B, r.N, r.seed = B, self.N, self.seed
         r.offsets, r.det_index, r.call, r.choice = (self.offsets.data_ptr(), self.det_index.data_ptr(),
                                                     self.call.data_ptr(), self.choice.data_ptr())
         self._ra = r
-        fa = _lib.DetFinalizeArgs()
-        fa.num_segments, fa.num_frustums, fa.capacity, fa.method, fa.dataset = 3 * F, B, self.R, self.method, 0
-        fa.top_k, fa.thresh = self.top_k, self.thresh
-        fa.counter, fa.records, fa.box2d = self.counter.data_ptr(), self.records.data_ptr(), self.box2d32.data_ptr()
-        fa.workspace, fa.workspace_bytes, fa.info = self._det_ws.data_ptr(), det_bytes, self.info.data_ptr()
-        fa.seg_offsets, fa.keep_count, fa.rows = (self.seg_offsets.data_ptr(), self.keep_count.data_ptr(),
-                                                  self.rows.data_ptr())
-        fa.mask, fa.mask_words = self.mask.data_ptr(), self.mask.numel()
-        self._fa = fa
-        self._plan = None
-        self._keep = None
+        self._init_collector(self.D)
 
     # ------------------------------------------------------------------ inputs
     def inputs(self):
@@ -227,32 +289,161 @@ class FrameDetector:
             self.call.add_(1)
             data = self.fb.build(self.choice)
             out = self._forward(data)
-            self._collect(out, data, st)
-        return FrameDetections(self.rows, self.seg_offsets, self.keep_count, self.seg_class, self.status,
-                               self.choice, self.valid)
+            self.box2d32.copy_(self.box2d)
+            self._collect(out, data["rot_angle"], self.rgb_prob, None, st)
+        return self._result()
 
-    def _forward(self, data):
-        """The model's eval forward on its plan for (F * D, N, T), launched on the current stream (no graph of its
-        own, so an enclosing capture records the kernels)."""
-        pc = data["point_cloud"]
-        centers = [data["center_ref%d" % (s + 1)] for s in range(len(self.fb.T))]
-        oh = data.get("one_hot") if self.model.num_vec > 0 else None
-        first = self._plan is None
-        if first:
-            self._plan = self.model.engine().plan(self.B, self.N, self.fb.T)
-        return self._plan.run(pc, centers, oh, use_graph=False, copy_out=False, trusted=not first)
 
-    def _collect(self, out, data, st):
-        cls_probs, center, heading, size, _, size_probs = out
-        B, T2 = self.B, self.T2
-        ts = [t.contiguous() for t in (cls_probs, center, heading, size, size_probs)]
-        a = _lib.DetCandidateArgs()
-        a.B, a.T2, a.NS, a.dataset, a.method = B, T2, int(ts[4].shape[-1]), 0, self.method
-        a.first, a.num_frustums, a.capacity = 0, B, self.R
-        a.cls_probs, a.center, a.heading, a.size, a.size_probs = (t.data_ptr() for t in ts)
-        a.rot_angle, a.rgb_prob, a.ref_center = data["rot_angle"].data_ptr(), self.rgb_prob.data_ptr(), None
-        a.seg_of_frustum, a.counter, a.records = self.seg.data_ptr(), self.counter.data_ptr(), self.records.data_ptr()
-        _lib.call("fcn_det_candidates_valid", C.byref(a), self.valid.data_ptr(), st)
-        self.box2d32.copy_(self.box2d)
-        _lib.call("fcn_det_finalize_capacity", C.byref(self._fa), self.status.data_ptr(), st)
-        self._keep = ts
+def section_widths(max_width, strides):
+    """W[s] = len(np.arange(-w / 2, w / 2, s)) for w = max_width: the sections of a refinement record whose enlarged
+    box is max_width wide, at every stride s."""
+    w = float(max_width)
+    return [len(np.arange(-w / 2, w / 2, float(s))) for s in strides]
+
+
+class FrameRefiner(_CapacityStage):
+    """The second stage of the KITTI cascade for a FrameDetector's results, in the same fixed capacities: refinement
+    frustums cut around the first stage's kept rows, device resampling, the refinement forward and the collector, with
+    no host sync (C ABI section (22)).  A detect and a refine call can be captured in one CUDA graph.
+
+        fd = FrameDetector(det_model, ("Car",), frames=F, points=P, dets=D)
+        fr = FrameRefiner(fd, refine_model, type_whitelist=("Car",), jobs=2 * D, max_width=4.8, seed=1)
+        inp = fd.inputs(); fd.stage(inp, frames)
+        out = fr.refine(inp, fd.detect(*inp))          # FrameDetections of the second stage
+
+    The chain is the offline one (RefineFrustumExtractor.from_collected, TrainBatchBuilder.from_frustums(..,
+    "refine", labels=False), the model, DetectionCollector) in capacity mode.  Frame f's jobs are the first stage's
+    kept rows of its whitelisted classes in to_dict order (slot f * J + j); the batch holds the kept frustums in slot
+    order, then dummy entries that add no row.  Batch width: the offline path pads each refinement batch to its own
+    widest item, so a refined box depends on its batch-mates; here every batch is padded to the fixed W[s], and the
+    result equals the offline path's for a batch padded to W.  Resampling draws are keyed on (seed, this refiner's
+    call counter, slot, point); the counter has bit 63 set, so no draw coincides with a first-stage draw.
+
+    Status: the result's status word is the first stage's with the second stage's FCN_FRAME_* bits OR-ed in:
+      4  a frame's refinement frustums had more than P2_out points (those past the budget were dropped)
+      8  the refinement gave more candidate rows than R2 (the result is incomplete)
+      16 a first-stage row had a non-finite box or a non-positive extent (it was not refined)
+      32 a frame had more than J whitelisted first-stage rows (the first J were refined)
+      64 a refinement frustum needed more sections than W[s] (it was dropped)"""
+
+    def __init__(self, detector, model, type_whitelist=("Car",), jobs=None, max_width=4.8, sections=None,
+                 frustum_points=None, rows=None, strides=REFINE_STRIDES, npoints=512, method="nms", thresh=0.1,
+                 top_k=300, seed=0):
+        """detector: the FrameDetector whose results this refines (its frames F, scan capacity P and device).
+        model: an eval-mode refinement det_base.PointNetDet (cfgs/refine_car.yaml: strides REFINE_STRIDES, npoints
+        512; the global cfg is the first stage's and is not read).  jobs J (default 2 * D) and max_width (4.8 m, the
+        widest enlarged box kept) are guesses, not measured distributions: size them to the first stage's rows per
+        frame and the boxes it produces.  sections=(W[0], ...) overrides the widths max_width gives; they must halve
+        from scale to scale like the model's section pyramid.
+        frustum_points P2_out (default P) and rows R2 (default B2 * W[1], B2 = F * J): the capacities of each frame's
+        frustum points and of the collector.  method / thresh / top_k: the collector's."""
+        bad = [t for t in type_whitelist if t not in CLASSES]
+        if bad:
+            raise ValueError("FrameRefiner: unknown types %s (KITTI: %s)" % (bad, CLASSES))
+        self.fd, self.model, self.device = detector, model, detector.device
+        self.class_mask = sum(1 << CLASSES.index(t) for t in type_whitelist)
+        self.method = 0 if method == "nms" else 1
+        self.thresh, self.top_k, self.seed = float(thresh), int(top_k), int(seed) & (2 ** 64 - 1)
+        self.F, self.P = detector.F, detector.P
+        self.J = int(jobs) if jobs is not None else 2 * detector.D
+        self.strides = [float(s) for s in strides]
+        self.N = int(npoints)
+        self.T = [int(w) for w in (sections if sections is not None else section_widths(max_width, self.strides))]
+        if len(self.T) != len(self.strides):
+            raise ValueError("FrameRefiner: %d sections for %d strides" % (len(self.T), len(self.strides)))
+        if any(self.T[s] != (self.T[s - 1] + 1) // 2 for s in range(1, len(self.T))):
+            raise ValueError("FrameRefiner: sections %s must halve from scale to scale (W[s] = (W[s-1] + 1) // 2), as "
+                             "the model's section pyramid does" % (self.T,))
+        self.B = self.F * self.J
+        self.P_out = int(frustum_points) if frustum_points is not None else self.P
+        self.R = int(rows) if rows is not None else self.B * self.T[1]
+        if min([self.J, self.P_out, self.R, self.N] + self.T) < 1:
+            raise ValueError("FrameRefiner: every capacity must be >= 1")
+        dev, B, F, S = self.device, self.B, self.F, len(self.strides)
+        e = lambda *shape, dtype=torch.int32: torch.empty(shape, dtype=dtype, device=dev)
+        self.points4 = e(F * self.P_out + B, 4, dtype=torch.float32)
+        self.points3 = e(F * self.P_out + B, 3, dtype=torch.float32)
+        self.offsets, self.offsets64 = e(B + 1), e(B + 1, dtype=torch.int64)
+        self.job_index, self.valid, self.cls_index, self.seg = e(B), e(B), e(B), e(B)
+        self.seg_class, self.box2d32 = e(F, 3), e(B, 4, dtype=torch.float32)
+        self.frustum_records = torch.zeros((B, C.sizeof(_lib.TrainFrustum)), dtype=torch.uint8, device=dev)
+        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.call = torch.full((1,), -2 ** 63, dtype=torch.int64, device=dev)     # bit 63 set: stage 2's draws
+        self.choice = e(B, self.N)
+        self.index = torch.arange(B, dtype=torch.int32, device=dev)
+        self.batch = {"point_cloud": e(B, 3, self.N, dtype=torch.float32), "rot_angle": e(B, dtype=torch.float32),
+                      "ref_center": e(B, 3, dtype=torch.float32), "rgb_prob": e(B, dtype=torch.float32),
+                      "one_hot": e(B, len(CLASSES), dtype=torch.float32)}
+        for s, w in enumerate(self.T):
+            self.batch["center_ref%d" % (s + 1)] = e(B, 3, w, dtype=torch.float32)
+
+        a = _lib.FrameRefineArgs()
+        a.num_frames, a.scan_capacity, a.job_capacity, a.out_capacity = F, self.P, self.J, self.P_out
+        a.num_rows, a.num_scales, a.class_mask = detector.R, S, self.class_mask
+        for s in range(S):
+            a.stride[s], a.widths[s] = self.strides[s], self.T[s]
+        a.frames = detector._frames.data_ptr()              # the calibs and image sizes its detect() packed
+        a.rows, a.seg_offsets = detector.rows.data_ptr(), detector.seg_offsets.data_ptr()
+        a.keep_count, a.seg_class = detector.keep_count.data_ptr(), detector.seg_class.data_ptr()
+        a.status, a.points, a.offsets = self.status.data_ptr(), self.points4.data_ptr(), self.offsets.data_ptr()
+        a.job_index, a.valid, a.cls_index = self.job_index.data_ptr(), self.valid.data_ptr(), self.cls_index.data_ptr()
+        a.seg, a.seg_class_out = self.seg.data_ptr(), self.seg_class.data_ptr()
+        a.records, a.box2d = self.frustum_records.data_ptr(), self.box2d32.data_ptr()
+        with torch.cuda.device(dev):
+            self._ws, a.workspace_bytes = workspace("fcn_frame_refine_extract_workspace_bytes", dev, C.byref(a))
+            a.workspace = self._ws.data_ptr()
+        self._xa = a
+        r = _lib.ResampleArgs()
+        r.B, r.N, r.seed = B, self.N, self.seed
+        r.offsets, r.det_index, r.call, r.choice = (self.offsets.data_ptr(), self.job_index.data_ptr(),
+                                                    self.call.data_ptr(), self.choice.data_ptr())
+        self._ra = r
+        t = _lib.TrainInputArgs()
+        t.kind, t.labels, t.rtc, t.extra_feat = _lib.TRAIN_REFINE, 0, 1, 0
+        t.B, t.N, t.num_scales, t.num_classes, t.num_frustums = B, self.N, S, len(CLASSES), B
+        for s in range(S):
+            t.stride[s] = self.strides[s]
+            t.centers[s] = self.batch["center_ref%d" % (s + 1)].data_ptr()
+        t.max_depth = 1.0
+        t.points, t.point_offsets, t.frustums = (self.points3.data_ptr(), self.offsets64.data_ptr(),
+                                                 self.frustum_records.data_ptr())
+        t.index, t.choice = self.index.data_ptr(), self.choice.data_ptr()
+        for k in ("point_cloud", "rot_angle", "ref_center", "rgb_prob", "one_hot"):
+            setattr(t, k, self.batch[k].data_ptr())
+        self._ta = t
+        self._widths = (C.c_int32 * S)(*self.T)
+        self._init_collector(self.J)
+
+    @torch.no_grad()
+    def refine(self, inputs, first):
+        """inputs: the detector's inputs() the first stage read; first: its detect() result of this call (the
+        calibrations and image sizes are those that detect() packed from the same inputs).  One call
+        on the current stream: no host sync, no allocation after the first call, so detect and refine can be captured
+        in one CUDA graph once both have run eagerly.  -> FrameDetections of the second stage (this refiner's
+        buffers, overwritten by the next call); choice holds the stage-2 resampling indices."""
+        (pts, npts), _, _, _ = inputs
+        if first.rows.data_ptr() != self.fd.rows.data_ptr():
+            raise ValueError("FrameRefiner.refine: `first` is not the result of this refiner's detector")
+        F, P = self.F, self.P
+        for name, t, shape, dt in (("scan points", pts, (F, P, 4), torch.float32),
+                                   ("scan counts", npts, (F,), torch.int32)):
+            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
+                raise ValueError("FrameRefiner.refine: %s must be a contiguous %s CUDA tensor of shape %s on %s"
+                                 % (name, dt, shape, self.device))
+        dev = self.device
+        with torch.cuda.device(dev):
+            st = torch.cuda.current_stream(dev).cuda_stream
+            self.status.copy_(first.status)
+            self.counter.zero_()
+            a = self._xa
+            a.scans, a.scan_counts = pts.data_ptr(), npts.data_ptr()
+            _lib.call("fcn_frame_refine_extract", C.byref(a), st)
+            self.points3.copy_(self.points4[:, :3])
+            self.offsets64.copy_(self.offsets)
+            _lib.call("fcn_resample_choice", C.byref(self._ra), st)
+            self.call.add_(1)
+            _lib.call("fcn_build_train_inputs_fixed", C.byref(self._ta), self._widths, st)
+            data = dict(self.batch)
+            out = self._forward(data)
+            self._collect(out, self.batch["rot_angle"], self.batch["rgb_prob"], self.batch["ref_center"], st)
+        return self._result()

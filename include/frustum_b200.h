@@ -1232,6 +1232,67 @@ FCN_API int fcn_resample_choice(const fcn_resample_args *args, fcn_stream_t stre
 FCN_API int fcn_det_candidates_valid(const fcn_det_candidate_args *args, const int32_t *valid, fcn_stream_t stream);
 FCN_API int fcn_det_finalize_capacity(const fcn_det_finalize_args *args, int32_t *status, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (22) Frame refinement in fixed capacities: sections (20), (16) and (11) for the result of one section (21) call,
+ *      with every size read on the device, so the refinement stage joins the detection stage in one CUDA graph.
+ *
+ *      fcn_frame_refine_extract : the refinement frustums of F frames, J jobs a frame (slot f * J + j), from the first
+ *        stage's rows (num_rows, 12), seg_offsets (3F + 1), keep_count (3F) and seg_class (F, 3), and the scans,
+ *        scan counts and frames the first stage read (frames of at most P = scan_capacity points).
+ *        Jobs: frame f's jobs are the kept rows of its segments 3f + r whose class seg_class[f, r] is set in
+ *          class_mask, in r order, rows k < keep_count in order (the dict path's job order); rows past J set
+ *          FCN_FRAME_JOBS and are not used.  Each job is section (20)'s FCN_REFINE_DET job (rj_jobs_kernel itself): the
+ *          row's text quantization, the x1.2 enlargement and the silent ymax - ymin < 5 / xmax - xmin < 1 drop; a row
+ *          with a non-finite box or a non-positive extent is dropped and sets FCN_FRAME_BAD_DET.
+ *        Points: the frames' in-image points (section (15)'s, recomputed here from the scans), then section (16)'s
+ *          count and write passes over the F * J slots.
+ *        Slots: a frustum whose record needs more sections than widths[s] at any scale s is dropped and sets
+ *          FCN_FRAME_SECTIONS; of the others, each frame's frustums fit, in slot order, while the frame's running
+ *          point count stays <= P2_out = out_capacity; a frustum past it is dropped whole (so is every later one of the
+ *          frame) and sets FCN_FRAME_OUT_POINTS.
+ *        Outputs, over B2 = F * J batch entries: the kept frustums first in slot order, then B2 - K dummy entries (one
+ *          point at the origin, a finite record with T[s] = 1, valid 0, box (0, 0, 1, 1)).
+ *          points (F * P2_out + B2, 4)   offsets (B2 + 1)   job_index (B2): the slot, -1 for a dummy
+ *          valid (B2)   cls_index (B2): the row's class   box2d (B2, 4) float32: the row's 2-D box as read back
+ *          seg (B2): 3 f + r, r the rank of the frustum's class among its frame's kept frustums by first appearance
+ *          seg_class_out (F * 3): the class of segment 3 f + r, -1 when the frame has fewer kept classes
+ *          records (B2): section (20)'s fcn_train_frustum records (fcn_refine_frustum_table, labels 0) for stride[0 ..
+ *            num_scales): rgb_prob is the row's score as read back.
+ *        *status gets FCN_FRAME_* bits OR-ed in (the caller sets it).  No store lands outside a buffer whatever the
+ *        inputs: rows outside [0, num_rows) are not read.
+ *      fcn_build_train_inputs_fixed : fcn_build_train_inputs (section (11)) with each scale's collate width widths[s]
+ *        (HOST, num_scales values >= 1) instead of the batch's largest T[s]; centers[s] is (B, 3, widths[s]) and columns
+ *        >= T[s] of an item repeat its last column (collate_fn's mode='edge'); an item with T[s] > widths[s] is cut.
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_FRAME_JOBS 32           /* a frame had more than J whitelisted first-stage rows (the first J were used) */
+#define FCN_FRAME_SECTIONS 64       /* a refinement frustum needed more sections than W[s] (dropped) */
+typedef struct {
+    int num_frames, scan_capacity, job_capacity, out_capacity;   /* F, P, J, P2_out */
+    int num_rows, num_scales;                                    /* R of the first stage, S */
+    uint32_t class_mask;
+    int reserved;
+    double stride[FCN_MAX_SCALES];
+    int32_t widths[FCN_MAX_SCALES];     /* W[s] */
+    const float *scans;                 /* DEVICE (F * P, 4), 16-byte aligned */
+    const int32_t *scan_counts;         /* DEVICE (F) */
+    const fcn_frustum_frame *frames;    /* DEVICE (F) */
+    const float *rows;                  /* DEVICE (num_rows, 12): the first stage's rows */
+    const int32_t *seg_offsets;         /* DEVICE (3F + 1) */
+    const int32_t *keep_count;          /* DEVICE (3F) */
+    const int32_t *seg_class;           /* DEVICE (F * 3) */
+    void *workspace;
+    long long workspace_bytes;
+    int32_t *status;                    /* DEVICE scalar */
+    float *points;                      /* outputs (DEVICE), see above */
+    int32_t *offsets, *job_index, *valid, *cls_index, *seg, *seg_class_out;
+    fcn_train_frustum *records;
+    float *box2d;
+} fcn_frame_refine_args;
+FCN_API long long fcn_frame_refine_extract_workspace_bytes(const fcn_frame_refine_args *args);
+FCN_API int fcn_frame_refine_extract(const fcn_frame_refine_args *args, fcn_stream_t stream);
+FCN_API int fcn_build_train_inputs_fixed(const fcn_train_input_args *args, const int32_t *widths,
+                                         fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
