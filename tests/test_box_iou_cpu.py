@@ -5,12 +5,12 @@ multiply-adds, so this is the same source, not the same arithmetic.  tests/test_
 header with and without contraction and checks both against exact arithmetic."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import box_iou as ob
+from toolchain import host_library
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -92,14 +92,14 @@ extern "C" void host_rbbox_iou(int M, const float* c, const float* q, float* out
 '''
 
 
-def test_device_arithmetic_compiled_for_the_host_matches_oracle(tmp_path):
+def _host_lib():
+    return host_library(HARNESS % os.path.join(ROOT, "frustum_convnet_b200", "csrc", "box_iou.cuh"),
+                        ("-ffp-contract=off",))
+
+
+def test_device_arithmetic_compiled_for_the_host_matches_oracle():
     """csrc/box_iou.cuh is plain C++ behind FCN_HD: build it with g++ and run the kernel's math on the CPU."""
-    hdr = os.path.join(ROOT, "frustum_convnet_b200", "csrc", "box_iou.cuh")
-    src = tmp_path / "harness.cpp"
-    src.write_text(HARNESS % hdr)
-    so = tmp_path / "libiou_host.so"
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-o", str(so), str(src)])
-    lib = ctypes.CDLL(str(so))
+    lib = _host_lib()
     g = _pairs()
     rng = np.random.default_rng(9)
     gt, pr = g["gt_corners"], g["pr_corners"]
@@ -122,22 +122,16 @@ def test_device_arithmetic_compiled_for_the_host_matches_oracle(tmp_path):
     assert not out[258].any() and not out[259].any()
 
 
-def _host_iou(tmp_path, pr, gt):
-    hdr = os.path.join(ROOT, "frustum_convnet_b200", "csrc", "box_iou.cuh")
-    src = tmp_path / "harness2.cpp"
-    src.write_text(HARNESS % hdr)
-    so = tmp_path / "libiou_host2.so"
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-ffp-contract=off", "-o", str(so), str(src)])
-    lib = ctypes.CDLL(str(so))
+def _host_iou(pr, gt):
     pr = np.ascontiguousarray(pr, dtype=np.float32)
     gt = np.ascontiguousarray(gt, dtype=np.float32)
     out = np.full((pr.shape[0], 2), -1.0, dtype=np.float32)
     P = ctypes.c_void_p
-    lib.host_rbbox_iou(ctypes.c_int(pr.shape[0]), P(pr.ctypes.data), P(gt.ctypes.data), P(out.ctypes.data))
+    _host_lib().host_rbbox_iou(ctypes.c_int(pr.shape[0]), P(pr.ctypes.data), P(gt.ctypes.data), P(out.ctypes.data))
     return out
 
 
-def test_degenerate_boxes(tmp_path):
+def test_degenerate_boxes():
     """Decoded boxes with negative sizes (untrained weights; the round-1 GPU failure): the pinned decision of
     oracle/box_iou.py - a counter-clockwise (invalid) BEV ring scores (0, 0); two negative footprint sizes are
     a valid box rotated by pi; a negative height gives IoU_3D = 0 through the reference's own max(0, .) terms -
@@ -164,7 +158,7 @@ def test_degenerate_boxes(tmp_path):
     bad = (s[:, 0] * s[:, 1]) <= 0
     assert bad.sum() > 50 and not want[bad].any()
     assert ((want >= 0) & (want <= 1 + 1e-9)).all() and (want[:, 1] <= want[:, 0] + 1e-9).all()
-    got = _host_iou(tmp_path, pr, gtb)
+    got = _host_iou(pr, gtb)
     assert np.isfinite(got).all() and np.abs(got - want).max() <= 5e-5
     assert not got[bad].any()
     assert ((got >= 0) & (got <= 1 + 1e-5)).all() and (got[:, 1] <= got[:, 0] + 1e-5).all()

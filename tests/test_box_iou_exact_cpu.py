@@ -32,7 +32,6 @@ families (errors up to ~0.5): without contraction both expressions round the sam
 """
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -40,12 +39,13 @@ import pytest
 import iou_exact_ref as ex
 from oracle import box_iou as ob
 from oracle import nms as onms
+from toolchain import fma_cpu, host_library
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HDR = os.path.join(ROOT, "frustum_convnet_b200", "csrc", "box_iou.cuh")
 N_PAIRS = 500
 SEED = 7
-MODES = {"no_contraction": ["-ffp-contract=off"], "contracted": ["-mfma", "-ffp-contract=fast"]}
+MODES = {"no_contraction": ("-ffp-contract=off",), "contracted": ("-mfma", "-ffp-contract=fast")}
 
 HARNESS = r'''
 #include "%s"
@@ -68,27 +68,10 @@ extern "C" void host_clip_count(int M, const float* c, const float* q, int* cnt)
 '''
 
 
-def _fma_cpu():
-    try:
-        with open("/proc/cpuinfo") as f:
-            return " fma " in f.read().replace("\n", " ")
-    except OSError:
-        return False
-
-
 @pytest.fixture(scope="module")
-def host_lib(tmp_path_factory):
-    d = tmp_path_factory.mktemp("iou_exact")
-    src = d / "harness.cpp"
-    src.write_text(HARNESS % HDR)
-    libs = {}
-    for mode, flags in MODES.items():
-        if mode == "contracted" and not _fma_cpu():
-            continue
-        so = d / ("libiou_%s.so" % mode)
-        subprocess.check_call(["g++", "-O2", "-shared", "-fPIC"] + flags + ["-o", str(so), str(src)])
-        libs[mode] = ctypes.CDLL(str(so))
-    return libs
+def host_lib():
+    return {mode: host_library(HARNESS % HDR, flags) for mode, flags in MODES.items()
+            if mode != "contracted" or fma_cpu()}
 
 
 def _run(lib, c, q):

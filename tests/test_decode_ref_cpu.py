@@ -11,7 +11,6 @@
 import ctypes
 import math
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,12 +18,13 @@ import torch
 
 import decode_ref as D
 from conftest import GOLDEN_CASES, load_golden
+from toolchain import fma_cpu, host_library
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HDR = os.path.join(ROOT, "frustum_convnet_b200", "csrc", "decode.cuh")
 NHS = (1, 2, 12, 24, 64)
 NSS = (1, 3, 10, 64)
-MODES = {"no_contraction": ["-ffp-contract=off"], "contracted": ["-mfma", "-ffp-contract=fast"]}
+MODES = {"no_contraction": ("-ffp-contract=off",), "contracted": ("-mfma", "-ffp-contract=fast")}
 
 # the CUDA intrinsics decode.cuh uses, as plain host functions (one rounding each)
 CUDA_SHIM = r'''
@@ -52,28 +52,12 @@ extern "C" void host_decode(int B, int T, int pitch, int ld, int NH, int NS, con
 '''
 
 
-def _fma_cpu():
-    try:
-        with open("/proc/cpuinfo") as f:
-            return " fma " in f.read().replace("\n", " ")
-    except OSError:
-        return False
-
-
 @pytest.fixture(scope="module")
 def host_lib(tmp_path_factory):
     d = tmp_path_factory.mktemp("decode_host")
     (d / "cuda_runtime.h").write_text(CUDA_SHIM)
-    src = d / "harness.cpp"
-    src.write_text(HARNESS % HDR)
-    libs = {}
-    for mode, flags in MODES.items():
-        if mode == "contracted" and not _fma_cpu():
-            continue
-        so = d / ("libdecode_%s.so" % mode)
-        subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-I", str(d)] + flags + ["-o", str(so), str(src)])
-        libs[mode] = ctypes.CDLL(str(so))
-    return libs
+    return {mode: host_library(HARNESS % HDR, flags, (str(d),)) for mode, flags in MODES.items()
+            if mode != "contracted" or fma_cpu()}
 
 
 def host_decode(lib, rows, B, T, NH, NS, center_ref, mean_size):

@@ -1,14 +1,13 @@
 """CPU: the numpy restatement of the per-image detection step (oracle/detect.py) reproduces what the reference's own
 ``test()`` handed to ``write_detection_results`` (tests/golden/detect_*.npz, oracle/make_golden_detect.py), and the
-C ABI of section (10) validates its arguments and matches its ctypes mirrors without a GPU."""
+C ABI of section (10) validates its arguments without a GPU."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN_DIR, ROOT
+from conftest import GOLDEN_DIR
 
 
 def load_fixture(name):
@@ -75,23 +74,9 @@ def test_fixture_covers_the_cases():
         assert len(np.unique(np.nonzero(ids == 7)[0] // int(g["batch_size"]))) >= 2   # non-adjacent batches
 
 
-def test_ctypes_mirrors_of_section_10(tmp_path):
-    from frustum_convnet_b200 import _lib
-    pairs = [("fcn_det_record", _lib.DetRecord), ("fcn_det_candidate_args", _lib.DetCandidateArgs),
-             ("fcn_det_finalize_args", _lib.DetFinalizeArgs)]
-    src = tmp_path / "sizes.c"
-    src.write_text('#include <stdio.h>\n#include "frustum_b200.h"\nint main(void) {\n' +
-                   "".join('    printf("%s %%zu\\n", sizeof(%s));\n' % (n, n) for n, _ in pairs) + "    return 0;\n}\n")
-    exe = tmp_path / "sizes"
-    subprocess.check_call(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    sizes = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    for name, cls in pairs:
-        assert int(sizes[name]) == ctypes.sizeof(cls), (name, sizes[name], ctypes.sizeof(cls))
-    assert ctypes.sizeof(_lib.DetRecord) == 48
-
-
 def test_argument_validation_without_gpu():
     from frustum_convnet_b200 import _lib
+    assert ctypes.sizeof(_lib.DetRecord) == 48            # the collector's (capacity, 12) int32 record rows
     lib = _lib.load()
     a = _lib.DetCandidateArgs()
     assert lib.fcn_det_candidates(None, None) == -1

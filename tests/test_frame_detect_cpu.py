@@ -1,14 +1,10 @@
 """CPU: the counter-based resampling draw of csrc/resample.cu restated in numpy (tests/resample_ref.py), the argument
 checks of the frame-detection entries (C ABI section (21)) and the ptxas usage of their kernels."""
-import os
-import re
-import subprocess
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from resample_ref import choice_row, philox4x32_10
+from toolchain import compile_cuda
 
 
 def test_philox_known_answers():
@@ -98,20 +94,11 @@ def C_ref(s):
     ("frame_extract.cu", ["frame_setup_kernel", "frame_pack_kernel", "frame_slots_kernel"]),
 ])
 def test_new_kernels_do_not_spill(src, kernels):
-    from frustum_convnet_b200 import build
-    nvcc = build._nvcc()
-    path = os.path.join(ROOT, "frustum_convnet_b200", "csrc", src)
-    out = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", path, "-o", os.devnull],
-                         capture_output=True, text=True, check=True).stderr
-    blocks = re.split(r"Compiling entry function '", out)
     seen = set()
-    for b in blocks[1:]:
-        name = b.split("'", 1)[0]
-        for k in kernels:
-            if k in name:
-                seen.add(k)
-                m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", b)
-                assert m and m.group(1) == "0" and m.group(2) == "0", (name, b[:400])
-                regs = int(re.search(r"Used (\d+) registers", b).group(1))
-                assert regs <= 64, (name, regs)          # 1024-thread CTAs need <= 64 registers a thread
+    for name, k in compile_cuda(src).kernels.items():
+        for want in kernels:
+            if want in name:
+                seen.add(want)
+                assert (k.spill_stores, k.spill_loads) == (0, 0), (name, k.report)
+                assert k.registers <= 64, (name, k.registers)          # 1024-thread CTAs need <= 64 registers a thread
     assert seen == set(kernels)

@@ -3,14 +3,11 @@ against the refinement provider's own arange, the ptxas usage of the new kernels
 that became a template instantiation."""
 import ctypes as C
 import hashlib
-import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from toolchain import compile_cuda, nvcc_release
 
 # cuobjdump -sass of build_train_inputs_kernel before it became the <false> instantiation (CUDA 12.9, sm_90a, the
 # build's flags): the fixed-width path must leave the batch-maximum path's instructions byte for byte as they were
@@ -96,46 +93,26 @@ def test_section_widths_follow_the_refine_ref_line(width):
         assert section_widths(width, REFINE_STRIDES) == Ts, (width, ry)
 
 
-def _compile(src, extra=()):
-    from frustum_convnet_b200 import build
-    nvcc = build._nvcc()
-    path = os.path.join(ROOT, "frustum_convnet_b200", "csrc", src)
-    return nvcc, subprocess.run([nvcc] + build.NVCC_FLAGS + list(extra) + ["-c", path, "-o", os.devnull],
-                                capture_output=True, text=True, check=True).stderr
-
-
 @pytest.mark.parametrize("src,kernels,max_regs", [
     ("frame_refine.cu", ["fr_plan_kernel", "fr_slots_kernel"], 64),
     ("train_inputs.cu", ["build_train_inputs_kernelILb1EE"], 255),
 ])
 def test_new_kernels_do_not_spill(src, kernels, max_regs):
-    _, out = _compile(src, ["-Xptxas", "-v"])
     seen = set()
-    for b in re.split(r"Compiling entry function '", out)[1:]:
-        name = b.split("'", 1)[0]
-        for k in kernels:
-            if k in name:
-                seen.add(k)
-                m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", b)
-                assert m and m.group(1) == "0" and m.group(2) == "0", (name, b[:400])
-                assert int(re.search(r"Used (\d+) registers", b).group(1)) <= max_regs, name
+    for name, k in compile_cuda(src).kernels.items():
+        for want in kernels:
+            if want in name:
+                seen.add(want)
+                assert (k.spill_stores, k.spill_loads) == (0, 0), (name, k.report)
+                assert k.registers <= max_regs, name
     assert seen == set(kernels)
 
 
-def test_batch_kernel_sass_is_the_parents(tmp_path):
-    from frustum_convnet_b200 import build
-    nvcc = build._nvcc()
-    version = re.search(r"release (\d+\.\d+)", subprocess.run([nvcc, "--version"], capture_output=True,
-                                                              text=True).stdout).group(1)
+def test_batch_kernel_sass_is_the_parents():
+    version = nvcc_release()
     if version not in PARENT_SASS:
         pytest.skip("the parent's SASS digest was taken with CUDA %s" % sorted(PARENT_SASS))
-    obj = str(tmp_path / "train_inputs.o")
-    subprocess.run([nvcc] + build.NVCC_FLAGS + ["-c", os.path.join(ROOT, "frustum_convnet_b200", "csrc",
-                                                                   "train_inputs.cu"), "-o", obj], check=True)
-    cuobjdump = os.path.join(os.path.dirname(nvcc), "cuobjdump")
-    sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    parts = re.split(r"^\s*Function : (\S+)\s*$", sass, flags=re.M)
-    bodies = {parts[i]: parts[i + 1] for i in range(1, len(parts), 2)}
+    bodies = compile_cuda("train_inputs.cu").sass()
     false = [b for n, b in bodies.items() if "build_train_inputs_kernelILb0E" in n]
     assert len(false) == 1 and any("build_train_inputs_kernelILb1E" in n for n in bodies)
     assert hashlib.sha256(false[0].encode()).hexdigest() == PARENT_SASS[version]

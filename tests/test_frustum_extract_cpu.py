@@ -4,14 +4,13 @@ edge cases, argument validation of the fcn_frustum_extract_* entries (on the hos
 wrappers' input checks and the kernels' register budget."""
 import ctypes
 import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import ROOT
+from toolchain import compile_cuda
 
 GOLDEN = os.path.join(ROOT, "tests", "golden", "frustum_extract.npz")
 
@@ -147,27 +146,10 @@ def test_wrappers_reject_cpu_tensors_and_mismatched_lists():
                                torch.zeros(1, 12, dtype=torch.float64))
 
 
-def test_detection_extraction_kernels_compile_without_spills(tmp_path):
+def test_detection_extraction_kernels_compile_without_spills():
     """The detection extractor's own kernels (csrc/frustum_extract.cu) and the stage it shares with the other
     extractors (csrc/frustum_fov.cu, the family's only CUB device scans) compile for sm_90a without spills."""
-    from frustum_convnet_b200 import build
-    try:
-        nvcc = build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc is not installed")
-    reports = {}
-    for src in ("frustum_extract", "frustum_fov"):
-        r = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, src + ".cu"),
-                            "-o", str(tmp_path / (src + ".o"))], capture_output=True, text=True)
-        assert r.returncode == 0, r.stdout + r.stderr
-        reports[src], name = {}, None
-        for ln in (r.stdout + r.stderr).splitlines():
-            m = re.search(r"Compiling entry function '(\S+)'", ln)
-            if m:
-                name = m.group(1)
-                reports[src][name] = ""
-            elif name is not None:
-                reports[src][name] += ln + "\n"
+    reports = {src: compile_cuda(src + ".cu").kernels for src in ("frustum_extract", "frustum_fov")}
 
     def named(src, *parts):
         return sorted(p for p in parts if any(p in k for k in reports[src]))
@@ -179,6 +161,5 @@ def test_detection_extraction_kernels_compile_without_spills(tmp_path):
     assert named("frustum_fov", *shared) == sorted(shared), sorted(reports["frustum_fov"])
     assert any("DeviceScanKernel" in k for k in reports["frustum_fov"]), sorted(reports["frustum_fov"])
     for src in reports:
-        for k, text in reports[src].items():
-            m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", text)
-            assert m and (int(m.group(1)), int(m.group(2))) == (0, 0), k + "\n" + text
+        for name, k in reports[src].items():
+            assert (k.spill_stores, k.spill_loads) == (0, 0), name + "\n" + k.report

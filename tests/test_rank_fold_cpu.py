@@ -3,13 +3,13 @@ argument checks before any launch, a kernel without stack frame or spills), the 
 multi-rank step, and the float32 fold reference the GPU tests compare against."""
 import os
 import re
-import subprocess
 
 import numpy as np
 import pytest
 
 from frustum_convnet_b200 import build
 from rank_fold_ref import F32, left_fold, order_sensitive, same_bits
+from toolchain import compile_cuda
 
 
 def test_the_entry_is_declared_and_exported():
@@ -40,22 +40,8 @@ def test_bad_arguments_are_rejected_before_any_launch():
         _lib.call("fcn_rank_fold", src, 3, 2, 4, dst, None)
 
 
-def test_fold_kernels_have_no_stack_frame_or_spills(tmp_path):
-    try:
-        nvcc = build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc is not installed")
-    r = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, "train.cu"),
-                        "-o", str(tmp_path / "train.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    usage, cur = {}, None
-    for ln in (r.stdout + r.stderr).splitlines():
-        m = re.search(r"Compiling entry function '(\S+)' for 'sm_90a'", ln)
-        if m:
-            cur = m.group(1)
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", ln)
-        if m and cur is not None:
-            usage[cur] = tuple(int(v) for v in m.groups())
+def test_fold_kernels_have_no_stack_frame_or_spills():
+    usage = {m: k.local_memory for m, k in compile_cuda("train.cu").kernels.items()}
     found = [v for k, v in usage.items() if "rank_fold_kernel" in k]
     assert found == [(0, 0, 0), (0, 0, 0)], usage          # the float4 and the scalar kernel
 

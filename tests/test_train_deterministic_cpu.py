@@ -3,12 +3,11 @@ sized from the layer's shape only."""
 import ctypes as C
 import os
 import re
-import subprocess
 
 import pytest
 
 from frustum_convnet_b200 import _lib, build
-from test_train_kernels_compile_cpu import kernel_key
+from toolchain import compile_cuda, kernel_key
 
 TRAIN_KERNELS = [
     "train_fwd_kernel<true>", "train_fwd_finish_kernel<true>", "train_slots_sum_kernel", "train_reduce_kernel<true>",
@@ -19,35 +18,21 @@ ENTRIES = ["fcn_train_deterministic_workspace_floats", "fcn_train_forward_determ
            "fcn_train_backward_deterministic", "fcn_det_loss_deterministic_scratch_floats", "fcn_det_loss_deterministic"]
 
 
-def _ptxas(src, tmp_path):
-    try:
-        nvcc = build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc is not installed")
-    r = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, src), "-o",
-                        str(tmp_path / "k.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    res, cur = {}, None
-    for ln in (r.stdout + r.stderr).splitlines():
-        m = re.search(r"Compiling entry function '(\S+)'", ln)
-        if m:
-            cur = kernel_key(m.group(1))
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", ln)
-        if m and cur is not None:
-            res[cur] = tuple(int(v) for v in m.groups())
-    return res
+def _usage(src):
+    """{kernel_key: Kernel.local_memory} of csrc/<src>."""
+    return {kernel_key(m): k.local_memory for m, k in compile_cuda(src).kernels.items()}
 
 
-def test_deterministic_train_kernels_no_stack_no_spills(tmp_path):
-    res = _ptxas("train.cu", tmp_path)
+def test_deterministic_train_kernels_no_stack_no_spills():
+    res = _usage("train.cu")
     for k in TRAIN_KERNELS:
-        assert res.get(k) == (0, 0, 0), "%s: %r (stack frame, spill stores, spill loads)" % (k, res.get(k))
+        assert res.get(k) == (0, 0, 0), "%s: %r (stack frame, bytes spilled: stores, loads)" % (k, res.get(k))
 
 
-def test_deterministic_loss_kernels_compile_like_the_default(tmp_path):
+def test_deterministic_loss_kernels_compile_like_the_default():
     """The ordered row kernel is the default one's template instantiation, whose corner arrays live in a local frame:
     the same frame, and no spills."""
-    res = _ptxas("loss.cu", tmp_path)
+    res = _usage("loss.cu")
     assert res["det_loss_rows_kernel<true>"] == res["det_loss_rows_kernel<false>"]
     assert res["det_loss_rows_kernel<true>"][1:] == (0, 0)
     assert res["det_loss_slots_kernel"] == (0, 0, 0)

@@ -3,15 +3,12 @@ frame or spills - and TrainStep.optimizer's torch state-dict handling for SGD (t
 stand-in for the flat parameter bucket: torch.optim.SGD states load into the flat momentum buffer and come back in
 torch's format, and states the fused step cannot continue are rejected with the optimizer left as it was."""
 import io
-import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from frustum_convnet_b200 import build
+from toolchain import compile_cuda
 
 
 def test_sgd_step_rejects_bad_arguments_before_any_launch():
@@ -30,22 +27,8 @@ def test_sgd_step_rejects_bad_arguments_before_any_launch():
         _lib.call("fcn_sgd_step", p, p, None, 4, 1e-2, 0.9, 0.0, 1, 1.0, None)
 
 
-def test_sgd_kernel_has_no_stack_frame_or_spills(tmp_path):
-    try:
-        nvcc = build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc is not installed")
-    r = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, "train.cu"),
-                        "-o", str(tmp_path / "train.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    usage, cur = {}, None
-    for ln in (r.stdout + r.stderr).splitlines():
-        m = re.search(r"Compiling entry function '(\S+)' for 'sm_90a'", ln)
-        if m:
-            cur = m.group(1)
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", ln)
-        if m and cur is not None:
-            usage[cur] = tuple(int(v) for v in m.groups())
+def test_sgd_kernel_has_no_stack_frame_or_spills():
+    usage = {m: k.local_memory for m, k in compile_cuda("train.cu").kernels.items()}
     found = [v for k, v in usage.items() if "train_sgd_kernel" in k]
     assert found == [(0, 0, 0)], usage
 

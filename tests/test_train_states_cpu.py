@@ -3,15 +3,12 @@ kernel without stack frame or spills - and TrainStep.optimizer's torch state-dic
 on a CPU stand-in for the flat parameter bucket: torch.optim.Adam states load into the flat moments and come back
 in torch's format, and states the fused step cannot continue are rejected with the optimizer left as it was."""
 import io
-import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from frustum_convnet_b200 import build
+from toolchain import compile_cuda
 
 
 def test_append_rejects_bad_arguments_before_any_launch():
@@ -29,22 +26,8 @@ def test_append_rejects_bad_arguments_before_any_launch():
         _lib.call("fcn_train_states_append", p, 4, p, 0, p, None)
 
 
-def test_append_kernel_has_no_stack_frame_or_spills(tmp_path):
-    try:
-        nvcc = build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc is not installed")
-    r = subprocess.run([nvcc] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build.CSRC, "validate.cu"),
-                        "-o", str(tmp_path / "validate.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    usage, cur = {}, None
-    for ln in (r.stdout + r.stderr).splitlines():
-        m = re.search(r"Compiling entry function '(\S+)' for 'sm_90a'", ln)
-        if m:
-            cur = m.group(1)
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", ln)
-        if m and cur is not None:
-            usage[cur] = tuple(int(v) for v in m.groups())
+def test_append_kernel_has_no_stack_frame_or_spills():
+    usage = {m: k.local_memory for m, k in compile_cuda("validate.cu").kernels.items()}
     for name in ("train_states_append_kernel", "val_final_kernel"):      # both append through one helper
         found = [v for k, v in usage.items() if name in k]
         assert found == [(0, 0, 0)], (name, usage)
