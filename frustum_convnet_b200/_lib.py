@@ -227,6 +227,7 @@ RefineFrustumTableArgs = STRUCTS["fcn_refine_frustum_table_args"]
 FrameExtractArgs = STRUCTS["fcn_frame_extract_args"]
 ResampleArgs = STRUCTS["fcn_resample_args"]
 FrameRefineArgs = STRUCTS["fcn_frame_refine_args"]
+SunrgbdFrameExtractArgs = STRUCTS["fcn_sunrgbd_frame_extract_args"]
 
 _lib = None
 

@@ -18,6 +18,7 @@
 #include "common.cuh"
 #include "frustum_fov.cuh"
 #include "input_builder.cuh"
+#include "sunrgbd_uv.cuh"
 
 namespace fcn {
 
@@ -46,9 +47,8 @@ sx_project_kernel(const float *__restrict__ scans, const int32_t *__restrict__ s
     v[i] = dot_fma(c0, K[3], c1, K[4], c2, K[5]) / w;
 }
 
-// prepare_data.py:191-192, in its order: u < xmax, u >= xmin, v < ymax, v >= ymin
 __device__ __forceinline__ bool sx_in_box2d(double u, double v, const fcn_gt_job &jb) {
-    return u < jb.box[2] && u >= jb.box[0] && v < jb.box[3] && v >= jb.box[1];
+    return sx_in_uv_box(u, v, jb.box);
 }
 
 // scan point i in upright camera coordinates (x, -z, y), exactly (flip_axis_to_camera)

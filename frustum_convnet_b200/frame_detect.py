@@ -37,6 +37,7 @@ from . import _lib
 from ._host import cuda_device, on_device, workspace
 from .input_builder import FrustumBatchBuilder
 from .refine_extract import REFINE_STRIDES
+from .train_inputs import SUNRGBD_CLASSES
 
 CLASSES = ("Car", "Pedestrian", "Cyclist")          # det_class values 0, 1, 2 (the model's one-hot index)
 _FRAME_BYTES = C.sizeof(_lib.FrustumFrame)         # 33 float64 (P2, Tr_velo_to_cam, R0_rect), then height, width
@@ -46,45 +47,53 @@ class FrameDetections:
     """The result of one FrameDetector.detect, on the device (overwritten by the next call).
 
     rows (R, 12) float32: kept row k of segment s at seg_offsets[s] + k, k < keep_count[s], in the row layout of
-    DetectionCollector.finalize_device(); segment s = 3 f + r is frame f's r-th class by first appearance among its
-    kept detections, seg_class[f, r] that class (-1: none).  status: the capacity bits.  choice (F * D, N) int32: the
-    resampling indices of the batch entries (kept frustums first)."""
+    DetectionCollector.finalize_device(); segment s = C f + r (C = len(classes)) is frame f's r-th class by first
+    appearance among its kept detections, seg_class[f, r] that class (-1: none).  status: the capacity bits.  choice
+    (F * D, N) int32: the resampling indices of the batch entries (kept frustums first).  classes: the names of the
+    class indices, dataset: "KITTI" or "SUNRGBD".  cap_choice (SunrgbdFrameDetector only, else None): the 2048-point
+    cap draws of the detection slots."""
 
-    def __init__(self, rows, seg_offsets, keep_count, seg_class, status, choice, valid):
+    cap_choice = None
+
+    def __init__(self, rows, seg_offsets, keep_count, seg_class, status, choice, valid, classes=CLASSES,
+                 dataset="KITTI"):
         self.rows, self.seg_offsets, self.keep_count = rows, seg_offsets, keep_count
         self.seg_class, self.status, self.choice, self.valid = seg_class, status, choice, valid
+        self.classes, self.dataset = tuple(classes), dataset
 
     def to_dict(self, frame_ids=None):
         """-> {frame id: {class name: float32 (n, 12)}} in the reference's dict order (frames with a kept frustum, each
         class by first appearance), what DetectionCollector.finalize() gives; frame_ids names frame f (default f).
         Reads the result back once (a host sync)."""
-        F = self.seg_class.shape[0]
+        F, C = self.seg_class.shape
+        S = C * F
         meta = torch.cat([self.seg_offsets, self.keep_count, self.seg_class.reshape(-1), self.status]).cpu().numpy()
-        n = int(meta[3 * F])
+        n = int(meta[S])
         rows = self.rows[:max(n, 1)].cpu().numpy()
-        off, kc, cls = meta[:3 * F + 1], meta[3 * F + 1:6 * F + 1], meta[6 * F + 1:9 * F + 1]
+        off, kc, cls = meta[:S + 1], meta[S + 1:2 * S + 1], meta[2 * S + 1:3 * S + 1]
         res = {}
-        for s in range(3 * F):
+        for s in range(S):
             if cls[s] < 0:
                 continue
-            f = s // 3
+            f = s // C
             key = f if frame_ids is None else frame_ids[f]
-            res.setdefault(key, {})[CLASSES[cls[s]]] = rows[off[s]:off[s] + kc[s]].copy()
+            res.setdefault(key, {})[self.classes[cls[s]]] = rows[off[s]:off[s] + kc[s]].copy()
         return res
 
     def collected(self, frame_ids=None):
         """-> detect.CollectedDetections over the same device rows, segments (frame id, class name) in to_dict's order
-        (frame_ids names frame f, default f), so a frame call's rows go to KittiEvaluator.evaluate_collected and
-        RefineFrustumExtractor.from_collected without leaving the device.  Reads the offsets, keep counts and classes
-        back once (a host sync); a segment of no class is named ""."""
+        (frame_ids names frame f, default f), so a frame call's rows go to KittiEvaluator.evaluate_collected (or
+        SunrgbdEvaluator.evaluate_collected) and RefineFrustumExtractor.from_collected without leaving the device.
+        Reads the offsets, keep counts and classes back once (a host sync); a segment of no class is named ""."""
         from .detect import CollectedDetections
-        F = self.seg_class.shape[0]
+        F, C = self.seg_class.shape
+        S = C * F
         meta = torch.cat([self.seg_offsets, self.keep_count, self.seg_class.reshape(-1)]).cpu().numpy()
-        off, kc, cls = meta[:3 * F + 1], meta[3 * F + 1:6 * F + 1], meta[6 * F + 1:9 * F + 1]
+        off, kc, cls = meta[:S + 1], meta[S + 1:2 * S + 1], meta[2 * S + 1:3 * S + 1]
         ids = list(range(F)) if frame_ids is None else list(frame_ids)
-        segments = [(ids[s // 3], CLASSES[cls[s]] if cls[s] >= 0 else "") for s in range(3 * F)]
-        order = [s for s in range(3 * F) if cls[s] >= 0]
-        return CollectedDetections("KITTI", self.rows, self.seg_offsets, self.keep_count, off, kc, segments, order,
+        segments = [(ids[s // C], self.classes[cls[s]] if cls[s] >= 0 else "") for s in range(S)]
+        order = [s for s in range(S) if cls[s] >= 0]
+        return CollectedDetections(self.dataset, self.rows, self.seg_offsets, self.keep_count, off, kc, segments, order,
                                    torch.cuda.current_stream(self.rows.device))
 
     def status_bits(self):
@@ -96,24 +105,27 @@ class _CapacityStage:
     """What the detection and refinement stages share: the model's eval forward on its plan for (B, N, T) and the
     collector's candidates and capacity finalize over B entries, of which only the valid ones add rows.  A subclass
     sets model, device, F, B, N, T (sections per scale), R, method, thresh, top_k and the entry tables seg, valid,
-    box2d32 and seg_class, then calls _init_collector."""
+    box2d32 and seg_class, then calls _init_collector.  Each frame has one segment per class of `classes`."""
+
+    classes, dataset = CLASSES, _lib.DET_KITTI
 
     def _init_collector(self, per_frame):
         """The collector's buffers; per_frame: the most entries of one frame (a segment holds rows of at most that
         many entries)."""
         dev, F, R, T2 = self.device, self.F, self.R, self.T[1]
+        S = len(self.classes) * F
         e = lambda *shape, dtype=torch.int32: torch.empty(shape, dtype=dtype, device=dev)
         self.counter = torch.zeros(1, dtype=torch.int32, device=dev)
         self.records = e(R, 12)
         self.rows = e(R, 12, dtype=torch.float32)
-        self.seg_offsets, self.keep_count = e(3 * F + 1), e(3 * F)
+        self.seg_offsets, self.keep_count = e(S + 1), e(S)
         self.info = e(4, dtype=torch.int64)
         m = min(R, per_frame * T2)                      # the most rows one (frame, class) segment can hold
         self.mask = e(max(R * ((m + 31) // 32), 1))
         with torch.cuda.device(dev):
-            self._det_ws, det_bytes = workspace("fcn_det_workspace_bytes", dev, R, 3 * F)
+            self._det_ws, det_bytes = workspace("fcn_det_workspace_bytes", dev, R, S)
         fa = _lib.DetFinalizeArgs()
-        fa.num_segments, fa.num_frustums, fa.capacity, fa.method, fa.dataset = 3 * F, self.B, R, self.method, 0
+        fa.num_segments, fa.num_frustums, fa.capacity, fa.method, fa.dataset = S, self.B, R, self.method, self.dataset
         fa.top_k, fa.thresh = self.top_k, self.thresh
         fa.counter, fa.records, fa.box2d = self.counter.data_ptr(), self.records.data_ptr(), self.box2d32.data_ptr()
         fa.workspace, fa.workspace_bytes, fa.info = self._det_ws.data_ptr(), det_bytes, self.info.data_ptr()
@@ -140,7 +152,7 @@ class _CapacityStage:
         cls_probs, center, heading, size, _, size_probs = out
         ts = [t.contiguous() for t in (cls_probs, center, heading, size, size_probs)]
         a = _lib.DetCandidateArgs()
-        a.B, a.T2, a.NS, a.dataset, a.method = self.B, self.T[1], int(ts[4].shape[-1]), 0, self.method
+        a.B, a.T2, a.NS, a.dataset, a.method = self.B, self.T[1], int(ts[4].shape[-1]), self.dataset, self.method
         a.first, a.num_frustums, a.capacity = 0, self.B, self.R
         a.cls_probs, a.center, a.heading, a.size, a.size_probs = (t.data_ptr() for t in ts)
         a.rot_angle, a.rgb_prob = rot_angle.data_ptr(), rgb_prob.data_ptr()
@@ -152,7 +164,8 @@ class _CapacityStage:
 
     def _result(self):
         return FrameDetections(self.rows, self.seg_offsets, self.keep_count, self.seg_class, self.status,
-                               self.choice, self.valid)
+                               self.choice, self.valid, self.classes,
+                               "SUNRGBD" if self.dataset == _lib.DET_SUNRGBD else "KITTI")
 
 
 class FrameDetector(_CapacityStage):
@@ -447,3 +460,207 @@ class FrameRefiner(_CapacityStage):
             out = self._forward(data)
             self._collect(out, self.batch["rot_angle"], self.batch["rgb_prob"], self.batch["ref_center"], st)
         return self._result()
+
+
+_SUNRGBD_FRAME_BYTES = C.sizeof(_lib.SunrgbdFrame)  # Rtilt, then K: 18 float64
+
+
+class SunrgbdFrameDetector(_CapacityStage):
+    """SUN-RGBD detection of single RGB-D frames in fixed capacities: depth clouds and 2-D detections to 3-D boxes with
+    no host round trip, so a serving loop can capture one call in a CUDA graph (C ABI section (23)).
+
+        fd = SunrgbdFrameDetector(model, frames=1, points=393216, dets=16)
+        inp = fd.inputs()
+        fd.stage(inp, [(cloud, {"Rtilt": Rtilt, "K": K}, [("chair", 0.9, box2d), ...])])
+        out = fd.detect(*inp)                              # no host sync; capturable after one eager call
+        results = out.to_dict()                            # {frame: {class: float32 (n, 12)}}
+
+    The chain is the offline one (SunrgbdFrustumExtractor.from_rgb_detections, TrainBatchBuilder.from_frustums(..,
+    "sunrgbd", labels=False), the model, DetectionCollector(dataset="SUNRGBD")) in capacity mode: the extraction runs
+    over all F * D detection slots, the reference's 2048-point cap (np.random.choice(n, 2048, replace=False)) and the
+    provider's resampling are drawn on the device, the forward runs on the model's plan for (F * D, N, T) and the
+    collector's finalize reads its sizes there.  The batch holds the kept frustums in (frame, detection) order, then
+    dummy entries that add no row.  Both draws are Philox4x32-10 values keyed on (seed, call counter, slot, point), as
+    FrameDetector's: the cap's counter has bit 62 set, so the two never coincide.  Given the same cap rows
+    (FrameDetections.cap_choice) and `choice`, frustums, rows, offsets and keep counts equal the offline chain's bit
+    for bit.
+
+    Capacities that a call exceeds set bits of FrameDetections.status (FCN_FRAME_* of the C header):
+      1  a frame had more than P cloud points (its first P were used)
+      2  a frame had more than D detections (its first D were used)
+      4  a frame's kept frustums had more than P_out points (those past the budget were dropped)
+      8  the frustums gave more candidate rows than R (the result is incomplete)
+      16 a detection had a class index outside SUNRGBD_CLASSES or a non-finite box (it was not extracted)
+    No store lands outside a buffer whatever the inputs."""
+
+    dataset = _lib.DET_SUNRGBD
+
+    def __init__(self, model, type_whitelist=SUNRGBD_CLASSES, method="top", thresh=0.1, top_k=300, seed=0, frames=1,
+                 points=393216, dets=16, rows=None, frustum_points=None, strides=None, max_depth=None, npoints=None,
+                 device=None):
+        """model: an eval-mode det_base_sunrgbd.PointNetDet.  type_whitelist: classes of SUNRGBD_CLASSES to detect
+        frames F, points P (< 2^24), dets D (<= 64): the capacities of one call; rows R (default
+        F * D * T2) and frustum_points P_out (default D * 2048, which no frame can exceed) those of the collector and
+        of each frame's frustum points.  strides, max_depth, npoints: the input cfg (default: the current cfg's
+        DATA.STRIDE, MAX_DEPTH, NUM_SAMPLES; cfgs/det_sample_sunrgbd.yaml).  method / thresh / top_k: the
+        collector's (the reference's SUN-RGBD cfg tests with "top")."""
+        from .config import get_cfg
+        cfg = get_cfg()
+        self.classes = SUNRGBD_CLASSES
+        bad = [t for t in type_whitelist if t not in SUNRGBD_CLASSES]
+        if bad:
+            raise ValueError("SunrgbdFrameDetector: unknown types %s (SUN-RGBD: %s)" % (bad, SUNRGBD_CLASSES))
+        self.model = model
+        self.device = cuda_device(device, "SunrgbdFrameDetector")
+        self.class_mask = sum(1 << SUNRGBD_CLASSES.index(t) for t in set(type_whitelist))
+        self.method = 0 if method == "nms" else 1
+        self.thresh, self.top_k, self.seed = float(thresh), int(top_k), int(seed) & (2 ** 64 - 1)
+        self.F, self.P, self.D = int(frames), int(points), int(dets)
+        self.B = self.F * self.D
+        self.strides = [float(s) for s in (cfg.DATA.STRIDE if strides is None else strides)]
+        self.max_depth = float(cfg.DATA.MAX_DEPTH if max_depth is None else max_depth)
+        self.N = int(cfg.DATA.NUM_SAMPLES if npoints is None else npoints)
+        if len(self.strides) != 5:
+            raise ValueError("SunrgbdFrameDetector: the SUN-RGBD model takes 5 strides, got %d" % len(self.strides))
+        self.T = [len(np.arange(0, self.max_depth, s)) for s in self.strides]
+        self.T2 = self.T[1]
+        self.R = int(rows) if rows is not None else self.B * self.T2
+        self.P_out = int(frustum_points) if frustum_points is not None else self.D * _lib.SUNRGBD_MAX_POINTS
+        if min(self.F, self.P, self.D, self.R, self.P_out, self.N) < 1:
+            raise ValueError("SunrgbdFrameDetector: every capacity must be >= 1")
+        if self.D > _lib.SUNRGBD_FRAME_MAX_DETS or self.P >= 2 ** 24 or self.N > _lib.SUNRGBD_MAX_POINTS:
+            raise ValueError("SunrgbdFrameDetector: need dets <= %d, points < 2^24 and npoints <= 2048"
+                             % _lib.SUNRGBD_FRAME_MAX_DETS)
+        dev, B, F, S, NC = self.device, self.B, self.F, len(self.strides), len(SUNRGBD_CLASSES)
+        e = lambda *shape, dtype=torch.int32: torch.empty(shape, dtype=dtype, device=dev)
+        f32 = torch.float32
+        self._frames = torch.zeros((F, _SUNRGBD_FRAME_BYTES), dtype=torch.uint8, device=dev)
+        self.points = e(F * self.P_out + B, 6, dtype=f32)
+        self.points3 = e(F * self.P_out + B, 3, dtype=f32)
+        self.offsets, self.offsets64 = e(B + 1), e(B + 1, dtype=torch.int64)
+        self.det_index, self.valid, self.cls_index, self.seg = e(B), e(B), e(B), e(B)
+        self.seg_class, self.rgb_prob, self.box2d32 = e(F, NC), e(B, dtype=f32), e(B, 4, dtype=f32)
+        self.cap_choice = e(B, _lib.SUNRGBD_MAX_POINTS)
+        self.frustum_records = torch.zeros((B, C.sizeof(_lib.TrainFrustum)), dtype=torch.uint8, device=dev)
+        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.call = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.cap_call = torch.full((1,), 2 ** 62, dtype=torch.int64, device=dev)    # bit 62 set: the cap's draws
+        self.choice = e(B, self.N)
+        self.index = torch.arange(B, dtype=torch.int32, device=dev)
+        self.batch = {"point_cloud": e(B, 3, self.N, dtype=f32), "rot_angle": e(B, dtype=f32),
+                      "rgb_prob": e(B, dtype=f32), "one_hot": e(B, NC, dtype=f32)}
+        for s, w in enumerate(self.T):
+            self.batch["center_ref%d" % (s + 1)] = e(B, 3, w, dtype=f32)
+
+        a = _lib.SunrgbdFrameExtractArgs()
+        a.num_frames, a.point_capacity, a.det_capacity, a.out_capacity = F, self.P, self.D, self.P_out
+        a.class_mask, a.num_scales, a.seed, a.max_depth = self.class_mask, S, self.seed, self.max_depth
+        for s in range(S):
+            a.stride[s] = self.strides[s]
+        a.frames, a.call, a.status = self._frames.data_ptr(), self.cap_call.data_ptr(), self.status.data_ptr()
+        a.points, a.xyz, a.offsets = self.points.data_ptr(), self.points3.data_ptr(), self.offsets.data_ptr()
+        a.det_index, a.valid, a.cls_index = self.det_index.data_ptr(), self.valid.data_ptr(), self.cls_index.data_ptr()
+        a.seg, a.seg_class, a.rgb_prob = self.seg.data_ptr(), self.seg_class.data_ptr(), self.rgb_prob.data_ptr()
+        a.box2d, a.cap_choice = self.box2d32.data_ptr(), self.cap_choice.data_ptr()
+        a.records = self.frustum_records.data_ptr()
+        with torch.cuda.device(dev):
+            self._ws, a.workspace_bytes = workspace("fcn_sunrgbd_frame_extract_workspace_bytes", dev, C.byref(a))
+            a.workspace = self._ws.data_ptr()
+        self._xa = a
+        r = _lib.ResampleArgs()
+        r.B, r.N, r.seed = B, self.N, self.seed
+        r.offsets, r.det_index, r.call, r.choice = (self.offsets.data_ptr(), self.det_index.data_ptr(),
+                                                    self.call.data_ptr(), self.choice.data_ptr())
+        self._ra = r
+        t = _lib.TrainInputArgs()
+        t.kind, t.labels, t.rtc, t.extra_feat = _lib.TRAIN_SUNRGBD, 0, 1, 0
+        t.B, t.N, t.num_scales, t.num_classes, t.num_frustums = B, self.N, S, NC, B
+        for s in range(S):
+            t.stride[s] = self.strides[s]
+            t.centers[s] = self.batch["center_ref%d" % (s + 1)].data_ptr()
+        t.max_depth = self.max_depth
+        t.points, t.point_offsets, t.frustums = (self.points3.data_ptr(), self.offsets64.data_ptr(),
+                                                 self.frustum_records.data_ptr())
+        t.index, t.choice = self.index.data_ptr(), self.choice.data_ptr()
+        for k in ("point_cloud", "rot_angle", "rgb_prob", "one_hot"):
+            setattr(t, k, self.batch[k].data_ptr())
+        self._ta = t
+        self._widths = (C.c_int32 * S)(*self.T)
+        self._init_collector(self.D)
+
+    # ------------------------------------------------------------------ inputs
+    def inputs(self):
+        """Fresh device input buffers of this detector's capacities, zero counts: (clouds, calibs, dets) with
+        clouds = (points (F, P, 6) float32, counts (F,) int32), calibs (F, 18) float64 (Rtilt, then K, row-major)
+        and dets = (boxes (F, D, 4) float64, classes (F, D) int32 (index in SUNRGBD_CLASSES), probs (F, D) float32,
+        counts (F,) int32)."""
+        dev, F, P, D = self.device, self.F, self.P, self.D
+        z = lambda *shape, dtype=torch.int32: torch.zeros(shape, dtype=dtype, device=dev)
+        return ((z(F, P, 6, dtype=torch.float32), z(F)), z(F, 18, dtype=torch.float64),
+                (z(F, D, 4, dtype=torch.float64), z(F, D), z(F, D, dtype=torch.float32), z(F)))
+
+    def stage(self, inputs, frames):
+        """Copy host frames into `inputs` (this detector's inputs()): frames is a list of at most F tuples
+        (cloud (n, 6) float32, calib dict with 'Rtilt' and 'K' (3 x 3), [(type name, prob, box2d), ...]); frames past
+        the list get zero counts.  Detections whose type is not one of SUNRGBD_CLASSES are skipped, as the offline
+        extractor's whitelist skips them (a 19-class 2-D detector is the usual input).  Rows past a capacity are
+        copied up to it and the counts are kept, so detect reports the overflow."""
+        (pts, npts), calib, (boxes, cls, prob, ndet) = inputs
+        F, P, D = self.F, self.P, self.D
+        if len(frames) > F:
+            raise ValueError("SunrgbdFrameDetector.stage: %d frames for a capacity of %d" % (len(frames), F))
+        h_pts, h_calib = np.zeros((F, P, 6), np.float32), np.zeros((F, 18))
+        h_box, h_cls = np.zeros((F, D, 4)), np.zeros((F, D), np.int32)
+        h_prob, h_n, h_nd = np.zeros((F, D), np.float32), np.zeros(F, np.int32), np.zeros(F, np.int32)
+        for f, (cloud, cal, det) in enumerate(frames):
+            cloud = np.asarray(cloud, np.float32).reshape(-1, 6)
+            h_n[f] = len(cloud)
+            h_pts[f, :min(len(cloud), P)] = cloud[:P]
+            h_calib[f] = np.concatenate([np.asarray(cal[k], np.float64).reshape(9) for k in ("Rtilt", "K")])
+            det = [d for d in det if d[0] in self.classes]
+            h_nd[f] = len(det)
+            for j, (t, p, b) in enumerate(det[:D]):
+                h_cls[f, j] = self.classes.index(t)
+                h_prob[f, j], h_box[f, j] = p, np.asarray(b, np.float64).reshape(4)
+        for dst, src in ((pts, h_pts), (npts, h_n), (calib, h_calib), (boxes, h_box), (cls, h_cls), (prob, h_prob),
+                         (ndet, h_nd)):
+            dst.copy_(torch.from_numpy(src), non_blocking=False)
+
+    # ------------------------------------------------------------------ the call
+    @torch.no_grad()
+    def detect(self, clouds, calibs, dets):
+        """One call on the current stream: no host sync, no allocation after the first call, so it can be captured
+        with torch.cuda.graph once it has run eagerly (the capture keeps the input tensors' addresses).
+        -> FrameDetections (this detector's buffers, overwritten by the next call), with cap_choice (F * D, 2048):
+        the cap draw of every candidate slot with more than 2048 in-box points, in draw order."""
+        (pts, npts), (boxes, cls, prob, ndet) = clouds, dets
+        F, P, D = self.F, self.P, self.D
+        specs = (("cloud points", pts, (F, P, 6), torch.float32), ("cloud counts", npts, (F,), torch.int32),
+                 ("calibs", calibs, (F, 18), torch.float64), ("boxes", boxes, (F, D, 4), torch.float64),
+                 ("classes", cls, (F, D), torch.int32), ("probs", prob, (F, D), torch.float32),
+                 ("det counts", ndet, (F,), torch.int32))
+        for name, t, shape, dt in specs:
+            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
+                raise ValueError("SunrgbdFrameDetector.detect: %s must be a contiguous %s CUDA tensor of shape %s on %s"
+                                 % (name, dt, shape, self.device))
+        dev = self.device
+        with torch.cuda.device(dev):
+            st = torch.cuda.current_stream(dev).cuda_stream
+            self.status.zero_()
+            self.counter.zero_()
+            self._frames.view(torch.float64).copy_(calibs)
+            a = self._xa
+            a.clouds, a.cloud_counts, a.boxes = pts.data_ptr(), npts.data_ptr(), boxes.data_ptr()
+            a.det_class, a.det_prob, a.det_counts = cls.data_ptr(), prob.data_ptr(), ndet.data_ptr()
+            _lib.call("fcn_sunrgbd_frame_extract", C.byref(a), st)
+            self.cap_call.add_(1)
+            self.offsets64.copy_(self.offsets)
+            _lib.call("fcn_resample_choice", C.byref(self._ra), st)
+            self.call.add_(1)
+            _lib.call("fcn_build_train_inputs_fixed", C.byref(self._ta), self._widths, st)
+            data = dict(self.batch)
+            out = self._forward(data)
+            self._collect(out, self.batch["rot_angle"], self.batch["rgb_prob"], None, st)
+        res = self._result()
+        res.cap_choice = self.cap_choice
+        return res

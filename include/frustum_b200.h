@@ -1293,6 +1293,69 @@ FCN_API int fcn_frame_refine_extract(const fcn_frame_refine_args *args, fcn_stre
 FCN_API int fcn_build_train_inputs_fixed(const fcn_train_input_args *args, const int32_t *widths,
                                          fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (23) SUN-RGBD frame extraction in fixed capacities: section (18)'s from_rgb_detection set (prepare_data.py:270-381)
+ *      for F frames of at most P cloud points and D 2-D detections each, with every size read on the device and the
+ *      2048-point cap drawn there.  No host sync, no allocation: a call can be captured in a CUDA graph.
+ *
+ *      fcn_sunrgbd_frame_extract : slot f * D + j is detection j of frame f.  Frame f holds min(cloud_counts[f], P)
+ *        points (rows [f * P, f * P + n) of clouds: x, y, z, r, g, b in upright depth coordinates) and
+ *        min(det_counts[f], D) detections; counts below 0 read as 0.  A detection is a candidate when its class
+ *        det_class (an index into SUNRGBD_CLASSES, 0..9) is set in class_mask and its box is finite; a class outside
+ *        0..9 or a non-finite box sets FCN_FRAME_BAD_DET.
+ *        In-box points: section (18)'s, u < xmax, u >= xmin, v < ymax, v >= ymin of the float64 projection, in scan
+ *          order (the rank of a point among its slot's in-box points is its scan-order rank).  A slot with n < 5
+ *          in-box points is dropped (prepare_data.py:352).
+ *        Cap: for every candidate with n > 2048, cap_choice[slot] holds 2048 distinct in-box ranks in random order,
+ *          fcn_resample_choice's n >= N draw (N = 2048) keyed on (seed, *call, slot): np.random.choice(n, 2048,
+ *          replace=False) of the reference.  The frustum keeps those points in that order; other rows of cap_choice
+ *          are 0.  The caller keeps *call apart from its other draws' counters and advances it per call.
+ *        Budget: each frame's kept frustums share P_out = out_capacity points, counting min(n, 2048) per frustum in
+ *          slot order; a frustum past the budget is dropped whole (so is every later one of the frame) and sets
+ *          FCN_FRAME_OUT_POINTS.
+ *        Outputs, over B = F * D batch entries: the kept frustums first in slot order, then B - K dummy entries (one
+ *          point at the origin, a finite record, valid 0, box (0, 0, 1, 1)).
+ *          points (F * P_out + B, 6): x, -z, y, r, g, b     xyz (F * P_out + B, 3): the first three columns
+ *          offsets (B + 1)   det_index (B): the slot, -1 for a dummy   valid (B)   cls_index (B): det_class
+ *          rgb_prob (B): det_prob   box2d (B, 4) float32: the detection's box
+ *          seg (B): 10 f + r, r the rank of the frustum's class among its frame's kept frustums by first appearance
+ *          seg_class (F * 10): the class of segment 10 f + r, -1 when the frame has fewer kept classes
+ *          records (B): the fcn_train_frustum of FCN_TRAIN_SUNRGBD, labels = 0: rot = pi / 2 + frustum_angle (the box
+ *            centre at depth 20 through project_image_to_upright_camera, Rtilt @ in dgemm order, then -atan2(z, x);
+ *            atan2, cos and sin are CUDA's float64 functions, within 2 ulp), cs, sn, cx, cy, K, Rtilt, rgb_prob,
+ *            cls_index and T[s] = len(np.arange(0, max_depth, stride[s])) for s < num_scales, dummies included.
+ *        *status gets FCN_FRAME_* bits OR-ed in (the caller clears it).  No store lands outside a buffer whatever the
+ *        inputs.  Needs 1 <= D <= 64 (each point carries one in-box bit per detection of its frame).
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_SUNRGBD_FRAME_CLASSES 10
+#define FCN_SUNRGBD_FRAME_MAX_DETS 64
+typedef struct {
+    int num_frames, point_capacity, det_capacity, out_capacity;   /* F, P, D, P_out */
+    uint32_t class_mask;                /* bit c: SUNRGBD_CLASSES[c] */
+    int num_scales;
+    unsigned long long seed;            /* the cap draw's key */
+    double max_depth;
+    double stride[FCN_MAX_SCALES];
+    const float *clouds;                /* DEVICE (F * P, 6), 4-byte aligned */
+    const int32_t *cloud_counts;        /* DEVICE (F) */
+    const fcn_sunrgbd_frame *frames;    /* DEVICE (F) */
+    const double *boxes;                /* DEVICE (F * D, 4) */
+    const int32_t *det_class;           /* DEVICE (F * D) */
+    const float *det_prob;              /* DEVICE (F * D) */
+    const int32_t *det_counts;          /* DEVICE (F) */
+    const long long *call;              /* DEVICE scalar: the cap draw's call counter */
+    void *workspace;
+    long long workspace_bytes;
+    int32_t *status;                    /* DEVICE scalar */
+    float *points, *xyz;                /* outputs (DEVICE), see above */
+    int32_t *offsets, *det_index, *valid, *cls_index, *seg, *seg_class;
+    float *rgb_prob, *box2d;
+    int32_t *cap_choice;                /* DEVICE (B, 2048) */
+    fcn_train_frustum *records;         /* DEVICE (B) */
+} fcn_sunrgbd_frame_extract_args;
+FCN_API long long fcn_sunrgbd_frame_extract_workspace_bytes(const fcn_sunrgbd_frame_extract_args *args);
+FCN_API int fcn_sunrgbd_frame_extract(const fcn_sunrgbd_frame_extract_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
