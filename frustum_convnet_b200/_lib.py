@@ -25,8 +25,8 @@ HEADER = os.path.join(os.path.dirname(_HERE), "include", "frustum_b200.h")   # F
 
 # The types a field or parameter may have by value.  A pointer may also point to void, char, an fcn_* struct or a
 # `struct fcn_*` tag.
-SCALARS = {"int": C.c_int, "int32_t": C.c_int, "int64_t": C.c_int64, "uint32_t": C.c_uint32, "uint8_t": C.c_uint8,
-           "long long": C.c_longlong, "unsigned long long": C.c_ulonglong, "float": C.c_float, "double": C.c_double,
+SCALARS = {"int": C.c_int, "int32_t": C.c_int, "int64_t": C.c_int64, "uint32_t": C.c_uint32, "uint16_t": C.c_uint16,
+           "uint8_t": C.c_uint8, "long long": C.c_longlong, "unsigned long long": C.c_ulonglong, "float": C.c_float, "double": C.c_double,
            "fcn_stream_t": C.c_void_p}
 # The header's conditionals as a C compiler sees them.
 _CONDITIONS = {"#ifndef FRUSTUM_B200_H_": True, "#if defined(__GNUC__)": True, "#ifdef __cplusplus": False}
@@ -228,6 +228,7 @@ FrameExtractArgs = STRUCTS["fcn_frame_extract_args"]
 ResampleArgs = STRUCTS["fcn_resample_args"]
 FrameRefineArgs = STRUCTS["fcn_frame_refine_args"]
 SunrgbdFrameExtractArgs = STRUCTS["fcn_sunrgbd_frame_extract_args"]
+SunrgbdDepthArgs = STRUCTS["fcn_sunrgbd_depth_args"]
 
 _lib = None
 

@@ -491,7 +491,13 @@ class SunrgbdFrameDetector(_CapacityStage):
       4  a frame's kept frustums had more than P_out points (those past the budget were dropped)
       8  the frustums gave more candidate rows than R (the result is incomplete)
       16 a detection had a class index outside SUNRGBD_CLASSES or a non-finite box (it was not extracted)
-    No store lands outside a buffer whatever the inputs."""
+    No store lands outside a buffer whatever the inputs.
+
+    From depth images instead of clouds (C ABI section (24), the reference's read_3d_points on the device):
+        inp = fd.inputs_depth(530, 730)
+        fd.stage_depth(inp, [(depth_uint16, rgb_uint8_or_None, {"Rtilt": Rtilt, "K": K}, dets)])
+        out = fd.detect_depth(*inp)                        # the conversion, then detect()'s chain
+    which adds status bit 128 for an image larger than the buffers."""
 
     dataset = _lib.DET_SUNRGBD
 
@@ -587,6 +593,7 @@ class SunrgbdFrameDetector(_CapacityStage):
         self._ta = t
         self._widths = (C.c_int32 * S)(*self.T)
         self._init_collector(self.D)
+        self._depth = None              # detect_depth's conversion and its (F, P, 6) clouds, made on its first call
 
     # ------------------------------------------------------------------ inputs
     def inputs(self):
@@ -605,25 +612,34 @@ class SunrgbdFrameDetector(_CapacityStage):
         the list get zero counts.  Detections whose type is not one of SUNRGBD_CLASSES are skipped, as the offline
         extractor's whitelist skips them (a 19-class 2-D detector is the usual input).  Rows past a capacity are
         copied up to it and the counts are kept, so detect reports the overflow."""
-        (pts, npts), calib, (boxes, cls, prob, ndet) = inputs
-        F, P, D = self.F, self.P, self.D
+        (pts, npts), calib, dets = inputs
+        F, P = self.F, self.P
         if len(frames) > F:
             raise ValueError("SunrgbdFrameDetector.stage: %d frames for a capacity of %d" % (len(frames), F))
-        h_pts, h_calib = np.zeros((F, P, 6), np.float32), np.zeros((F, 18))
-        h_box, h_cls = np.zeros((F, D, 4)), np.zeros((F, D), np.int32)
-        h_prob, h_n, h_nd = np.zeros((F, D), np.float32), np.zeros(F, np.int32), np.zeros(F, np.int32)
-        for f, (cloud, cal, det) in enumerate(frames):
+        h_pts, h_n = np.zeros((F, P, 6), np.float32), np.zeros(F, np.int32)
+        for f, (cloud, _, _) in enumerate(frames):
             cloud = np.asarray(cloud, np.float32).reshape(-1, 6)
             h_n[f] = len(cloud)
             h_pts[f, :min(len(cloud), P)] = cloud[:P]
+        for dst, src in ((pts, h_pts), (npts, h_n)):
+            dst.copy_(torch.from_numpy(src), non_blocking=False)
+        self._stage_calib_dets(calib, dets, [(cal, det) for _, cal, det in frames])
+
+    def _stage_calib_dets(self, calib, dets, frames):
+        """stage()'s calibrations and detections: frames is a list of (calib, [(type name, prob, box2d), ...])."""
+        boxes, cls, prob, ndet = dets
+        F, D = self.F, self.D
+        h_calib = np.zeros((F, 18))
+        h_box, h_cls = np.zeros((F, D, 4)), np.zeros((F, D), np.int32)
+        h_prob, h_nd = np.zeros((F, D), np.float32), np.zeros(F, np.int32)
+        for f, (cal, det) in enumerate(frames):
             h_calib[f] = np.concatenate([np.asarray(cal[k], np.float64).reshape(9) for k in ("Rtilt", "K")])
             det = [d for d in det if d[0] in self.classes]
             h_nd[f] = len(det)
             for j, (t, p, b) in enumerate(det[:D]):
                 h_cls[f, j] = self.classes.index(t)
                 h_prob[f, j], h_box[f, j] = p, np.asarray(b, np.float64).reshape(4)
-        for dst, src in ((pts, h_pts), (npts, h_n), (calib, h_calib), (boxes, h_box), (cls, h_cls), (prob, h_prob),
-                         (ndet, h_nd)):
+        for dst, src in ((calib, h_calib), (boxes, h_box), (cls, h_cls), (prob, h_prob), (ndet, h_nd)):
             dst.copy_(torch.from_numpy(src), non_blocking=False)
 
     # ------------------------------------------------------------------ the call
@@ -645,22 +661,107 @@ class SunrgbdFrameDetector(_CapacityStage):
                                  % (name, dt, shape, self.device))
         dev = self.device
         with torch.cuda.device(dev):
-            st = torch.cuda.current_stream(dev).cuda_stream
             self.status.zero_()
-            self.counter.zero_()
-            self._frames.view(torch.float64).copy_(calibs)
-            a = self._xa
-            a.clouds, a.cloud_counts, a.boxes = pts.data_ptr(), npts.data_ptr(), boxes.data_ptr()
-            a.det_class, a.det_prob, a.det_counts = cls.data_ptr(), prob.data_ptr(), ndet.data_ptr()
-            _lib.call("fcn_sunrgbd_frame_extract", C.byref(a), st)
-            self.cap_call.add_(1)
-            self.offsets64.copy_(self.offsets)
-            _lib.call("fcn_resample_choice", C.byref(self._ra), st)
-            self.call.add_(1)
-            _lib.call("fcn_build_train_inputs_fixed", C.byref(self._ta), self._widths, st)
-            data = dict(self.batch)
-            out = self._forward(data)
-            self._collect(out, self.batch["rot_angle"], self.batch["rgb_prob"], None, st)
+            return self._chain(clouds, calibs, dets)
+
+    def _chain(self, clouds, calibs, dets):
+        """The extraction, the resampling, the forward and the collector on the current stream, with the status as the
+        caller left it."""
+        (pts, npts), (boxes, cls, prob, ndet) = clouds, dets
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        self.counter.zero_()
+        self._frames.view(torch.float64).copy_(calibs)
+        a = self._xa
+        a.clouds, a.cloud_counts, a.boxes = pts.data_ptr(), npts.data_ptr(), boxes.data_ptr()
+        a.det_class, a.det_prob, a.det_counts = cls.data_ptr(), prob.data_ptr(), ndet.data_ptr()
+        _lib.call("fcn_sunrgbd_frame_extract", C.byref(a), st)
+        self.cap_call.add_(1)
+        self.offsets64.copy_(self.offsets)
+        _lib.call("fcn_resample_choice", C.byref(self._ra), st)
+        self.call.add_(1)
+        _lib.call("fcn_build_train_inputs_fixed", C.byref(self._ta), self._widths, st)
+        data = dict(self.batch)
+        out = self._forward(data)
+        self._collect(out, self.batch["rot_angle"], self.batch["rgb_prob"], None, st)
         res = self._result()
         res.cap_choice = self.cap_choice
         return res
+
+    # ------------------------------------------------------------------ from depth images (C ABI section (24))
+    def inputs_depth(self, height, width, rgb=True):
+        """Fresh device input buffers for frames of at most height x width pixels, zero sizes and counts:
+        (images, calibs, dets) with images = (depth (F, H, W) uint16, rgb (F, H, W, 3) uint8 or None (rgb=False),
+        image_hw (F, 2) int32), and calibs and dets as inputs() makes them."""
+        dev, F, D, H, W = self.device, self.F, self.D, int(height), int(width)
+        if min(H, W) < 1:
+            raise ValueError("SunrgbdFrameDetector.inputs_depth: height and width must be >= 1")
+        z = lambda *shape, dtype=torch.int32: torch.zeros(shape, dtype=dtype, device=dev)
+        depth = z(F, H, W, dtype=torch.int16).view(torch.uint16)
+        images = (depth, z(F, H, W, 3, dtype=torch.uint8) if rgb else None, z(F, 2))
+        return (images, z(F, 18, dtype=torch.float64),
+                (z(F, D, 4, dtype=torch.float64), z(F, D), z(F, D, dtype=torch.float32), z(F)))
+
+    def stage_depth(self, inputs, frames):
+        """Copy host frames into `inputs` (this detector's inputs_depth()): frames is a list of at most F tuples
+        (depth (h, w) uint16, rgb (h, w, 3) uint8 in RGB order or None, calib dict with 'Rtilt' and 'K' (3 x 3),
+        [(type name, prob, box2d), ...]); frames past the list get zero sizes and counts.  An image larger than the
+        buffers is copied as its top-left crop with its own size kept, so detect_depth reports it; a None rgb gives
+        that frame colour 0 (the rgb buffer's zeros) and needs no rgb buffer.  Detections as stage() takes them."""
+        (depth, rgb, hw), calib, dets = inputs
+        F, (H, W) = self.F, depth.shape[1:]
+        if len(frames) > F:
+            raise ValueError("SunrgbdFrameDetector.stage_depth: %d frames for a capacity of %d" % (len(frames), F))
+        h_depth, h_hw = np.zeros((F, H, W), np.uint16), np.zeros((F, 2), np.int32)
+        h_rgb = np.zeros((F, H, W, 3), np.uint8)
+        for f, (d, c, _, _) in enumerate(frames):
+            d = np.asarray(d)
+            if d.ndim != 2 or d.dtype != np.uint16:
+                raise ValueError("SunrgbdFrameDetector.stage_depth: frame %d's depth must be (h, w) uint16" % f)
+            h_hw[f] = d.shape
+            h, w = min(d.shape[0], H), min(d.shape[1], W)
+            h_depth[f, :h, :w] = d[:h, :w]
+            if c is not None:
+                if rgb is None:
+                    raise ValueError("SunrgbdFrameDetector.stage_depth: an rgb image for inputs without rgb buffers")
+                c = np.asarray(c, np.uint8)
+                if c.shape != d.shape + (3,):
+                    raise ValueError("SunrgbdFrameDetector.stage_depth: frame %d's rgb must be (h, w, 3)" % f)
+                h_rgb[f, :h, :w] = c[:h, :w]
+        self._stage_calib_dets(calib, dets, [(cal, det) for _, _, cal, det in frames])
+        depth.view(torch.int16).copy_(torch.from_numpy(h_depth.view(np.int16)))
+        hw.copy_(torch.from_numpy(h_hw))
+        if rgb is not None:
+            rgb.copy_(torch.from_numpy(h_rgb))
+
+    @torch.no_grad()
+    def detect_depth(self, images, calibs, dets):
+        """detect() from depth images (inputs_depth()'s buffers): the status cleared, the frames converted into this
+        detector's internal (F, P, 6) clouds (fcn_sunrgbd_depth_cloud), then detect()'s chain.  One call on the current
+        stream with no host sync; it allocates on the first call for an image size only, so it can be captured with
+        torch.cuda.graph after one eager call.  Status bits besides detect()'s:
+          1   a frame had more than P valid pixels (its first P in row-major order were used)
+          128 a frame's image_hw was larger than the buffers (their top-left crop was read)"""
+        depth, rgb, hw = images
+        (boxes, cls, prob, ndet) = dets
+        F, D = self.F, self.D
+        if depth.dim() != 3:
+            raise ValueError("SunrgbdFrameDetector.detect_depth: depth must be (F, H, W)")
+        H, W = depth.shape[1:]
+        if self._depth is None or (self._depth.H, self._depth.W) != (H, W):
+            from .sunrgbd_depth import DepthCloudStage
+            dev = self.device
+            self._depth = DepthCloudStage(F, H, W, self.P, dev)
+            self._depth_clouds = (torch.empty((F, self.P, 6), dtype=torch.float32, device=dev),
+                                  torch.empty(F, dtype=torch.int32, device=dev))
+        self._depth.check("SunrgbdFrameDetector.detect_depth", depth, rgb, hw, calibs)
+        for name, t, shape, dt in (("boxes", boxes, (F, D, 4), torch.float64), ("classes", cls, (F, D), torch.int32),
+                                   ("probs", prob, (F, D), torch.float32), ("det counts", ndet, (F,), torch.int32)):
+            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
+                raise ValueError("SunrgbdFrameDetector.detect_depth: %s must be a contiguous %s CUDA tensor of shape "
+                                 "%s on %s" % (name, dt, shape, self.device))
+        with torch.cuda.device(self.device):
+            self.status.zero_()
+            pts, npts = self._depth_clouds
+            self._depth.run(depth, rgb, hw, calibs, pts, npts, self.status,
+                            torch.cuda.current_stream(self.device).cuda_stream)
+            return self._chain(self._depth_clouds, calibs, dets)

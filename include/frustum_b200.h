@@ -1356,6 +1356,42 @@ typedef struct {
 FCN_API long long fcn_sunrgbd_frame_extract_workspace_bytes(const fcn_sunrgbd_frame_extract_args *args);
 FCN_API int fcn_sunrgbd_frame_extract(const fcn_sunrgbd_frame_extract_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (24) SUN-RGBD depth clouds: the SUNRGBD toolbox's read3dPoints as the reference's port restates it
+ *      (sunrgbd/read_3d_points.py), for F depth images of at most H x W pixels, into section (23)'s `clouds` input.
+ *      No host sync, no allocation: a call can be captured in a CUDA graph.
+ *
+ *      fcn_sunrgbd_depth_cloud : frame f is the top-left min(h, H) x min(w, W) crop of depth[f] (h, w = image_hw[f];
+ *        values below 0 read as 0); pixel (v, u) is depth[f, v, u], 0-based row v and column u.
+ *        Per pixel, with raw = depth[f, v, u]: a pixel is valid when raw != 0;
+ *          r = (raw >> 3) | (raw << 13) in uint16 (a rotate right by 3), d = min(float(r) / 1000, 8) in float32;
+ *          x3 = ((u - cx) * d) / fx, y3 = ((v - cy) * d) / fy in float64 (cx = K[0, 2], cy = K[1, 2], fx = K[0, 0],
+ *          fy = K[1, 1]); the point (x3, d, -y3) times Rtilt in float64, each row as np.matmul(Rtilt, points.T) sums it
+ *          (dgemm's a0 b0 rounded, then one FMA per further term; a frame of exactly one valid pixel goes through
+ *          gemv instead: a1 b1 rounded, then FMAs of term 0 and term 2), rounded to float32 once;
+ *          r, g, b = float(rgb[f, v, u, c]) / 255 in float32, or 0 when rgb is NULL.
+ *        Outputs: clouds[f, k] (x, y, z, r, g, b) for the k-th valid pixel of the frame in row-major order, k < P;
+ *          counts[f] = min(valid pixels, P).  Rows at and past counts[f] are not written.
+ *        *status gets bits OR-ed in (the caller clears it): FCN_FRAME_SCAN_POINTS when a frame has more than P valid
+ *        pixels (the first P are kept, in order), FCN_FRAME_PIXELS when h > H or w > W (the crop is read).
+ *        No store lands outside a buffer whatever the inputs.
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_FRAME_PIXELS 128        /* an image larger than the H x W capacity (its top-left H x W crop was read) */
+typedef struct {
+    int num_frames, height, width, point_capacity;   /* F, H, W, P */
+    const uint16_t *depth;              /* DEVICE (F, H, W), 2-byte aligned */
+    const uint8_t *rgb;                 /* DEVICE (F, H, W, 3) in RGB order, or NULL */
+    const int32_t *image_hw;            /* DEVICE (F, 2): h, w of each frame */
+    const double *calibs;               /* DEVICE (F, 18): Rtilt, then K, row-major, 8-byte aligned */
+    void *workspace;
+    long long workspace_bytes;
+    int32_t *status;                    /* DEVICE scalar */
+    float *clouds;                      /* DEVICE (F, P, 6), 4-byte aligned */
+    int32_t *counts;                    /* DEVICE (F) */
+} fcn_sunrgbd_depth_args;
+FCN_API long long fcn_sunrgbd_depth_cloud_workspace_bytes(const fcn_sunrgbd_depth_args *args);
+FCN_API int fcn_sunrgbd_depth_cloud(const fcn_sunrgbd_depth_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
