@@ -229,6 +229,8 @@ ResampleArgs = STRUCTS["fcn_resample_args"]
 FrameRefineArgs = STRUCTS["fcn_frame_refine_args"]
 SunrgbdFrameExtractArgs = STRUCTS["fcn_sunrgbd_frame_extract_args"]
 SunrgbdDepthArgs = STRUCTS["fcn_sunrgbd_depth_args"]
+FrameStoreCursor = STRUCTS["fcn_frame_store_cursor"]
+FrameStoreArgs = STRUCTS["fcn_frame_store_args"]
 
 _lib = None
 

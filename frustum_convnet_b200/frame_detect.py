@@ -765,3 +765,123 @@ class SunrgbdFrameDetector(_CapacityStage):
             self._depth.run(depth, rgb, hw, calibs, pts, npts, self.status,
                             torch.cuda.current_stream(self.device).cuda_stream)
             return self._chain(self._depth_clouds, calibs, dets)
+
+
+class FrameStore:
+    """The kept rows of many calls of one frame stage (FrameDetector, FrameRefiner or SunrgbdFrameDetector) collected
+    on the device (C ABI section (25)), so a whole split run through the stage's CUDA graph is scored or refined from
+    one table: every append is one launch sequence with no host sync, captured in the same graph as the call.
+
+        store = FrameStore(fd, rows=200000, segments=30000)
+        with torch.cuda.graph(g):                          # after one eager detect
+            out = fd.detect(*inp); store.append(out)
+        store.reset()
+        for frames, ids in split:                          # at most F frames a call
+            fd.stage(inp, frames); store.stage_ids(ids); g.replay()
+        res = KittiEvaluator(...).evaluate_collected(store.collected())
+
+    A call's segments (frame slot, then class by first appearance, as FrameDetections.to_dict orders them) are those of
+    slots with an id >= 0; they are appended with their rows copied bit for bit, zero-row segments included.  A call
+    is stored whole or not at all: when its rows or segments do not fit, nothing of it is stored and the store's
+    status gets FCN_STORE_ROWS (1) or FCN_STORE_SEGMENTS (2); earlier calls stay intact.  Each stored call's own
+    status word (FCN_FRAME_*) is OR-ed into the store's frame status, so one read at the end tells whether any call
+    of the split hit a frame capacity."""
+
+    def __init__(self, stage, rows, segments):
+        """stage: the frame stage whose results are appended (its frames F, classes, dataset, device and result
+        buffers); rows, segments: the store's capacities."""
+        self.stage, self.device = stage, stage.device
+        self.F, self.classes = stage.F, tuple(stage.classes)
+        self.dataset = "SUNRGBD" if stage.dataset == _lib.DET_SUNRGBD else "KITTI"
+        self.row_capacity, self.segment_capacity = int(rows), int(segments)
+        if min(self.row_capacity, self.segment_capacity) < 1 or max(self.row_capacity, self.segment_capacity) >= 2 ** 31:
+            raise ValueError("FrameStore: rows and segments must lie in [1, 2^31)")
+        dev, n = self.device, self.segment_capacity
+        e = lambda *shape, dtype=torch.int32: torch.empty(shape, dtype=dtype, device=dev)
+        self.rows = e(self.row_capacity, 12, dtype=torch.float32)
+        self.image, self.seg_class, self.frame = e(n, dtype=torch.int64), e(n), e(n)
+        self.seg_offsets, self.keep_count = torch.zeros(n + 1, dtype=torch.int32, device=dev), e(n)
+        self.cursor = torch.zeros(C.sizeof(_lib.FrameStoreCursor) // 4, dtype=torch.int32, device=dev)
+        self.ids = torch.full((self.F,), -1, dtype=torch.int64, device=dev)
+        a = _lib.FrameStoreArgs()
+        a.num_frames, a.num_classes, a.num_rows = self.F, len(self.classes), stage.R
+        a.row_capacity, a.segment_capacity = self.row_capacity, n
+        a.rows, a.seg_offsets, a.keep_count = stage.rows.data_ptr(), stage.seg_offsets.data_ptr(), \
+            stage.keep_count.data_ptr()
+        a.seg_class, a.status, a.ids = stage.seg_class.data_ptr(), stage.status.data_ptr(), self.ids.data_ptr()
+        a.store_rows, a.store_image, a.store_class = self.rows.data_ptr(), self.image.data_ptr(), \
+            self.seg_class.data_ptr()
+        a.store_frame, a.store_offset, a.store_keep = self.frame.data_ptr(), self.seg_offsets.data_ptr(), \
+            self.keep_count.data_ptr()
+        a.cursor = self.cursor.data_ptr()
+        with torch.cuda.device(dev):
+            self._ws, a.workspace_bytes = workspace("fcn_frame_store_append_workspace_bytes", dev, C.byref(a))
+            a.workspace = self._ws.data_ptr()
+        self._a = a
+
+    def stage_ids(self, ids):
+        """Copy the image ids of the next call's frame slots into `ids`: at most F values, slots past them get -1 (a
+        slot with a negative id contributes nothing)."""
+        ids = list(ids)
+        if len(ids) > self.F:
+            raise ValueError("FrameStore.stage_ids: %d ids for %d frame slots" % (len(ids), self.F))
+        h = np.full(self.F, -1, np.int64)
+        h[:len(ids)] = ids
+        self.ids.copy_(torch.from_numpy(h), non_blocking=False)
+
+    def append(self, out):
+        """Append `out`, the stage's result of this call, on the current stream: no host sync, no allocation, so it is
+        captured in the same CUDA graph as the call."""
+        if out.rows.data_ptr() != self.stage.rows.data_ptr():
+            raise ValueError("FrameStore.append: `out` is not a result of this store's stage")
+        with torch.cuda.device(self.device):
+            _lib.call("fcn_frame_store_append", C.byref(self._a), torch.cuda.current_stream(self.device).cuda_stream)
+
+    def reset(self):
+        """Empty the store on the current stream (capturable): zeroes the cursor block, status words included."""
+        with torch.cuda.device(self.device):
+            self.cursor.zero_()
+
+    def collected(self):
+        """-> detect.CollectedDetections over the store's device rows, segments (image id, class name) in append
+        order, for KittiEvaluator / SunrgbdEvaluator.evaluate_collected and RefineFrustumExtractor.from_collected.
+        One host read, of the cursor block and the segment table; no row crosses to the host.  Raises RuntimeError
+        when a call did not fit (a store status bit is set) and ValueError naming an image id that was appended from
+        two frame slots."""
+        from .detect import CollectedDetections
+        n = self.segment_capacity
+        with torch.cuda.device(self.device):
+            meta = torch.cat([t.view(torch.uint8).reshape(-1) for t in (self.cursor, self.image, self.seg_class,
+                                                                         self.frame, self.seg_offsets,
+                                                                         self.keep_count)]).cpu().numpy()
+        cur = meta[:self.cursor.numel() * 4].view(np.int32)
+        pieces, at = [], len(cur) * 4
+        for dt, k in ((np.int64, n), (np.int32, n), (np.int32, n), (np.int32, n + 1), (np.int32, n)):
+            size = np.dtype(dt).itemsize * k
+            pieces.append(meta[at:at + size].view(dt))
+            at += size
+        image, cls, frame, off, kc = pieces
+        used, total, status = int(cur[0]), int(cur[1]), int(cur[3])
+        if status:
+            raise RuntimeError("FrameStore: store status %d: a call's %s did not fit and was not stored (capacities: "
+                               "%d rows, %d segments)" % (status, " and ".join(
+                                   w for b, w in ((_lib.STORE_ROWS, "rows"), (_lib.STORE_SEGMENTS, "segments"))
+                                   if status & b), self.row_capacity, n))
+        image, frame = image[:used], frame[:used]
+        pairs = np.unique(np.stack([image, frame.astype(np.int64)], axis=1), axis=0)
+        twice = pairs[1:, 0][pairs[1:, 0] == pairs[:-1, 0]]
+        if len(twice):
+            raise ValueError("FrameStore: image id %d was appended from two frame slots" % int(twice[0]))
+        segments = [(int(i), self.classes[c]) for i, c in zip(image.tolist(), cls[:used].tolist())]
+        return CollectedDetections(self.dataset, self.rows, self.seg_offsets, self.keep_count,
+                                   np.append(off[:used], total), kc[:used], segments, np.arange(used),
+                                   torch.cuda.current_stream(self.device))
+
+    def to_dict(self):
+        """-> {image id: {class name: float32 (n, 12)}}: collected().to_dict()."""
+        return self.collected().to_dict()
+
+    def status_bits(self):
+        """-> (the store's FCN_STORE_* bits, the OR of the stored calls' FCN_FRAME_* words), read back (a host sync)."""
+        cur = self.cursor.cpu().numpy()
+        return int(cur[3]), int(cur[4])

@@ -1392,6 +1392,58 @@ typedef struct {
 FCN_API long long fcn_sunrgbd_depth_cloud_workspace_bytes(const fcn_sunrgbd_depth_args *args);
 FCN_API int fcn_sunrgbd_depth_cloud(const fcn_sunrgbd_depth_args *args, fcn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (25) Frame detection store: the kept rows of many section (21), (22) or (23) calls appended to one device table, so
+ *      a split run through a captured CUDA graph is scored or refined from one read.  Every size is read on the
+ *      device: an append is captured in the same graph as the call it stores.
+ *
+ *      fcn_frame_store_append : one call's result, rows (num_rows, 12), seg_offsets (S + 1), keep_count (S) and
+ *        seg_class (F, C) with S = C * F (segment s = C f + r), its status word, and ids (F): the image id of frame
+ *        slot f, negative for a slot that contributes nothing.  The call's segments are those with seg_class >= 0 and
+ *        ids[f] >= 0, in s order (frame slot, then class by first appearance), zero-keep segments included; segment
+ *        s's rows are [seg_offsets[s], seg_offsets[s] + keep_count[s]) cut to [0, num_rows).
+ *        A call is stored whole or not at all.  With n segments and m rows, when cursor->segments + n <=
+ *        segment_capacity and cursor->rows + m <= row_capacity, the call's j-th segment becomes store segment
+ *        d = cursor->segments + j: store_image[d] = ids[f], store_class[d] = seg_class[s], store_frame[d] =
+ *        cursor->calls * F + f (mod 2^32), store_offset[d] = its first store row, store_keep[d] = its rows; then
+ *        store_offset[cursor->segments + n] = cursor->rows + m, the rows are copied bit for bit, the cursor's
+ *        segments and rows advance, calls grows by one and frame_status |= *status.  Otherwise nothing of the call is
+ *        written and cursor->status gets FCN_STORE_SEGMENTS and / or FCN_STORE_ROWS.  Earlier calls stay intact, and
+ *        no store lands outside a buffer whatever the call's tables hold.  The cursor starts zeroed; appends on one
+ *        stream are ordered and nothing else writes the store meanwhile.
+ * ------------------------------------------------------------------------------------------ */
+#define FCN_STORE_ROWS 1            /* a call's rows did not fit the store's row capacity (the call was not stored) */
+#define FCN_STORE_SEGMENTS 2        /* a call's segments did not fit the segment capacity (the call was not stored) */
+#define FCN_STORE_MAX_FRAMES 65535
+#define FCN_STORE_MAX_CLASSES 64
+typedef struct {
+    int32_t segments, rows;             /* store segments and rows used */
+    int32_t calls;                      /* calls stored */
+    int32_t status;                     /* FCN_STORE_* bits */
+    int32_t frame_status;               /* OR of the stored calls' FCN_FRAME_* words */
+} fcn_frame_store_cursor;
+typedef struct {
+    int num_frames, num_classes, num_rows;          /* F, C and the row capacity R of the appended call */
+    int row_capacity, segment_capacity;             /* the store's */
+    int reserved;
+    const float *rows;                  /* DEVICE (num_rows, 12), 16-byte aligned */
+    const int32_t *seg_offsets;         /* DEVICE (S + 1) */
+    const int32_t *keep_count;          /* DEVICE (S) */
+    const int32_t *seg_class;           /* DEVICE (F, C) */
+    const int32_t *status;              /* DEVICE scalar: the call's FCN_FRAME_* word */
+    const int64_t *ids;                 /* DEVICE (F) */
+    void *workspace;
+    long long workspace_bytes;
+    float *store_rows;                  /* DEVICE (row_capacity, 12), 16-byte aligned */
+    int64_t *store_image;               /* DEVICE (segment_capacity) */
+    int32_t *store_class, *store_frame; /* DEVICE (segment_capacity) */
+    int32_t *store_offset;              /* DEVICE (segment_capacity + 1) */
+    int32_t *store_keep;                /* DEVICE (segment_capacity) */
+    fcn_frame_store_cursor *cursor;     /* DEVICE */
+} fcn_frame_store_args;
+FCN_API long long fcn_frame_store_append_workspace_bytes(const fcn_frame_store_args *args);
+FCN_API int fcn_frame_store_append(const fcn_frame_store_args *args, fcn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
