@@ -27,6 +27,15 @@ def on_device(t, dev):
     return t.device.index == (dev.index if dev.index is not None else torch.cuda.current_device())
 
 
+def check_tensors(who, dev, specs):
+    """specs: (name, tensor, shape, dtype) tuples; raises ValueError naming `who` and the first tensor that is not a
+    contiguous CUDA tensor of that shape and dtype on dev."""
+    for name, t, shape, dt in specs:
+        if not on_device(t, dev) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
+            raise ValueError("%s: %s must be a contiguous %s CUDA tensor of shape %s on %s"
+                             % (who, name, dt, shape, dev))
+
+
 def csr_offsets(counts):
     """Per-group record counts -> int32 CSR offsets [0, n0, n0 + n1, ...] (len(counts) + 1 entries)."""
     off = np.zeros(len(counts) + 1, dtype=np.int32)

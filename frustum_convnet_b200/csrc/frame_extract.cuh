@@ -9,8 +9,8 @@ namespace fcn {
 cudaError_t frame_setup(const fcn_frame_extract_args &a, int32_t *so, int32_t *det_frame, float4 *packed,
                         cudaStream_t s);
 
-// frame_slots_kernel after the count pass: c2, kpos, base (F * D each) for the write kernel, rank (F * 3) scratch
-cudaError_t frame_slots(const fcn_frame_extract_args &a, const int32_t *det_points, const long long *cnt_pos,
-                        int32_t *c2, int32_t *kpos, long long *base, int32_t *rank, cudaStream_t s);
+// frame_slots_kernel after the count pass: c2, kpos, base (F * D each) for the write kernel
+cudaError_t frame_slots(const fcn_frame_extract_args &a, const int32_t *det_points, int32_t *c2, int32_t *kpos,
+                        long long *base, cudaStream_t s);
 
 }  // namespace fcn

@@ -4,16 +4,15 @@
 //   fr_plan   each slot's first-stage row, as section (20)'s gather plan of one-job pieces (rj_jobs_kernel reads it);
 //   fr_slots  after the count pass and a table pass over every slot: the W[s] section test, each frame's P2_out
 //             budget, the batch entry and output position of every kept frustum (what rx_write_kernel is handed), the
-//             batch tables and the dummy entries.
+//             batch tables and the dummy entries (frame_plan).
 // The in-image points are recomputed from the scans (frame_setup, frame_pack and fov_stage of section (21)) rather
 // than kept from the detection call: that costs one more pass over the F * P scan points (a flag, a scan and a
 // compaction) and saves keeping F * P float4 points and their scan alive between the two calls.
 #include <cmath>
 
-#include <cub/block/block_scan.cuh>
-
 #include "common.cuh"
 #include "frame_extract.cuh"
+#include "frame_plan.cuh"
 #include "frame_refine.cuh"
 #include "frustum_fov.cuh"
 
@@ -53,83 +52,41 @@ __global__ void __launch_bounds__(FR_THREADS) fr_plan_kernel(const fcn_frame_ref
     if (j == 0 && total > J) atomicOr(a.status, FCN_FRAME_JOBS);
 }
 
-// One CTA, after the count pass and the table pass over every slot (words: T per scale of each slot's record).  Per
-// frame (one thread each, its J slots in order): a counted frustum whose T[s] exceeds widths[s] is dropped; the
-// others fit while the frame's running point count stays <= P2_out, so the budget drops a suffix.  Class ranks are
-// taken among the kept frustums only.  Exclusive sums over the frames give each kept frustum its batch entry k and
-// output position base; then the B - K dummy entries, whose record is the one-section box of job_data[B].
+// One CTA, after the count pass and the table pass over every slot (words: T per scale of each slot's record):
+// frame_plan over the F frames of J job slots, where a counted frustum whose T[s] exceeds widths[s] is dropped.  The
+// dummy entries' record is the one-section box of job_data[B].
 __global__ void __launch_bounds__(FR_SLOT_THREADS)
 fr_slots_kernel(const fcn_frame_refine_args a, FrPlan p, const int32_t *__restrict__ job_status,
                 const int32_t *__restrict__ job_points, const int32_t *__restrict__ words,
                 fcn_refine_job_data *__restrict__ job_data, int32_t *__restrict__ c2, int32_t *__restrict__ kpos,
                 long long *__restrict__ base, int32_t *__restrict__ kept) {
-    using Scan = cub::BlockScan<int, FR_SLOT_THREADS>;
-    __shared__ typename Scan::TempStorage tmp;
-    const int F = a.num_frames, J = a.job_capacity, B = F * J, S = a.num_scales, Pout = a.out_capacity;
-    int bits = 0, k_run = 0, m_run = 0;
-    for (int f0 = 0; f0 < F; f0 += FR_SLOT_THREADS) {
-        const int f = f0 + threadIdx.x;
-        int rank[3] = {-1, -1, -1}, k = 0, m = 0;
-        if (f < F) {
-            int n = 0, run = 0;
-            for (int j = 0; j < J; ++j) {
-                const int d = f * J + j;
-                int c = -1;
-                if (p.frame[d] >= 0 && (job_status[d] & (FCN_REFINE_ROW_NONFINITE | FCN_REFINE_ROW_EXTENTS)))
-                    bits |= FCN_FRAME_BAD_DET;
-                if (job_points[d] >= 0) {
-                    bool fits = true;
-                    for (int s = 0; s < S; ++s) fits = fits && words[(size_t)d * (S + 1) + s] <= a.widths[s];
-                    if (!fits) {
-                        bits |= FCN_FRAME_SECTIONS;
-                    } else {
-                        run = min(run + job_points[d], Pout + 1);      // saturates: the budget drops a suffix
-                        if (run > Pout) bits |= FCN_FRAME_OUT_POINTS;
-                        else c = job_points[d];
-                    }
-                }
-                c2[d] = c;
-                if (c >= 0) {
-                    const int cls = p.cls[d];
-                    if (rank[cls] < 0) {
-                        a.seg_class_out[3 * f + n] = cls;
-                        rank[cls] = n++;
-                    }
-                    ++k;
-                    m += c;
-                }
-            }
-            for (int q = n; q < 3; ++q) a.seg_class_out[3 * f + q] = -1;
-        }
-        int kx, kt, mx, mt;
-        Scan(tmp).ExclusiveSum(k, kx, kt);
-        __syncthreads();
-        Scan(tmp).ExclusiveSum(m, mx, mt);
-        if (f < F) {
-            int kk = k_run + kx;
-            long long mm = m_run + mx;
-            for (int j = 0; j < J; ++j) {
-                const int d = f * J + j, c = c2[d];
-                kpos[d] = kk;
-                base[d] = mm;
-                if (c < 0) continue;
-                const int cls = p.cls[d];
-                a.valid[kk] = 1;
-                a.cls_index[kk] = cls;
-                a.seg[kk] = 3 * f + rank[cls];
-                a.job_index[kk] = d;
-                kept[kk] = d;
-                for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)kk + i] = (float)job_data[d].box2d[i];
-                ++kk;
-                mm += c;
-            }
-        }
-        k_run += kt;
-        m_run += mt;
-        __syncthreads();
-    }
+    const int B = a.num_frames * a.job_capacity, S = a.num_scales;
+    frame_plan<3, FR_SLOT_THREADS>(
+        a.num_frames, a.job_capacity, a.out_capacity, p.cls, c2, base, a.seg_class_out, a.offsets, a.valid,
+        a.cls_index, a.seg, a.status,
+        [&](int d, int &bits) {
+            if (p.frame[d] >= 0 && (job_status[d] & (FCN_REFINE_ROW_NONFINITE | FCN_REFINE_ROW_EXTENTS)))
+                bits |= FCN_FRAME_BAD_DET;
+            if (job_points[d] < 0) return -1;
+            bool fits = true;
+            for (int s = 0; s < S; ++s) fits = fits && words[(size_t)d * (S + 1) + s] <= a.widths[s];
+            if (!fits) bits |= FCN_FRAME_SECTIONS;
+            return fits ? job_points[d] : -1;
+        },
+        [&](int k, int d, int, long long) {
+            kpos[d] = k;
+            a.job_index[k] = d;
+            kept[k] = d;
+            for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)k + i] = (float)job_data[d].box2d[i];
+        },
+        [&](int k, int pt) {
+            reinterpret_cast<float4 *>(a.points)[pt] = make_float4(0.f, 0.f, 0.f, 0.f);
+            a.job_index[k] = -1;
+            kept[k] = B;
+            const float bx[4] = {0.f, 0.f, 1.f, 1.f};
+            for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)k + i] = bx[i];
+        });
     if (threadIdx.x == 0) {
-        a.offsets[0] = 0;
         double w = a.stride[0];                     // T[s] = ceil(w / stride[s]) = 1 at every scale
         for (int s = 1; s < S; ++s) w = fmin(w, a.stride[s]);
         fcn_refine_job_data dd;
@@ -141,19 +98,6 @@ fr_slots_kernel(const fcn_frame_refine_args a, FrPlan p, const int32_t *__restri
         dd.cls_index = 0;
         job_data[B] = dd;
     }
-    for (int k = k_run + threadIdx.x; k < B; k += FR_SLOT_THREADS) {
-        const int pt = m_run + (k - k_run);
-        a.offsets[k + 1] = pt + 1;
-        reinterpret_cast<float4 *>(a.points)[pt] = make_float4(0.f, 0.f, 0.f, 0.f);
-        a.valid[k] = 0;
-        a.cls_index[k] = 0;
-        a.seg[k] = 0;
-        a.job_index[k] = -1;
-        kept[k] = B;
-        const float bx[4] = {0.f, 0.f, 1.f, 1.f};
-        for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)k + i] = bx[i];
-    }
-    if (bits) atomicOr(a.status, bits);
 }
 
 // ------------------------------------------------------------------------------------------------ host side

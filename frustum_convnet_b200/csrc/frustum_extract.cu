@@ -140,7 +140,7 @@ static int fx_prepare(const fcn_frustum_extract_args *a, const char *fn, FxWs &w
 
 struct FrameWs : FxWs {
     float4 *packed;
-    int32_t *so, *det_frame, *det_points, *c2, *kpos, *rank;
+    int32_t *so, *det_frame, *det_points, *c2, *kpos;
     long long *base, *info;
 };
 
@@ -155,7 +155,6 @@ static cudaError_t frame_layout(const fcn_frame_extract_args *a, Carve &c, Frame
     w.det_points = (int32_t *)c.take(FD * 4);
     w.c2 = (int32_t *)c.take(FD * 4);
     w.kpos = (int32_t *)c.take(FD * 4);
-    w.rank = (int32_t *)c.take(F * 3 * 4);
     w.base = (long long *)c.take(FD * 8);
     w.info = (long long *)c.take(32);
     return e;
@@ -213,7 +212,7 @@ extern "C" int fcn_frame_extract(const fcn_frame_extract_args *a, fcn_stream_t s
                                              w.det_points, w.keep, w.cnt, w.box, w.angle, w.bad);
     FCN_LAUNCH_CHECK();
     FCN_CUDA(job_totals(w, B, w.info, s));
-    FCN_CUDA(frame_slots(*a, w.det_points, w.cnt_pos, w.c2, w.kpos, w.base, w.rank, s));
+    FCN_CUDA(frame_slots(*a, w.det_points, w.c2, w.kpos, w.base, s));
     fx_write_kernel<<<B, FX_THREADS, 0, s>>>(B, (long long)F * a->out_capacity, w.so, a->frames, w.det_frame, w.c2,
                                              w.kpos, w.base, w.box, w.angle, w.pos, w.fov_pts, w.fov_u, w.fov_v,
                                              (float4 *)a->points, a->offsets, a->frustum_angle, a->box2d, a->P,

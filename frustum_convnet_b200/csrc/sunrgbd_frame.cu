@@ -20,6 +20,7 @@
 #include <cub/block/block_scan.cuh>
 
 #include "common.cuh"
+#include "frame_plan.cuh"
 #include "input_builder.cuh"
 #include "sunrgbd_uv.cuh"
 
@@ -56,22 +57,8 @@ __global__ void __launch_bounds__(SF_THREADS) sf_setup_kernel(const fcn_sunrgbd_
     const int d = blockIdx.x * SF_THREADS + threadIdx.x;
     if (d >= B) return;
     int bits = 0;
-    if (d < F) {
-        const int c = a.cloud_counts[d], nd = a.det_counts[d];
-        w.n[d] = c < 0 ? 0 : (c > P ? P : c);
-        bits |= (c > P ? FCN_FRAME_SCAN_POINTS : 0) | (nd > D ? FCN_FRAME_DETS : 0);
-    }
-    const int f = d / D;
-    int fr = -1;
-    if (d - f * D < a.det_counts[f]) {
-        const int c = a.det_class[d];
-        const double *b = a.boxes + 4 * (size_t)d;
-        const bool ok = c >= 0 && c < SF_CLASSES && isfinite(b[0]) && isfinite(b[1]) && isfinite(b[2]) &&
-                        isfinite(b[3]);
-        if (!ok) bits |= FCN_FRAME_BAD_DET;
-        else if ((a.class_mask >> c) & 1u) fr = f;
-    }
-    w.det_frame[d] = fr;
+    if (d < F) w.n[d] = frame_count(a.cloud_counts[d], a.det_counts[d], P, D, bits);
+    w.det_frame[d] = frame_candidate(d, D, SF_CLASSES, a.class_mask, a.det_counts, a.det_class, a.boxes, bits);
     w.ident[d] = d;
     if (bits) atomicOr(a.status, bits);
 }
@@ -200,87 +187,35 @@ __global__ void __launch_bounds__(SF_THREADS) sf_scan_kernel(SfWs w, int C) {
     if (threadIdx.x == 0) w.det_points[d] = w.det_frame[d] >= 0 ? run : -1;
 }
 
-// One CTA, after the scan.  Per frame (one thread each, its D slots in order): a candidate with n >= 5 keeps
-// min(n, 2048) points while the frame's running count stays <= P_out (saturating, so the budget drops a suffix);
-// class ranks among the kept frustums, 4 bits a class (15: none).  Exclusive sums over the frames give each kept
-// frustum its batch entry and output position; then the B - K dummy entries and the cap draw's offsets.
+// One CTA, after the scan: frame_plan over the F frames of D detection slots, where a candidate with n >= 5 keeps
+// min(n, 2048) points; then the cap draw's offsets.
 __global__ void __launch_bounds__(SF_SLOT_THREADS) sf_slots_kernel(const fcn_sunrgbd_frame_extract_args a, SfWs w) {
     using Scan = cub::BlockScan<int, SF_SLOT_THREADS>;
     __shared__ typename Scan::TempStorage tmp;
-    const int F = a.num_frames, D = a.det_capacity, B = F * D, Pout = a.out_capacity;
-    int bits = 0, k_run = 0, m_run = 0;
-    for (int f0 = 0; f0 < F; f0 += SF_SLOT_THREADS) {
-        const int f = f0 + threadIdx.x;
-        unsigned long long rank = ~0ull;
-        int k = 0, m = 0;
-        if (f < F) {
-            int nr = 0, run = 0;
-            for (int j = 0; j < D; ++j) {
-                const int d = f * D + j, np = w.det_points[d];
-                int c = -1;
-                if (np >= SF_MIN_POINTS) {
-                    const int kp = np < SF_CAP ? np : SF_CAP;
-                    run = min(run + kp, Pout + 1);
-                    if (run > Pout) bits |= FCN_FRAME_OUT_POINTS;
-                    else c = kp;
-                }
-                w.c2[d] = c;
-                if (c >= 0) {
-                    const int cls = a.det_class[d];
-                    if (((rank >> (4 * cls)) & 15) == 15) {
-                        a.seg_class[SF_CLASSES * f + nr] = cls;
-                        rank &= ~(15ull << (4 * cls));
-                        rank |= (unsigned long long)nr++ << (4 * cls);
-                    }
-                    ++k;
-                    m += c;
-                }
-            }
-            for (int q = nr; q < SF_CLASSES; ++q) a.seg_class[SF_CLASSES * f + q] = -1;
-        }
-        int kx, kt, mx, mt;
-        Scan(tmp).ExclusiveSum(k, kx, kt);
-        __syncthreads();
-        Scan(tmp).ExclusiveSum(m, mx, mt);
-        if (f < F) {
-            int kk = k_run + kx;
-            long long mm = m_run + mx;
-            for (int j = 0; j < D; ++j) {
-                const int d = f * D + j, c = w.c2[d];
-                w.base[d] = mm;
-                if (c < 0) continue;
-                const int cls = a.det_class[d];
-                a.valid[kk] = 1;
-                a.cls_index[kk] = cls;
-                a.seg[kk] = SF_CLASSES * f + (int)((rank >> (4 * cls)) & 15);
-                a.det_index[kk] = d;
-                a.rgb_prob[kk] = a.det_prob[d];
-                for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)kk + i] = (float)a.boxes[4 * (size_t)d + i];
-                w.kept[kk] = d;
-                mm += c;
-                a.offsets[kk + 1] = (int32_t)mm;
-                ++kk;
-            }
-        }
-        k_run += kt;
-        m_run += mt;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) a.offsets[0] = 0;
-    for (int k = k_run + threadIdx.x; k < B; k += SF_SLOT_THREADS) {
-        const int p = m_run + (k - k_run);
-        a.offsets[k + 1] = p + 1;
-        for (int i = 0; i < 6; ++i) a.points[6 * (size_t)p + i] = 0.f;
-        for (int i = 0; i < 3; ++i) a.xyz[3 * (size_t)p + i] = 0.f;
-        a.valid[k] = 0;
-        a.cls_index[k] = 0;
-        a.seg[k] = 0;
-        a.det_index[k] = -1;
-        a.rgb_prob[k] = 0.f;
-        const float bx[4] = {0.f, 0.f, 1.f, 1.f};
-        for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)k + i] = bx[i];
-        w.kept[k] = -1;
-    }
+    const int B = a.num_frames * a.det_capacity;
+    frame_plan<SF_CLASSES, SF_SLOT_THREADS>(
+        a.num_frames, a.det_capacity, a.out_capacity, a.det_class, w.c2, w.base, a.seg_class, a.offsets, a.valid,
+        a.cls_index, a.seg, a.status,
+        [&](int d, int &) {
+            const int n = w.det_points[d];
+            return n < SF_MIN_POINTS ? -1 : (n < SF_CAP ? n : SF_CAP);
+        },
+        [&](int k, int d, int c, long long m) {
+            a.det_index[k] = d;
+            a.rgb_prob[k] = a.det_prob[d];
+            for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)k + i] = (float)a.boxes[4 * (size_t)d + i];
+            w.kept[k] = d;
+            a.offsets[k + 1] = (int32_t)(m + c);
+        },
+        [&](int k, int p) {
+            for (int i = 0; i < 6; ++i) a.points[6 * (size_t)p + i] = 0.f;
+            for (int i = 0; i < 3; ++i) a.xyz[3 * (size_t)p + i] = 0.f;
+            a.det_index[k] = -1;
+            a.rgb_prob[k] = 0.f;
+            const float bx[4] = {0.f, 0.f, 1.f, 1.f};
+            for (int i = 0; i < 4; ++i) a.box2d[4 * (size_t)k + i] = bx[i];
+            w.kept[k] = -1;
+        });
     int run = 0;
     for (int d0 = 0; d0 < B; d0 += SF_SLOT_THREADS) {
         const int d = d0 + threadIdx.x;
@@ -292,7 +227,6 @@ __global__ void __launch_bounds__(SF_SLOT_THREADS) sf_slots_kernel(const fcn_sun
         __syncthreads();
     }
     if (threadIdx.x == 0) w.cap_off[B] = run;
-    if (bits) atomicOr(a.status, bits);
 }
 
 // one CTA per slot: a kept capped slot's 2048 drawn ranks sorted, with the draw position (output row) of each

@@ -34,7 +34,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._host import cuda_device, on_device, workspace
+from ._host import check_tensors, cuda_device, workspace
 from .input_builder import FrustumBatchBuilder
 from .refine_extract import REFINE_STRIDES
 from .train_inputs import SUNRGBD_CLASSES
@@ -104,10 +104,58 @@ class FrameDetections:
 class _CapacityStage:
     """What the detection and refinement stages share: the model's eval forward on its plan for (B, N, T) and the
     collector's candidates and capacity finalize over B entries, of which only the valid ones add rows.  A subclass
-    sets model, device, F, B, N, T (sections per scale), R, method, thresh, top_k and the entry tables seg, valid,
-    box2d32 and seg_class, then calls _init_collector.  Each frame has one segment per class of `classes`."""
+    calls _settings, sets model, device, F, B, N, T (sections per scale), R and the entry tables seg, valid, box2d32
+    and seg_class, then calls _init_collector.  Each frame has one segment per class of `classes`."""
 
     classes, dataset = CLASSES, _lib.DET_KITTI
+
+    def _settings(self, who, classes, type_whitelist, method, thresh, top_k, seed):
+        """class_mask of type_whitelist (names of `classes`; any other raises ValueError before a device is
+        touched), the collector's method, thresh and top_k, and the resampling seed."""
+        bad = [t for t in type_whitelist if t not in classes]
+        if bad:
+            raise ValueError("%s: unknown types %s (classes: %s)" % (who, bad, classes))
+        self.class_mask = sum(1 << classes.index(t) for t in set(type_whitelist))
+        self.method = 0 if method == "nms" else 1
+        self.thresh, self.top_k, self.seed = float(thresh), int(top_k), int(seed) & (2 ** 64 - 1)
+
+    def _init_resample(self, index):
+        """The fcn_resample_choice arguments: N indices into each of the B entries' points (offsets) written to
+        choice, drawn under the key (seed, call, index[k], point)."""
+        r = _lib.ResampleArgs()
+        r.B, r.N, r.seed = self.B, self.N, self.seed
+        r.offsets, r.det_index, r.call, r.choice = (self.offsets.data_ptr(), index.data_ptr(), self.call.data_ptr(),
+                                                    self.choice.data_ptr())
+        self._ra = r
+
+    def _init_fixed_batch(self, kind, num_classes, max_depth, keys):
+        """The fixed-width batch of fcn_build_train_inputs_fixed over points3, offsets64 and frustum_records (the
+        extraction's records, zeroed here): the tensors `keys` of point_cloud, rot_angle, ref_center, rgb_prob and
+        one_hot, then center_ref1.. of widths T at the strides."""
+        dev, B, N, S = self.device, self.B, self.N, len(self.strides)
+        e = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
+        self.offsets64 = torch.empty(B + 1, dtype=torch.int64, device=dev)
+        self.frustum_records = torch.zeros((B, C.sizeof(_lib.TrainFrustum)), dtype=torch.uint8, device=dev)
+        self.index = torch.arange(B, dtype=torch.int32, device=dev)
+        shapes = {"point_cloud": (B, 3, N), "rot_angle": (B,), "ref_center": (B, 3), "rgb_prob": (B,),
+                  "one_hot": (B, num_classes)}
+        self.batch = {k: e(*shapes[k]) for k in keys}
+        for s, w in enumerate(self.T):
+            self.batch["center_ref%d" % (s + 1)] = e(B, 3, w)
+        t = _lib.TrainInputArgs()
+        t.kind, t.labels, t.rtc, t.extra_feat = kind, 0, 1, 0
+        t.B, t.N, t.num_scales, t.num_classes, t.num_frustums = B, N, S, num_classes, B
+        for s in range(S):
+            t.stride[s] = self.strides[s]
+            t.centers[s] = self.batch["center_ref%d" % (s + 1)].data_ptr()
+        t.max_depth = max_depth
+        t.points, t.point_offsets, t.frustums = (self.points3.data_ptr(), self.offsets64.data_ptr(),
+                                                 self.frustum_records.data_ptr())
+        t.index, t.choice = self.index.data_ptr(), self.choice.data_ptr()
+        for k in keys:
+            setattr(t, k, self.batch[k].data_ptr())
+        self._ta = t
+        self._widths = (C.c_int32 * S)(*self.T)
 
     def _init_collector(self, per_frame):
         """The collector's buffers; per_frame: the most entries of one frame (a segment holds rows of at most that
@@ -178,14 +226,9 @@ class FrameDetector(_CapacityStage):
         current cfg's DATA.STRIDE, MAX_DEPTH, NUM_SAMPLES).  method / thresh / top_k: the collector's."""
         from .config import get_cfg
         cfg = get_cfg()
-        bad = [t for t in type_whitelist if t not in CLASSES]
-        if bad:
-            raise ValueError("FrameDetector: unknown types %s (KITTI first stage: %s)" % (bad, CLASSES))
+        self._settings("FrameDetector", CLASSES, type_whitelist, method, thresh, top_k, seed)
         self.model = model
         self.device = cuda_device(device, "FrameDetector")
-        self.class_mask = sum(1 << CLASSES.index(t) for t in type_whitelist)
-        self.method = 0 if method == "nms" else 1
-        self.thresh, self.top_k, self.seed = float(thresh), int(top_k), int(seed) & (2 ** 64 - 1)
         self.F, self.P, self.D = int(frames), int(points), int(dets)
         self.B = self.F * self.D
         self.fb = FrustumBatchBuilder(cfg.DATA.STRIDE if strides is None else strides,
@@ -225,11 +268,7 @@ class FrameDetector(_CapacityStage):
             self._ws, a.workspace_bytes = workspace("fcn_frame_extract_workspace_bytes", dev, C.byref(a))
             a.workspace = self._ws.data_ptr()
         self._xa = a
-        r = _lib.ResampleArgs()
-        r.B, r.N, r.seed = B, self.N, self.seed
-        r.offsets, r.det_index, r.call, r.choice = (self.offsets.data_ptr(), self.det_index.data_ptr(),
-                                                    self.call.data_ptr(), self.choice.data_ptr())
-        self._ra = r
+        self._init_resample(self.det_index)
         self._init_collector(self.D)
 
     # ------------------------------------------------------------------ inputs
@@ -278,14 +317,11 @@ class FrameDetector(_CapacityStage):
         -> FrameDetections (this detector's buffers, overwritten by the next call)."""
         (pts, npts), (boxes, cls, prob, ndet) = scans, dets
         F, P, D = self.F, self.P, self.D
-        specs = (("scan points", pts, (F, P, 4), torch.float32), ("scan counts", npts, (F,), torch.int32),
-                 ("calibs", calibs, (F, 33), torch.float64), ("image_hw", image_hw, (F, 2), torch.int32),
-                 ("boxes", boxes, (F, D, 4), torch.float64), ("classes", cls, (F, D), torch.int32),
-                 ("probs", prob, (F, D), torch.float32), ("det counts", ndet, (F,), torch.int32))
-        for name, t, shape, dt in specs:
-            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
-                raise ValueError("FrameDetector.detect: %s must be a contiguous %s CUDA tensor of shape %s on %s"
-                                 % (name, dt, shape, self.device))
+        check_tensors("FrameDetector.detect", self.device, (
+            ("scan points", pts, (F, P, 4), torch.float32), ("scan counts", npts, (F,), torch.int32),
+            ("calibs", calibs, (F, 33), torch.float64), ("image_hw", image_hw, (F, 2), torch.int32),
+            ("boxes", boxes, (F, D, 4), torch.float64), ("classes", cls, (F, D), torch.int32),
+            ("probs", prob, (F, D), torch.float32), ("det counts", ndet, (F,), torch.int32)))
         dev = self.device
         with torch.cuda.device(dev):
             st = torch.cuda.current_stream(dev).cuda_stream
@@ -350,13 +386,8 @@ class FrameRefiner(_CapacityStage):
         from scale to scale like the model's section pyramid.
         frustum_points P2_out (default P) and rows R2 (default B2 * W[1], B2 = F * J): the capacities of each frame's
         frustum points and of the collector.  method / thresh / top_k: the collector's."""
-        bad = [t for t in type_whitelist if t not in CLASSES]
-        if bad:
-            raise ValueError("FrameRefiner: unknown types %s (KITTI: %s)" % (bad, CLASSES))
+        self._settings("FrameRefiner", CLASSES, type_whitelist, method, thresh, top_k, seed)
         self.fd, self.model, self.device = detector, model, detector.device
-        self.class_mask = sum(1 << CLASSES.index(t) for t in type_whitelist)
-        self.method = 0 if method == "nms" else 1
-        self.thresh, self.top_k, self.seed = float(thresh), int(top_k), int(seed) & (2 ** 64 - 1)
         self.F, self.P = detector.F, detector.P
         self.J = int(jobs) if jobs is not None else 2 * detector.D
         self.strides = [float(s) for s in strides]
@@ -376,19 +407,14 @@ class FrameRefiner(_CapacityStage):
         e = lambda *shape, dtype=torch.int32: torch.empty(shape, dtype=dtype, device=dev)
         self.points4 = e(F * self.P_out + B, 4, dtype=torch.float32)
         self.points3 = e(F * self.P_out + B, 3, dtype=torch.float32)
-        self.offsets, self.offsets64 = e(B + 1), e(B + 1, dtype=torch.int64)
+        self.offsets = e(B + 1)
         self.job_index, self.valid, self.cls_index, self.seg = e(B), e(B), e(B), e(B)
         self.seg_class, self.box2d32 = e(F, 3), e(B, 4, dtype=torch.float32)
-        self.frustum_records = torch.zeros((B, C.sizeof(_lib.TrainFrustum)), dtype=torch.uint8, device=dev)
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self.call = torch.full((1,), -2 ** 63, dtype=torch.int64, device=dev)     # bit 63 set: stage 2's draws
         self.choice = e(B, self.N)
-        self.index = torch.arange(B, dtype=torch.int32, device=dev)
-        self.batch = {"point_cloud": e(B, 3, self.N, dtype=torch.float32), "rot_angle": e(B, dtype=torch.float32),
-                      "ref_center": e(B, 3, dtype=torch.float32), "rgb_prob": e(B, dtype=torch.float32),
-                      "one_hot": e(B, len(CLASSES), dtype=torch.float32)}
-        for s, w in enumerate(self.T):
-            self.batch["center_ref%d" % (s + 1)] = e(B, 3, w, dtype=torch.float32)
+        self._init_fixed_batch(_lib.TRAIN_REFINE, len(CLASSES), 1.0,
+                               ("point_cloud", "rot_angle", "ref_center", "rgb_prob", "one_hot"))
 
         a = _lib.FrameRefineArgs()
         a.num_frames, a.scan_capacity, a.job_capacity, a.out_capacity = F, self.P, self.J, self.P_out
@@ -406,25 +432,7 @@ class FrameRefiner(_CapacityStage):
             self._ws, a.workspace_bytes = workspace("fcn_frame_refine_extract_workspace_bytes", dev, C.byref(a))
             a.workspace = self._ws.data_ptr()
         self._xa = a
-        r = _lib.ResampleArgs()
-        r.B, r.N, r.seed = B, self.N, self.seed
-        r.offsets, r.det_index, r.call, r.choice = (self.offsets.data_ptr(), self.job_index.data_ptr(),
-                                                    self.call.data_ptr(), self.choice.data_ptr())
-        self._ra = r
-        t = _lib.TrainInputArgs()
-        t.kind, t.labels, t.rtc, t.extra_feat = _lib.TRAIN_REFINE, 0, 1, 0
-        t.B, t.N, t.num_scales, t.num_classes, t.num_frustums = B, self.N, S, len(CLASSES), B
-        for s in range(S):
-            t.stride[s] = self.strides[s]
-            t.centers[s] = self.batch["center_ref%d" % (s + 1)].data_ptr()
-        t.max_depth = 1.0
-        t.points, t.point_offsets, t.frustums = (self.points3.data_ptr(), self.offsets64.data_ptr(),
-                                                 self.frustum_records.data_ptr())
-        t.index, t.choice = self.index.data_ptr(), self.choice.data_ptr()
-        for k in ("point_cloud", "rot_angle", "ref_center", "rgb_prob", "one_hot"):
-            setattr(t, k, self.batch[k].data_ptr())
-        self._ta = t
-        self._widths = (C.c_int32 * S)(*self.T)
+        self._init_resample(self.job_index)
         self._init_collector(self.J)
 
     @torch.no_grad()
@@ -438,11 +446,8 @@ class FrameRefiner(_CapacityStage):
         if first.rows.data_ptr() != self.fd.rows.data_ptr():
             raise ValueError("FrameRefiner.refine: `first` is not the result of this refiner's detector")
         F, P = self.F, self.P
-        for name, t, shape, dt in (("scan points", pts, (F, P, 4), torch.float32),
-                                   ("scan counts", npts, (F,), torch.int32)):
-            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
-                raise ValueError("FrameRefiner.refine: %s must be a contiguous %s CUDA tensor of shape %s on %s"
-                                 % (name, dt, shape, self.device))
+        check_tensors("FrameRefiner.refine", self.device, (("scan points", pts, (F, P, 4), torch.float32),
+                                                           ("scan counts", npts, (F,), torch.int32)))
         dev = self.device
         with torch.cuda.device(dev):
             st = torch.cuda.current_stream(dev).cuda_stream
@@ -513,14 +518,9 @@ class SunrgbdFrameDetector(_CapacityStage):
         from .config import get_cfg
         cfg = get_cfg()
         self.classes = SUNRGBD_CLASSES
-        bad = [t for t in type_whitelist if t not in SUNRGBD_CLASSES]
-        if bad:
-            raise ValueError("SunrgbdFrameDetector: unknown types %s (SUN-RGBD: %s)" % (bad, SUNRGBD_CLASSES))
+        self._settings("SunrgbdFrameDetector", SUNRGBD_CLASSES, type_whitelist, method, thresh, top_k, seed)
         self.model = model
         self.device = cuda_device(device, "SunrgbdFrameDetector")
-        self.class_mask = sum(1 << SUNRGBD_CLASSES.index(t) for t in set(type_whitelist))
-        self.method = 0 if method == "nms" else 1
-        self.thresh, self.top_k, self.seed = float(thresh), int(top_k), int(seed) & (2 ** 64 - 1)
         self.F, self.P, self.D = int(frames), int(points), int(dets)
         self.B = self.F * self.D
         self.strides = [float(s) for s in (cfg.DATA.STRIDE if strides is None else strides)]
@@ -543,20 +543,16 @@ class SunrgbdFrameDetector(_CapacityStage):
         self._frames = torch.zeros((F, _SUNRGBD_FRAME_BYTES), dtype=torch.uint8, device=dev)
         self.points = e(F * self.P_out + B, 6, dtype=f32)
         self.points3 = e(F * self.P_out + B, 3, dtype=f32)
-        self.offsets, self.offsets64 = e(B + 1), e(B + 1, dtype=torch.int64)
+        self.offsets = e(B + 1)
         self.det_index, self.valid, self.cls_index, self.seg = e(B), e(B), e(B), e(B)
         self.seg_class, self.rgb_prob, self.box2d32 = e(F, NC), e(B, dtype=f32), e(B, 4, dtype=f32)
         self.cap_choice = e(B, _lib.SUNRGBD_MAX_POINTS)
-        self.frustum_records = torch.zeros((B, C.sizeof(_lib.TrainFrustum)), dtype=torch.uint8, device=dev)
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
         self.call = torch.zeros(1, dtype=torch.int64, device=dev)
         self.cap_call = torch.full((1,), 2 ** 62, dtype=torch.int64, device=dev)    # bit 62 set: the cap's draws
         self.choice = e(B, self.N)
-        self.index = torch.arange(B, dtype=torch.int32, device=dev)
-        self.batch = {"point_cloud": e(B, 3, self.N, dtype=f32), "rot_angle": e(B, dtype=f32),
-                      "rgb_prob": e(B, dtype=f32), "one_hot": e(B, NC, dtype=f32)}
-        for s, w in enumerate(self.T):
-            self.batch["center_ref%d" % (s + 1)] = e(B, 3, w, dtype=f32)
+        self._init_fixed_batch(_lib.TRAIN_SUNRGBD, NC, self.max_depth, ("point_cloud", "rot_angle", "rgb_prob",
+                                                                        "one_hot"))
 
         a = _lib.SunrgbdFrameExtractArgs()
         a.num_frames, a.point_capacity, a.det_capacity, a.out_capacity = F, self.P, self.D, self.P_out
@@ -573,25 +569,7 @@ class SunrgbdFrameDetector(_CapacityStage):
             self._ws, a.workspace_bytes = workspace("fcn_sunrgbd_frame_extract_workspace_bytes", dev, C.byref(a))
             a.workspace = self._ws.data_ptr()
         self._xa = a
-        r = _lib.ResampleArgs()
-        r.B, r.N, r.seed = B, self.N, self.seed
-        r.offsets, r.det_index, r.call, r.choice = (self.offsets.data_ptr(), self.det_index.data_ptr(),
-                                                    self.call.data_ptr(), self.choice.data_ptr())
-        self._ra = r
-        t = _lib.TrainInputArgs()
-        t.kind, t.labels, t.rtc, t.extra_feat = _lib.TRAIN_SUNRGBD, 0, 1, 0
-        t.B, t.N, t.num_scales, t.num_classes, t.num_frustums = B, self.N, S, NC, B
-        for s in range(S):
-            t.stride[s] = self.strides[s]
-            t.centers[s] = self.batch["center_ref%d" % (s + 1)].data_ptr()
-        t.max_depth = self.max_depth
-        t.points, t.point_offsets, t.frustums = (self.points3.data_ptr(), self.offsets64.data_ptr(),
-                                                 self.frustum_records.data_ptr())
-        t.index, t.choice = self.index.data_ptr(), self.choice.data_ptr()
-        for k in ("point_cloud", "rot_angle", "rgb_prob", "one_hot"):
-            setattr(t, k, self.batch[k].data_ptr())
-        self._ta = t
-        self._widths = (C.c_int32 * S)(*self.T)
+        self._init_resample(self.det_index)
         self._init_collector(self.D)
         self._depth = None              # detect_depth's conversion and its (F, P, 6) clouds, made on its first call
 
@@ -651,14 +629,11 @@ class SunrgbdFrameDetector(_CapacityStage):
         the cap draw of every candidate slot with more than 2048 in-box points, in draw order."""
         (pts, npts), (boxes, cls, prob, ndet) = clouds, dets
         F, P, D = self.F, self.P, self.D
-        specs = (("cloud points", pts, (F, P, 6), torch.float32), ("cloud counts", npts, (F,), torch.int32),
-                 ("calibs", calibs, (F, 18), torch.float64), ("boxes", boxes, (F, D, 4), torch.float64),
-                 ("classes", cls, (F, D), torch.int32), ("probs", prob, (F, D), torch.float32),
-                 ("det counts", ndet, (F,), torch.int32))
-        for name, t, shape, dt in specs:
-            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
-                raise ValueError("SunrgbdFrameDetector.detect: %s must be a contiguous %s CUDA tensor of shape %s on %s"
-                                 % (name, dt, shape, self.device))
+        check_tensors("SunrgbdFrameDetector.detect", self.device, (
+            ("cloud points", pts, (F, P, 6), torch.float32), ("cloud counts", npts, (F,), torch.int32),
+            ("calibs", calibs, (F, 18), torch.float64), ("boxes", boxes, (F, D, 4), torch.float64),
+            ("classes", cls, (F, D), torch.int32), ("probs", prob, (F, D), torch.float32),
+            ("det counts", ndet, (F,), torch.int32)))
         dev = self.device
         with torch.cuda.device(dev):
             self.status.zero_()
@@ -754,11 +729,9 @@ class SunrgbdFrameDetector(_CapacityStage):
             self._depth_clouds = (torch.empty((F, self.P, 6), dtype=torch.float32, device=dev),
                                   torch.empty(F, dtype=torch.int32, device=dev))
         self._depth.check("SunrgbdFrameDetector.detect_depth", depth, rgb, hw, calibs)
-        for name, t, shape, dt in (("boxes", boxes, (F, D, 4), torch.float64), ("classes", cls, (F, D), torch.int32),
-                                   ("probs", prob, (F, D), torch.float32), ("det counts", ndet, (F,), torch.int32)):
-            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
-                raise ValueError("SunrgbdFrameDetector.detect_depth: %s must be a contiguous %s CUDA tensor of shape "
-                                 "%s on %s" % (name, dt, shape, self.device))
+        check_tensors("SunrgbdFrameDetector.detect_depth", self.device, (
+            ("boxes", boxes, (F, D, 4), torch.float64), ("classes", cls, (F, D), torch.int32),
+            ("probs", prob, (F, D), torch.float32), ("det counts", ndet, (F,), torch.int32)))
         with torch.cuda.device(self.device):
             self.status.zero_()
             pts, npts = self._depth_clouds

@@ -21,7 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._host import cuda_device, on_device, workspace
+from ._host import check_tensors, cuda_device, workspace
 from .sunrgbd_extract import calib_mats
 
 
@@ -45,10 +45,7 @@ class DepthCloudStage:
                  ("calibs", calibs, (F, 18), torch.float64)]
         if rgb is not None:
             specs.append(("rgb", rgb, (F, H, W, 3), torch.uint8))
-        for name, t, shape, dt in specs:
-            if not on_device(t, self.device) or tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
-                raise ValueError("%s: %s must be a contiguous %s CUDA tensor of shape %s on %s"
-                                 % (who, name, dt, shape, self.device))
+        check_tensors(who, self.device, specs)
 
     def run(self, depth, rgb, image_hw, calibs, clouds, counts, status, stream):
         """Launch on `stream` (a cudaStream_t): clouds (F, P, 6) float32 and counts (F,) int32 written, status bits

@@ -59,10 +59,10 @@ def budget(det_points, P_out):
     return np.asarray(out, dtype=np.int64)
 
 
-def class_ranks(classes, fits):
-    """One frame's slot classes and budget flags -> (rank of each class 0..2 or -1, seg_class (3,)): classes by first
-    appearance among the slots that fit."""
-    rank, seg_class = [-1, -1, -1], [-1, -1, -1]
+def class_ranks(classes, fits, num_classes=3):
+    """One frame's slot classes and budget flags -> (rank of each class 0..num_classes - 1 or -1, seg_class
+    (num_classes,)): classes by first appearance among the slots that fit."""
+    rank, seg_class = [-1] * num_classes, [-1] * num_classes
     n = 0
     for c, ok in zip(classes, fits):
         if ok and rank[c] < 0:

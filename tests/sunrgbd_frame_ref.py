@@ -3,8 +3,11 @@ inputs and status bits, the extraction of each clamped frame by oracle/sunrgbd_e
 tests/resample_ref.choice_row under the cap's key, each frame's P_out budget, the ten-class ranks, the B = F * D batch
 entries with their dummy tail, and the fcn_train_frustum records (frustum_table of the kept frustums; the frustum
 angle is sunrgbd_extract.frustum_angle)."""
+from functools import partial
+
 import numpy as np
 
+from frame_ref import budget, class_ranks as _class_ranks
 from frustum_convnet_b200 import _lib
 from frustum_convnet_b200.train_inputs import SUNRGBD_CLASSES, frustum_table
 from oracle import sunrgbd_extract as ox
@@ -12,6 +15,7 @@ from resample_ref import choice_row
 
 SCAN_POINTS, DETS, OUT_POINTS, BAD_DET = 1, 2, 4, 16          # FCN_FRAME_* bits of the C header
 CAP, MIN_POINTS, NC = 2048, 5, len(SUNRGBD_CLASSES)
+class_ranks = partial(_class_ranks, num_classes=NC)          # KITTI's budget and ranks over ten classes
 
 
 def synth_frames(seed, F, H=240, W=320, n_objects=6):
@@ -60,31 +64,6 @@ class _Rows:
         want_n, row = self.rows.pop(0)
         assert (int(n), size, replace) == (want_n, CAP, False)
         return row.astype(np.int64)
-
-
-def budget(det_points, P_out):
-    """One frame's slots (kept points min(n, 2048) of each, -1 when dropped before the budget) -> the points of the
-    slots that fit P_out, -1 for the others: the longest prefix of the kept slots whose points add up to <= P_out."""
-    out, run = [], 0
-    for c in det_points:
-        if c < 0:
-            out.append(-1)
-            continue
-        run += c
-        out.append(c if run <= P_out else -1)
-    return np.asarray(out, dtype=np.int64)
-
-
-def class_ranks(classes, fits):
-    """One frame's slot classes and budget flags -> (rank of each class or -1, seg_class (10,)): classes by first
-    appearance among the slots that fit."""
-    rank, seg_class = [-1] * NC, [-1] * NC
-    n = 0
-    for c, ok in zip(classes, fits):
-        if ok and rank[c] < 0:
-            rank[c], seg_class[n] = n, c
-            n += 1
-    return rank, np.asarray(seg_class, dtype=np.int32)
 
 
 def dummy_record(strides, max_depth):
