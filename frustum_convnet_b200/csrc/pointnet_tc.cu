@@ -9,8 +9,8 @@
 //           permutation turns the accumulator fragments into the A fragments of layer 3 (resident for the tile)
 //   layer 3 D3[64 x N3-channel chunk] = A2 * W3^T (A from registers) -> +bias, ReLU, max over the rows of each
 //           section part in a warp's 16 rows, then one integer atomicMax per (section part, channel) into the
-//           position-major feature map.  A warp with one or two sections reduce-scatters each section's max over
-//           its lanes (14 shuffles per 64 channels); three or more take a segmented suffix max (112).
+//           position-major feature map.  A warp takes one masked reduce-scatter pass over its lanes per section
+//           that starts in its rows (7 shuffles per 32 channels and section, one coalesced atomic per lane).
 // Only the weights go through shared memory.  A loader warp streams (or keeps resident) the pre-swizzled W2/W3
 // stage images; both warpgroups read every stage, and a stage is released when both have retired the wgmma group
 // that read it.  The loader is a whole warpgroup that gives its registers to the two consumer warpgroups
@@ -96,7 +96,7 @@ __device__ __forceinline__ uint32_t layer1_tf32(const float4 &r, const float4 &w
 // becomes -inf by a select before any fmaxf.  The 8 values of a thread are reduce-scattered over the 8 lanes g = 0..7 that share
 // q (butterfly over lane bits 16, 8, 4: each level keeps one half and receives the partner's max of the other half,
 // 4 + 2 + 1 shuffles), so lane g ends up with the section max of value g, i.e. column 8 (j0 + g / 2) + 2q + g % 2;
-// then +bias, TF32 and one integer atomicMax if positive, as on the general path.  dst / bias point at column 0 of
+// then +bias, TF32 and one integer atomicMax if positive.  dst / bias point at column 0 of
 // the chunk.  32 columns at a time keep the temporaries at 8 registers next to the A fragments and accumulators.
 template <int H>            // one butterfly level over lane bit 4H: 2H values in, H out
 __device__ __forceinline__ void max_scatter_level(float (&v)[8], int lane) {
@@ -336,10 +336,10 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
             for (int s = 0; s < Cfg::KB2 * 4; ++s) fence_frag(a2[s]);
 
             // ---- layer 3 + section max.  Warp-uniform shape of the warp's 16 rows: sections are contiguous runs and
-            //      the rows past nrows (sect -1) a suffix, so the rows 1..15 that start a new section give the number
-            //      of sections.  One or two sections (almost every warp at C1 >= 128) take section_max_32 per section;
-            //      three or more the segmented suffix max below.  +bias, ReLU, TF32 rounding commute with the max
-            //      (monotone), values >= 0 so the integer atomicMax on the float bits is exact.
+            //      the rows past nrows (sect -1) a suffix, so the rows that start a section give the warp's sections;
+            //      each takes its own section_max_32 passes (1 or 2 sections in almost every warp at C1 >= 128, up to
+            //      16 at the small scales).  +bias, ReLU, TF32 rounding commute with the max (monotone), values >= 0
+            //      so the integer atomicMax on the float bits is exact.
             int *feat = (int *)(p.out + (size_t)b * p.feat_pitch * p.ld_feat);
             for (int nc = 0; nc < Cfg::NCH3; ++nc) {
                 float acc3[Cfg::N3 / 2];
@@ -370,66 +370,21 @@ pointnet_tc_kernel(const __grid_constant__ fcn_pointnet_args p) {
                 fence_acc(acc3);
                 release_prev();
                 // the warp's section shape (re-read per chunk from shared memory rather than held in registers
-                // through the MMAs)
+                // through the MMAs): bit i of `starts` marks row i of the warp's 16 as the first of a section in
+                // them (row 0 whenever it is below nrows); the rows past nrows (sect -1) start nothing
                 const int sa = sect_s[ra], sb = sect_s[ra + 8];
                 const int r0 = ra - g, rl = r0 + (lane & 15);
-                const int s0 = sect_s[r0], sl = sect_s[rl];
-                const unsigned starts =
-                    __ballot_sync(0xffffffffu, lane >= 1 && lane < 16 && sl >= 0 && sl != sect_s[rl - 1]);
-                const int nsec = s0 < 0 ? 0 : 1 + __popc(starts);
-                const int s1 = nsec == 2 ? sect_s[r0 + __ffs(starts) - 1] : -1;
-                if (nsec == 0) continue;
-                if (nsec <= 2) {
-                    const int c0 = nc * Cfg::N3;
+                const int sl = sect_s[rl];
+                unsigned starts =
+                    __ballot_sync(0xffffffffu, lane < 16 && sl >= 0 && (lane == 0 || sl != sect_s[rl - 1]));
+                const int c0 = nc * Cfg::N3;
+                while (starts) {                       // one reduce-scatter pass per section, 0..16 of them
+                    const int s = __shfl_sync(0xffffffffu, sl, __ffs(starts) - 1);
+                    starts &= starts - 1;
     #pragma unroll
-                    for (int h = 0; h < Cfg::N3 / 32; ++h) {
-                        section_max_32(acc3, 4 * h, sa == s0, sb == s0, feat + (size_t)s0 * p.ld_feat + c0, b3s + c0,
+                    for (int h = 0; h < Cfg::N3 / 32; ++h)
+                        section_max_32(acc3, 4 * h, sa == s, sb == s, feat + (size_t)s * p.ld_feat + c0, b3s + c0,
                                        lane);
-                        if (nsec == 2)
-                            section_max_32(acc3, 4 * h, sa == s1, sb == s1, feat + (size_t)s1 * p.ld_feat + c0,
-                                           b3s + c0, lane);
-                    }
-                    continue;
-                }
-                // segmented suffix max: rows ra (fragment half 0) and ra + 8 (half 1) of this thread; the suffix max
-                // over the rows of a section runs over the 8 lanes l/4 = 0..7 of each half, then half 0 takes in
-                // half 1's head when the section crosses row 8 of the warp
-                const int s8 = sect_s[r0 + 8];
-                unsigned oka = 0, okb = 0;             // bit d: row + (1 << d) is in the same section and 8-row half
-    #pragma unroll
-                for (int d = 0; d < 3; ++d) {
-                    const int o = 1 << d;
-                    if (g + o < 8 && sa >= 0 && sect_s[ra + o] == sa) oka |= 1u << d;
-                    if (g + o < 8 && sb >= 0 && sect_s[ra + 8 + o] == sb) okb |= 1u << d;
-                }
-                const bool merge_a = sa >= 0 && sa == s8;
-                const bool head_a = sa >= 0 && (g == 0 || sect_s[ra - 1] != sa);
-                const bool head_b = sb >= 0 && sect_s[ra + 7] != sb;
-    #pragma unroll
-                for (int j = 0; j < Cfg::N3 / 8; ++j) {
-                    float v[4] = {acc3[4 * j], acc3[4 * j + 1], acc3[4 * j + 2], acc3[4 * j + 3]};
-    #pragma unroll
-                    for (int d = 0; d < 3; ++d) {
-    #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const float x = __shfl_down_sync(0xffffffffu, v[e], 4 << d);
-                            if (((e < 2 ? oka : okb) >> d) & 1u) v[e] = fmaxf(v[e], x);
-                        }
-                    }
-    #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const float x = __shfl_sync(0xffffffffu, v[2 + e], lane & 3);   // row 8 of this warp
-                        if (merge_a) v[e] = fmaxf(v[e], x);
-                    }
-                    const int c = nc * Cfg::N3 + 8 * j + 2 * q;
-                    const float2 bb = *(const float2 *)(b3s + c);
-    #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const bool head = e < 2 ? head_a : head_b;
-                        const float o = to_tf32(v[e] + ((e & 1) ? bb.y : bb.x));
-                        if (head && o > 0.f)
-                            atomicMax(feat + (size_t)(e < 2 ? sa : sb) * p.ld_feat + c + (e & 1), __float_as_int(o));
-                    }
                 }
             }
             if (!STAGE_AFTER_L2 && it + 1 < my_tiles) stage_rec((it + 1) & 1, rec_next, td_next.z);
