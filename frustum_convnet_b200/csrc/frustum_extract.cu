@@ -127,7 +127,7 @@ static int fx_check(const fcn_frustum_extract_args *a, const char *fn, int *max_
     if (a->num_frames == 0 || a->num_dets == 0) return FCN_OK;
     if (!a->scan_offsets || !a->frames || !a->boxes || !a->det_frame || (a->num_points > 0 && !a->scans))
         return invalid(fn, "NULL pointer");
-    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, max_n);
+    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, 16, max_n);
 }
 
 static int fx_prepare(const fcn_frustum_extract_args *a, const char *fn, FxWs &w, int *max_n) {

@@ -123,13 +123,19 @@ cudaError_t fov_carve(Carve &c, int num_points, int num_jobs, bool uv, FovWs &w)
     return job_carve(c, num_jobs, t0, w);
 }
 
+cudaError_t job_reset(const JobWs &w, int num_jobs, cudaStream_t s) {
+    cudaError_t e;
+    if ((e = cudaMemsetAsync(w.keep + num_jobs, 0, 4, s)) != cudaSuccess ||
+        (e = cudaMemsetAsync(w.cnt + num_jobs, 0, 8, s)) != cudaSuccess)
+        return e;
+    return cudaMemsetAsync(w.bad, 0, 4, s);
+}
+
 cudaError_t fov_stage(const FovWs &w, int num_points, int num_jobs, int num_frames, int max_n, const void *scans,
                       const int32_t *scan_offsets, const fcn_frustum_frame *frames, cudaStream_t s) {
     cudaError_t e;
     if ((e = cudaMemsetAsync(w.flags + num_points, 0, 4, s)) != cudaSuccess ||
-        (e = cudaMemsetAsync(w.keep + num_jobs, 0, 4, s)) != cudaSuccess ||
-        (e = cudaMemsetAsync(w.cnt + num_jobs, 0, 8, s)) != cudaSuccess ||
-        (e = cudaMemsetAsync(w.bad, 0, 4, s)) != cudaSuccess)
+        (e = job_reset(w, num_jobs, s)) != cudaSuccess)
         return e;
     const float4 *pts = (const float4 *)scans;
     const dim3 grid(ceil_div(max_n, FX_THREADS), num_frames);

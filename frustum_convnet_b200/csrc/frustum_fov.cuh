@@ -38,7 +38,10 @@ cudaError_t job_carve(Carve &c, int num_jobs, size_t min_temp_bytes, JobWs &w);
 // Takes the shared pieces for num_points scan points and num_jobs jobs from c (fov_u, fov_v only when uv).
 cudaError_t fov_carve(Carve &c, int num_points, int num_jobs, bool uv, FovWs &w);
 
-// The in-image stage of a count entry on stream s: clears the scan tails and the bad counter, then flags every scan
+// The start of every count entry on stream s: clears the tails of the keep and cnt scans and the bad counter.
+cudaError_t job_reset(const JobWs &w, int num_jobs, cudaStream_t s);
+
+// The in-image stage of a count entry on stream s: clears the flag scan's tail, job_reset, then flags every scan
 // point, scans the flags into pos and compacts the in-image points of each frame, in scan order, to fov_pts (and
 // fov_u, fov_v).  max_n is the largest scan (check_scans), the x extent of the flag and compact grids.
 cudaError_t fov_stage(const FovWs &w, int num_points, int num_jobs, int num_frames, int max_n, const void *scans,
@@ -104,13 +107,17 @@ __device__ __forceinline__ void job_scatter(int p0, int p1, int c, long long bas
     }
 }
 
-// Host check of the scans every extractor takes: 16-byte-aligned float4 points and the host copy of the scan offsets
-// (num_frames + 1 entries).  Raises *max_n (0 on entry) to the largest scan, the x extent of the flag and compact
-// grids.
+// Host check of the scans every extractor takes: points aligned to `align` bytes (16 for the KITTI float4 points, 4
+// for SUN-RGBD's 6-float rows) and the host copy of the scan offsets (num_frames + 1 entries).  Raises *max_n (0 on
+// entry) to the largest scan, the x extent of the flag and compact grids.
 inline int check_scans(const char *fn, const int32_t *host_so, int num_frames, int num_points, const void *scans,
-                       int *max_n) {
+                       int align, int *max_n) {
     if (!host_so) return invalid(fn, "NULL host_scan_offsets");
-    if (((uintptr_t)scans & 15) != 0) return invalid(fn, "scans must be 16-byte aligned");
+    if (((uintptr_t)scans & (align - 1)) != 0) {
+        char msg[32];
+        snprintf(msg, sizeof(msg), "scans must be %d-byte aligned", align);
+        return invalid(fn, msg);
+    }
     if (!offsets_ok(host_so, num_frames, num_points))
         return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
     for (int f = 0; f < num_frames; ++f)

@@ -93,7 +93,7 @@ static int gx_check(const fcn_gt_extract_args *a, const char *fn, int *max_n) {
     if (!a->scan_offsets || !a->frames || !a->jobs || (a->num_labels > 0 && !a->label_boxes) ||
         (a->num_points > 0 && !a->scans))
         return invalid(fn, "NULL pointer");
-    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, max_n);
+    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, 16, max_n);
 }
 
 static int gx_prepare(const fcn_gt_extract_args *a, const char *fn, FovWs &w, int *max_n) {

@@ -265,7 +265,7 @@ static int rx_check(const fcn_refine_extract_args *a, const char *fn, int *max_n
         (a->num_dets == 0 || !a->det_frame || !a->gt_offsets || !a->pair_offsets ||
          (a->num_pairs > 0 && (!a->gt_corners || !a->det_corners))))
         return invalid(fn, "matched mode needs num_dets > 0 and det_frame, gt_offsets, pair_offsets and corners");
-    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, max_n);
+    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, 16, max_n);
 }
 
 static int rx_prepare(const fcn_refine_extract_args *a, const char *fn, RxWs &w, int *max_n) {

@@ -214,14 +214,7 @@ static int sx_check(const fcn_sunrgbd_extract_args *a, const char *fn, int *max_
     if (!a->scan_offsets || !a->frames || !a->jobs || (a->labelled && !a->label_boxes) ||
         (a->num_points > 0 && !a->scans))
         return invalid(fn, "NULL pointer");
-    if (!a->host_scan_offsets) return invalid(fn, "NULL host_scan_offsets");
-    if (((uintptr_t)a->scans & 3) != 0) return invalid(fn, "scans must be 4-byte aligned");
-    if (!offsets_ok(a->host_scan_offsets, a->num_frames, a->num_points))
-        return invalid(fn, "scan offsets must start at 0, never decrease and end at num_points");
-    for (int f = 0; f < a->num_frames; ++f)
-        if (a->host_scan_offsets[f + 1] - a->host_scan_offsets[f] > *max_n)
-            *max_n = a->host_scan_offsets[f + 1] - a->host_scan_offsets[f];
-    return FCN_OK;
+    return check_scans(fn, a->host_scan_offsets, a->num_frames, a->num_points, a->scans, 4, max_n);
 }
 
 static int sx_prepare(const fcn_sunrgbd_extract_args *a, const char *fn, SxWs &w, int *max_n) {
@@ -251,10 +244,7 @@ extern "C" int fcn_sunrgbd_extract_project(const fcn_sunrgbd_extract_args *a, fc
     const int st = sx_prepare(a, __func__, w, &max_n);
     if (st != FCN_OK || sx_empty(a)) return st;
     cudaStream_t s = (cudaStream_t)stream;
-    const int J = a->num_jobs;
-    FCN_CUDA(cudaMemsetAsync(w.keep + J, 0, 4, s));
-    FCN_CUDA(cudaMemsetAsync(w.cnt + J, 0, 8, s));
-    FCN_CUDA(cudaMemsetAsync(w.bad, 0, 4, s));
+    FCN_CUDA(job_reset(w, a->num_jobs, s));
     if (max_n == 0) return FCN_OK;
     sx_project_kernel<<<dim3(ceil_div(max_n, FX_THREADS), a->num_frames), FX_THREADS, 0, s>>>(
         a->scans, a->scan_offsets, a->frames, w.u, w.v);

@@ -130,43 +130,52 @@ def read_counts(summary, n, who, bad_what):
     return K, M, words, kept
 
 
-def run_extract(family, a, sc, so, n, word_fields, outputs, dev, stream, timer, bad_what, extra_words=0, before=None):
-    """The two device calls of an extractor family ('frustum_extract', 'refine_extract', 'gt_extract') on the current
-    stream `stream`.  a: the family's args struct with its counts and inputs filled; sc, so: scan_table's scans and
-    host scan offsets.  Uploads the scans, queries the workspace, runs fcn_<family>_count into one summary (info, then
-    the per-job int32 words: n of them for each args field of word_fields), reads it back once (read_counts, naming
-    bad_what), then runs fcn_<family>_write into new points, offsets and the tensors of outputs(K, M, words), a dict
-    {args field: tensor or None}.  `timer(name)` (optional) marks "start", "count", "write_start" and "write".
-    extra_words int32 words follow the fields' words in the summary; before(their device address) (optional) runs just
-    before the count call, so a job-building launch can leave per-job words in the same read.
+def run_extract(family, a, sc, so, n, word_fields, outputs, dev, stream, timer, bad_what, extra_words=0, count=None,
+                cols=4):
+    """The two device calls of an extractor family ('frustum_extract', 'refine_extract', 'gt_extract',
+    'sunrgbd_extract') on the current stream `stream`.  a: the family's args struct with its counts and inputs filled;
+    sc, so: the frames' scans and host scan offsets.  Uploads the scans, queries the workspace, runs the count into one
+    summary (info, then the per-job int32 words: n of them for each args field of word_fields, then extra_words more),
+    reads it back once (read_counts, naming bad_what), then runs fcn_<family>_write into new points (M, cols),
+    offsets and the tensors of outputs(K, M, words), a dict {args field: tensor or None}.
+    count(the summary's int32 words on the device) enqueues the count-side device work and marks its own timer
+    names; the default runs fcn_<family>_count and marks "count".  A family whose count is several calls, or which
+    builds its jobs on the device (writing per-job words into the extra words), passes its own.  `timer(name)`
+    (optional) also marks "start" before the count, "write_start" and "write".
     -> (the int32 words, the kept jobs, {args field: output tensor}, points and offsets included)."""
+    mark = timer if timer is not None else (lambda name: None)
+    if count is None:
+        def count(words):
+            _lib.call("fcn_%s_count" % family, C.byref(a), stream.cuda_stream)
+            mark("count")
     scan_dev = upload_scans(sc, dev)            # like so and the caller's upload, alive until the write is enqueued
     a.scans = scan_dev.data_ptr() if int(so[-1]) > 0 else None
     a.host_scan_offsets = so.ctypes.data
     ws, nbytes = workspace("fcn_%s_workspace_bytes" % family, dev, C.byref(a))
     summary = torch.empty(4 + (len(word_fields) * n + extra_words + 1) // 2, dtype=torch.int64, device=dev)
+    words_dev = summary[4:].view(torch.int32)
     a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), nbytes, summary.data_ptr()
     for k, field in enumerate(word_fields):
-        setattr(a, field, summary.data_ptr() + 32 + 4 * n * k)
-    if timer is not None:
-        timer("start")
-    if before is not None:
-        before(summary.data_ptr() + 32 + 4 * n * len(word_fields))
-    _lib.call("fcn_%s_count" % family, C.byref(a), stream.cuda_stream)
-    if timer is not None:
-        timer("count")
+        setattr(a, field, words_dev.data_ptr() + 4 * n * k)
+    mark("start")
+    count(words_dev)
     K, M, words, kept = read_counts(summary, n, "fcn_" + family, bad_what)
-    out = {"points": torch.empty((M, 4), dtype=torch.float32, device=dev),
+    out = {"points": torch.empty((M, cols), dtype=torch.float32, device=dev),
            "offsets": torch.empty(K + 1, dtype=torch.int32, device=dev), **outputs(K, M, words)}
     a.num_kept, a.num_out_points = K, M
     for field, t in out.items():
         setattr(a, field, None if t is None else t.data_ptr())
-    if timer is not None:
-        timer("write_start")
+    mark("write_start")
     _lib.call("fcn_%s_write" % family, C.byref(a), stream.cuda_stream)
-    if timer is not None:
-        timer("write")
+    mark("write")
     return words, kept, out
+
+
+def empty_outputs(dev, cols, labels):
+    """The device tensors of an extraction without frustums: points (0, cols) float32, offsets [0] int32 and label
+    (0,) uint8, or None without labels."""
+    return (torch.zeros((0, cols), dtype=torch.float32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev),
+            torch.zeros(0, dtype=torch.uint8, device=dev) if labels else None)
 
 
 class LabelledFrustums:
@@ -243,10 +252,8 @@ class FrustumExtractor:
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
             if F == 0 or D == 0:
-                return self._result(torch.zeros((0, 4), dtype=torch.float32, device=dev),
-                                    torch.zeros(1, dtype=torch.int32, device=dev), *self._empty(dev),
-                                    np.zeros(0, np.int64), [], id_list, type_list, prob_list, box2d_list, calibs,
-                                    image_hw)
+                return self._result(*empty_outputs(dev, 4, False)[:2], *self._empty(dev), np.zeros(0, np.int64), [],
+                                    id_list, type_list, prob_list, box2d_list, calibs, image_hw)
             inp, ptrs = upload([bytes(frames), boxes, so, det_frame], dev)
             a = _lib.FrustumExtractArgs()
             a.num_frames, a.num_points, a.num_dets = F, N, D

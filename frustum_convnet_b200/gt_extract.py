@@ -38,7 +38,7 @@ import torch
 
 from . import _lib
 from ._host import cuda_device, upload
-from .frustum_extract import LabelledFrustums, frame_order, run_extract, scan_table
+from .frustum_extract import LabelledFrustums, empty_outputs, frame_order, run_extract, scan_table
 from .refine_extract import _check_box, box_record, iou_thresh, obj_array, objects_of
 
 SHIFT_RATIO = 0.1          # random_shift_box2d(box2d, H, W, 0.1) of the training sets (prepare_data.py:187, :321)
@@ -255,10 +255,8 @@ class GtFrustumExtractor:
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
             if F == 0 or J == 0:
-                return GtFrustums(torch.zeros((0, 4), dtype=torch.float32, device=dev),
-                                  torch.zeros(1, dtype=torch.int32, device=dev),
-                                  torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.int64),
-                                  np.zeros(0, np.int64), job_lists([], calibs), stream)
+                return GtFrustums(*empty_outputs(dev, 4, True), np.zeros(0, np.int64), np.zeros(0, np.int64),
+                                  job_lists([], calibs), stream)
             sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "GtFrustumExtractor")
             job_rec = np.zeros(J, dtype=np.dtype(_lib.GtJob))
             job_rec["box"] = np.stack([jb["cut"] for jb in jobs])

@@ -49,7 +49,7 @@ import torch
 
 from . import _lib
 from ._host import csr_offsets, cuda_device, upload
-from .frustum_extract import LabelledFrustums, frame_order, run_extract, scan_table
+from .frustum_extract import LabelledFrustums, empty_outputs, frame_order, run_extract, scan_table
 from .kitti_eval import detection_records
 from .train_inputs import KITTI_CLASSES
 
@@ -248,6 +248,13 @@ def job_table(mode, image_ids, objects, gt_objects, type_whitelist, remove_diff=
     return jobs, gts
 
 
+def gt_table(frame_ids, gts):
+    """The ground truth {frame id: [KittiObject]} of the frames frame_ids (none without an entry) -> (their objects
+    in frame_ids order, each frame's first position among them: F + 1 int32 offsets)."""
+    per_frame = [gts.get(k, []) for k in frame_ids]
+    return [o for g in per_frame for o in g], csr_offsets([len(g) for g in per_frame])
+
+
 def check_matched_extents(jobs, gt_flat, job_gt):
     """Matched mode: extract_frustum_det_data triangulates a detection's box and its ground truth's only once the
     detection is matched (:493-532), so only matched pairs need positive extents.  job_gt[j] >= 0: job j matched
@@ -335,60 +342,36 @@ class RefineFrustumExtractor:
             dets = objects_from_detections(dets)
         return {int(i): list(dets.get(int(i), [])) for i in image_ids}
 
-    # ------------------------------------------------------------------ device call
+    # ------------------------------------------------------------------ device calls
     def _run(self, mode, scans, calibs, image_hw, jobs, gts, stream, timer):
         dev = self.device
         frame_ids, fpos = frame_order(jb["frame"] for jb in jobs)
-        gt_flat, gt_off = [], [0]
-        for k in frame_ids:
-            gt_flat += gts.get(k, [])
-            gt_off.append(len(gt_flat))
-        gt_base = {k: gt_off[fpos[k]] for k in frame_ids}
-        J, F, G = len(jobs), len(frame_ids), len(gt_flat)
+        gt_flat, gt_off = gt_table(frame_ids, gts)
+        J = len(jobs)
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
-            if F == 0 or J == 0:
-                return self._result(mode, torch.zeros((0, 4), dtype=torch.float32, device=dev),
-                                    torch.zeros(1, dtype=torch.int32, device=dev),
-                                    None if mode == _lib.REFINE_DET else torch.zeros(0, dtype=torch.uint8, device=dev),
-                                    np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, np.int64), jobs,
-                                    gt_flat, calibs, stream)
-            sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "RefineFrustumExtractor")
-            job_box = np.array([box_record(jb["cut"]) for jb in jobs], dtype=np.dtype(_lib.RefineBox))
+            if J == 0:
+                return self._result(mode, *empty_outputs(dev, 4, mode != _lib.REFINE_DET), np.zeros(0, np.int64),
+                                    np.zeros(0, np.int64), np.zeros(0, np.int64), jobs, gt_flat, calibs, stream)
             job_frame = np.array([fpos[jb["frame"]] for jb in jobs], dtype=np.int32)
-            gt_box = np.array([box_record(obj_array(o)) for o in gt_flat], dtype=np.dtype(_lib.RefineBox))
             if mode == _lib.REFINE_GT:
-                job_ref = np.array([gt_base[jb["frame"]] + jb["gt"] for jb in jobs], dtype=np.int32)
+                job_ref = np.array([gt_off[f] + jb["gt"] for f, jb in zip(job_frame, jobs)], dtype=np.int32)
             elif mode == _lib.REFINE_MATCHED:
                 job_ref = np.arange(J, dtype=np.int32)                 # one job per detection
             else:
                 job_ref = np.zeros(J, dtype=np.int32)
-            parts = [bytes(frames), job_box, so, job_frame, job_ref, gt_box]
-            D = P = 0
-            if mode == _lib.REFINE_MATCHED:
-                D = J
-                po = csr_offsets([gt_off[f + 1] - gt_off[f] for f in job_frame])
-                P = int(po[-1])
-                det_c = iou_corners(np.stack([jb["box"] for jb in jobs]))
-                gt_c = iou_corners(np.stack([obj_array(o) for o in gt_flat]))
-                parts += [det_c, gt_c, np.asarray(gt_off, np.int32), po]
-            inp, ptrs = upload(parts, dev)
             a = _lib.RefineExtractArgs()
-            a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, F, int(so[-1]), J, G
-            a.num_dets, a.num_pairs, a.iou_thresh = D, P, self.iou_thresh
-            a.frames, a.jobs, a.scan_offsets, a.job_frame, a.job_ref = ptrs[:5]
-            a.gt_boxes = ptrs[5] if G > 0 else None
+            parts = [(a, "jobs", np.array([box_record(jb["cut"]) for jb in jobs], dtype=np.dtype(_lib.RefineBox))),
+                     (a, "job_frame", job_frame), (a, "job_ref", job_ref)]
             if mode == _lib.REFINE_MATCHED:
-                a.det_frame = a.job_frame
-                a.det_corners, a.gt_corners, a.gt_offsets, a.pair_offsets = ptrs[6:10]
+                parts.append((a, "det_corners", iou_corners(np.stack([jb["box"] for jb in jobs]))))
 
-            def outputs(K, M, words):
+            def check(words):
                 if mode == _lib.REFINE_MATCHED:
                     check_matched_extents(jobs, gt_flat, words[J:2 * J])
-                return {"labels": None if mode == _lib.REFINE_DET else torch.empty(M, dtype=torch.uint8, device=dev)}
 
-            words, kept, out = run_extract("refine_extract", a, sc, so, J, ("job_points", "job_gt"), outputs, dev,
-                                           stream, timer, "jobs or pairs reference no frame or box")
+            words, kept, out = self._extract(a, mode, scans, calibs, image_hw, frame_ids, gt_flat, gt_off, job_frame,
+                                             parts, check, stream, timer)
         job_points, job_gt = words[:J], words[J:2 * J]
         return self._result(mode, out["points"], out["offsets"], out["labels"], job_points[kept].astype(np.int64),
                             kept.astype(np.int64), job_gt[kept].astype(np.int64), jobs, gt_flat, calibs, stream)
@@ -396,6 +379,7 @@ class RefineFrustumExtractor:
     def _run_collected(self, mode, scans, calibs, image_hw, image_ids, collected, gt, remove_diff, strides, stream,
                        timer):
         dev = self.device
+        mark = timer if timer is not None else (lambda name: None)
         strides = [float(s) for s in strides]
         if not 1 <= len(strides) <= _lib.MAX_SCALES:
             raise ValueError("need 1..%d strides" % _lib.MAX_SCALES)
@@ -405,10 +389,7 @@ class RefineFrustumExtractor:
             gts = {int(i): ground_truth_boxes(gt[int(i)], self.type_whitelist, remove_diff) for i in image_ids}
         plan = collected_plan(image_ids, collected, self.type_whitelist, gts)
         frame_ids, J = plan["frame_ids"], int(plan["offsets"][-1])
-        gt_flat, gt_off = [], [0]
-        for k in frame_ids:
-            gt_flat += gts[k] if gts is not None else []
-            gt_off.append(len(gt_flat))
+        gt_flat, gt_off = gt_table(frame_ids, gts or {})
         G = len(gt_flat)
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
         with torch.cuda.device(dev), torch.cuda.stream(stream):
@@ -416,55 +397,40 @@ class RefineFrustumExtractor:
                 stream.wait_stream(collected.stream)
             if J == 0:
                 return CollectedRefineFrustums.empty(mode, dev, strides, stream)
-            sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "RefineFrustumExtractor")
-            gt_arr = [obj_array(o) for o in gt_flat]
-            parts = [bytes(frames), so, plan["offsets"], plan["row"], plan["frame"], plan["image"], plan["class"],
-                     np.array([box_record(a) for a in gt_arr], dtype=np.dtype(_lib.RefineBox))]
-            if mode == _lib.REFINE_MATCHED:
-                job_frame = np.repeat(plan["frame"], np.diff(plan["offsets"]))
-                po = csr_offsets(np.diff(np.asarray(gt_off, np.int64))[job_frame])
-                parts += [iou_corners(np.stack(gt_arr)) if G else np.zeros(0), np.asarray(gt_off, np.int32), po,
-                          gt_terms(gt_flat, gt_arr)]
-            inp, ptrs = upload(parts, dev)
             f64 = lambda *shape: torch.empty(shape, dtype=torch.float64, device=dev)
             i32 = lambda n: torch.empty(n, dtype=torch.int32, device=dev)
             jobs = f64(J, 8)                                       # fcn_refine_box
-            job_frame_d, job_ref = i32(J), i32(J)
+            job_frame, job_ref = i32(J), i32(J)
             job_data = torch.empty((J, C.sizeof(_lib.RefineJobData)), dtype=torch.uint8, device=dev)
             det_c = f64(J, 24) if mode == _lib.REFINE_MATCHED else None
             ja = _lib.RefineJobsArgs()
             ja.mode, ja.num_pieces, ja.num_jobs, ja.num_rows = mode, len(plan["row"]), J, collected.num_rows
             ja.rows = collected.rows.data_ptr()
-            ja.piece_offsets, ja.piece_row, ja.piece_frame, ja.piece_image, ja.piece_class = ptrs[2:7]
             ja.host_piece_offsets, ja.host_piece_row = plan["offsets"].ctypes.data, plan["row"].ctypes.data
-            ja.jobs, ja.job_frame, ja.job_ref = jobs.data_ptr(), job_frame_d.data_ptr(), job_ref.data_ptr()
             ja.job_data = job_data.data_ptr()
-            ja.det_corners = None if det_c is None else det_c.data_ptr()
-
-            def build_jobs(status_ptr):
-                ja.status = status_ptr
-                _lib.call("fcn_refine_jobs_from_rows", C.byref(ja), stream.cuda_stream)
-
             a = _lib.RefineExtractArgs()
-            a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, len(frame_ids), int(so[-1]), J, G
-            a.iou_thresh = self.iou_thresh
-            a.frames, a.scan_offsets = ptrs[0], ptrs[1]
-            a.jobs, a.job_frame, a.job_ref = jobs.data_ptr(), job_frame_d.data_ptr(), job_ref.data_ptr()
-            a.gt_boxes = ptrs[7] if G > 0 else None
-            if mode == _lib.REFINE_MATCHED:
-                a.num_dets, a.num_pairs = J, int(po[-1])
-                a.det_frame, a.det_corners = a.job_frame, det_c.data_ptr()
-                a.gt_corners, a.gt_offsets, a.pair_offsets = ptrs[8:11]
-
-            def outputs(K, M, words):
-                check_collected(mode, plan, collected, words[J:2 * J], words[2 * J:3 * J], gt_flat, gt_arr)
-                return {"labels": None if mode == _lib.REFINE_DET else torch.empty(M, dtype=torch.uint8, device=dev)}
-
-            words, kept, out = run_extract("refine_extract", a, sc, so, J, ("job_points", "job_gt"), outputs, dev,
-                                           stream, timer, "jobs or pairs reference no frame or box", J, build_jobs)
-            K, S = len(kept), len(strides)
+            for args in (ja, a):                # the jobs ja writes and a reads
+                args.jobs, args.job_frame, args.job_ref = jobs.data_ptr(), job_frame.data_ptr(), job_ref.data_ptr()
+                args.det_corners = None if det_c is None else det_c.data_ptr()
             labels = mode == _lib.REFINE_MATCHED
-            kept_d = torch.from_numpy(kept.astype(np.int32)).to(dev, non_blocking=False)
+            gt_arr = [obj_array(o) for o in gt_flat]
+            terms = gt_terms(gt_flat, gt_arr) if labels else None       # host work, ahead of the device calls
+
+            def count(words):                   # the jobs' status words follow job_points and job_gt
+                ja.status = words.data_ptr() + 8 * J
+                _lib.call("fcn_refine_jobs_from_rows", C.byref(ja), stream.cuda_stream)
+                _lib.call("fcn_refine_extract_count", C.byref(a), stream.cuda_stream)
+                mark("count")
+
+            words, kept, out = self._extract(
+                a, mode, scans, calibs, image_hw, frame_ids, gt_flat, gt_off,
+                np.repeat(plan["frame"], np.diff(plan["offsets"])),
+                [(ja, "piece_" + k, plan[k]) for k in ("offsets", "row", "frame", "image", "class")],
+                lambda words: check_collected(mode, plan, collected, words[J:2 * J], words[2 * J:3 * J], gt_flat,
+                                              gt_arr),
+                stream, timer, count, J)
+            K, S = len(kept), len(strides)
+            tab, tptrs = upload([kept.astype(np.int32)] + ([words[J:2 * J], terms] if labels else []), dev)
             lists = f64(K, _lib.REFINE_LIST_COLS)
             records = torch.zeros((K, C.sizeof(_lib.TrainFrustum)), dtype=torch.uint8, device=dev)
             rwords = torch.empty((K, S + 1), dtype=torch.int32, device=dev)
@@ -472,17 +438,13 @@ class RefineFrustumExtractor:
             ta.mode, ta.labels, ta.num_kept, ta.num_jobs, ta.num_gt, ta.num_scales = mode, int(labels), K, J, G, S
             for q, st in enumerate(strides):
                 ta.stride[q] = st
-            ta.kept, ta.job_data = kept_d.data_ptr(), job_data.data_ptr()
-            job_gt_d = None
+            ta.kept, ta.job_data = tptrs[0], job_data.data_ptr()
             if labels:
-                job_gt_d = torch.from_numpy(np.ascontiguousarray(words[J:2 * J])).to(dev)
-                ta.job_gt, ta.gt_terms = job_gt_d.data_ptr(), ptrs[11]
+                ta.job_gt, ta.gt_terms = tptrs[1:]
             ta.lists, ta.records, ta.words = lists.data_ptr(), records.data_ptr(), rwords.data_ptr()
-            if timer is not None:
-                timer("table_start")
+            mark("table_start")
             _lib.call("fcn_refine_frustum_table", C.byref(ta), stream.cuda_stream)
-            if timer is not None:
-                timer("table")
+            mark("table")
         pk = np.searchsorted(plan["offsets"], kept, side="right") - 1
         kept_gt = words[J:2 * J][kept].astype(np.int64)
         return CollectedRefineFrustums(mode, out["points"], out["offsets"], out["labels"],
@@ -490,6 +452,38 @@ class RefineFrustumExtractor:
                                        plan["image"][pk].tolist(), [plan["types"][p] for p in pk.tolist()],
                                        bool((plan["class"][pk] >= 0).all()), lists, records, rwords, strides,
                                        kept_gt, gt_flat, calibs, stream)
+
+    def _extract(self, a, mode, scans, calibs, image_hw, frame_ids, gt_flat, gt_off, job_frame, parts, check, stream,
+                 timer, count=None, extra_words=0):
+        """Both job sources' run_extract into the RefineExtractArgs `a`, jobs in frames job_frame.  The frames, the
+        ground truth (gt_table's) and, in matched mode, its corners and pair offsets go up in one copy with `parts`,
+        the job source's (struct, field, host array) triples, each field set to its array's device address.
+        check(words) runs before the outputs are allocated.  -> run_extract's (words, kept, out)."""
+        dev = self.device
+        J, G = len(job_frame), len(gt_flat)
+        sc, frames, so = scan_table(scans, calibs, image_hw, frame_ids, dev, "RefineFrustumExtractor")
+        gt_arr = [obj_array(o) for o in gt_flat]
+        common = [bytes(frames), so, np.array([box_record(g) for g in gt_arr], dtype=np.dtype(_lib.RefineBox))]
+        if mode == _lib.REFINE_MATCHED:
+            po = csr_offsets(np.diff(gt_off)[job_frame])
+            common += [iou_corners(np.stack(gt_arr)) if G else np.zeros(0), gt_off, po]
+        inp, ptrs = upload(common + [p for _, _, p in parts], dev)
+        for (struct, field, _), ptr in zip(parts, ptrs[len(common):]):
+            setattr(struct, field, ptr)
+        a.mode, a.num_frames, a.num_points, a.num_jobs, a.num_gt = mode, len(frame_ids), int(so[-1]), J, G
+        a.iou_thresh = self.iou_thresh
+        a.frames, a.scan_offsets = ptrs[:2]
+        a.gt_boxes = ptrs[2] if G > 0 else None
+        if mode == _lib.REFINE_MATCHED:
+            a.num_dets, a.num_pairs, a.det_frame = J, int(po[-1]), a.job_frame
+            a.gt_corners, a.gt_offsets, a.pair_offsets = ptrs[3:6]
+
+        def outputs(K, M, words):
+            check(words)
+            return {"labels": None if mode == _lib.REFINE_DET else torch.empty(M, dtype=torch.uint8, device=dev)}
+
+        return run_extract("refine_extract", a, sc, so, J, ("job_points", "job_gt"), outputs, dev, stream, timer,
+                           "jobs or pairs reference no frame or box", extra_words, count)
 
     @staticmethod
     def _result(mode, points, offsets, label, counts, kept, kept_gt, jobs, gt_flat, calibs, stream):
@@ -629,8 +623,7 @@ class CollectedRefineFrustums(RefineFrustums):
     @classmethod
     def empty(cls, mode, dev, strides, stream):
         z = lambda *shape, dt=torch.float64: torch.zeros(shape, dtype=dt, device=dev)
-        return cls(mode, z(0, 4, dt=torch.float32), z(1, dt=torch.int32),
-                   None if mode == _lib.REFINE_DET else z(0, dt=torch.uint8), np.zeros(0, np.int64),
+        return cls(mode, *empty_outputs(dev, 4, mode != _lib.REFINE_DET), np.zeros(0, np.int64),
                    np.zeros(0, np.int64), [], [], True, z(0, _lib.REFINE_LIST_COLS),
                    z(0, C.sizeof(_lib.TrainFrustum), dt=torch.uint8), z(0, len(strides) + 1, dt=torch.int32), strides,
                    np.zeros(0, np.int64), [], {}, stream)

@@ -36,8 +36,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._host import csr_offsets, cuda_device, upload, workspace
-from .frustum_extract import LabelledFrustums, _scan, frame_order, upload_scans
+from ._host import csr_offsets, cuda_device, upload
+from .frustum_extract import LabelledFrustums, _scan, empty_outputs, frame_order, run_extract
 
 TYPE_WHITELIST = ("bed", "table", "sofa", "chair", "toilet", "desk", "dresser", "night_stand", "bookshelf",
                   "bathtub")                         # prepare_data.py:405-408 (--num_classes 10)
@@ -394,7 +394,8 @@ class SunrgbdFrustumExtractor:
             so = csr_offsets([s.shape[0] for s in sc])
             if J == 0:                                  # nothing to count: only the skipped jobs' box draws
                 replay(slots, perturb, rng, None)
-                return self._empty(dev, labelled, stream)
+                return SunrgbdFrustums(*empty_outputs(dev, 6, labelled), np.zeros(0, np.int64), np.zeros(0, np.int64),
+                                       _job_lists([], labelled), stream)
             frames = np.zeros(F, dtype=np.dtype(_lib.SunrgbdFrame))
             for k in frame_ids:
                 frames[fpos[k]]["Rtilt"] = np.asarray(mats[k][0], np.float64).reshape(9)
@@ -407,78 +408,55 @@ class SunrgbdFrustumExtractor:
             boxes = np.array([box_record(jb["obj"]) for jb in jobs] if labelled else np.zeros(0),
                              dtype=np.dtype(_lib.RefineBox))
             inp, (d_frames, d_jobs, d_boxes, d_so) = upload([frames, rec, boxes, so], dev)
-            scan_dev = upload_scans(sc, dev)
             a = _lib.SunrgbdExtractArgs()
             a.num_frames, a.num_points, a.num_jobs = F, int(so[-1]), J
             a.num_labels, a.labelled = (J if labelled else 0), int(labelled)
-            a.scans = scan_dev.data_ptr() if int(so[-1]) > 0 else None
-            a.scan_offsets, a.host_scan_offsets, a.frames, a.jobs = d_so, so.ctypes.data, d_frames, d_jobs
+            a.scan_offsets, a.frames, a.jobs = d_so, d_frames, d_jobs
             a.label_boxes = d_boxes if labelled else None
-            ws, nbytes = workspace("fcn_sunrgbd_extract_workspace_bytes", dev, C.byref(a))
-            summary = torch.empty(4 + J, dtype=torch.int64, device=dev)      # info, then 2 J int32 words
-            words = summary[4:].view(torch.int32)
-            a.workspace, a.workspace_bytes, a.info = ws.data_ptr(), nbytes, summary.data_ptr()
-            a.job_points, a.job_labelled = words.data_ptr(), words.data_ptr() + 4 * J
             jb_bytes = C.sizeof(_lib.GtJob)
             jobs_dev = inp[d_jobs - inp.data_ptr():d_jobs - inp.data_ptr() + J * jb_bytes]
-            mark("start")
-            _lib.call("fcn_sunrgbd_extract_project", C.byref(a), stream.cuda_stream)
-            mark("project")
-
-            def count(begin, end, cuts):
-                if perturb:
-                    rec["box"][begin:end] = cuts
-                    jobs_dev[begin * jb_bytes:end * jb_bytes].copy_(torch.from_numpy(rec[begin:end].view(np.uint8)))
-                a.job_begin, a.job_end = begin, end
-                mark("round_start")
-                _lib.call("fcn_sunrgbd_extract_count", C.byref(a), stream.cuda_stream)
-                mark("round_end")
-                return words[begin:end].cpu().numpy()
-
-            cuts, n, choices, rounds = replay(slots, perturb, rng, count, window)
-            mark("count")
             live = np.flatnonzero([not s["skip"] for s in slots])
-            job_choice = np.full(J, -1, np.int32)
-            ranks = np.zeros((len(choices), CAP), np.int32)
-            order = np.zeros((len(choices), CAP), np.int32)
-            for c, k in enumerate(sorted(choices)):       # job order
-                ch = np.asarray(choices[k])
-                order[c] = np.argsort(ch, kind="stable")
-                ranks[c] = ch[order[c]]
-                job_choice[np.searchsorted(live, k)] = c
-            sel, (d_choice, d_ranks, d_slots) = upload([job_choice, ranks, order], dev)
-            a.num_choices, a.job_choice, a.choice_ranks, a.choice_slots = len(choices), d_choice, d_ranks, d_slots
-            _lib.call("fcn_sunrgbd_extract_select", C.byref(a), stream.cuda_stream)
-            mark("select")
-            back = summary.cpu().numpy()
-            K, M, bad = int(back[0]), int(back[1]), int(back[2])
-            if bad:
-                raise RuntimeError("fcn_sunrgbd_extract: %d jobs reference no frame or label box, or disagree with "
-                                   "their draws" % bad)
-            kept_n = back[4:].view(np.int32)[:J]
-            kept = np.flatnonzero(kept_n >= 0)
-            assert len(kept) == K and int(kept_n[kept].sum()) == M
-            pts = torch.empty((M, 6), dtype=torch.float32, device=dev)
-            offsets = torch.empty(K + 1, dtype=torch.int32, device=dev)
-            label = torch.empty(M, dtype=torch.uint8, device=dev) if labelled else None
-            a.num_kept, a.num_out_points = K, M
-            a.points, a.offsets = pts.data_ptr(), offsets.data_ptr()
-            a.labels = label.data_ptr() if labelled else None
-            mark("write_start")
-            _lib.call("fcn_sunrgbd_extract_write", C.byref(a), stream.cuda_stream)
-            mark("write")
+            cuts = rounds = sel = None
+
+            def count(words):
+                nonlocal cuts, rounds, sel          # sel: the choice tables, alive until the write is enqueued
+                _lib.call("fcn_sunrgbd_extract_project", C.byref(a), stream.cuda_stream)
+                mark("project")
+
+                def count_round(begin, end, win):
+                    if perturb:
+                        rec["box"][begin:end] = win
+                        jobs_dev[begin * jb_bytes:end * jb_bytes].copy_(torch.from_numpy(rec[begin:end].view(np.uint8)))
+                    a.job_begin, a.job_end = begin, end
+                    mark("round_start")
+                    _lib.call("fcn_sunrgbd_extract_count", C.byref(a), stream.cuda_stream)
+                    mark("round_end")
+                    return words[begin:end].cpu().numpy()
+
+                cuts, n, choices, rounds = replay(slots, perturb, rng, count_round, window)
+                mark("count")
+                job_choice = np.full(J, -1, np.int32)
+                ranks = np.zeros((len(choices), CAP), np.int32)
+                order = np.zeros((len(choices), CAP), np.int32)
+                for c, k in enumerate(sorted(choices)):       # job order
+                    ch = np.asarray(choices[k])
+                    order[c] = np.argsort(ch, kind="stable")
+                    ranks[c] = ch[order[c]]
+                    job_choice[np.searchsorted(live, k)] = c
+                sel, (d_choice, d_ranks, d_slots) = upload([job_choice, ranks, order], dev)
+                a.num_choices, a.job_choice, a.choice_ranks, a.choice_slots = len(choices), d_choice, d_ranks, d_slots
+                _lib.call("fcn_sunrgbd_extract_select", C.byref(a), stream.cuda_stream)
+                mark("select")
+
+            words, kept, out = run_extract(
+                "sunrgbd_extract", a, sc, so, J, ("job_points", "job_labelled"),
+                lambda K, M, words: {"labels": torch.empty(M, dtype=torch.uint8, device=dev) if labelled else None},
+                dev, stream, timer, "jobs reference no frame or label box, or disagree with their draws", count=count,
+                cols=6)
         kept_slots = live[kept]
         for k in kept_slots.tolist():
             slots[k]["cut"] = cuts[k]
             slots[k]["calib"] = mats[slots[k]["frame"]]
         lists = _job_lists([slots[k] for k in kept_slots.tolist()], labelled)
-        return SunrgbdFrustums(pts, offsets, label, kept_n[kept].astype(np.int64), kept_slots.astype(np.int64), lists,
-                               stream, rounds)
-
-    @staticmethod
-    def _empty(dev, labelled, stream):
-        lists = _job_lists([], labelled)
-        return SunrgbdFrustums(torch.zeros((0, 6), dtype=torch.float32, device=dev),
-                               torch.zeros(1, dtype=torch.int32, device=dev),
-                               torch.zeros(0, dtype=torch.uint8, device=dev) if labelled else None,
-                               np.zeros(0, np.int64), np.zeros(0, np.int64), lists, stream)
+        return SunrgbdFrustums(out["points"], out["offsets"], out["labels"], words[kept].astype(np.int64),
+                               kept_slots.astype(np.int64), lists, stream, rounds)
